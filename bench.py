@@ -20,6 +20,9 @@ Chains are independent trajectories (one b2s handle / CUDA stream each), the uni
   config3/4/5  : the other configurations of BASELINE.json, device-timed in the same run (open3d_slam_b200/benchmarks.py)
   cpu_baseline : the CPU oracle (oracle/, "port" of the reference's Open3D path) on a bounded sample, rank 0 only
   --impl reference : the same workload on the host cores through the oracle only (no GPU code on that path)
+  --dump-outputs DIR : after the timed steps, what their last step computed, as DIR/<name>.npy (float64): every chain's
+          RegistrationResult of its last scan and its pose, and a fixed sample of chain 0's map (points sorted, then sampled
+          with a fixed seed), so that two builds can be compared output for output on identical inputs
 """
 from __future__ import annotations
 
@@ -63,7 +66,7 @@ def make_config(args):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -201,6 +204,24 @@ def cpu_baseline_sample(lp, ratio, n_sample):
     return {"value": n_sample / dt, "unit": UNIT, "cores": O.num_threads(), "kind": "port", "map_points": int(len(ch.map_x)),
             "sample": f"1 chain x {n_sample} consecutive scans on its steady-state map (crop+voxel+normals+select, KD-tree rebuild + ICP, map fusion), "
                       f"{O.num_threads()} OpenMP threads"}
+
+
+DUMP_MAP_ROWS = 1 << 17   # map points kept in the dump (48 B each as float64 xyz + normal)
+
+
+def dump_outputs(out_dir, results, poses, map_cloud):
+    """What the timed path handed back in its last step: per chain the RegistrationResult of its last scan and the pose state, plus
+    chain 0's map cloud sorted by coordinates and sampled with a fixed seed (rows are independent of the device's storage order)."""
+    os.makedirs(out_dir, exist_ok=True)
+    xyz, nrm = map_cloud
+    order = np.lexsort((xyz[:, 2], xyz[:, 1], xyz[:, 0]))
+    if len(order) > DUMP_MAP_ROWS:
+        order = order[np.sort(np.random.default_rng(0).choice(len(order), DUMP_MAP_ROWS, replace=False))]
+    arrays = {"transformation": np.array([r.transformation_ for r in results]), "fitness": np.array([r.fitness_ for r in results]),
+              "inlier_rmse": np.array([r.inlier_rmse_ for r in results]), "n_corr": np.array([r.n_corr for r in results]),
+              "iters": np.array([r.iters for r in results]), "pose": np.array(poses), "map_xyz": xyz[order], "map_normals": nrm[order]}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -342,6 +363,8 @@ def run_b2s_arm(args):
     nsrc_last = np.array([r.n_corr / max(r.fitness_, 1e-12) for r in last])
     pose_err = max(float(np.linalg.norm(maps[c].submap.getPose()[:3, 3] - lp.map_frame_pose(kpos[c] - 1)[:3, 3])) for c in range(chains))
     map_pts = int(np.mean([m.submap.size() for m in maps[:chains]]))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last, [maps[c].submap.getPose() for c in range(chains)], maps[0].submap.getMapPointCloud())
 
     # ---------------- chain sweep (N = 1): same resident measurement at other chain counts ----------------
     sweep_out, latency_ms = {}, None
@@ -430,16 +453,8 @@ def run_b2s_arm(args):
     ab = bytes_by_kind[dom_for_roof]
     dur_ms = prof[dom_for_roof][0] / max(prof[dom_for_roof][1], 1)
     achieved = ab / (dur_ms * 1e-3) / 1e9
-    traffic, traffic_src = None, None   # DRAM bytes per launch of that kernel from the committed ncu --set full capture
-    for tp in ("r02_traffic.json", "r01_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", tp)
-        if os.path.exists(tpath):
-            ent = json.load(open(tpath)).get(dom_for_roof)
-            if ent:
-                traffic, traffic_src = ent["bytes_per_launch"], ent["source"]
-                break
     roofline = {"bound": "hbm", "kernel": dom_for_roof, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "bytes_per_launch": ab, "avg_launch_ms": dur_ms,
+                "peak_source": peak_src, "bytes_per_launch": ab, "avg_launch_ms": dur_ms,
                 "note": "latency-bound: a single registration's working set is L2-resident and its iterations are sequential (SURVEY.md 8d); "
                         "the streaming kernels' fractions are under config3, the batched ICP's under config4"}
     profile = {k: {"ms_per_scan": v[0] / kp, "launch_groups_per_scan": v[1] / kp} for k, v in prof.items()}
@@ -528,6 +543,7 @@ def main():
     ap.add_argument("--host-threads", type=int, default=0, help="host threads issuing the chains' launches (0 = auto: 1 with graph replay, 8 eager)")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel eagerly instead of replaying one CUDA graph per scan")
     ap.add_argument("--nn-cell", type=float, default=0.0, help="NN grid cell edge in metres (0 = max_corr_dist / 4)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

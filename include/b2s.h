@@ -1,5 +1,5 @@
 /*
- * b2s.h -- C ABI of the B200-native scan-to-map registration and voxel-map fusion engine.
+ * b2s.h -- C ABI of the H100-native scan-to-map registration and voxel-map fusion engine.
  *
  * This is the drop-in boundary behind open3d_slam's CloudRegistration / ScanToMapRegistration /
  * Submap interfaces.  The reference has NO C/FFI boundary today: its seam is a pair of abstract C++

@@ -91,7 +91,7 @@ def lib():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise ImportError(f"{LIB_PATH} is missing: build it with __graft_entry__.build() (nvcc, sm_100a). "
+            raise ImportError(f"{LIB_PATH} is missing: build it with __graft_entry__.build() (nvcc, sm_90a). "
                               "There is no CPU fallback.")
         L = C.CDLL(LIB_PATH)
         L.b2s_last_error.restype = C.c_char_p

@@ -4,8 +4,6 @@ torch is plumbing here: streams, events, the flush buffer and torch.distributed 
 from __future__ import annotations
 
 import ctypes as C
-import json
-import os
 import time
 
 import numpy as np
@@ -16,14 +14,9 @@ from . import engine as E
 from . import slam as S
 from . import workloads as W
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
 
 def hbm_peak():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 700 W card); not a measured figure"
 
 
 class Timer:

@@ -301,7 +301,7 @@ void b2s_default_config(b2s_config* cfg) {
 }
 
 const char* b2s_last_error(void) { return get_error(); }
-const char* b2s_version(void) { return "b2s 0.1 (sm_100a, fp64)"; }
+const char* b2s_version(void) { return "b2s 0.1 (sm_90a, fp64)"; }
 int32_t b2s_device_count(void) { int n = 0; if (cudaGetDeviceCount(&n) != cudaSuccess) return 0; return n; }
 int64_t b2s_launch_count(const b2s_handle* h) { return h ? h->launches : 0; }
 

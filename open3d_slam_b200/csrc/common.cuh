@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers and the host-side runtime types of the b2s engine (sm_100a only).
+// common.cuh -- shared device helpers and the host-side runtime types of the b2s engine (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -333,8 +333,10 @@ int32_t op_submap_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan
 int32_t op_dense_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw, const double* T_host, const double* T_dev, const b2s_cropper* crop,
                         const int32_t* enable_dev = nullptr);
 
-// upper bound of the CTAs of a streaming kernel: 2 per SM (B2S_GRID_CAP overrides).  Measured at 16 concurrent chains: 148 .. 592
-// CTAs give 9.1 - 9.2 k registrations/s, 2368 (the round-1 value) 8.1 k -- few fat CTAs leave the SMs to the other chains' kernels
+// SMs of the current device (132 on an H100 SXM), queried once per device: the grid sizes below are multiples of it
+int device_sms();
+// upper bound of the CTAs of a streaming kernel: 2 per SM (B2S_GRID_CAP overrides).  With many concurrent chains, few fat CTAs
+// leave the SMs to the other chains' kernels; a much larger cap (16 per SM) lost throughput there
 int grid_cap();
 // The stand-alone operators (voxel down-sample, normals, crop of ONE large cloud: config 3) are not sharing the GPU with other chains'
 // kernels: for the duration of such a call the cap is lifted so that a 2^20-point cloud fills every SM.
@@ -352,7 +354,7 @@ inline int grid_for(size_t n, int threads, int max_blocks = 0) {
 }
 
 bool pdl_enabled();   // runtime.cu: true inside a PdlScope unless B2S_PDL=0 (A/B)
-// Launches carry the attribute only inside the per-scan mapper chain (b2s_mapper_step_*), where it was measured (+2.2 % at 16 chains);
+// Launches carry the attribute only inside the per-scan mapper chain (b2s_mapper_step_*), where it was measured to help at 16 chains;
 // everywhere else kernels launch exactly as before.
 struct PdlScope {
   PdlScope();
@@ -388,7 +390,7 @@ namespace b2s {
 // predecessor in the stream instead of starting after it -- a scan is a chain of 42 kernels of 3-50 us.  Past the wait the predecessor
 // grid has completed and its writes are visible, so nothing else changes.  Without the launch attribute the instruction is a no-op.
 // (An explicit early griddepcontrol.launch_dependents at the top of every kernel was measured too: the successors' CTAs become resident
-// long before they can run and hold registers / shared memory that the other chains' kernels need -- 10.4 k -> 7.9 k registrations/s.)
+// long before they can run and hold registers / shared memory that the other chains' kernels need, and throughput dropped.)
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // order-preserving map double -> uint64 so that atomicMin/atomicMax work on doubles

@@ -323,7 +323,7 @@ int32_t fuse_reserve(b2s_handle* h, b2s_submap* sm) {
   B2S_TRY(sm->pstamp.ensure((sm->capacity + 1) * 4, h->stream));
   B2S_TRY(sm->dups.ensure((size_t)2 * FUSE_DUP_CAP * 4, h->stream));
   sm->vcap = vcap;
-  launch_pdl(fuse_table_clear_kernel, 148 * 4, 256, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vstamp.as<int32_t>(), vcap,
+  launch_pdl(fuse_table_clear_kernel, 4 * device_sms(), 256, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vstamp.as<int32_t>(), vcap,
                                                          sm->mstate.as<int32_t>(), nullptr);
   h->launches++;
   B2S_CUDA(cudaGetLastError());
@@ -336,13 +336,13 @@ int32_t fuse_rehash(b2s_handle* h, b2s_submap* sm, const int32_t* enable_dev) {
   const size_t n_max = sm->graph_mode ? sm->capacity : (map->n_max > 0 ? map->n_max : 1);
   int32_t* ms = sm->mstate.as<int32_t>();
   ProfScope prof(h, PK_FUSE);
-  launch_pdl(fuse_table_clear_kernel, 148 * 4, 256, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vstamp.as<int32_t>(), sm->vcap,
+  launch_pdl(fuse_table_clear_kernel, 4 * device_sms(), 256, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vstamp.as<int32_t>(), sm->vcap,
                                                          ms, enable_dev);
   launch_pdl(fuse_table_link_kernel, grid_for(n_max, FZ_THREADS), FZ_THREADS, 0, h->stream, map->xyz.as<double>(), map->dn.as<int32_t>(),
                                                                                    1.0 / h->cfg.map_voxel_size, sm->vkeys.as<unsigned long long>(),
                                                                                    sm->vhead.as<int32_t>(), sm->vcap - 1, sm->vnext.as<int32_t>(),
                                                                                    sm->pstamp.as<int32_t>(), ms, h->status.as<uint32_t>(), enable_dev);
-  launch_pdl(fuse_table_dups_kernel, 148 * 4, FZ_THREADS, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vcap,
+  launch_pdl(fuse_table_dups_kernel, 4 * device_sms(), FZ_THREADS, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vcap,
                                                                sm->vnext.as<int32_t>(), sm->dups.as<int32_t>(), ms, h->status.as<uint32_t>(), enable_dev);
   h->launches += 3;
   B2S_CUDA(cudaGetLastError());
@@ -521,7 +521,7 @@ int32_t dense_init(b2s_handle* h, b2s_submap* sm, size_t cap, double voxel) {
   B2S_TRY(sm->dense_cnt.ensure(cap * 4, h->stream));
   B2S_TRY(sm->dense_used.ensure(16, h->stream));
   sm->dense_cap = cap; sm->dense_voxel = voxel;
-  launch_pdl(dense_init_kernel, 148 * 4, 256, 0, h->stream, sm->dense_keys.as<unsigned long long>(), sm->dense_sum.as<double>(),
+  launch_pdl(dense_init_kernel, 4 * device_sms(), 256, 0, h->stream, sm->dense_keys.as<unsigned long long>(), sm->dense_sum.as<double>(),
                                                     sm->dense_cnt.as<int32_t>(), cap, sm->dense_used.as<int32_t>());
   h->launches++;
   B2S_CUDA(cudaGetLastError());
@@ -575,10 +575,10 @@ int32_t dense_to_cloud(b2s_handle* h, b2s_submap* sm, double* d_xyz, int32_t* d_
   const size_t cap = sm->dense_cap;
   B2S_TRY(h->flags.ensure((cap + 1) * 4, h->stream));
   B2S_TRY(h->offs.ensure((cap + 2) * 4, h->stream));
-  launch_pdl(dense_flags_kernel, 148 * 4, 256, 0, h->stream, sm->dense_cnt.as<int32_t>(), cap, h->flags.as<int32_t>());
+  launch_pdl(dense_flags_kernel, 4 * device_sms(), 256, 0, h->stream, sm->dense_cnt.as<int32_t>(), cap, h->flags.as<int32_t>());
   h->launches++;
   B2S_TRY(scan_exclusive_i32(h, h->flags.as<int32_t>(), h->offs.as<int32_t>(), nullptr, cap, nullptr));
-  launch_pdl(dense_gather_kernel, 148 * 4, 256, 0, h->stream, sm->dense_keys.as<unsigned long long>(), sm->dense_sum.as<double>(),
+  launch_pdl(dense_gather_kernel, 4 * device_sms(), 256, 0, h->stream, sm->dense_keys.as<unsigned long long>(), sm->dense_sum.as<double>(),
                                                       sm->dense_cnt.as<int32_t>(), cap, h->flags.as<int32_t>(), h->offs.as<int32_t>(), d_xyz,
                                                       d_keys, d_out_n);
   h->launches++;
@@ -667,7 +667,7 @@ int32_t op_dense_remove(b2s_handle* h, b2s_submap* sm, const b2s_cloud* pts) {
 int32_t op_dense_count(b2s_handle* h, const b2s_submap* sm, int32_t* out_dev) {
   B2S_CUDA(cudaMemsetAsync(out_dev, 0, 4, h->stream));
   if (sm->dense_cap == 0) return B2S_OK;
-  launch_pdl(dense_count_kernel, 148 * 4, 256, 0, h->stream, sm->dense_cnt.as<int32_t>(), sm->dense_cap, out_dev);
+  launch_pdl(dense_count_kernel, 4 * device_sms(), 256, 0, h->stream, sm->dense_cnt.as<int32_t>(), sm->dense_cap, out_dev);
   h->launches++;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;
@@ -807,14 +807,14 @@ int32_t op_dense_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, con
   const double voxel = sm->dense_voxel;
   const double s0 = sensor ? sensor[0] : 0.0, s1 = sensor ? sensor[1] : 0.0, s2 = sensor ? sensor[2] : 0.0;
   ProfScope prof(h, PK_FUSE);
-  launch_pdl(dcarve_init_kernel, 148 * 8, 256, 0, h->stream, keys, first, cap, rm, sm->dense_cap, enable_dev, removed_dev);
+  launch_pdl(dcarve_init_kernel, 8 * device_sms(), 256, 0, h->stream, keys, first, cap, rm, sm->dense_cap, enable_dev, removed_dev);
   launch_pdl(dcarve_first_kernel, grid_for(n_max, FZ_THREADS), FZ_THREADS, 0, h->stream, scan->xyz.as<double>(), scan->dn.as<int32_t>(), 1.0 / voxel, keys, first,
                                                                                 cap - 1, slot_of, enable_dev);
   launch_pdl(dcarve_march_kernel, grid_for(n_max, FZ_THREADS), FZ_THREADS, 0, h->stream, scan->xyz.as<double>(), scan->dn.as<int32_t>(), slot_of, first, s0, s1, s2,
                                                                                 sensor_dev, voxel, radius, trunc, max_len,
                                                                                 sm->dense_keys.as<unsigned long long>(), sm->dense_cnt.as<int32_t>(),
                                                                                 sm->dense_cap, rm, enable_dev);
-  launch_pdl(dcarve_apply_kernel, 148 * 8, 256, 0, h->stream, rm, sm->dense_cap, sm->dense_sum.as<double>(), sm->dense_cnt.as<int32_t>(), removed_dev, enable_dev,
+  launch_pdl(dcarve_apply_kernel, 8 * device_sms(), 256, 0, h->stream, rm, sm->dense_cap, sm->dense_sum.as<double>(), sm->dense_cnt.as<int32_t>(), removed_dev, enable_dev,
                                                       sm->mstate.as<int32_t>());
   h->launches += 4;
   B2S_CUDA(cudaGetLastError());

@@ -231,7 +231,7 @@ int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double c
   launch_pdl(grid_bbox_init_kernel, 1, 32, 0, h->stream, g->bbox.as<unsigned long long>());
   launch_pdl(grid_bbox_kernel, blocks, GB_THREADS, 0, h->stream, cloud->xyz.as<double>(), d_n, cd, use_crop, g->bbox.as<unsigned long long>());
   launch_pdl(grid_header_kernel, 1, 32, 0, h->stream, g->bbox.as<unsigned long long>(), cell, g->cap_cells, hdr);
-  launch_pdl(grid_zero_kernel, 148 * 4, 256, 0, h->stream, hdr, counts);
+  launch_pdl(grid_zero_kernel, 4 * device_sms(), 256, 0, h->stream, hdr, counts);
   launch_pdl(grid_count_kernel, blocks, GB_THREADS, 0, h->stream, cloud->xyz.as<double>(), d_n, cd, use_crop, hdr, counts, g->rank.as<int32_t>());
   h->launches += 5;
   // scan over ncell (device-known) counts; launch sized for the capacity
@@ -306,13 +306,13 @@ int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* co
   B2S_CUDA(cudaMemsetAsync(dev + off_state, 0, st_bytes * (size_t)n, h->stream));
   const GridJob* dj = reinterpret_cast<const GridJob*>(dev);
   const ScanJob* ds = reinterpret_cast<const ScanJob*>(dev + off_scan);
-  int bx = grid_for(max_pts, GB_THREADS, 148 * 2);   // x blocks per job; y = job
+  int bx = grid_for(max_pts, GB_THREADS, 2 * device_sms());   // x blocks per job; y = job
   const dim3 gpts((unsigned)bx, (unsigned)n);
   ProfScope prof(h, PK_GRID);
   launch_pdl(gridb_init_kernel, (n * 6 + 127) / 128, 128, 0, h->stream, dj, n);
   launch_pdl(gridb_bbox_kernel, gpts, GB_THREADS, 0, h->stream, dj);
   launch_pdl(gridb_header_kernel, (n + 127) / 128, 128, 0, h->stream, dj, n, cell);
-  launch_pdl(gridb_zero_kernel, dim3(148, (unsigned)n), 256, 0, h->stream, dj);
+  launch_pdl(gridb_zero_kernel, dim3((unsigned)device_sms(), (unsigned)n), 256, 0, h->stream, dj);
   launch_pdl(gridb_count_kernel, gpts, GB_THREADS, 0, h->stream, dj);
   h->launches += 5;
   B2S_TRY(scan_exclusive_i32_batch(h, ds, n, max_cells));

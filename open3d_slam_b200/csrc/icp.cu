@@ -41,7 +41,7 @@ constexpr int NACC = 29;  // 21 upper-triangular JtJ + 6 Jtr + sum d2 + count
 // (every contribution is warp-reduced at once into a per-warp accumulator in shared memory) and run 768 threads = 24 warps per SM
 // at 80 registers; the generalized-ICP kernel carries 3x3 covariance algebra per correspondence and stays at 512 threads
 #ifndef B2S_ICP_PLANE_THREADS
-#define B2S_ICP_PLANE_THREADS 768   // measured on B200: 768 beats 512 and 1024 on latency and throughput (make alt ALT_THREADS=... builds libb2s_alt<N>.so for A/B runs)
+#define B2S_ICP_PLANE_THREADS 768   // 768 threads: 80 registers each still fit one CTA per SM (make alt ALT_THREADS=... builds libb2s_alt<N>.so for A/B runs)
 #endif
 constexpr int icp_threads(int mode) { return mode == 2 ? 512 : B2S_ICP_PLANE_THREADS; }
 constexpr int ICP_TILE = 64;   // points per tile of the source cloud (tile t belongs to CTA t % cluster size)
@@ -1154,7 +1154,7 @@ int32_t icp_launch(b2s_handle* h, const IcpProblem* single_host, const IcpProble
     const size_t smem_pts = (size_t)((ICP_DYN_SMEM - fixed) / ICP_BYTES_PER_POINT) - 64;
     static const int forced = getenv("B2S_ICP_BATCH_CSIZE") ? atoi(getenv("B2S_ICP_BATCH_CSIZE")) : 0;
     if (n_problems > 1 && forced > 0) csize = forced;
-    else while (csize > 1 && (size_t)n_problems * (size_t)csize > 148 * 2 && icp_chunk_points(max_src_points, csize / 2) <= smem_pts) csize /= 2;
+    else while (csize > 1 && (size_t)n_problems * (size_t)csize > 2 * (size_t)device_sms() && icp_chunk_points(max_src_points, csize / 2) <= smem_pts) csize /= 2;
   }
   // shared memory is sized for THIS launch's chunk only: whatever is not claimed stays L1, and the candidate gathers of
   // neighbouring queries hit the same lines (4 target points per 128-byte line)

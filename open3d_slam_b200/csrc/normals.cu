@@ -884,7 +884,7 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
   const size_t n_max = c->n_max > 0 ? c->n_max : 1;
   B2S_TRY(c->nrm.ensure(n_max * 24, h->stream));
   int blocks = (int)((n_max + NK_THREADS - 1) / NK_THREADS);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 16 * device_sms()) blocks = 16 * device_sms();
   if (blocks < 1) blocks = 1;
   // phase-2 queue: counter + one slot per point
   B2S_TRY(h->tmp_i32.ensure((2 * n_max + 64) * 4, h->stream));
@@ -894,7 +894,7 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
   const int32_t* qcount = flags ? qn + 1 : nullptr;
   // rings the thread-per-query kernel may walk before handing a query to the warp-cooperative kernel
   // (B2S_NORMALS_RING_LIMIT: tuning knob; -1 = every query goes to the warp-cooperative kernel)
-  // measured on B200 (config 2, 11 k queries): all-warp 0.13 ms, thread kernel + warp stragglers 0.35 ms -> default -1
+  // default -1: on the config-2 scans the all-warp path beat the thread kernel plus warp stragglers
   static const int ring_limit_env = getenv("B2S_NORMALS_RING_LIMIT") ? atoi(getenv("B2S_NORMALS_RING_LIMIT")) : -1;
   const int ring_limit = ring_limit_env;
   ProfScope prof(h, PK_NORMALS);
@@ -912,8 +912,7 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
   if (ring_limit == -1) {   // default: gather + select (one warp per query), stragglers to the general warp kernel
     // one warp per query, grid-stride (B2S_NS2_GRID: A/B knob of the grid size)
     static const int ns2_grid_env = getenv("B2S_NS2_GRID") ? atoi(getenv("B2S_NS2_GRID")) : 0;
-    // measured at 16 chains / 1 chain: 2368 CTAs 10.21 k/s, 0.600 ms; 592: 10.28 k/s, 0.619 ms; 296: 10.41 k/s, 0.640 ms -> the large grid stays
-    const int ns2_cap = ns2_grid_env > 0 ? ns2_grid_env : 148 * 16;
+    const int ns2_cap = ns2_grid_env > 0 ? ns2_grid_env : 16 * device_sms();
     int wblocks = (int)((n_max + (NK_THREADS / 32) - 1) / (NK_THREADS / 32));
     if (wblocks > ns2_cap) wblocks = ns2_cap;
     if (wblocks < 1) wblocks = 1;
@@ -940,7 +939,7 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
     fprintf(stderr, "[b2s normals] indexed %d queries %d fallback %d cell %.3f dims %dx%dx%d\n", gh.n, flags ? hq[1] : gh.n, hq[0], gh.cell,
             gh.dims[0], gh.dims[1], gh.dims[2]);
   }
-  launch_pdl(normals_phase2_kernel, 148 * 4, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, queue, qn, out);
+  launch_pdl(normals_phase2_kernel, 4 * device_sms(), NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, queue, qn, out);
   h->launches += 3;
   c->has_normals = true;
   B2S_CUDA(cudaGetLastError());

@@ -1,6 +1,6 @@
 // runtime.cu -- host runtime (errors, buffers) and the two device-wide primitives everything else is built
 // from: a single-pass decoupled-look-back exclusive scan and a stable LSD radix sort (8-bit digits,
-// match_any warp ranking).  Hand-written for sm_100a; no CUB/Thrust on the product path.
+// match_any warp ranking).  Hand-written for sm_90a; no CUB/Thrust on the product path.
 #include <cooperative_groups.h>
 #include <stdarg.h>
 #include <stdlib.h>
@@ -20,13 +20,24 @@ void set_error(const char* fmt, ...) {
 const char* get_error() { return g_err; }
 
 unsigned long long g_alloc_generation = 1;
+static int g_device_sms[64] = {0};
+int device_sms() {
+  int d = 0;
+  if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64) d = 0;
+  int v = __atomic_load_n(&g_device_sms[d], __ATOMIC_RELAXED);
+  if (v <= 0) {
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d) != cudaSuccess || v <= 0) v = 132;
+    __atomic_store_n(&g_device_sms[d], v, __ATOMIC_RELAXED);
+  }
+  return v;
+}
 static thread_local int g_grid_cap_override = 0;
 int grid_cap() {
   if (g_grid_cap_override > 0) return g_grid_cap_override;
-  static const int v = getenv("B2S_GRID_CAP") ? atoi(getenv("B2S_GRID_CAP")) : 148 * 2;
-  return v > 0 ? v : 148 * 2;
+  static const int v = getenv("B2S_GRID_CAP") ? atoi(getenv("B2S_GRID_CAP")) : 0;
+  return v > 0 ? v : 2 * device_sms();
 }
-WideGridScope::WideGridScope(size_t n) : on(n >= ((size_t)1 << 19) && g_grid_cap_override == 0) { if (on) g_grid_cap_override = 148 * 16; }
+WideGridScope::WideGridScope(size_t n) : on(n >= ((size_t)1 << 19) && g_grid_cap_override == 0) { if (on) g_grid_cap_override = 16 * device_sms(); }
 WideGridScope::~WideGridScope() { if (on) g_grid_cap_override = 0; }
 static thread_local int g_pdl_depth = 0;
 bool pdl_enabled() {

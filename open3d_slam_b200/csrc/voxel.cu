@@ -646,7 +646,7 @@ int32_t op_submap_transform(b2s_handle* h, b2s_submap* sm, const double* T_host)
   launch_pdl(pose_right_multiply_kernel, 1, 32, 0, h->stream, sm->pose.as<double>(), M);
   h->launches += 2;
   if (sm->dense_cap > 0) {
-    launch_pdl(dense_transform_kernel, 148 * 4, 256, 0, h->stream, sm->dense_sum.as<double>(), sm->dense_cnt.as<int32_t>(), sm->dense_cap, M);
+    launch_pdl(dense_transform_kernel, 4 * device_sms(), 256, 0, h->stream, sm->dense_sum.as<double>(), sm->dense_cnt.as<int32_t>(), sm->dense_cap, M);
     h->launches++;
   }
   B2S_CUDA(cudaGetLastError());

@@ -193,7 +193,7 @@ int32_t b2s_voxel_map_create(b2s_handle* h, const double voxel_size[3], size_t c
   if (rc == B2S_OK) rc = vm->cnt.ensure(cap * 4 * VM_LAYERS, h->stream);
   if (rc == B2S_OK) rc = vm->used.ensure(64, h->stream);
   if (rc != B2S_OK) { vm->keys.release(); vm->head.release(); vm->cnt.release(); vm->used.release(); delete vm; return rc; }
-  launch_pdl(vm_clear_kernel, 148 * 4, VM_THREADS, 0, h->stream, vm->keys.as<unsigned long long>(), vm->head.as<int32_t>(), vm->cnt.as<int32_t>(), cap,
+  launch_pdl(vm_clear_kernel, 4 * device_sms(), VM_THREADS, 0, h->stream, vm->keys.as<unsigned long long>(), vm->head.as<int32_t>(), vm->cnt.as<int32_t>(), cap,
                                                          vm->used.as<int32_t>());
   h->launches++;
   *out = vm;
@@ -212,7 +212,7 @@ void b2s_voxel_map_destroy(b2s_voxel_map* vm) {
 int32_t b2s_voxel_map_clear(b2s_handle* h, b2s_voxel_map* vm) {
   B2S_REQUIRE(h && vm, B2S_E_INVALID, "null argument");
   VM_LOCK(h);
-  launch_pdl(vm_clear_kernel, 148 * 4, VM_THREADS, 0, h->stream, vm->keys.as<unsigned long long>(), vm->head.as<int32_t>(), vm->cnt.as<int32_t>(), vm->cap,
+  launch_pdl(vm_clear_kernel, 4 * device_sms(), VM_THREADS, 0, h->stream, vm->keys.as<unsigned long long>(), vm->head.as<int32_t>(), vm->cnt.as<int32_t>(), vm->cap,
                                                          vm->used.as<int32_t>());
   h->launches++;
   vm->entries_bound = 0;

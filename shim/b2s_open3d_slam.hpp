@@ -1,4 +1,4 @@
-// b2s_open3d_slam.hpp -- the C++ subclasses a maintainer adds to open3d_slam to run the hot path on a B200 through the
+// b2s_open3d_slam.hpp -- the C++ subclasses a maintainer adds to open3d_slam to run the hot path on an H100 through the
 // C ABI of include/b2s.h.  They implement the reference's own abstract interfaces
 //     o3d_slam::CloudRegistration        (include/open3d_slam/CloudRegistration.hpp:19-27)
 //     o3d_slam::ScanToMapRegistration    (include/open3d_slam/ScanToMapRegistration.hpp:29-38)

@@ -1,4 +1,4 @@
-"""Summaries of ncu outputs for profiles/ (run here on the CPU box; ncu reads the reports without a GPU).
+"""Summaries of ncu outputs as markdown tables (ncu reads the reports without a GPU).
   python tools/summarize_ncu.py launches <launches.csv> <out.md> [title]
   python tools/summarize_ncu.py report <file.ncu-rep> <out.md> [title]
   python tools/summarize_ncu.py table <file.ncu-rep | raw.csv> <out.md> [title]     one row per launch, the columns the round's analysis uses"""
