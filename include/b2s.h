@@ -332,6 +332,24 @@ int32_t b2s_voxel_map_indices_in_voxel(b2s_handle* h, const b2s_voxel_map* vm, i
  * the merge_ cloud in its overlap buffer, src/SubmapCollection.cpp:83-92,180).  Either output may be NULL. */
 int32_t b2s_mapper_processed_scan(b2s_handle* h, b2s_cloud* merge_out, b2s_cloud* match_out);
 
+/* ---- loop-closure features: Submap::computeFeatures -> [O3D] ComputeFPFHFeature (src/Submap.cpp:244) ----------------------
+ *      A b2s_feature is the device-resident [O3D] pipelines::registration::Feature: B2S_FEATURE_DIM x n fp64, stored point after
+ *      point (the memory order of the reference's column-major data_ matrix), so host arrays hold n * B2S_FEATURE_DIM doubles.
+ *      b2s_compute_fpfh(cloud, radius, knn): FPFH over the exact hybrid neighbourhood (the knn nearest points with d^2 < radius^2,
+ *      ascending (d^2, index)).  Errors: radius <= 0 or knn <= 0 -> B2S_E_INVALID; knn > B2S_FEATURE_MAX_KNN -> B2S_E_UNSUPPORTED;
+ *      a non-empty cloud without normals -> B2S_E_NO_NORMALS ([O3D] LogError); an empty cloud gives a feature of zero points.
+ *      A feature belongs to the handle that created it: passing it with another handle -> B2S_E_INVALID.
+ *      Synchronises once (point count).  Semantics and deterministic choices: DESIGN.md, row K-fpfh. */
+#define B2S_FEATURE_DIM 33
+#define B2S_FEATURE_MAX_KNN 128
+typedef struct b2s_feature b2s_feature;
+int32_t b2s_feature_create(b2s_handle* h, b2s_feature** out);
+void b2s_feature_destroy(b2s_feature* f);
+int32_t b2s_feature_size(b2s_handle* h, const b2s_feature* f, size_t* n);
+int32_t b2s_feature_download(b2s_handle* h, const b2s_feature* f, double* data, size_t capacity_points, size_t* n);
+int32_t b2s_feature_upload(b2s_handle* h, b2s_feature* f, const double* data, size_t n);
+int32_t b2s_compute_fpfh(b2s_handle* h, const b2s_cloud* cloud, double radius, int32_t knn, b2s_feature* feature);
+
 /* ---- device-to-device hand-over of a cloud's arrays (SURVEY.md section 8e: a submap that is the registration target on
  *      several GPUs is built once by its owner and broadcast over NVLink by the host side -- torch.distributed / NCCL own
  *      the transfer, this library only copies between its cloud and the caller's device buffers on the handle's stream).

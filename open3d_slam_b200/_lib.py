@@ -73,7 +73,9 @@ SYMBOLS = [
     "b2s_voxel_map_create", "b2s_voxel_map_destroy", "b2s_voxel_map_clear", "b2s_voxel_map_insert_cloud", "b2s_voxel_map_size",
     "b2s_voxel_map_has_voxel", "b2s_voxel_map_indices_in_voxel", "b2s_mapper_processed_scan",
     "b2s_cloud_export_device", "b2s_cloud_import_device", "b2s_submap_to_cloud", "b2s_nearest_neighbors",
+    "b2s_feature_create", "b2s_feature_destroy", "b2s_feature_size", "b2s_feature_download", "b2s_feature_upload", "b2s_compute_fpfh",
 ]
+FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 PROFILE_KINDS = ["icp", "normals", "radix_sort", "nn_grid_build", "voxel", "fuse", "select", "crop"]
 
 _lib = None
@@ -108,6 +110,8 @@ def lib():
         L.b2s_submap_destroy.argtypes = [C.c_void_p]
         L.b2s_voxel_map_destroy.restype = None
         L.b2s_voxel_map_destroy.argtypes = [C.c_void_p]
+        L.b2s_feature_destroy.restype = None
+        L.b2s_feature_destroy.argtypes = [C.c_void_p]
         _lib = L
     return _lib
 

@@ -1124,4 +1124,71 @@ int32_t b2s_scan_result_fetch(b2s_handle* h, int32_t slot, b2s_result* out) {
   return rc;
 }
 
+// ---- loop-closure features ---------------------------------------------------------------------------------------------
+int32_t b2s_feature_create(b2s_handle* h, b2s_feature** out) {
+  B2S_REQUIRE(h && out, B2S_E_INVALID, "null argument");
+  LOCK(h);
+  b2s_feature* f = new (std::nothrow) b2s_feature();
+  B2S_REQUIRE(f, B2S_E_INVALID, "out of host memory");
+  f->h = h;
+  f->device = h->device;
+  f->data.tracked = f->nb_idx.tracked = f->nb_d2.tracked = f->nb_cnt.tracked = f->spfh.tracked = false;   // caller-owned, never in a graph
+  *out = f;
+  return B2S_OK;
+}
+
+void b2s_feature_destroy(b2s_feature* f) {
+  if (!f) return;
+  cudaSetDevice(f->device);   // the owning handle may already be gone (see b2s_cloud_destroy)
+  cudaDeviceSynchronize();
+  DevBuf* bufs[] = {&f->data, &f->nb_idx, &f->nb_d2, &f->nb_cnt, &f->spfh};
+  for (DevBuf* b : bufs) b->release();
+  delete f;
+}
+
+int32_t b2s_feature_size(b2s_handle* h, const b2s_feature* f, size_t* n) {
+  B2S_REQUIRE(h && f && n, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(f->h == h, B2S_E_INVALID, "the feature belongs to another handle");
+  LOCK(h);
+  *n = f->n;
+  return B2S_OK;
+}
+
+int32_t b2s_feature_download(b2s_handle* h, const b2s_feature* f, double* data, size_t capacity_points, size_t* n_out) {
+  B2S_REQUIRE(h && f && (data || f->n == 0), B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(f->h == h, B2S_E_INVALID, "the feature belongs to another handle");
+  LOCK(h);
+  if (n_out) *n_out = f->n;
+  B2S_REQUIRE(f->n <= capacity_points, B2S_E_CAPACITY, "download buffer too small: %zu points, capacity %zu", f->n, capacity_points);
+  if (f->n) B2S_CUDA(cudaMemcpyAsync(data, f->data.p, f->n * B2S_FEATURE_DIM * 8, cudaMemcpyDeviceToHost, h->stream));
+  return check_status(h);
+}
+
+int32_t b2s_feature_upload(b2s_handle* h, b2s_feature* f, const double* data, size_t n) {
+  B2S_REQUIRE(h && f && (data || n == 0), B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(n < (size_t)0x7fffffff / B2S_FEATURE_DIM, B2S_E_INVALID, "feature too large");
+  B2S_REQUIRE(f->h == h, B2S_E_INVALID, "the feature belongs to another handle");
+  LOCK(h);
+  if (n) {
+    B2S_TRY(f->data.ensure(n * B2S_FEATURE_DIM * 8, h->stream));
+    B2S_CUDA(cudaMemcpyAsync(f->data.p, data, n * B2S_FEATURE_DIM * 8, cudaMemcpyHostToDevice, h->stream));
+  }
+  f->n = n;
+  return B2S_OK;
+}
+
+int32_t b2s_compute_fpfh(b2s_handle* h, const b2s_cloud* cloud, double radius, int32_t knn, b2s_feature* feature) {
+  B2S_REQUIRE(h && cloud && feature, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(feature->h == h, B2S_E_INVALID, "the feature belongs to another handle");
+  B2S_REQUIRE(cloud->device == h->device, B2S_E_INVALID, "the cloud lives on device %d, the handle on device %d", cloud->device, h->device);
+  B2S_REQUIRE(radius > 0.0, B2S_E_INVALID, "ComputeFPFHFeature: radius must be > 0");
+  B2S_REQUIRE(knn > 0, B2S_E_INVALID, "ComputeFPFHFeature: max_nn must be > 0");
+  B2S_REQUIRE(knn <= B2S_FEATURE_MAX_KNN, B2S_E_UNSUPPORTED, "ComputeFPFHFeature: max_nn %d > %d is not supported", knn, B2S_FEATURE_MAX_KNN);
+  LOCK(h);
+  size_t n = 0;
+  B2S_TRY(cloud_count_sync(h, cloud, &n));
+  B2S_REQUIRE(n == 0 || cloud->has_normals, B2S_E_NO_NORMALS, "ComputeFPFHFeature: the point cloud has no normals");
+  return op_compute_fpfh(h, cloud, n, radius, knn, feature);
+}
+
 }  // extern "C"

@@ -156,6 +156,14 @@ struct b2s_submap {
   unsigned long long graph_cfg_gen = 0;     // value of b2s_handle::cfg_gen when the graph was captured
 };
 
+struct b2s_feature {
+  b2s_handle* h = nullptr;
+  int device = 0;
+  b2s::DevBuf data;      // B2S_FEATURE_DIM x f64 per point, point after point ([O3D] Feature::data_, a column-major dim x n matrix)
+  size_t n = 0;
+  b2s::DevBuf nb_idx, nb_d2, nb_cnt, spfh;   // scratch of b2s_compute_fpfh: neighbour lists (knn per point) and the SPFH rows
+};
+
 namespace b2s {
 // device-side state words of the mapper chain (b2s_submap::mstate)
 enum MapperStateWord {
@@ -326,6 +334,8 @@ int32_t op_undistort(b2s_handle* h, const b2s_cloud* in, const double* lin_vel, 
 // L1 overlap selection in front of the loop-closure ICP (overlap.cu); T_dev = sourceToTarget (device, row-major)
 int32_t op_overlap(b2s_handle* h, const b2s_cloud* source, const b2s_cloud* target, const double* T_dev, double voxel, int min_pts,
                    b2s_cloud* source_overlap, b2s_cloud* target_overlap);
+// K-fpfh (features.cu): [O3D] ComputeFPFHFeature of the n points of c (normals required, 1 <= knn <= B2S_FEATURE_MAX_KNN)
+int32_t op_compute_fpfh(b2s_handle* h, const b2s_cloud* c, size_t n, double radius, int knn, b2s_feature* f);
 // C1 space carving of the sparse map (carve.cu); removed_dev (optional) receives the number of removed points
 int32_t op_submap_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan, const double* T_dev, const CropDev& crop,
                         const b2s_carving_params& prm, int32_t* removed_dev, const int32_t* enable_dev = nullptr);

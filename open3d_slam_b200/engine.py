@@ -369,6 +369,57 @@ def nearestNeighbors(eng: Engine, queries: Cloud, target: Cloud, maxCorresponden
     return idx[:n], d2[:n]
 
 
+class Feature:
+    """Device-resident [O3D] pipelines::registration::Feature (33 x n fp64), what Submap::computeFeatures keeps in feature_."""
+
+    def __init__(self, eng: Engine, data=None):
+        self.eng = eng
+        self._f = C.c_void_p()
+        L.check(L.lib().b2s_feature_create(eng._h, C.byref(self._f)))
+        if data is not None:
+            self.upload(data)
+
+    def upload(self, data):
+        """data_ as [O3D] holds it: a Dimension() x Num() matrix."""
+        d = np.ascontiguousarray(np.asarray(data, dtype=np.float64).reshape(L.FEATURE_DIM, -1).T)
+        L.check(L.lib().b2s_feature_upload(self.eng._h, self._f, _pd(d), C.c_size_t(len(d))))
+        return self
+
+    def Num(self) -> int:
+        n = C.c_size_t()
+        L.check(L.lib().b2s_feature_size(self.eng._h, self._f, C.byref(n)))
+        return int(n.value)
+
+    def Dimension(self) -> int:
+        return L.FEATURE_DIM
+
+    @property
+    def data_(self) -> np.ndarray:
+        n = self.Num()
+        buf = np.empty((max(n, 1), L.FEATURE_DIM))
+        m = C.c_size_t()
+        L.check(L.lib().b2s_feature_download(self.eng._h, self._f, _pd(buf), C.c_size_t(len(buf)), C.byref(m)))
+        return buf[:n].T.copy()
+
+    def free(self):
+        if self._f:
+            L.lib().b2s_feature_destroy(self._f)
+        self._f = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def computeFPFHFeature(eng: Engine, cloud: Cloud, radius: float, max_nn: int) -> Feature:
+    """[O3D] ComputeFPFHFeature(cloud, KDTreeSearchParamHybrid(radius, max_nn)) as called at src/Submap.cpp:244 (max_nn <= 128)."""
+    f = Feature(eng)
+    L.check(L.lib().b2s_compute_fpfh(eng._h, cloud._c, C.c_double(radius), C.c_int32(max_nn), f._f))
+    return f
+
+
 class CloudRegistration:
     def registerClouds(self, source: Cloud, target: Cloud, init) -> RegistrationResult:  # pragma: no cover - abstract
         raise NotImplementedError
