@@ -2,6 +2,10 @@
 
 Tolerances: the north star asks for 1e-4 relative on the converged SE(3); because the device path is fp64 and
 reproduces the oracle's neighbour decisions bit-for-bit, the tests hold it to 1e-9 (transform) / 1e-12 (voxel means).
+
+The inputs here are typical ones.  The size switches of the kernels (ICP cluster size, 64-point tiles, shared or global memory,
+batch cluster shrink, certificates; normals knn, select exits, coarsened grid; voxel key width, one-cluster or multi-kernel sort,
+wide grid, grid-size independence) are crossed from both sides in test_gpu_boundaries.py.
 """
 import ctypes as C
 
