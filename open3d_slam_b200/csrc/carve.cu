@@ -156,8 +156,8 @@ int32_t compact_cloud(b2s_handle* h, const b2s_cloud* in, const int32_t* flags, 
 
 int32_t op_submap_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan, const double* T_dev, const CropDev& crop,
                         const b2s_carving_params& prm, int32_t* removed_dev, const int32_t* enable_dev) {
-  b2s_cloud* map = sm->cloud[0];
-  b2s_cloud* tmp = sm->cloud[1];
+  b2s_cloud* map = sm->cloud[0].get();
+  b2s_cloud* tmp = sm->cloud[1].get();
   // graph replay: constant launch dimensions (the map's host-side bound moves from scan to scan)
   const size_t n_max = sm->graph_mode ? sm->capacity : (map->n_max > 0 ? map->n_max : 1);
   size_t cap = 1024;

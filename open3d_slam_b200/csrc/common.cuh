@@ -4,8 +4,11 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <memory>
 #include <mutex>
+#include <new>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/b2s.h"
@@ -42,17 +45,55 @@ const char* get_error();
   } while (0)
 
 // ------------------------------------------------------------------------------------------------
-// grow-only device buffer
+// owning buffers: the destructor frees the allocation, so an object holding them needs no release code.  They are move-only
+// (declaring the move operations deletes the copies): a moved-from buffer takes over what the target held and frees it.
 // ------------------------------------------------------------------------------------------------
-struct DevBuf {
+struct DevBuf {          // grow-only device buffer
   void* p = nullptr;
   size_t cap = 0;
   bool tracked = true;   // a re-allocation invalidates captured graphs (false for clouds the caller owns: a graph never holds them)
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept { *this = std::move(o); }
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); std::swap(tracked, o.tracked); return *this; }
+  ~DevBuf() { release(); }
   int32_t ensure(size_t bytes, cudaStream_t s, bool preserve = false);
   void release();
   template <typename T>
   T* as() const { return reinterpret_cast<T*>(p); }
 };
+
+struct PinnedBuf {       // page-locked host memory (cudaHostAlloc)
+  void* p = nullptr;
+  size_t cap = 0;
+  PinnedBuf() = default;
+  PinnedBuf(PinnedBuf&& o) noexcept { *this = std::move(o); }
+  PinnedBuf& operator=(PinnedBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+  ~PinnedBuf() { release(); }
+  int32_t alloc(size_t bytes, unsigned flags = cudaHostAllocDefault);   // frees what it held first: nothing may still use that
+  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
+  template <typename T>
+  T* as() const { return reinterpret_cast<T*>(p); }
+};
+
+// Builds a new T with init(T*) and hands it out through *out only when init succeeded; a half-built T is deleted (its members free
+// what they own), so a failed create leaves nothing behind.
+template <typename T, typename Init>
+int32_t create_object(T** out, Init&& init) {
+  T* obj = new (std::nothrow) T();
+  B2S_REQUIRE(obj, B2S_E_INVALID, "out of host memory");
+  const int32_t rc = init(obj);
+  if (rc != B2S_OK) { delete obj; return rc; }
+  *out = obj;
+  return B2S_OK;
+}
+// Deletes an object a b2s_*_create made.  The owning handle may already be gone: wait for the whole device instead of touching it.
+template <typename T>
+void destroy_object(T* obj) {
+  if (!obj) return;
+  cudaSetDevice(obj->device);
+  cudaDeviceSynchronize();
+  delete obj;
+}
 
 // device-side status word: kernels OR error bits into it, the host checks it when it synchronises
 enum : uint32_t { ST_KEY_OVERFLOW = 1u, ST_CAPACITY = 2u, ST_EMPTY = 4u, ST_HASH_FULL = 8u };
@@ -75,7 +116,6 @@ struct GridIndex {
   DevBuf pts;            // double4 per indexed point: x,y,z, bits(original index)
   DevBuf nrm;            // double4 per indexed point: nx,ny,nz,0
   int32_t cap_cells = 0;
-  void release();
 };
 
 struct ScanScratch {     // decoupled look-back scan state
@@ -107,9 +147,10 @@ struct b2s_cloud {
 };
 
 struct b2s_submap {
+  ~b2s_submap() { if (gexec) cudaGraphExecDestroy(gexec); if (cnt_ev) cudaEventDestroy(cnt_ev); }   // the buffers and clouds free themselves
   b2s_handle* h = nullptr;
   int device = 0;
-  b2s_cloud* cloud[2] = {nullptr, nullptr};  // ping-pong map cloud (mapCloud_)
+  std::unique_ptr<b2s_cloud> cloud[2];  // ping-pong map cloud (mapCloud_)
   int cur = 0;
   size_t capacity = 0;
   // dense map (VoxelizedPointCloud): open-addressing hash of running sums
@@ -122,7 +163,7 @@ struct b2s_submap {
   bool dense_has_normals = false;
   b2s::DevBuf pose;          // 4 x (4x4 f64): [0] mapToRangeSensor_ state, [1] insertion pose, [2] odometry motion, [3] initial guess
   // asynchronous read-back of the map size (keeps the host-side launch bound tight without ever synchronising)
-  int32_t* pinned_cnt = nullptr;
+  b2s::PinnedBuf pinned_cnt;          // int32 map size, written by the copy cnt_ev marks
   cudaEvent_t cnt_ev = nullptr;
   bool cnt_pending = false;
   size_t adds_after_readback = 0;
@@ -132,8 +173,8 @@ struct b2s_submap {
   int graph_warm = 0;                 // eager steps still to run before the capture (sizes every scratch buffer)
   cudaGraphExec_t gexec = nullptr;
   int64_t graph_kernels = 0;          // kernels per replay (for the launch counter)
-  b2s_cloud* staging = nullptr;       // fixed-capacity input cloud the caller uploads each scan into
-  double* odom_ring = nullptr;        // pinned, device-mapped: 64 x (4x4) odometry motions
+  std::unique_ptr<b2s_cloud> staging; // fixed-capacity input cloud the caller uploads each scan into
+  b2s::PinnedBuf odom_ring;           // device-mapped: 64 x (4x4 f64) odometry motions
   long long host_step = 0;
   b2s::DevBuf gstate;                 // int32 [0] device step counter, [1] current result slot
   double g_min_fitness = 0.0;
@@ -201,8 +242,13 @@ extern thread_local bool g_capture_broken;
 }  // namespace b2s
 
 struct b2s_handle {
+  ~b2s_handle() {   // the buffers and clouds free themselves
+    for (auto& r : prof_recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
+    for (cudaEvent_t e : prof_pool) cudaEventDestroy(e);
+    if (own_stream && stream) cudaStreamDestroy(stream);
+  }
   bool prof_enabled = false;
-  long long* icp_dbg = nullptr;       // optional device buffer of clock64 stamps (b2s_debug_icp_clocks)
+  b2s::DevBuf icp_dbg;                // optional clock64 stamps (b2s_debug_icp_clocks); unallocated while they are off
   std::vector<b2s::ProfRec> prof_recs;
   std::vector<cudaEvent_t> prof_pool;
   int device = 0;
@@ -213,7 +259,7 @@ struct b2s_handle {
   unsigned long long cfg_gen = 1;     // bumped by b2s_set_config: captured graphs bake the configuration in
   int64_t launches = 0;
 
-  b2s::DevBuf status;                 // uint32 device status word
+  b2s::DevBuf status;                 // uint32 [16]: [0] device status word, the rest scratch words (b2s::SW_*)
   b2s::ScanScratch scan;
   b2s::SortScratch sort;
   b2s::GridIndex grid_a, grid_b;      // target index (ICP) / self index (normals)
@@ -222,25 +268,37 @@ struct b2s_handle {
   b2s::DevBuf problems;               // IcpProblem array (device)
   b2s::DevBuf results;                // b2s_result array (device)
   b2s::DevBuf slots;                  // per-slot results for the async mapper step
-  b2s::DevBuf poses;                  // small device-resident transforms
-  void* pinned = nullptr;             // pinned host staging
-  size_t pinned_cap = 0;
+  b2s::DevBuf poses;                  // 64 small device-resident transforms (4x4 f64, all allocated by b2s_create); scratch slots b2s::PS_*
+  b2s::PinnedBuf pinned;              // host staging of check_status and read_back (runtime.cu owns its layout)
   // temporaries for the fused chains
-  b2s_cloud* t0 = nullptr; b2s_cloud* t1 = nullptr; b2s_cloud* t2 = nullptr; b2s_cloud* t3 = nullptr;
-  std::vector<b2s::GridIndex*> batch_grids;
+  std::unique_ptr<b2s_cloud> t0, t1, t2, t3;
+  std::vector<std::unique_ptr<b2s::GridIndex>> batch_grids;
   b2s::DevBuf batch_jobs;             // GridJob + ScanJob tables and the scan tile states of a batched index build
   std::vector<unsigned char> batch_jobs_host;
 };
 
+// every entry point that touches a handle's stream or buffers holds its lock and works on its device
+#define LOCK(h) std::lock_guard<std::recursive_mutex> _lk((h)->mu); cudaSetDevice((h)->device)
+
 namespace b2s {
+
+// extra words of b2s_handle::status (uint32): removed count of b2s_submap_carve / b2s_dense_carve, voxel count of b2s_dense_size,
+// point count of the chunk b2s_nearest_neighbors works on
+enum StatusWord : int { SW_REMOVED = 8, SW_DENSE_SIZE = 12, SW_NN_CHUNK = 14 };
+// scratch slots of b2s_handle::poses: T of b2s_voxel_map_has_voxel; sourceToTarget of b2s_overlap and the host-given pose of
+// op_dense_insert (shared: each call writes the slot before its kernels read it, on the handle's stream); T of op_transform
+enum PoseSlot : int { PS_VOXEL_MAP = 61, PS_CALL = 62, PS_TRANSFORM = 63 };
 
 struct ProfScope {   // records an event pair around the launches issued during its lifetime (no-op unless enabled)
   b2s_handle* h; int idx;
   ProfScope(b2s_handle* h_, int kind);
   ~ProfScope();
 };
-int32_t ensure_pinned(b2s_handle* h, size_t bytes);
 int32_t check_status(b2s_handle* h);     // synchronises and converts device status bits into an error
+struct ReadBack { void* dst; const void* src; size_t bytes; };   // host destination, device source
+// small device -> host reads through pinned staging, then check_status; the destinations are written even when the device status
+// reports an error, and check_status's code is returned
+int32_t read_back(b2s_handle* h, std::initializer_list<ReadBack> copies);
 
 // ---- primitives (scan.cu / radix_sort.cu / grid_index.cu / ...) : all asynchronous on h->stream ----
 // exclusive scan of in[0..*d_n) into out[0..*d_n]; out[*d_n] and *d_total (optional) receive the total

@@ -332,7 +332,7 @@ int32_t fuse_reserve(b2s_handle* h, b2s_submap* sm) {
 
 int32_t fuse_rehash(b2s_handle* h, b2s_submap* sm, const int32_t* enable_dev) {
   B2S_TRY(fuse_reserve(h, sm));
-  b2s_cloud* map = sm->cloud[0];
+  b2s_cloud* map = sm->cloud[0].get();
   const size_t n_max = sm->graph_mode ? sm->capacity : (map->n_max > 0 ? map->n_max : 1);
   int32_t* ms = sm->mstate.as<int32_t>();
   ProfScope prof(h, PK_FUSE);
@@ -357,27 +357,27 @@ __global__ void __launch_bounds__(FZ_THREADS) fuse_alive_flags_kernel(const doub
 }
 int32_t compact_cloud(b2s_handle* h, const b2s_cloud* in, const int32_t* flags, b2s_cloud* out, const int32_t* d_n_override = nullptr);   // voxel.cu
 int32_t submap_compact_view(b2s_handle* h, b2s_submap* sm, b2s_cloud** view) {
-  b2s_cloud* map = sm->cloud[0];
+  b2s_cloud* map = sm->cloud[0].get();
   const size_t n_max = map->n_max > 0 ? map->n_max : 1;
   B2S_TRY(h->flags.ensure((n_max + 1) * 4, h->stream));
   launch_pdl(fuse_alive_flags_kernel, grid_for(n_max, FZ_THREADS), FZ_THREADS, 0, h->stream, map->xyz.as<double>(), map->dn.as<int32_t>(), h->flags.as<int32_t>());
   h->launches++;
-  B2S_TRY(compact_cloud(h, map, h->flags.as<int32_t>(), sm->cloud[1]));
-  *view = sm->cloud[1];
+  B2S_TRY(compact_cloud(h, map, h->flags.as<int32_t>(), sm->cloud[1].get()));
+  *view = sm->cloud[1].get();
   return B2S_OK;
 }
 
 int32_t op_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, const double* T_dev, const int32_t* gate_dev) {
   B2S_REQUIRE(scan->has_normals || h->cfg.icp.reg_type == B2S_REG_POINT_TO_POINT, B2S_E_NO_NORMALS,
               "Submap::insertScan: the pre-processed scan must carry normals (isMergeScanValid) unless the registration is point-to-point");
-  b2s_cloud* map = sm->cloud[0];
+  b2s_cloud* map = sm->cloud[0].get();
   const double v = h->cfg.map_voxel_size;
   B2S_REQUIRE(v > 0.0, B2S_E_UNSUPPORTED, "map_voxel_size <= 0 (no voxelisation) is not supported on the device path");
   B2S_TRY(fuse_reserve(h, sm));
   // host-side upper bound of the map size.  The exact size is read back asynchronously after an insertion (pinned
   // host word + event); once that copy has landed the bound becomes exact-size + what was appended since.
   if (sm->cnt_pending && cudaEventQuery(sm->cnt_ev) == cudaSuccess) {
-    map->n_max = (size_t)sm->pinned_cnt[0] + sm->adds_after_readback;
+    map->n_max = (size_t)sm->pinned_cnt.as<int32_t>()[0] + sm->adds_after_readback;
     sm->cnt_pending = false;
   }
   const size_t m_max = 2 * (scan->n_max > 0 ? scan->n_max : 1);   // the duplication quirk doubles the scan
@@ -424,12 +424,12 @@ int32_t op_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, c
   map->has_normals = true;
   B2S_CUDA(cudaGetLastError());
   if (!sm->graph_mode) {
-    if (!sm->pinned_cnt) {
-      B2S_CUDA(cudaMallocHost(&sm->pinned_cnt, 64));
+    if (!sm->cnt_ev) {
+      B2S_TRY(sm->pinned_cnt.alloc(64));
       B2S_CUDA(cudaEventCreateWithFlags(&sm->cnt_ev, cudaEventDisableTiming));
     }
     if (!sm->cnt_pending) {
-      B2S_CUDA(cudaMemcpyAsync(sm->pinned_cnt, map->dn.p, 4, cudaMemcpyDeviceToHost, h->stream));
+      B2S_CUDA(cudaMemcpyAsync(sm->pinned_cnt.p, map->dn.p, 4, cudaMemcpyDeviceToHost, h->stream));
       B2S_CUDA(cudaEventRecord(sm->cnt_ev, h->stream));
       sm->cnt_pending = true;
       sm->adds_after_readback = 0;
@@ -533,8 +533,7 @@ int32_t op_dense_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw, con
   B2S_REQUIRE(sm->dense_cap > 0, B2S_E_INVALID, "dense map not initialised");
   const double* Td = T_dev;
   if (!Td) {
-    B2S_TRY(h->poses.ensure(64 * 16 * 8, h->stream, true));
-    double* slot = h->poses.as<double>() + 16 * 62;
+    double* slot = h->poses.as<double>() + 16 * PS_CALL;
     B2S_TRY(pose_to_device(h, T_host, slot));
     Td = slot;
   }

@@ -1144,7 +1144,8 @@ int32_t icp_launch(b2s_handle* h, const IcpProblem* single_host, const IcpProble
   const int estimator = single_host ? single_host->estimator : h->cfg.icp.reg_type;   // uniform over a batch
   int csize = 1;
   const int cmax = icp_max_cluster(h);
-  const int mode = estimator == B2S_REG_GENERALIZED ? 2 : (estimator == B2S_REG_POINT_TO_PLANE ? (h->icp_dbg ? 3 : 0) : 1);
+  long long* const dbg = h->icp_dbg.as<long long>();
+  const int mode = estimator == B2S_REG_GENERALIZED ? 2 : (estimator == B2S_REG_POINT_TO_PLANE ? (dbg ? 3 : 0) : 1);
   const int threads = icp_threads(mode);
   while (csize < cmax && (size_t)csize * threads < max_src_points) csize *= 2;
   const int fixed = icp_fixed_smem_bytes(threads);
@@ -1178,10 +1179,10 @@ int32_t icp_launch(b2s_handle* h, const IcpProblem* single_host, const IcpProble
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 2 : 1;
   ProfScope prof(h, PK_ICP);
-  if (estimator == B2S_REG_GENERALIZED) B2S_CUDA(cudaLaunchKernelEx(&cfg, icp_kernel<2>, single, problems_dev, pts_cap, h->icp_dbg));
-  else if (estimator == B2S_REG_POINT_TO_PLANE && h->icp_dbg) B2S_CUDA(cudaLaunchKernelEx(&cfg, icp_kernel<3>, single, problems_dev, pts_cap, h->icp_dbg));
-  else if (estimator == B2S_REG_POINT_TO_PLANE) B2S_CUDA(cudaLaunchKernelEx(&cfg, icp_kernel<0>, single, problems_dev, pts_cap, h->icp_dbg));
-  else B2S_CUDA(cudaLaunchKernelEx(&cfg, icp_kernel<1>, single, problems_dev, pts_cap, h->icp_dbg));
+  if (estimator == B2S_REG_GENERALIZED) B2S_CUDA(cudaLaunchKernelEx(&cfg, icp_kernel<2>, single, problems_dev, pts_cap, dbg));
+  else if (estimator == B2S_REG_POINT_TO_PLANE && dbg) B2S_CUDA(cudaLaunchKernelEx(&cfg, icp_kernel<3>, single, problems_dev, pts_cap, dbg));
+  else if (estimator == B2S_REG_POINT_TO_PLANE) B2S_CUDA(cudaLaunchKernelEx(&cfg, icp_kernel<0>, single, problems_dev, pts_cap, dbg));
+  else B2S_CUDA(cudaLaunchKernelEx(&cfg, icp_kernel<1>, single, problems_dev, pts_cap, dbg));
   h->launches++;
   return B2S_OK;
 }

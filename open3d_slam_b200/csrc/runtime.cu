@@ -64,7 +64,9 @@ int32_t DevBuf::ensure(size_t bytes, cudaStream_t s, bool preserve) {
   ncap = (ncap + 255) & ~(size_t)255;
   if (ncap < 256) ncap = 256;
   void* np = nullptr;
-  B2S_CUDA(cudaMalloc(&np, ncap));
+  const cudaError_t me = cudaMalloc(&np, ncap);
+  // the runtime also keeps the failure as this thread's last error: clear it, so that this call reports it and no later one does
+  if (me != cudaSuccess) { cudaGetLastError(); B2S_CUDA(me); }
   if (p) {
     if (preserve) B2S_CUDA(cudaMemcpyAsync(np, p, cap, cudaMemcpyDeviceToDevice, s));
     B2S_CUDA(cudaStreamSynchronize(s));  // earlier kernels may still read the old allocation
@@ -80,9 +82,12 @@ void DevBuf::release() {
   p = nullptr;
   cap = 0;
 }
-void GridIndex::release() {
-  hdr.release(); bbox.release(); cell_start.release(); rank.release(); pts.release(); nrm.release();
-  cap_cells = 0;
+int32_t PinnedBuf::alloc(size_t bytes, unsigned flags) {
+  release();
+  const cudaError_t me = cudaHostAlloc(&p, bytes, flags);
+  if (me != cudaSuccess) { p = nullptr; cudaGetLastError(); B2S_CUDA(me); }   // last error cleared as in DevBuf::ensure
+  cap = bytes;
+  return B2S_OK;
 }
 
 ProfScope::ProfScope(b2s_handle* h_, int kind) : h(h_), idx(-1) {
@@ -102,25 +107,20 @@ ProfScope::~ProfScope() {
   if (idx >= 0) cudaEventRecord(h->prof_recs[(size_t)idx].b, h->stream);
 }
 
-int32_t ensure_pinned(b2s_handle* h, size_t bytes) {
-  if (bytes <= h->pinned_cap) return B2S_OK;
-  if (h->pinned) {
-    B2S_CUDA(cudaStreamSynchronize(h->stream));
-    cudaFreeHost(h->pinned);
-    h->pinned = nullptr; h->pinned_cap = 0;
-  }
-  size_t cap = (bytes + 4095) & ~(size_t)4095;
-  B2S_CUDA(cudaMallocHost(&h->pinned, cap));
-  h->pinned_cap = cap;
-  return B2S_OK;
+constexpr size_t PINNED_READ_BACK = 256;   // layout of h->pinned: the status word at byte 0, read_back's copies from here on
+
+static int32_t ensure_pinned(b2s_handle* h, size_t bytes) {
+  if (bytes <= h->pinned.cap) return B2S_OK;
+  if (h->pinned.p) B2S_CUDA(cudaStreamSynchronize(h->stream));
+  return h->pinned.alloc((bytes + 4095) & ~(size_t)4095);
 }
 
 int32_t check_status(b2s_handle* h) {
   // through pinned memory: a pageable device->host copy goes through a driver staging path that serialises the host
   // threads of all chains
   B2S_TRY(ensure_pinned(h, 4096));
-  volatile uint32_t* pst = reinterpret_cast<volatile uint32_t*>(h->pinned);
-  B2S_CUDA(cudaMemcpyAsync(h->pinned, h->status.p, 4, cudaMemcpyDeviceToHost, h->stream));
+  volatile uint32_t* pst = h->pinned.as<volatile uint32_t>();
+  B2S_CUDA(cudaMemcpyAsync(h->pinned.p, h->status.p, 4, cudaMemcpyDeviceToHost, h->stream));
   B2S_CUDA(cudaStreamSynchronize(h->stream));
   const uint32_t st = pst[0];
   if (st == 0) return B2S_OK;
@@ -131,6 +131,18 @@ int32_t check_status(b2s_handle* h) {
   if (st & ST_EMPTY) { set_error("cloud is empty where the reference asserts a non-empty cloud (status 0x%x)", st); return B2S_E_EMPTY; }
   set_error("unknown device status 0x%x", st);
   return B2S_E_INVALID;
+}
+
+int32_t read_back(b2s_handle* h, std::initializer_list<ReadBack> copies) {
+  size_t end = PINNED_READ_BACK;
+  for (const ReadBack& c : copies) end += c.bytes;
+  B2S_TRY(ensure_pinned(h, end));   // rounded up to whole pages, so check_status keeps this allocation
+  char* stage = h->pinned.as<char>() + PINNED_READ_BACK;
+  for (const ReadBack& c : copies) { B2S_CUDA(cudaMemcpyAsync(stage, c.src, c.bytes, cudaMemcpyDeviceToHost, h->stream)); stage += c.bytes; }
+  const int32_t rc = check_status(h);   // synchronises
+  stage = h->pinned.as<char>() + PINNED_READ_BACK;
+  for (const ReadBack& c : copies) { memcpy(c.dst, stage, c.bytes); stage += c.bytes; }
+  return rc;
 }
 
 // =================================================================================================

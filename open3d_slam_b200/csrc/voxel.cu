@@ -511,8 +511,7 @@ int32_t pose_to_device(b2s_handle* h, const double* T, double* dst) {
 int32_t op_transform(b2s_handle* h, const b2s_cloud* in, const double* T_host, b2s_cloud* out) {
   const size_t n_max = in->n_max > 0 ? in->n_max : 1;
   B2S_TRY(cloud_reserve(h, out, 2 * n_max, in->has_normals));
-  B2S_TRY(h->poses.ensure(64 * 16 * 8, h->stream, true));
-  double* Td = h->poses.as<double>() + 16 * 63;  // slot 63: scratch pose for standalone transforms
+  double* Td = h->poses.as<double>() + 16 * PS_TRANSFORM;
   B2S_TRY(pose_to_device(h, T_host, Td));
   launch_pdl(transform_kernel, grid_for(n_max, VX_THREADS), VX_THREADS, 0, h->stream, in->xyz.as<double>(),
                                                                               in->has_normals ? in->nrm.as<double>() : nullptr,
@@ -638,7 +637,7 @@ __global__ void dense_transform_kernel(double* __restrict__ sums, const int32_t*
 int32_t op_submap_transform(b2s_handle* h, b2s_submap* sm, const double* T_host) {
   Mat4 M;
   for (int i = 0; i < 16; i++) M.m[i] = T_host[i];
-  b2s_cloud* map = sm->cloud[0];
+  b2s_cloud* map = sm->cloud[0].get();
   const size_t n_max = map->n_max > 0 ? map->n_max : 1;
   launch_pdl(o3d_transform_inplace_kernel, grid_for(n_max, VX_THREADS), VX_THREADS, 0, h->stream, map->xyz.as<double>(),
                                                                                           map->has_normals ? map->nrm.as<double>() : nullptr,

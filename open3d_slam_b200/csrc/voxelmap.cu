@@ -11,8 +11,6 @@
 // reference's layer names, e.g. Submap::voxelMapLayer = "map", to 0..B2S_VOXEL_MAP_LAYERS-1).
 // getIndicesInVoxel answers come back sorted ascending, which is the reference's order whenever a layer was filled by
 // insertCloud(layer, cloud) (iota indices, appended in order).
-#include <new>
-
 #include "common.cuh"
 
 using namespace b2s;
@@ -173,45 +171,31 @@ __global__ void __launch_bounds__(VM_THREADS) vm_fill_kernel(const double* __res
 
 }  // namespace b2s
 
-#define VM_LOCK(h) std::lock_guard<std::recursive_mutex> _lk((h)->mu); cudaSetDevice((h)->device)
-
 extern "C" {
 
 int32_t b2s_voxel_map_create(b2s_handle* h, const double voxel_size[3], size_t capacity_voxels, b2s_voxel_map** out) {
   B2S_REQUIRE(h && voxel_size && out && capacity_voxels > 0, B2S_E_INVALID, "bad argument");
   B2S_REQUIRE(voxel_size[0] > 0.0 && voxel_size[1] > 0.0 && voxel_size[2] > 0.0, B2S_E_INVALID, "voxel size must be > 0");
-  VM_LOCK(h);
-  b2s_voxel_map* vm = new (std::nothrow) b2s_voxel_map();
-  B2S_REQUIRE(vm, B2S_E_INVALID, "out of host memory");
-  vm->h = h; vm->device = h->device;
-  for (int d = 0; d < 3; d++) { vm->voxel[d] = voxel_size[d]; vm->inv[d] = 1.0 / voxel_size[d]; }   // fromVoxelSize, VoxelHashMap.hpp:43-45
-  size_t cap = 1024;
-  while (cap < 2 * capacity_voxels) cap <<= 1;
-  vm->cap = cap;
-  int32_t rc = vm->keys.ensure(cap * 8, h->stream);
-  if (rc == B2S_OK) rc = vm->head.ensure(cap * 4 * VM_LAYERS, h->stream);
-  if (rc == B2S_OK) rc = vm->cnt.ensure(cap * 4 * VM_LAYERS, h->stream);
-  if (rc == B2S_OK) rc = vm->used.ensure(64, h->stream);
-  if (rc != B2S_OK) { vm->keys.release(); vm->head.release(); vm->cnt.release(); vm->used.release(); delete vm; return rc; }
-  launch_pdl(vm_clear_kernel, 4 * device_sms(), VM_THREADS, 0, h->stream, vm->keys.as<unsigned long long>(), vm->head.as<int32_t>(), vm->cnt.as<int32_t>(), cap,
-                                                         vm->used.as<int32_t>());
-  h->launches++;
-  *out = vm;
-  B2S_CUDA(cudaGetLastError());
-  return B2S_OK;
+  LOCK(h);
+  return create_object(out, [&](b2s_voxel_map* vm) -> int32_t {
+    vm->h = h; vm->device = h->device;
+    for (int d = 0; d < 3; d++) { vm->voxel[d] = voxel_size[d]; vm->inv[d] = 1.0 / voxel_size[d]; }   // fromVoxelSize, VoxelHashMap.hpp:43-45
+    size_t cap = 1024;
+    while (cap < 2 * capacity_voxels) cap <<= 1;
+    vm->cap = cap;
+    B2S_TRY(vm->keys.ensure(cap * 8, h->stream));
+    B2S_TRY(vm->head.ensure(cap * 4 * VM_LAYERS, h->stream));
+    B2S_TRY(vm->cnt.ensure(cap * 4 * VM_LAYERS, h->stream));
+    B2S_TRY(vm->used.ensure(64, h->stream));
+    return b2s_voxel_map_clear(h, vm);
+  });
 }
 
-void b2s_voxel_map_destroy(b2s_voxel_map* vm) {
-  if (!vm) return;
-  cudaSetDevice(vm->device);
-  cudaDeviceSynchronize();
-  vm->keys.release(); vm->head.release(); vm->cnt.release(); vm->next.release(); vm->eidx.release(); vm->used.release();
-  delete vm;
-}
+void b2s_voxel_map_destroy(b2s_voxel_map* vm) { destroy_object(vm); }
 
 int32_t b2s_voxel_map_clear(b2s_handle* h, b2s_voxel_map* vm) {
   B2S_REQUIRE(h && vm, B2S_E_INVALID, "null argument");
-  VM_LOCK(h);
+  LOCK(h);
   launch_pdl(vm_clear_kernel, 4 * device_sms(), VM_THREADS, 0, h->stream, vm->keys.as<unsigned long long>(), vm->head.as<int32_t>(), vm->cnt.as<int32_t>(), vm->cap,
                                                          vm->used.as<int32_t>());
   h->launches++;
@@ -223,7 +207,7 @@ int32_t b2s_voxel_map_clear(b2s_handle* h, b2s_voxel_map* vm) {
 int32_t b2s_voxel_map_insert_cloud(b2s_handle* h, b2s_voxel_map* vm, int32_t layer, const b2s_cloud* cloud) {
   B2S_REQUIRE(h && vm && cloud, B2S_E_INVALID, "null argument");
   B2S_REQUIRE(layer >= 0 && layer < VM_LAYERS, B2S_E_INVALID, "layer must be in [0, %d)", VM_LAYERS);
-  VM_LOCK(h);
+  LOCK(h);
   const size_t n_max = cloud->n_max;
   if (n_max == 0) return B2S_OK;
   const size_t want = vm->entries_bound + n_max;
@@ -242,19 +226,17 @@ int32_t b2s_voxel_map_insert_cloud(b2s_handle* h, b2s_voxel_map* vm, int32_t lay
 
 int32_t b2s_voxel_map_size(b2s_handle* h, const b2s_voxel_map* vm, size_t* n_voxels) {
   B2S_REQUIRE(h && vm && n_voxels, B2S_E_INVALID, "null argument");
-  VM_LOCK(h);
-  B2S_TRY(ensure_pinned(h, 4096));
-  int32_t* pr = reinterpret_cast<int32_t*>(static_cast<char*>(h->pinned) + 1280);
-  B2S_CUDA(cudaMemcpyAsync(pr, vm->used.p, 8, cudaMemcpyDeviceToHost, h->stream));
-  const int32_t rc = check_status(h);
-  *n_voxels = (size_t)pr[0];
+  LOCK(h);
+  int32_t used = 0;
+  const int32_t rc = read_back(h, {{&used, vm->used.p, 4}});
+  *n_voxels = (size_t)used;
   return rc;
 }
 
 int32_t b2s_voxel_map_has_voxel(b2s_handle* h, const b2s_voxel_map* vm, const b2s_cloud* points, const double T_or_null[16], int32_t* flags_or_null,
                                 size_t capacity, size_t* n_hits) {
   B2S_REQUIRE(h && vm && points, B2S_E_INVALID, "null argument");
-  VM_LOCK(h);
+  LOCK(h);
   const size_t n_max = points->n_max > 0 ? points->n_max : 1;
   B2S_REQUIRE(!flags_or_null || capacity >= points->n_max, B2S_E_CAPACITY, "flag array holds %zu entries, the cloud has up to %zu points", capacity,
               points->n_max);
@@ -264,8 +246,7 @@ int32_t b2s_voxel_map_has_voxel(b2s_handle* h, const b2s_voxel_map* vm, const b2
   B2S_CUDA(cudaMemsetAsync(d_hits, 0, 4, h->stream));
   const double* Td = nullptr;
   if (T_or_null) {
-    B2S_TRY(h->poses.ensure(64 * 16 * 8, h->stream, true));
-    double* slot = h->poses.as<double>() + 16 * 61;
+    double* slot = h->poses.as<double>() + 16 * PS_VOXEL_MAP;
     B2S_TRY(pose_to_device(h, T_or_null, slot));
     Td = slot;
   }
@@ -273,12 +254,10 @@ int32_t b2s_voxel_map_has_voxel(b2s_handle* h, const b2s_voxel_map* vm, const b2
   launch_pdl(vm_has_kernel, grid_for(n_max, VM_THREADS), VM_THREADS, 0, h->stream, points->xyz.as<double>(), points->dn.as<int32_t>(), Td, v,
                                                                           flags_or_null ? d_flags : nullptr, d_hits);
   h->launches++;
-  B2S_TRY(ensure_pinned(h, 4096));
-  int32_t* pr = reinterpret_cast<int32_t*>(static_cast<char*>(h->pinned) + 1280);
-  B2S_CUDA(cudaMemcpyAsync(pr, d_hits, 4, cudaMemcpyDeviceToHost, h->stream));
   if (flags_or_null && points->n_max) B2S_CUDA(cudaMemcpyAsync(flags_or_null, d_flags, points->n_max * 4, cudaMemcpyDeviceToHost, h->stream));
-  const int32_t rc = check_status(h);
-  if (n_hits) *n_hits = (size_t)pr[0];
+  int32_t hits = 0;
+  const int32_t rc = read_back(h, {{&hits, d_hits, 4}});
+  if (n_hits) *n_hits = (size_t)hits;
   return rc;
 }
 
@@ -286,7 +265,7 @@ int32_t b2s_voxel_map_indices_in_voxel(b2s_handle* h, const b2s_voxel_map* vm, i
                                        size_t offsets_capacity, int32_t* indices, size_t indices_capacity, size_t* n_indices) {
   B2S_REQUIRE(h && vm && points && offsets, B2S_E_INVALID, "null argument");
   B2S_REQUIRE(layer >= 0 && layer < VM_LAYERS, B2S_E_INVALID, "layer must be in [0, %d)", VM_LAYERS);
-  VM_LOCK(h);
+  LOCK(h);
   const size_t n_max = points->n_max;
   B2S_REQUIRE(offsets_capacity >= n_max + 1, B2S_E_CAPACITY, "offsets must hold n + 1 = %zu entries", n_max + 1);
   const size_t nm = n_max > 0 ? n_max : 1;
