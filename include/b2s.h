@@ -174,7 +174,13 @@ int32_t b2s_register_host(b2s_handle* h, const double* src_xyz, size_t n_src, co
 /* ---- submap (Submap::mapCloud_ / denseMap_)   include/open3d_slam/Submap.hpp:38-45 ----------------------- */
 int32_t b2s_submap_create(b2s_handle* h, size_t capacity_points, b2s_submap** out);
 void b2s_submap_destroy(b2s_submap* sm);
-/* F1  Submap::insertScan without carving: transform, append, voxelizeWithinCroppingVolume around the sensor
+/* Key limit of the map side.  The fusion hash, the dense map, sparse carving (map points), the overlap and the voxel map key a
+ * point by k = floor(p * (1/voxel)) on the global-origin grid, packed as three 21-bit fields: |k| <= 2^20 - 2 per axis.  A point
+ * with |k| >= 2^20 - 1 (about 52 km at a 0.05 m voxel, 105 km at 0.1 m) is refused: the insertion reports B2S_E_INVALID at the
+ * next synchronising call, and a query reports its voxel as absent.  The ray set of dense carving (b2s_dense_carve) keys with
+ * the full int32 range instead, like the reference, so a far return still casts its ray.
+ *
+ * F1  Submap::insertScan without carving: transform, append, voxelizeWithinCroppingVolume around the sensor
  *     src/Submap.cpp:39-75, src/helpers.cpp:115-183 */
 int32_t b2s_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* preprocessed_scan, const double map_to_sensor[16]);
 /* C1  Submap::carve of the sparse map (space carving)   src/Submap.cpp:55-60,109-123, src/helpers.cpp:235-271,

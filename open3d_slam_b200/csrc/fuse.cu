@@ -30,10 +30,15 @@ int32_t pose_to_device(b2s_handle* h, const double* T, double* dst);  // voxel.c
 //                   point): AccumulatedPoint over the in-cropper members in map order -- old map points first (each counts as
 //                   ONE member, helpers.cpp:30-70), then the scan points in scan order -- mean, normalized mean normal; the result
 //                   takes the slot of the oldest member (or a fresh slot), merged-away map points become tombstones (NaN),
-//                   out-of-cropper members pass through (a staged one gets a slot of its own), the chain is rebuilt;
+//                   out-of-cropper members pass through (a staged one gets a slot of its own), the chain is rebuilt.  The
+//                   mean of three or more members can round across a face of the voxel: such a result is left out of the
+//                   chain and marked (pstamp = -stamp) for K3;
 //   K3 renormalize  the reference's pass also rewrites the normal of every UNTOUCHED in-cropper point as normalized(n / 1)
 //                   (helpers.cpp:172), which is not idempotent in floating point: one streaming pass over the map applies it to
-//                   the points K2 did not rewrite, so normals stay bit-faithful; + commit of the counters and the pose.
+//                   the points K2 did not rewrite, so normals stay bit-faithful.  The same pass links every marked mean into
+//                   the chain of the voxel its position now keys to (the reference re-buckets it there at the next insertion),
+//                   and queues that voxel as a duplicate when it already held a point; + commit of the counters and the pose.
+//                   No chain is walked in K3, so relinking cannot race with a reader.
 // Positions of untouched voxels are unchanged by the reference's pass (mean of one member = p / 1), so the map is identical
 // as a keyed set.  Tombstones are skipped by every reader (NaN never passes a cropper or enters an index) and dropped whenever
 // the map is compacted (carving) or leaves the device.
@@ -134,9 +139,9 @@ __global__ void __launch_bounds__(FZ_THREADS) fuse_stage_kernel(const double* __
 
 // K2
 __global__ void __launch_bounds__(128) fuse_merge_kernel(const int32_t* __restrict__ gate, const int32_t* __restrict__ d_nscan, CropDev crop,
-                                                         FuseView v, int32_t* vhead, const int32_t* __restrict__ vstamp,
-                                                         const int32_t* __restrict__ touched, int32_t* dups, int32_t* d_nmap, size_t capacity,
-                                                         int32_t* ms, uint32_t* status) {
+                                                         FuseView v, const unsigned long long* __restrict__ vkeys, double inv, int32_t* vhead,
+                                                         int32_t* vstamp, const int32_t* __restrict__ touched, int32_t* dups, int32_t* d_nmap,
+                                                         size_t capacity, int32_t* ms, uint32_t* status) {
   pdl_wait();
   if (!((gate == nullptr || *gate != 0) && *d_nscan > 0)) return;
   const int cur = ms[MS_STAMP] + 1;
@@ -150,7 +155,8 @@ __global__ void __launch_bounds__(128) fuse_merge_kernel(const int32_t* __restri
     if (t < ntouched) slot = touched[t];
     else {
       slot = dup_cur[t - ntouched];
-      if (vstamp[slot] == cur) continue;   // touched by this insertion as well: its own thread deals with it
+      // touched by this insertion as well, or listed twice (K3 may queue a voxel K2 queued already): one thread deals with it
+      if (atomicExch(&vstamp[slot], cur) == cur) continue;
     }
     // pass 1: who is in the bucket?  (a map point counts when it is alive and inside the cropper; a staged one by its flag)
     int nin = 0, dest = 0x7fffffff;
@@ -228,8 +234,15 @@ __global__ void __launch_bounds__(128) fuse_merge_kernel(const int32_t* __restri
       const double zz = __dadd_rn(__dadd_rn(__dmul_rn(a0, a0), __dmul_rn(a1, a1)), __dmul_rn(a2, a2));
       if (zz > 0.0) { const double sn = sqrt(zz); a0 = __ddiv_rn(a0, sn); a1 = __ddiv_rn(a1, sn); a2 = __ddiv_rn(a2, sn); }  // .normalized()
       v.mnrm[3 * (size_t)dest] = a0; v.mnrm[3 * (size_t)dest + 1] = a1; v.mnrm[3 * (size_t)dest + 2] = a2;
-      v.pstamp[dest] = cur;
-      v.vnext[dest] = newhead; newhead = dest; survivors++;
+      unsigned long long key;
+      const double* m = v.mxyz + 3 * (size_t)dest;
+      if (fv_key(m[0], m[1], m[2], inv, &key) && key == vkeys[slot]) {
+        v.pstamp[dest] = cur;
+        v.vnext[dest] = newhead; newhead = dest; survivors++;
+      } else {
+        v.pstamp[dest] = -cur;   // the mean left the voxel: K3 links it where it now belongs
+        v.vnext[dest] = -1;
+      }
     }
     vhead[slot] = newhead;
     if (survivors >= 2) {   // more than one map point in this voxel: they merge as soon as both are inside the cropper
@@ -239,17 +252,37 @@ __global__ void __launch_bounds__(128) fuse_merge_kernel(const int32_t* __restri
   }
 }
 
-// K3: normalized(n / 1) for the in-cropper points this insertion did not rewrite; the last block commits the insertion
+// K3: normalized(n / 1) for the in-cropper points this insertion did not rewrite, relinking of the means that left their voxel;
+// the last block commits the insertion
 __global__ void __launch_bounds__(FZ_THREADS) fuse_renorm_commit_kernel(const int32_t* __restrict__ gate, const int32_t* __restrict__ d_nscan,
                                                                         CropDev crop, const double* __restrict__ mxyz, double* __restrict__ mnrm,
-                                                                        const int32_t* __restrict__ pstamp, const int32_t* __restrict__ d_nmap,
-                                                                        int32_t* ms, double* last_pose, const double* __restrict__ Tdev) {
+                                                                        int32_t* __restrict__ pstamp, const int32_t* __restrict__ d_nmap, double inv,
+                                                                        unsigned long long* vkeys, int32_t* vhead, size_t vmask, int32_t* __restrict__ vnext,
+                                                                        int32_t* dups, int32_t* ms, uint32_t* status, double* last_pose,
+                                                                        const double* __restrict__ Tdev) {
   pdl_wait();
   if (!((gate == nullptr || *gate != 0) && *d_nscan > 0)) return;
   const int cur = ms[MS_STAMP] + 1;
   const int n = *d_nmap;
+  const int nxt = (ms[MS_DUPSEL] & 1) ^ 1;   // the list K2 filled for the next insertion
+  int32_t* dup_nxt = dups + (size_t)nxt * FUSE_DUP_CAP;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    if (pstamp[i] == cur) continue;
+    const int ps = pstamp[i];
+    if (ps == -cur) {   // a mean K2 left out of its chain: find-or-insert the voxel it keys to now (a far key stays unlinked, like a rehash)
+      pstamp[i] = cur;
+      unsigned long long key;
+      if (!fv_key(mxyz[3 * (size_t)i], mxyz[3 * (size_t)i + 1], mxyz[3 * (size_t)i + 2], inv, &key)) continue;
+      const long long s = fv_find_or_insert(vkeys, vhead, vmask, key, ms, status);
+      if (s < 0) continue;
+      const int prev = atomicExch(&vhead[s], i);
+      vnext[i] = prev;
+      if (prev >= 0) {   // the voxel holds another map point now: they merge once both are inside the cropper (K2 skips a repeat)
+        const int k = atomicAdd(&ms[MS_NDUP + nxt], 1);
+        if (k < FUSE_DUP_CAP) dup_nxt[k] = (int32_t)s; else atomicOr(status, ST_CAPACITY);
+      }
+      continue;
+    }
+    if (ps == cur) continue;
     const double x = mxyz[3 * (size_t)i], y = mxyz[3 * (size_t)i + 1], z = mxyz[3 * (size_t)i + 2];
     if (!(x == x) || !crop_within(crop, x, y, z)) continue;
     double a0 = mnrm[3 * (size_t)i], a1 = mnrm[3 * (size_t)i + 1], a2 = mnrm[3 * (size_t)i + 2];
@@ -411,12 +444,16 @@ int32_t op_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, c
         sm->stage_xyz.as<double>(),
         sm->stage_nrm.as<double>(), sm->stage_next.as<int32_t>(), sm->stage_in.as<int32_t>(), sm->vkeys.as<unsigned long long>(),
         sm->vhead.as<int32_t>(), sm->vstamp.as<int32_t>(), sm->vcap - 1, sm->touched.as<int32_t>(), ms, h->status.as<uint32_t>());
-    launch_pdl(fuse_merge_kernel, grid_for(m_max + 4096, 128), 128, 0, h->stream, gate_dev, scan->dn.as<int32_t>(), crop, fv, sm->vhead.as<int32_t>(),
+    launch_pdl(fuse_merge_kernel, grid_for(m_max + 4096, 128), 128, 0, h->stream, gate_dev, scan->dn.as<int32_t>(), crop, fv,
+                                                                         sm->vkeys.as<unsigned long long>(), inv, sm->vhead.as<int32_t>(),
                                                                          sm->vstamp.as<int32_t>(), sm->touched.as<int32_t>(), sm->dups.as<int32_t>(),
                                                                          map->dn.as<int32_t>(), sm->capacity, ms, h->status.as<uint32_t>());
     launch_pdl(fuse_renorm_commit_kernel, grid_for(tot_max, FZ_THREADS), FZ_THREADS, 0, h->stream, gate_dev, scan->dn.as<int32_t>(), crop, map->xyz.as<double>(),
                                                                                          map->nrm.as<double>(), sm->pstamp.as<int32_t>(),
-                                                                                         map->dn.as<int32_t>(), ms, sm->pose.as<double>() + 5 * 16, T_dev);
+                                                                                         map->dn.as<int32_t>(), inv, sm->vkeys.as<unsigned long long>(),
+                                                                                         sm->vhead.as<int32_t>(), sm->vcap - 1, sm->vnext.as<int32_t>(),
+                                                                                         sm->dups.as<int32_t>(), ms, h->status.as<uint32_t>(),
+                                                                                         sm->pose.as<double>() + 5 * 16, T_dev);
     h->launches += 3;
   }
   map->n_max = tot_max;   // upper bound only; the exact count lives on the device
@@ -694,31 +731,45 @@ __device__ __forceinline__ long long dense_find_key(const unsigned long long* __
   return -1;
 }
 
+// The ray set is keyed with the full int32 range of the reference's Eigen::Vector3i, not the 21-bit fields of the map: a
+// return 2^20 voxels out still casts a ray through the voxels near the sensor.  A key is three int32 in 16 bytes (z = ~0: empty
+// slot) claimed by one 128-bit compare-and-swap; its home slot is the dense map's hash of the key's low 21 bits per axis, which is
+// the dense map's own home slot wherever the map can key a point.
+struct alignas(16) RayKey { unsigned long long xy, z; };
+constexpr unsigned long long RAY_EMPTY = ~0ull;
+// (int32_t)floor(v) as the reference computes it on x86-64 (cvttsd2si): NaN and values outside int32 become INT32_MIN
+__device__ __forceinline__ int ray_i32(double f) { return (f >= -2147483648.0 && f < 2147483648.0) ? (int)f : INT32_MIN; }
+__device__ __forceinline__ unsigned long long ray_home(int x, int y, int z) {
+  const unsigned long long m = 0x1FFFFF;
+  return dense_hash(((((unsigned)x + 1048576u) & m) << 42) | ((((unsigned)y + 1048576u) & m) << 21) | (((unsigned)z + 1048576u) & m));
+}
+
 __global__ void __launch_bounds__(FZ_THREADS) dcarve_first_kernel(const double* __restrict__ xyz, const int32_t* __restrict__ d_n, double inv,
-                                                                  unsigned long long* keys, int32_t* first, size_t mask,
+                                                                  RayKey* keys, int32_t* first, size_t mask,
                                                                   int32_t* __restrict__ slot_of, const int32_t* __restrict__ enable) {
   pdl_wait();
   if (enable != nullptr && *enable == 0) return;
   const int n = *d_n;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double fx = floor(__dmul_rn(xyz[3 * i], inv)), fy = floor(__dmul_rn(xyz[3 * i + 1], inv)), fz = floor(__dmul_rn(xyz[3 * i + 2], inv));
+    const int kx = ray_i32(floor(__dmul_rn(xyz[3 * i], inv))), ky = ray_i32(floor(__dmul_rn(xyz[3 * i + 1], inv))),
+              kz = ray_i32(floor(__dmul_rn(xyz[3 * i + 2], inv)));
     slot_of[i] = -1;
-    if (!(fabs(fx) < 1048575.0 && fabs(fy) < 1048575.0 && fabs(fz) < 1048575.0)) continue;   // NaN / far away: never a ray
-    const unsigned long long key = dense_pack((int)fx, (int)fy, (int)fz);
-    size_t s = (size_t)dense_hash(key) & mask;
+    const RayKey key{((unsigned long long)(unsigned)kx << 32) | (unsigned)ky, (unsigned long long)(unsigned)kz};
+    const RayKey empty{RAY_EMPTY, RAY_EMPTY};
+    size_t s = (size_t)ray_home(kx, ky, kz) & mask;
     for (size_t probe = 0; probe <= mask; ++probe, s = (s + 1) & mask) {
-      const unsigned long long old = atomicCAS(&keys[s], DENSE_EMPTY, key);
-      if (old == DENSE_EMPTY || old == key) { atomicMin(&first[s], i); slot_of[i] = (int32_t)s; break; }
+      const RayKey old = atomicCAS(&keys[s], empty, key);
+      if (old.z == RAY_EMPTY || (old.xy == key.xy && old.z == key.z)) { atomicMin(&first[s], i); slot_of[i] = (int32_t)s; break; }
     }
   }
 }
 
-__global__ void dcarve_init_kernel(unsigned long long* keys, int32_t* first, size_t cap, int32_t* rm, size_t dense_cap,
+__global__ void dcarve_init_kernel(RayKey* keys, int32_t* first, size_t cap, int32_t* rm, size_t dense_cap,
                                    const int32_t* __restrict__ enable, int32_t* removed) {
   pdl_wait();
   if (blockIdx.x == 0 && threadIdx.x == 0 && removed) *removed = 0;
   if (enable != nullptr && *enable == 0) return;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (size_t)gridDim.x * blockDim.x) { keys[i] = DENSE_EMPTY; first[i] = 0x7fffffff; }
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (size_t)gridDim.x * blockDim.x) { keys[i] = RayKey{RAY_EMPTY, RAY_EMPTY}; first[i] = 0x7fffffff; }
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < dense_cap; i += (size_t)gridDim.x * blockDim.x) rm[i] = 0;
 }
 
@@ -795,11 +846,11 @@ int32_t op_dense_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, con
   const size_t n_max = scan->n_max > 0 ? scan->n_max : 1;
   size_t cap = 1024;
   while (cap < 2 * n_max) cap <<= 1;
-  B2S_TRY(h->keys.ensure(cap * 8, h->stream));
+  B2S_TRY(h->keys.ensure(cap * sizeof(RayKey), h->stream));
   B2S_TRY(h->vals.ensure(cap * 4, h->stream));
   B2S_TRY(h->tmp_i32.ensure((n_max + 64) * 4, h->stream));
   B2S_TRY(h->offs.ensure((sm->dense_cap + 2) * 4, h->stream));   // removal flags per dense slot
-  unsigned long long* keys = h->keys.as<unsigned long long>();
+  RayKey* keys = h->keys.as<RayKey>();
   int32_t* first = h->vals.as<int32_t>();
   int32_t* slot_of = h->tmp_i32.as<int32_t>();
   int32_t* rm = h->offs.as<int32_t>();
