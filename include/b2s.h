@@ -356,6 +356,30 @@ int32_t b2s_feature_download(b2s_handle* h, const b2s_feature* f, double* data, 
 int32_t b2s_feature_upload(b2s_handle* h, b2s_feature* f, const double* data, size_t n);
 int32_t b2s_compute_fpfh(b2s_handle* h, const b2s_cloud* cloud, double radius, int32_t knn, b2s_feature* feature);
 
+/* The feature-cloud front end of Submap::computeFeatures (src/Submap.cpp:239-244) on the submap's map cloud, read in place:
+ *     sparse = VoxelDownSample(map, feature_voxel_size)              normals averaged per voxel, like b2s_voxel_down_sample
+ *     sparse.EstimateNormals(Hybrid(normal_estimation_radius, normal_knn)), NormalizeNormals,
+ *     OrientNormalsTowardsCameraLocation(0)                          the sparse cloud HAS normals (the voxel means): [O3D] keeps
+ *                                                                    the prior where the solver returns a zero vector and flips a
+ *                                                                    normal that points against it (DESIGN.md, row K-features)
+ *     feature = ComputeFPFHFeature(sparse, Hybrid(feature_radius, feature_knn))
+ * b2s_default_feature_params gives the Lua defaults (parameter_structure_definitions.lua:155-159): 0.5 / 2.0 / 20 / 2.5 / 100.
+ * The C++ struct PlaceRecognitionParameters (Parameters.hpp:118-122) defaults differ: normalEstimationRadius_ 1.0, normalKnn_ 10.
+ * Errors: a size <= 0 or a knn <= 0 -> B2S_E_INVALID; normal_knn > 32 or feature_knn > B2S_FEATURE_MAX_KNN -> B2S_E_UNSUPPORTED;
+ * a submap or an output of another handle -> B2S_E_INVALID.  An empty map gives an empty sparse cloud and a feature of zero points.
+ * A map loaded without normals (point-to-point, stored as NaN) gives zero prior normals, which change nothing.
+ * Synchronises once (the sparse cloud's point count, as b2s_compute_fpfh does). */
+typedef struct b2s_feature_params {     /* PlaceRecognitionParameters, the fields computeFeatures reads */
+  double feature_voxel_size;            /* featureVoxelSize_ */
+  double normal_estimation_radius;      /* normalEstimationRadius_ */
+  int32_t normal_knn;                   /* normalKnn_ (<= 32) */
+  double feature_radius;                /* featureRadius_ */
+  int32_t feature_knn;                  /* featureKnn_ (<= B2S_FEATURE_MAX_KNN) */
+} b2s_feature_params;
+void b2s_default_feature_params(b2s_feature_params* p);
+int32_t b2s_submap_compute_features(b2s_handle* h, b2s_submap* sm, const b2s_feature_params* params, b2s_cloud* sparse_out,
+                                    b2s_feature* feature_out);
+
 /* ---- device-to-device hand-over of a cloud's arrays (SURVEY.md section 8e: a submap that is the registration target on
  *      several GPUs is built once by its owner and broadcast over NVLink by the host side -- torch.distributed / NCCL own
  *      the transfer, this library only copies between its cloud and the caller's device buffers on the handle's stream).

@@ -53,6 +53,11 @@ class MapperOptions(C.Structure):
                 ("dense_carving", CarvingParams), ("dense_cropper", Cropper)]
 
 
+class FeatureParams(C.Structure):
+    _fields_ = [("feature_voxel_size", C.c_double), ("normal_estimation_radius", C.c_double), ("normal_knn", C.c_int32),
+                ("feature_radius", C.c_double), ("feature_knn", C.c_int32)]
+
+
 class MapperCounters(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("steps", "accepted", "inserted_map", "inserted_dense", "carve_runs", "carved_points_total",
                                          "dense_carve_runs", "carved_voxels_total")]
@@ -74,6 +79,7 @@ SYMBOLS = [
     "b2s_voxel_map_has_voxel", "b2s_voxel_map_indices_in_voxel", "b2s_mapper_processed_scan",
     "b2s_cloud_export_device", "b2s_cloud_import_device", "b2s_submap_to_cloud", "b2s_nearest_neighbors",
     "b2s_feature_create", "b2s_feature_destroy", "b2s_feature_size", "b2s_feature_download", "b2s_feature_upload", "b2s_compute_fpfh",
+    "b2s_default_feature_params", "b2s_submap_compute_features",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 PROFILE_KINDS = ["icp", "normals", "radix_sort", "nn_grid_build", "voxel", "fuse", "select", "crop"]
@@ -105,6 +111,7 @@ def lib():
         L.b2s_submap_destroy.restype = None
         L.b2s_default_config.restype = None
         L.b2s_default_mapper_options.restype = None
+        L.b2s_default_feature_params.restype = None
         L.b2s_destroy.argtypes = [C.c_void_p]
         L.b2s_cloud_destroy.argtypes = [C.c_void_p]
         L.b2s_submap_destroy.argtypes = [C.c_void_p]

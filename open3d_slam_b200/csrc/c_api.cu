@@ -1130,4 +1130,36 @@ int32_t b2s_compute_fpfh(b2s_handle* h, const b2s_cloud* cloud, double radius, i
   return op_compute_fpfh(h, cloud, n, radius, knn, feature);
 }
 
+void b2s_default_feature_params(b2s_feature_params* p) {   // parameter_structure_definitions.lua:155-159
+  memset(p, 0, sizeof(*p));
+  p->feature_voxel_size = 0.5; p->normal_estimation_radius = 2.0; p->normal_knn = 20; p->feature_radius = 2.5; p->feature_knn = 100;
+}
+
+// Submap::computeFeatures (src/Submap.cpp:239-244) without the host: map -> sparse cloud -> normals (the voxel-mean normals as
+// priors) -> FPFH.  The map's count is never read; the one synchronisation reads the sparse cloud's count for the FPFH launch
+// and reports a voxel key beyond the fixed width.
+int32_t b2s_submap_compute_features(b2s_handle* h, b2s_submap* sm, const b2s_feature_params* p, b2s_cloud* sparse, b2s_feature* f) {
+  B2S_REQUIRE(h && sm && p && sparse && f, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(sm->h == h, B2S_E_INVALID, "the submap belongs to another handle");
+  B2S_REQUIRE(sparse->h == h, B2S_E_INVALID, "the sparse cloud belongs to another handle");
+  B2S_REQUIRE(f->h == h, B2S_E_INVALID, "the feature belongs to another handle");
+  B2S_REQUIRE(!sparse->fixed_cap, B2S_E_INVALID, "the sparse cloud must not be a fixed-capacity staging cloud");
+  B2S_REQUIRE(p->feature_voxel_size > 0.0 && p->normal_estimation_radius > 0.0 && p->feature_radius > 0.0, B2S_E_INVALID,
+              "computeFeatures: featureVoxelSize_, normalEstimationRadius_ and featureRadius_ must be > 0");
+  B2S_REQUIRE(p->normal_knn > 0 && p->feature_knn > 0, B2S_E_INVALID, "computeFeatures: normalKnn_ and featureKnn_ must be > 0");
+  B2S_REQUIRE(p->normal_knn <= 32, B2S_E_UNSUPPORTED, "computeFeatures: normalKnn_ %d > 32 is not supported", p->normal_knn);
+  B2S_REQUIRE(p->feature_knn <= B2S_FEATURE_MAX_KNN, B2S_E_UNSUPPORTED, "computeFeatures: featureKnn_ %d > %d is not supported", p->feature_knn,
+              B2S_FEATURE_MAX_KNN);
+  LOCK(h);
+  b2s_cloud* view = nullptr;
+  B2S_TRY(submap_compact_view(h, sm, &view));   // getMapPointCloudCopy: the live points in map order, normals included (NaN = none)
+  // VoxelDownSample: the full key width, so that the extent need not be read back; a map wider than 2^21 voxels is reported below
+  B2S_TRY(op_voxel_down_sample(h, view, nullptr, p->feature_voxel_size, sparse, 21));
+  B2S_TRY(op_estimate_normals(h, sparse, p->normal_knn, p->normal_estimation_radius, 0.0, nullptr, sparse->has_normals));
+  int32_t n = 0;
+  B2S_TRY(read_back(h, {{&n, sparse->dn.p, 4}}));
+  sparse->n_known = n;
+  return op_compute_fpfh(h, sparse, (size_t)n, p->feature_radius, p->feature_knn, f);
+}
+
 }  // extern "C"

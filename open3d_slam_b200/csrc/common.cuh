@@ -332,9 +332,13 @@ int32_t cloud_set_count(b2s_handle* h, b2s_cloud* c, size_t n);
 
 // stages
 int32_t op_crop(b2s_handle* h, const b2s_cloud* in, const CropDev& crop, b2s_cloud* out);
-int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, b2s_cloud* out);
-// flags (optional, one int per point of c): only flagged points get a normal
-int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius, double cell_hint, const int32_t* flags = nullptr);
+// fixed_key_bits > 0: key width per axis given by the caller instead of measured (no synchronisation); a voxel index outside it
+// sets ST_KEY_OVERFLOW, reported by the next check_status
+int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, b2s_cloud* out, int fixed_key_bits = 0);
+// flags (optional, one int per point of c): only flagged points get a normal.  with_prior: c's normals on entry are the priors of
+// [O3D] EstimateNormals on a cloud that has normals (keep the prior for a zero solver result, flip against it otherwise)
+int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius, double cell_hint, const int32_t* flags = nullptr,
+                            bool with_prior = false);
 int32_t select_flags(b2s_handle* h, const b2s_cloud* in, double ratio, uint32_t seed);
 int32_t select_compact(b2s_handle* h, const b2s_cloud* in, double ratio, b2s_cloud* out);
 int32_t op_random_down_sample(b2s_handle* h, const b2s_cloud* in, double ratio, uint32_t seed, b2s_cloud* out);

@@ -130,7 +130,10 @@ __device__ void fast_eigen3x3_dev(const double* cov, double* out) {
 
 // Post-search part shared by all KMAX: covariance in the reference's neighbour order (ascending (d2, index)) with
 // the reference's single-pass cumulant formula in explicitly rounded fp64, analytic eigen-solver, normalise, orient.
-__device__ __forceinline__ void finish_normal(const double c_in[9], int kk, double qx, double qy, double qz, double* nr) {
+// prior (optional): the query's normal before the estimation -- [O3D] EstimateNormals on a cloud that already has normals keeps
+// the prior where the solver returns a zero vector and otherwise flips the new normal when it points against the prior.  The
+// caller reads it from the very slot nr is stored to afterwards (see op_estimate_normals).
+__device__ __forceinline__ void finish_normal(const double c_in[9], int kk, double qx, double qy, double qz, const double* prior, double* nr) {
   double cov[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};  // [O3D] fewer than 3 neighbours -> identity covariance
   if (kk >= 3) {
     double c[9];
@@ -145,7 +148,13 @@ __device__ __forceinline__ void finish_normal(const double c_in[9], int kk, doub
     cov[5] = cov[7] = __dsub_rn(c[7], __dmul_rn(c[1], c[2]));
   }
   fast_eigen3x3_dev(cov, nr);
-  if (sqrt(dot3d(nr, nr)) == 0.0) { nr[0] = 0; nr[1] = 0; nr[2] = 1; }
+  if (prior) {
+    const double pv[3] = {prior[0], prior[1], prior[2]};
+    if (sqrt(dot3d(nr, nr)) == 0.0) { nr[0] = pv[0]; nr[1] = pv[1]; nr[2] = pv[2]; }
+    else if (__dadd_rn(__dadd_rn(__dmul_rn(nr[0], pv[0]), __dmul_rn(nr[1], pv[1])), __dmul_rn(nr[2], pv[2])) < 0.0) {
+      nr[0] *= -1.0; nr[1] *= -1.0; nr[2] *= -1.0;
+    }
+  } else if (sqrt(dot3d(nr, nr)) == 0.0) { nr[0] = 0; nr[1] = 0; nr[2] = 1; }
   const double zz = dot3d(nr, nr);  // NormalizeNormals
   if (zz > 0) { const double sn = sqrt(zz); nr[0] /= sn; nr[1] /= sn; nr[2] /= sn; }
   if (nr[0] != nr[0]) { nr[0] = 0; nr[1] = 0; nr[2] = 1; }
@@ -170,7 +179,7 @@ __global__ void __launch_bounds__(NK_THREADS) normals_kernel(const GridHeader* _
                                                              const double4* __restrict__ pts, int knn, double radius, int ring_limit,
                                                              int32_t* __restrict__ queue, int32_t* queue_n,
                                                              const int32_t* __restrict__ qlist, const int32_t* __restrict__ qcount,
-                                                             double* __restrict__ out_nrm) {
+                                                             const double* prior_nrm, double* out_nrm) {
   pdl_wait();
   __shared__ GridHeader g;
   if (threadIdx.x == 0) g = *hdr;
@@ -273,7 +282,7 @@ __global__ void __launch_bounds__(NK_THREADS) normals_kernel(const GridHeader* _
       }
     }
     double nr[3];
-    finish_normal(c, kk, qx, qy, qz, nr);
+    finish_normal(c, kk, qx, qy, qz, prior_nrm ? prior_nrm + 3 * (size_t)qi : nullptr, nr);
     out_nrm[3 * (size_t)qi] = nr[0]; out_nrm[3 * (size_t)qi + 1] = nr[1]; out_nrm[3 * (size_t)qi + 2] = nr[2];
   }
 }
@@ -285,7 +294,7 @@ __global__ void __launch_bounds__(NK_THREADS) normals_kernel(const GridHeader* _
 __global__ void __launch_bounds__(NK_THREADS) normals_phase2_kernel(const GridHeader* __restrict__ hdr, const int32_t* __restrict__ cs,
                                                                     const double4* __restrict__ pts, int knn, double radius,
                                                                     const int32_t* __restrict__ queue, const int32_t* __restrict__ queue_n,
-                                                                    double* __restrict__ out_nrm) {
+                                                                    const double* prior_nrm, double* out_nrm) {
   pdl_wait();
   __shared__ GridHeader g;
   if (threadIdx.x == 0) g = *hdr;
@@ -388,7 +397,7 @@ __global__ void __launch_bounds__(NK_THREADS) normals_phase2_kernel(const GridHe
     }
     if (lane == 0) {
       double nr[3];
-      finish_normal(c, kk, qx, qy, qz, nr);
+      finish_normal(c, kk, qx, qy, qz, prior_nrm ? prior_nrm + 3 * (size_t)qi : nullptr, nr);
       out_nrm[3 * (size_t)qi] = nr[0]; out_nrm[3 * (size_t)qi + 1] = nr[1]; out_nrm[3 * (size_t)qi + 2] = nr[2];
     }
   }
@@ -834,7 +843,7 @@ __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2
 // eigen-solver + normalise + orient for the queries the select kernel resolved: one THREAD per query
 __global__ void __launch_bounds__(NK_THREADS) normals_finish_kernel(const GridHeader* __restrict__ hdr, const double4* __restrict__ pts,
                                                                     const int32_t* __restrict__ qlist, const int32_t* __restrict__ qcount,
-                                                                    const double* __restrict__ cum, double* __restrict__ out_nrm) {
+                                                                    const double* __restrict__ cum, const double* prior_nrm, double* out_nrm) {
   pdl_wait();
   const int nq = qlist ? *qcount : hdr->n;
   for (int tq = blockIdx.x * blockDim.x + threadIdx.x; tq < nq; tq += gridDim.x * blockDim.x) {
@@ -844,9 +853,9 @@ __global__ void __launch_bounds__(NK_THREADS) normals_finish_kernel(const GridHe
 #pragma unroll
     for (int t = 0; t < 9; t++) c9[t] = cum[10 * (size_t)tq + t];
     const double4 qp = pts[qlist ? qlist[tq] : tq];
-    double nr[3];
-    finish_normal(c9, (int)kkd, qp.x, qp.y, qp.z, nr);
     const size_t qi = (size_t)(int)__double_as_longlong(qp.w);
+    double nr[3];
+    finish_normal(c9, (int)kkd, qp.x, qp.y, qp.z, prior_nrm ? prior_nrm + 3 * qi : nullptr, nr);
     out_nrm[3 * qi] = nr[0]; out_nrm[3 * qi + 1] = nr[1]; out_nrm[3 * qi + 2] = nr[2];
   }
 }
@@ -874,15 +883,16 @@ __global__ void __launch_bounds__(NK_THREADS) normals_qlist_kernel(const GridHea
   }
 }
 
-int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius, double cell_hint, const int32_t* flags) {
+int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius, double cell_hint, const int32_t* flags, bool with_prior) {
   B2S_REQUIRE(radius > 0.0, B2S_E_INVALID, "maxRadiusNormalEstimation_ must be > 0");  // CloudRegistration.cpp:50
   B2S_REQUIRE(knn > 0, B2S_E_INVALID, "knnNormalEstimation_ must be > 0");            // CloudRegistration.cpp:51
   B2S_REQUIRE(knn <= 32, B2S_E_UNSUPPORTED, "knn > 32 is not supported by the register-resident k-best list yet");
+  B2S_REQUIRE(!with_prior || c->has_normals, B2S_E_NO_NORMALS, "prior normals requested for a cloud without normals");
   double cell = cell_hint > 0.0 ? cell_hint : radius / 4.0;
   if (cell < radius / 16.0) cell = radius / 16.0;  // bound the ring count of the worst case
   B2S_TRY(grid_build(h, &h->grid_b, c, cell, nullptr, false));
   const size_t n_max = c->n_max > 0 ? c->n_max : 1;
-  B2S_TRY(c->nrm.ensure(n_max * 24, h->stream));
+  B2S_TRY(c->nrm.ensure(n_max * 24, h->stream, with_prior));
   int blocks = (int)((n_max + NK_THREADS - 1) / NK_THREADS);
   if (blocks > 16 * device_sms()) blocks = 16 * device_sms();
   if (blocks < 1) blocks = 1;
@@ -902,6 +912,11 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
   const int32_t* cs = grid_starts(&h->grid_b);
   const double4* pts = h->grid_b.pts.as<double4>();
   double* out = c->nrm.as<double>();
+  // The prior normals are the output array itself.  That is safe because every kernel below reads only the POSITIONS of other
+  // points, and each point's normal slot is read (its prior) and then written by exactly one thread: the finish kernel, the
+  // phase-2 kernel or the thread-per-query kernel, whichever resolves the query.  Keep it so: a kernel that read another
+  // point's normal, or two kernels writing the same slot, would see overwritten priors.
+  const double* prior = with_prior ? out : nullptr;
   launch_pdl(zero_i32_kernel, 1, 1, 0, h->stream, qn);
   if (flags) {
     launch_pdl(normals_qlist_kernel, blocks, NK_THREADS, 0, h->stream, hdr, pts, flags, qlist, qn + 1);
@@ -921,13 +936,13 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
     static const bool use_v1 = getenv("B2S_NORMALS_SELECT_V1") != nullptr;   // A/B knob: fixed 3x3x3 block, register gather
     if (use_v1) launch_pdl(normals_select_kernel, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn, cum);
     else launch_pdl(normals_select2_kernel, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn, cum);
-    launch_pdl(normals_finish_kernel, blocks, NK_THREADS, 0, h->stream, hdr, pts, qlist, qcount, cum, out);
+    launch_pdl(normals_finish_kernel, blocks, NK_THREADS, 0, h->stream, hdr, pts, qlist, qcount, cum, prior, out);
     h->launches++;
-  } else if (knn == 20) launch_pdl(normals_kernel<20, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, out);
-  else if (knn == 10) launch_pdl(normals_kernel<10, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, out);
-  else if (knn == 5) launch_pdl(normals_kernel<5, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, out);
-  else if (knn <= 16) launch_pdl(normals_kernel<16, false>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, out);
-  else launch_pdl(normals_kernel<32, false>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, out);
+  } else if (knn == 20) launch_pdl(normals_kernel<20, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
+  else if (knn == 10) launch_pdl(normals_kernel<10, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
+  else if (knn == 5) launch_pdl(normals_kernel<5, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
+  else if (knn <= 16) launch_pdl(normals_kernel<16, false>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
+  else launch_pdl(normals_kernel<32, false>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
   static const bool dbg_counts = getenv("B2S_DEBUG_NORMALS") != nullptr;
   if (dbg_counts) {   // debug aid: how many queries the fast path left to the general kernel
     int32_t hq[6] = {0, 0, 0, 0, 0, 0};
@@ -939,7 +954,7 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
     fprintf(stderr, "[b2s normals] indexed %d queries %d fallback %d cell %.3f dims %dx%dx%d\n", gh.n, flags ? hq[1] : gh.n, hq[0], gh.cell,
             gh.dims[0], gh.dims[1], gh.dims[2]);
   }
-  launch_pdl(normals_phase2_kernel, 4 * device_sms(), NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, queue, qn, out);
+  launch_pdl(normals_phase2_kernel, 4 * device_sms(), NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, queue, qn, prior, out);
   h->launches += 3;
   c->has_normals = true;
   B2S_CUDA(cudaGetLastError());

@@ -263,7 +263,7 @@ static int32_t voxel_impl(b2s_handle* h, const b2s_cloud* in, const CropDev* cro
   return B2S_OK;
 }
 
-int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, b2s_cloud* out) {
+int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, b2s_cloud* out, int fixed_key_bits) {
   if (voxel <= 0.0) {  // helpers.cpp:108-110: voxelize() is a no-op for voxelSize <= 0 (the crop still applies)
     if (crop) return op_crop(h, in, *crop, out);
     B2S_TRY(cloud_reserve(h, out, in->n_max, in->has_normals));
@@ -280,7 +280,8 @@ int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* 
   int bits;
   const bool bounded = crop && !crop->invert && !crop->pose_dev &&
                        (crop->kind == B2S_CROP_MAX_RADIUS || crop->kind == B2S_CROP_MINMAX_RADIUS);
-  if (bounded) bits = bits_for(2.0 * crop->rmax, voxel);
+  if (fixed_key_bits > 0) bits = fixed_key_bits;
+  else if (bounded) bits = bits_for(2.0 * crop->rmax, voxel);
   else {
     unsigned long long hb[6];
     B2S_CUDA(cudaMemcpyAsync(hb, bbox, 48, cudaMemcpyDeviceToHost, h->stream));

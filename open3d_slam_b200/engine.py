@@ -85,6 +85,21 @@ class CloudRegistrationParameters:
 
 
 @dataclass
+class PlaceRecognitionParameters:
+    """The fields of include/open3d_slam/Parameters.hpp:118-122 that Submap::computeFeatures reads.  Defaults = the Lua values
+    (parameter_structure_definitions.lua:155-159); the C++ struct's own defaults differ (normalEstimationRadius_ 1.0, normalKnn_ 10)."""
+    featureVoxelSize: float = 0.5
+    normalEstimationRadius: float = 2.0
+    normalKnn: int = 20
+    featureRadius: float = 2.5
+    featureKnn: int = 100
+
+    def to_c(self) -> L.FeatureParams:
+        return L.FeatureParams(float(self.featureVoxelSize), float(self.normalEstimationRadius), int(self.normalKnn), float(self.featureRadius),
+                               int(self.featureKnn))
+
+
+@dataclass
 class MapperParameters:
     scanToMapRegType: str = "PointToPlaneIcp"
     minRefinementFitness: float = 0.7
@@ -518,6 +533,8 @@ class Submap:
         self.nScansInsertedDenseMap_ = 0
         self._cropperPose = np.eye(4)   # mapBuilderCropper_'s pose: set AFTER each insertion (Submap.cpp:71), Identity before the first
         self.lastCarvedCount = 0
+        self.sparseMapCloud_: Cloud | None = None
+        self.feature_: Feature | None = None
 
     def setMapperOptions(self, *, minMovement: float = 0.0, carving: "SpaceCarvingParameters | None" = None, dense: bool = False,
                          denseCarving: "SpaceCarvingParameters | None" = None, denseCropper: "ScanCroppingParameters | None" = None) -> None:
@@ -636,6 +653,25 @@ class Submap:
     def setMapPointCloud(self, cloud: Cloud):
         L.check(L.lib().b2s_submap_set_cloud(self.eng._h, self._s, cloud._c))
 
+    def computeFeatures(self, params: PlaceRecognitionParameters | None = None) -> None:
+        """The feature half of Submap::computeFeatures (src/Submap.cpp:239-244): sparse cloud (voxel down-sample of the map), its
+        normals, their FPFH -- on the device, kept on this object.  Repeated calls reuse the same cloud and feature."""
+        prm = (params or PlaceRecognitionParameters()).to_c()
+        if self.sparseMapCloud_ is None:
+            self.sparseMapCloud_ = Cloud(self.eng)
+            self.feature_ = Feature(self.eng)
+        L.check(L.lib().b2s_submap_compute_features(self.eng._h, self._s, C.byref(prm), self.sparseMapCloud_._c, self.feature_._f))
+
+    def getSparseMapPointCloud(self) -> Cloud:
+        if self.sparseMapCloud_ is None:
+            raise RuntimeError("Submap::getSparseMapPointCloud: computeFeatures has not run")
+        return self.sparseMapCloud_
+
+    def getFeatures(self) -> "Feature":
+        if self.feature_ is None:
+            raise RuntimeError("Feature ptr is nullptr")   # Submap.cpp:250 assert_nonNullptr
+        return self.feature_
+
     def setPose(self, T):
         T = _mat(T)
         L.check(L.lib().b2s_submap_set_pose(self.eng._h, self._s, _pd(T)))
@@ -646,6 +682,10 @@ class Submap:
         return T
 
     def free(self):
+        for o in (getattr(self, "sparseMapCloud_", None), getattr(self, "feature_", None)):
+            if o is not None:
+                o.free()
+        self.sparseMapCloud_ = self.feature_ = None
         if self._s:
             L.lib().b2s_submap_destroy(self._s)
             self._s = C.c_void_p()

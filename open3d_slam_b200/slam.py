@@ -57,6 +57,8 @@ class SubmapRecord:
     origin: np.ndarray                  # mapToSubmap_ translation at creation
     center: np.ndarray | None = None    # computeSubmapCenter() once finished
     has_voxel_map: bool = False
+    sparse: object = None               # computeFeatures(): sparseMapCloud_ (backend cloud) ...
+    feature: object = None              # ... and feature_ (backend feature)
 
     def mapToSubmapCenter(self) -> np.ndarray:   # Submap::getMapToSubmapCenter
         return self.center if self.center is not None else self.origin
@@ -127,6 +129,17 @@ class SubmapCollection:
         rec.center = self.backend.map_center(rec.handle)
         self.backend.build_voxel_map(rec.handle)
         rec.has_voxel_map = True
+
+    def computeFeatures(self, params: E.PlaceRecognitionParameters | None = None) -> list[int]:
+        """SubmapCollection::computeFeatures (src/SubmapCollection.cpp:219-243): the loop-closure features of every finished submap
+        (Submap::computeFeatures, src/Submap.cpp:239-244), kept on its record.  Returns the submaps it computed, in order -- the
+        reference queues them as loop-closure candidates.  The reference's worker thread, its odometry constraints and the
+        minSecondsBetweenFeatureComputation_ timer are host policy and stay with the caller; the mapper never calls this."""
+        params = params or E.PlaceRecognitionParameters()
+        for idx in self.finishedSubmapsIdxs:
+            rec = self.submaps[idx]
+            rec.sparse, rec.feature = self.backend.compute_features(rec.handle, params)
+        return list(self.finishedSubmapsIdxs)
 
     # -- the call the mapper makes after an accepted registration (:172-207).  The scan itself has ALREADY been fused into the
     # submap that was active during the registration (with carving), because the device chain does that without a host
@@ -297,6 +310,11 @@ class DeviceBackend:
         c = sm.toCloud()
         vm.insertCloud(VOXEL_MAP_LAYER, c)
         c.free()
+
+    def compute_features(self, sm, params: E.PlaceRecognitionParameters):
+        """Submap::computeFeatures on the device: (sparse cloud, Feature), both owned by the submap object"""
+        sm.computeFeatures(params)
+        return sm.getSparseMapPointCloud(), sm.getFeatures()
 
     def revisit_fitness(self, sm, scan, mapToRangeSensor) -> float:
         vm = self._voxel_maps[id(sm)]

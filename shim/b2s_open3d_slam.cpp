@@ -258,7 +258,11 @@ SubmapB200::SubmapB200(const MapperParameters& p, size_t capacityPoints)
   if (rc != B2S_OK) b2sThrow(rc);
 }
 
-SubmapB200::~SubmapB200() { b2s_submap_destroy(sm_); }
+SubmapB200::~SubmapB200() {
+  b2s_feature_destroy(feature_);
+  b2s_cloud_destroy(sparse_);
+  b2s_submap_destroy(sm_);
+}
 
 bool SubmapB200::insertScan(const PointCloud& rawScan, const PointCloud& preProcessedScan, const Transform& mapToRangeSensor, bool isPerformCarving) {
   if (preProcessedScan.IsEmpty()) return true;   // Submap.cpp:41-43
@@ -335,6 +339,52 @@ void SubmapB200::setMapPointCloud(const PointCloud& cloud) {
   const int32_t rc = b2s_submap_set_cloud(h_, sm_, d.c);
   if (rc != B2S_OK) b2sThrow(rc);
   cacheValid_ = false;
+}
+
+void SubmapB200::computeFeatures(const PlaceRecognitionParameters& p) {
+  int32_t rc = B2S_OK;
+  if (!sparse_ && (rc = b2s_cloud_create(h_, &sparse_)) != B2S_OK) b2sThrow(rc);
+  if (!feature_ && (rc = b2s_feature_create(h_, &feature_)) != B2S_OK) b2sThrow(rc);
+  b2s_feature_params fp;
+  b2s_default_feature_params(&fp);
+  fp.feature_voxel_size = p.featureVoxelSize_;              // src/Submap.cpp:241
+  fp.normal_estimation_radius = p.normalEstimationRadius_;  // :242
+  fp.normal_knn = p.normalKnn_;
+  fp.feature_radius = p.featureRadius_;                     // :245
+  fp.feature_knn = p.featureKnn_;
+  rc = b2s_submap_compute_features(h_, sm_, &fp, sparse_, feature_);
+  if (rc != B2S_OK) b2sThrow(rc);
+  sparseValid_ = featureValid_ = false;
+}
+
+const PointCloud& SubmapB200::getSparseMapPointCloud() const {
+  if (sparse_ && !sparseValid_) {   // before the first computeFeatures: the empty default cloud, like the reference's member
+    size_t n = 0;
+    int32_t hasN = 0;
+    int32_t rc = b2s_cloud_size(h_, sparse_, &n, &hasN);
+    if (rc != B2S_OK) b2sThrow(rc);
+    sparseCache_.points_.resize(n);
+    sparseCache_.normals_.resize(hasN ? n : 0);
+    rc = b2s_cloud_download(h_, sparse_, n ? sparseCache_.points_.front().data() : nullptr, (hasN && n) ? sparseCache_.normals_.front().data() : nullptr,
+                            n, &n);
+    if (rc != B2S_OK) b2sThrow(rc);
+    sparseValid_ = true;
+  }
+  return sparseCache_;
+}
+
+const SubmapB200::Feature& SubmapB200::getFeatures() const {
+  if (!feature_) throw std::runtime_error("Feature ptr is nullptr");   // src/Submap.cpp:250 assert_nonNullptr
+  if (!featureValid_) {
+    size_t n = 0;
+    int32_t rc = b2s_feature_size(h_, feature_, &n);
+    if (rc != B2S_OK) b2sThrow(rc);
+    featureCache_.Resize(B2S_FEATURE_DIM, (int)n);   // data_ is column-major: point after point, the ABI's layout
+    rc = b2s_feature_download(h_, feature_, n ? featureCache_.data_.data() : nullptr, n, &n);
+    if (rc != B2S_OK) b2sThrow(rc);
+    featureValid_ = true;
+  }
+  return featureCache_;
 }
 
 void ScanToMapIcpB200::prepareInitialMap(PointCloud* map) const {

@@ -16,6 +16,7 @@
 #include <memory>
 #include <mutex>
 #include "b2s.h"
+#include "open3d/pipelines/registration/Feature.h"
 
 namespace o3d_slam {
 
@@ -68,9 +69,15 @@ void carveB200(const PointCloud& rawScan, const Transform& mapToRangeSensor, con
 //     Submap::transform             src/Submap.cpp:94-107
 //     Submap::getMapPointCloud      src/Submap.cpp:184-186   (download on demand, cached until the next change)
 //     Submap::isEmpty               src/Submap.cpp:221-223
-// The b2s_submap lives on the handle of the thread that created the SubmapB200 (the mapping thread).
+//     Submap::computeFeatures       src/Submap.cpp:239-244   (the feature half: sparse cloud, its normals, FPFH; the voxel map of
+//                                                            the revisit check and the minSecondsBetweenFeatureComputation_
+//                                                            timer stay with the caller)
+//     Submap::getFeatures / getSparseMapPointCloud          (download on demand, cached until the next computeFeatures)
+// The b2s_submap lives on the handle of the thread that created the SubmapB200 (the mapping thread); computeFeatures must run on
+// that handle too (the reference runs it on a worker thread: hand the call to the mapping thread, or build the SubmapB200 there).
 class SubmapB200 {
  public:
+  using Feature = open3d::pipelines::registration::Feature;
   SubmapB200(const MapperParameters& p, size_t capacityPoints = 2000000);
   ~SubmapB200();
   SubmapB200(const SubmapB200&) = delete;
@@ -81,6 +88,9 @@ class SubmapB200 {
   const PointCloud& getMapPointCloud() const;
   bool isEmpty() const;
   void setMapPointCloud(const PointCloud& cloud);           // initial map (SlamWrapper::setInitialMap)
+  void computeFeatures(const PlaceRecognitionParameters& p);
+  const PointCloud& getSparseMapPointCloud() const;
+  const Feature& getFeatures() const;                       // throws before the first computeFeatures, like the reference
   b2s_submap* handle() const { return sm_; }
   b2s_handle* engine() const { return h_; }
 
@@ -94,6 +104,11 @@ class SubmapB200 {
   Transform cropperPose_ = Transform::Identity();           // mapBuilderCropper_'s pose: set after every insertion (Submap.cpp:71)
   mutable PointCloud cache_;
   mutable bool cacheValid_ = false;
+  b2s_cloud* sparse_ = nullptr;                             // sparseMapCloud_, device-resident
+  b2s_feature* feature_ = nullptr;                          // feature_, device-resident
+  mutable PointCloud sparseCache_;
+  mutable Feature featureCache_;
+  mutable bool sparseValid_ = false, featureValid_ = false;
 };
 
 class ScanToMapIcpB200 : public ScanToMapRegistration {

@@ -2,7 +2,7 @@
 // signatures the shim overrides so that it can be type-checked without Open3D / Eigen / the reference tree:
 //   CloudRegistration          include/open3d_slam/CloudRegistration.hpp:19-27
 //   ScanToMapRegistration      include/open3d_slam/ScanToMapRegistration.hpp:24-38
-//   parameter structs          include/open3d_slam/Parameters.hpp:51-98,148-153
+//   parameter structs          include/open3d_slam/Parameters.hpp:51-98,118-122,148-153
 // In a real build, include the reference's own headers instead (INTEGRATION.md).
 #pragma once
 #include <Eigen/Dense>
@@ -23,6 +23,7 @@ struct SpaceCarvingParameters { double voxelSize_ = 0.1, maxRaytracingLength_ = 
 struct MapBuilderParameters { double mapVoxelSize_ = 0.03; ScanCroppingParameters cropper_; SpaceCarvingParameters carving_; };
 enum class ScanToMapRegistrationType : int { PointToPlaneIcp, PointToPointIcp, GeneralizedIcp };   // Parameters.hpp:44-49
 struct ScanToMapRegistrationParameters { double minRefinementFitness_ = 0.7; IcpParameters icp_; ScanToMapRegistrationType scanToMapRegType_ = ScanToMapRegistrationType::PointToPlaneIcp; };
+struct PlaceRecognitionParameters { double normalEstimationRadius_ = 1.0, featureVoxelSize_ = 0.5, featureRadius_ = 2.5; int featureKnn_ = 100, normalKnn_ = 10; };   // Parameters.hpp:118-122
 struct MapperParameters { ScanToMapRegistrationParameters scanMatcher_; ScanProcessingParameters scanProcessing_; MapBuilderParameters mapBuilder_; MapBuilderParameters denseMapBuilder_; };
 class Submap;  // the shim only needs getMapPointCloud(); see b2s_open3d_slam.cpp
 class CloudRegistration {
