@@ -102,7 +102,7 @@ static int32_t check_icp_params(const b2s_icp_params& p) {
 // global working copy of a source of n points (positions + per-point search state); only touched by sources too large for shared memory
 static inline size_t icp_work_bytes(size_t n) { return (n + 1) * 24 + (n + 1) * 4 + 16; }
 
-static void fill_problem(b2s_handle* h, IcpProblem* P, const b2s_cloud* src, const GridIndex* g, const double* init_host,
+static void fill_problem(b2s_handle* h, IcpProblem* P, const b2s_cloud* src, const GridIndex* g, const b2s_cloud* tgt, const double* init_host,
                          const double* init_dev, double* work, b2s_result* out_dev) {
   memset(P, 0, sizeof(*P));
   P->src_xyz = src->xyz.as<double>();
@@ -110,7 +110,7 @@ static void fill_problem(b2s_handle* h, IcpProblem* P, const b2s_cloud* src, con
   P->ghdr = g->hdr.as<GridHeader>();
   P->cell_start = grid_starts(g);
   P->tgt_pts = g->pts.as<double>();
-  P->tgt_nrm = g->nrm.as<double>();
+  P->tgt_nrm = tgt->has_normals ? tgt->nrm.as<double>() : nullptr;
   P->work_xyz = work;
   P->work_prev = reinterpret_cast<int32_t*>(work + 3 * (src->n_max + 1));   // callers size the work buffer with icp_work_bytes()
   P->init_dev = init_dev;
@@ -559,12 +559,12 @@ int32_t b2s_register(b2s_handle* h, const b2s_cloud* source, const b2s_cloud* ta
               "[RegistrationICP] TransformationEstimationPointToPlane requires target normals");
   B2S_REQUIRE(source->has_normals || h->cfg.icp.reg_type != B2S_REG_GENERALIZED, B2S_E_NO_NORMALS,
               "GeneralizedIcp on the device derives the covariances from normals: call estimateNormalsOrCovariancesIfNeeded on both clouds");
-  B2S_TRY(grid_build(h, &h->grid_a, target, nn_cell(h, h->cfg.icp.max_corr_dist), nullptr, true));
+  B2S_TRY(grid_build(h, &h->grid_a, target, nn_cell(h, h->cfg.icp.max_corr_dist), nullptr));
   B2S_TRY(h->work_xyz.ensure(icp_work_bytes(source->n_max), h->stream));
   B2S_TRY(h->problems.ensure(sizeof(IcpProblem), h->stream));
   B2S_TRY(h->results.ensure(sizeof(b2s_result), h->stream));
   IcpProblem P;
-  fill_problem(h, &P, source, &h->grid_a, init, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
+  fill_problem(h, &P, source, &h->grid_a, target, init, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
   B2S_TRY(icp_launch(h, &P, nullptr, 1, source->n_max));
   B2S_CUDA(cudaMemcpyAsync(out, h->results.p, sizeof(b2s_result), cudaMemcpyDeviceToHost, h->stream));
   return check_status(h);
@@ -599,13 +599,13 @@ int32_t b2s_register_batch(b2s_handle* h, int32_t n, const b2s_cloud* const* sou
     if (sources[i]->n_max > max_src) max_src = sources[i]->n_max;
   }
   // R2 for every distinct target in one set of launches (blockIdx.y = target)
-  B2S_TRY(grid_build_batch(h, grids.data(), seen.data(), (int)seen.size(), nn_cell(h, h->cfg.icp.max_corr_dist), true));
+  B2S_TRY(grid_build_batch(h, grids.data(), seen.data(), (int)seen.size(), nn_cell(h, h->cfg.icp.max_corr_dist)));
   B2S_TRY(h->work_xyz.ensure(work_total * 8, h->stream));
   B2S_TRY(h->problems.ensure(sizeof(IcpProblem) * (size_t)n, h->stream));
   B2S_TRY(h->results.ensure(sizeof(b2s_result) * (size_t)n, h->stream));
   size_t woff = 0;
   for (int i = 0; i < n; i++) {
-    fill_problem(h, &probs[i], sources[i], grids[grid_of[i]], inits + 16 * (size_t)i, nullptr, h->work_xyz.as<double>() + woff,
+    fill_problem(h, &probs[i], sources[i], grids[grid_of[i]], targets[i], inits + 16 * (size_t)i, nullptr, h->work_xyz.as<double>() + woff,
                  h->results.as<b2s_result>() + i);
     woff += (icp_work_bytes(sources[i]->n_max) + 7) / 8;
   }
@@ -693,11 +693,11 @@ int32_t b2s_information_matrix(b2s_handle* h, const b2s_cloud* source, const b2s
   B2S_REQUIRE(h && source && target && T && info_out, B2S_E_INVALID, "null argument");
   B2S_REQUIRE(max_corr > 0.0, B2S_E_INVALID, "[GetInformationMatrixFromPointClouds] Invalid max_correspondence_distance.");
   LOCK(h);
-  B2S_TRY(grid_build(h, &h->grid_a, target, max_corr * 0.25, nullptr, false));
+  B2S_TRY(grid_build(h, &h->grid_a, target, max_corr * 0.25, nullptr));
   B2S_TRY(h->work_xyz.ensure(icp_work_bytes(source->n_max), h->stream));
   B2S_TRY(h->results.ensure(sizeof(b2s_result) + 36 * 8 + 64, h->stream));
   IcpProblem P;
-  fill_problem(h, &P, source, &h->grid_a, T, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
+  fill_problem(h, &P, source, &h->grid_a, target, T, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
   P.max_corr = max_corr;
   P.max_iter = 0;
   P.estimator = EST_INFORMATION;
@@ -717,7 +717,7 @@ int32_t b2s_nearest_neighbors(b2s_handle* h, const b2s_cloud* queries, const b2s
   if (n_queries) *n_queries = n;
   B2S_REQUIRE(n <= capacity, B2S_E_CAPACITY, "output arrays hold %zu entries, the cloud has %zu points", capacity, n);
   if (n == 0) return B2S_OK;
-  B2S_TRY(grid_build(h, &h->grid_a, target, nn_cell(h, max_corr), nullptr, false));
+  B2S_TRY(grid_build(h, &h->grid_a, target, nn_cell(h, max_corr), nullptr));
   constexpr size_t CHUNK = 36864;   // what one launch keeps in shared memory (8 CTAs x 72 tiles of 64 points at 40 bytes per point)
   B2S_TRY(h->work_xyz.ensure(icp_work_bytes(CHUNK), h->stream));
   B2S_TRY(h->results.ensure(sizeof(b2s_result) + 36 * 8 + 64, h->stream));
@@ -730,7 +730,7 @@ int32_t b2s_nearest_neighbors(b2s_handle* h, const b2s_cloud* queries, const b2s
     launch_pdl(write_i32_kernel, 1, 1, 0, h->stream, d_cnt, (int32_t)cnt);
     h->launches++;
     IcpProblem P;
-    fill_problem(h, &P, queries, &h->grid_a, T ? T : I, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
+    fill_problem(h, &P, queries, &h->grid_a, target, T ? T : I, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
     P.src_xyz = queries->xyz.as<double>() + 3 * off;
     P.work_prev = reinterpret_cast<int32_t*>(h->work_xyz.as<double>() + 3 * (CHUNK + 1));   // the work buffer is sized for a chunk, not for the cloud
     P.src_n = d_cnt;
@@ -926,11 +926,11 @@ static int32_t register_to_submap_async(b2s_handle* h, const b2s_cloud* scan, co
   b2s_cropper c = h->cfg.scan.scan_matcher_cropper;  // ScanToMapRegistration.cpp:58 setPose(mapToRangeSensor)
   if (sensor_pose_host) { c.center[0] = sensor_pose_host[3]; c.center[1] = sensor_pose_host[7]; c.center[2] = sensor_pose_host[11]; }
   CropDev patch = make_crop(&c, sensor_pose_dev);
-  B2S_TRY(grid_build(h, &h->grid_a, map, nn_cell(h, h->cfg.icp.max_corr_dist), &patch, true));
+  B2S_TRY(grid_build(h, &h->grid_a, map, nn_cell(h, h->cfg.icp.max_corr_dist), &patch));
   B2S_TRY(h->work_xyz.ensure(icp_work_bytes(scan->n_max), h->stream));
   B2S_TRY(h->problems.ensure(sizeof(IcpProblem), h->stream));
   IcpProblem P;
-  fill_problem(h, &P, scan, &h->grid_a, init_host, init_dev, h->work_xyz.as<double>(), out_dev);
+  fill_problem(h, &P, scan, &h->grid_a, map, init_host, init_dev, h->work_xyz.as<double>(), out_dev);
   return icp_launch(h, &P, nullptr, 1, scan->n_max);
 }
 

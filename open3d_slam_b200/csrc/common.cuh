@@ -113,8 +113,7 @@ struct GridIndex {
   DevBuf bbox;           // 6 x uint64 ordered-double min/max
   DevBuf cell_start;     // int32 [cap_cells + 1]
   DevBuf rank;           // int32 per point: rank within its cell (-1 = not indexed)
-  DevBuf pts;            // double4 per indexed point: x,y,z, bits(original index)
-  DevBuf nrm;            // double4 per indexed point: nx,ny,nz,0
+  DevBuf pts;            // double4 per indexed point: x,y,z, bits(original index); normals are read from the cloud through it
   int32_t cap_cells = 0;
 };
 
@@ -322,9 +321,9 @@ struct CropDev {      // cropper passed by value to kernels; centre may come fro
   const double* pose_dev;   // if non-null the centre is (pose[3], pose[7], pose[11])
 };
 CropDev make_crop(const b2s_cropper* c, const double* pose_dev = nullptr);
-int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch, bool with_normals);
+int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch);
 // the same for n clouds at once (batched registration: every pair brings its own target), blockIdx.y = cloud
-int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* const* clouds, int n, double cell, bool with_normals);
+int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* const* clouds, int n, double cell);
 
 int32_t pose_to_device(b2s_handle* h, const double* T, double* dst);   // host 4x4 -> device slot, no staging buffer (voxel.cu)
 int32_t cloud_reserve(b2s_handle* h, b2s_cloud* c, size_t n, bool normals);
@@ -350,7 +349,7 @@ struct IcpProblem {
   const GridHeader* ghdr;
   const int32_t* cell_start;
   const double* tgt_pts;    // double4
-  const double* tgt_nrm;    // double4
+  const double* tgt_nrm;    // the target cloud's normals (3 x f64 per point, cloud order), indexed by tgt_pts[k].w
   double* work_xyz;         // global working copy of the source (used when it does not fit in shared memory) ...
   int32_t* work_prev;       // ... and its per-point search state
   const double* init_dev;   // optional device-resident init (overrides init)

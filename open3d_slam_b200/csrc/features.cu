@@ -262,7 +262,7 @@ int32_t op_compute_fpfh(b2s_handle* h, const b2s_cloud* c, size_t n, double radi
   f->n = 0;
   if (n == 0) return B2S_OK;
   // cell edge as for the normals (radius / 4): a hybrid search ends within about four rings
-  B2S_TRY(grid_build(h, &h->grid_b, c, radius / 4.0, nullptr, false));
+  B2S_TRY(grid_build(h, &h->grid_b, c, radius / 4.0, nullptr));
   B2S_TRY(f->data.ensure(n * 33 * 8, h->stream));
   B2S_TRY(f->spfh.ensure(n * 33 * 8, h->stream));
   B2S_TRY(f->nb_idx.ensure(n * (size_t)knn * 4, h->stream));

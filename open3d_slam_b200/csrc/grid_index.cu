@@ -2,7 +2,9 @@
 // [O3D] RegistrationICP / EstimateNormals call (KDTreeFlann::SetGeometry; SURVEY.md section 8a row R2).
 //
 // Layout (HBM): a dense grid of cells over the (optionally cropped) point set; points are counting-sorted by
-// linear cell id (x fastest) into a packed double4 array {x,y,z,bits(original index)}; normals likewise.
+// linear cell id (x fastest) into a packed double4 array {x,y,z,bits(original index)}.  Normals are not copied: a
+// search needs them only for its final correspondences, and reads them from the cloud through the original index
+// (copying them was half of the scatter's bytes, for every indexed point of every build).
 // cell_start[c] .. cell_start[c+1] is the slot range of cell c.  Because x is the fastest axis, a run of
 // neighbouring cells along x is ONE contiguous slot range, so a 3x3x3 neighbourhood is 9 ranges.
 // Points outside the grid box are clamped into the border cells, which the search treats as semi-infinite.
@@ -117,10 +119,9 @@ __global__ void __launch_bounds__(GB_THREADS) grid_count_kernel(const double* __
   grid_count_body(xyz, d_n, crop, use_crop, hdr, counts, rank);
 }
 
-__device__ __forceinline__ void grid_scatter_body(const double* __restrict__ xyz, const double* __restrict__ nrm,
-                                                  const int32_t* __restrict__ d_n, GridHeader* hdr,
+__device__ __forceinline__ void grid_scatter_body(const double* __restrict__ xyz, const int32_t* __restrict__ d_n, GridHeader* hdr,
                                                   const int32_t* __restrict__ cell_start, const int32_t* __restrict__ rank,
-                                                  double4* __restrict__ pts, double4* __restrict__ onrm) {
+                                                  double4* __restrict__ pts) {
   const int n = *d_n;
   __shared__ GridHeader g;
   if (threadIdx.x == 0) g = *hdr;
@@ -132,23 +133,20 @@ __device__ __forceinline__ void grid_scatter_body(const double* __restrict__ xyz
     double x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
     int slot = cell_start[grid_cell_of(g, x, y, z)] + r;
     pts[slot] = make_double4(x, y, z, __longlong_as_double((long long)i));
-    if (nrm) onrm[slot] = make_double4(nrm[3 * i], nrm[3 * i + 1], nrm[3 * i + 2], 0.0);
   }
 }
 
-__global__ void __launch_bounds__(GB_THREADS) grid_scatter_kernel(const double* __restrict__ xyz, const double* __restrict__ nrm,
-                                                                  const int32_t* __restrict__ d_n, GridHeader* hdr,
-                                                                  const int32_t* __restrict__ cell_start,
-                                                                  const int32_t* __restrict__ rank, double4* __restrict__ pts,
-                                                                  double4* __restrict__ onrm) {
+__global__ void __launch_bounds__(GB_THREADS) grid_scatter_kernel(const double* __restrict__ xyz, const int32_t* __restrict__ d_n,
+                                                                  GridHeader* hdr, const int32_t* __restrict__ cell_start,
+                                                                  const int32_t* __restrict__ rank, double4* __restrict__ pts) {
   pdl_wait();
-  grid_scatter_body(xyz, nrm, d_n, hdr, cell_start, rank, pts, onrm);
+  grid_scatter_body(xyz, d_n, hdr, cell_start, rank, pts);
 }
 
 // ---- batched build: blockIdx.y = job -------------------------------------------------------------------------------
 struct GridJob {
-  const double* xyz; const double* nrm; const int32_t* d_n;
-  unsigned long long* bbox; GridHeader* hdr; int32_t* counts; int32_t* starts; int32_t* rank; double4* pts; double4* onrm;
+  const double* xyz; const int32_t* d_n;
+  unsigned long long* bbox; GridHeader* hdr; int32_t* counts; int32_t* starts; int32_t* rank; double4* pts;
   int32_t cap_cells; int32_t pad;
 };
 
@@ -185,7 +183,7 @@ __global__ void __launch_bounds__(GB_THREADS) gridb_count_kernel(const GridJob* 
 __global__ void __launch_bounds__(GB_THREADS) gridb_scatter_kernel(const GridJob* __restrict__ jobs) {
   pdl_wait();
   const GridJob j = jobs[blockIdx.y];
-  grid_scatter_body(j.xyz, j.nrm, j.d_n, j.hdr, j.starts, j.rank, j.pts, j.onrm);
+  grid_scatter_body(j.xyz, j.d_n, j.hdr, j.starts, j.rank, j.pts);
 }
 
 CropDev make_crop(const b2s_cropper* c, const double* pose_dev) {
@@ -199,7 +197,7 @@ CropDev make_crop(const b2s_cropper* c, const double* pose_dev) {
   return d;
 }
 
-int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch, bool with_normals) {
+int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch) {
   B2S_REQUIRE(cell > 0.0, B2S_E_INVALID, "grid_build: cell size must be > 0");
   const size_t n_max = cloud->n_max > 0 ? cloud->n_max : 1;
   // buffers follow the ALLOCATION of the cloud, not its current size: a growing map never re-allocates its index
@@ -219,7 +217,6 @@ int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double c
   B2S_TRY(g->bbox.ensure(64, h->stream));
   B2S_TRY(g->rank.ensure(n_alloc * 4, h->stream));
   B2S_TRY(g->pts.ensure(n_alloc * 32, h->stream));
-  if (with_normals) B2S_TRY(g->nrm.ensure(n_alloc * 32, h->stream));
   CropDev cd = patch ? *patch : make_crop(nullptr);
   const int use_crop = patch ? 1 : 0;
   const int blocks = grid_for(n_max, GB_THREADS);
@@ -236,17 +233,15 @@ int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double c
   h->launches += 5;
   // scan over ncell (device-known) counts; launch sized for the capacity
   B2S_TRY(scan_exclusive_i32(h, counts, starts, &hdr->ncell, (size_t)g->cap_cells, nullptr));
-  launch_pdl(grid_scatter_kernel, blocks, GB_THREADS, 0, h->stream, cloud->xyz.as<double>(),
-                                                            (with_normals && cloud->has_normals) ? cloud->nrm.as<double>() : nullptr, d_n,
-                                                            hdr, starts, g->rank.as<int32_t>(), g->pts.as<double4>(),
-                                                            with_normals ? g->nrm.as<double4>() : nullptr);
+  launch_pdl(grid_scatter_kernel, blocks, GB_THREADS, 0, h->stream, cloud->xyz.as<double>(), d_n, hdr, starts, g->rank.as<int32_t>(),
+             g->pts.as<double4>());
   h->launches++;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;
 }
 
 
-static int32_t grid_reserve(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, bool with_normals, size_t* n_alloc_out) {
+static int32_t grid_reserve(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, size_t* n_alloc_out) {
   const size_t n_max = cloud->n_max > 0 ? cloud->n_max : 1;
   size_t n_alloc = cloud->xyz.cap / 24;
   if (n_alloc < n_max) n_alloc = n_max;
@@ -261,18 +256,17 @@ static int32_t grid_reserve(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud,
   B2S_TRY(g->bbox.ensure(64, h->stream));
   B2S_TRY(g->rank.ensure(n_alloc * 4, h->stream));
   B2S_TRY(g->pts.ensure(n_alloc * 32, h->stream));
-  if (with_normals) B2S_TRY(g->nrm.ensure(n_alloc * 32, h->stream));
   *n_alloc_out = n_alloc;
   return B2S_OK;
 }
 
-int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* const* clouds, int n, double cell, bool with_normals) {
+int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* const* clouds, int n, double cell) {
   B2S_REQUIRE(cell > 0.0, B2S_E_INVALID, "grid_build: cell size must be > 0");
   if (n <= 0) return B2S_OK;
   size_t max_pts = 1, max_cells = 1;
   for (int i = 0; i < n; i++) {
     size_t n_alloc;
-    B2S_TRY(grid_reserve(h, g[i], clouds[i], with_normals, &n_alloc));
+    B2S_TRY(grid_reserve(h, g[i], clouds[i], &n_alloc));
     if (clouds[i]->n_max > max_pts) max_pts = clouds[i]->n_max;
     if ((size_t)g[i]->cap_cells > max_cells) max_cells = (size_t)g[i]->cap_cells;
   }
@@ -292,12 +286,10 @@ int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* co
     int32_t* starts = counts + g[i]->cap_cells + 4;
     GridHeader* hdr = g[i]->hdr.as<GridHeader>();
     gj[i].xyz = clouds[i]->xyz.as<double>();
-    gj[i].nrm = (with_normals && clouds[i]->has_normals) ? clouds[i]->nrm.as<double>() : nullptr;
     gj[i].d_n = clouds[i]->dn.as<int32_t>();
     gj[i].bbox = g[i]->bbox.as<unsigned long long>();
     gj[i].hdr = hdr; gj[i].counts = counts; gj[i].starts = starts; gj[i].rank = g[i]->rank.as<int32_t>();
     gj[i].pts = g[i]->pts.as<double4>();
-    gj[i].onrm = with_normals ? g[i]->nrm.as<double4>() : nullptr;
     gj[i].cap_cells = g[i]->cap_cells;
     unsigned long long* st = reinterpret_cast<unsigned long long*>(dev + off_state + st_bytes * (size_t)i);
     sj[i].in = counts; sj[i].out = starts; sj[i].d_n = &hdr->ncell; sj[i].state = st; sj[i].counter = reinterpret_cast<int32_t*>(st + ntiles);

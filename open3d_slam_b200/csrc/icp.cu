@@ -82,8 +82,13 @@ struct GridView {
   int nx, ny, nz;
   const int32_t* __restrict__ cs;
   const double4* __restrict__ pts;
-  const double4* __restrict__ nrm;
+  const double* __restrict__ nrm;   // the target cloud's normals in cloud order: point pts[slot] has nrm[3 * bits(pts[slot].w)]
 };
+
+__device__ __forceinline__ double4 target_normal(const GridView& g, const double4& q) {
+  const double* n = g.nrm + 3 * (size_t)__double_as_longlong(q.w);
+  return make_double4(n[0], n[1], n[2], 0.0);
+}
 
 struct NNState {
   double best;     // d2 of the best candidate so far (or the search limit while bslot < 0)
@@ -564,7 +569,7 @@ template <bool LANE0>
 __device__ __forceinline__ void icp_contribute_plane(double* wacc, const GridView& g, int slot, double px, double py, double pz, int lane) {
   const bool ok = slot >= 0;
   double4 q = make_double4(0, 0, 0, 0), nn = make_double4(0, 0, 0, 0);
-  if (ok) { q = g.pts[slot]; nn = g.nrm[slot]; }
+  if (ok) { q = g.pts[slot]; nn = target_normal(g, q); }
   const double d2 = ok ? dist2_exact(px, py, pz, q.x, q.y, q.z) : 0.0;
   const double r = (px - q.x) * nn.x + (py - q.y) * nn.y + (pz - q.z) * nn.z;   // zero normal for a lane without correspondence: all terms vanish
   double J[6];
@@ -628,7 +633,7 @@ __device__ __forceinline__ void icp_contribute_gicp(double* wacc, const GridView
   // a lane without correspondence runs the algebra on a harmless stand-in (unit normals) and contributes with weight zero
   double4 q = make_double4(px, py, pz, 0), nt = make_double4(1, 0, 0, 0);
   double sn[3] = {1.0, 0.0, 0.0};
-  if (ok) { q = g.pts[slot]; nt = g.nrm[slot]; sn[0] = sn_ptr[0]; sn[1] = sn_ptr[1]; sn[2] = sn_ptr[2]; }
+  if (ok) { q = g.pts[slot]; nt = target_normal(g, q); sn[0] = sn_ptr[0]; sn[1] = sn_ptr[1]; sn[2] = sn_ptr[2]; }
   const double wgt = ok ? 1.0 : 0.0;
   const double d2 = ok ? dist2_exact(px, py, pz, q.x, q.y, q.z) : 0.0;
   double Ct[9], Cs0[9], M[9];
@@ -790,7 +795,7 @@ __global__ void __launch_bounds__(icp_threads(MODE), 1) icp_kernel(const __grid_
   g.nx = s_g->dims[0]; g.ny = s_g->dims[1]; g.nz = s_g->dims[2];
   g.cs = P.cell_start;
   g.pts = reinterpret_cast<const double4*>(P.tgt_pts);
-  g.nrm = reinterpret_cast<const double4*>(P.tgt_nrm);
+  g.nrm = P.tgt_nrm;
   const double r2 = P.max_corr * P.max_corr;
   const int max_iter = P.max_iter;
   constexpr bool GICP = MODE == 2;

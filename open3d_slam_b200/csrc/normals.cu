@@ -890,7 +890,7 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
   B2S_REQUIRE(!with_prior || c->has_normals, B2S_E_NO_NORMALS, "prior normals requested for a cloud without normals");
   double cell = cell_hint > 0.0 ? cell_hint : radius / 4.0;
   if (cell < radius / 16.0) cell = radius / 16.0;  // bound the ring count of the worst case
-  B2S_TRY(grid_build(h, &h->grid_b, c, cell, nullptr, false));
+  B2S_TRY(grid_build(h, &h->grid_b, c, cell, nullptr));
   const size_t n_max = c->n_max > 0 ? c->n_max : 1;
   B2S_TRY(c->nrm.ensure(n_max * 24, h->stream, with_prior));
   int blocks = (int)((n_max + NK_THREADS - 1) / NK_THREADS);
