@@ -380,6 +380,49 @@ void b2s_default_feature_params(b2s_feature_params* p);
 int32_t b2s_submap_compute_features(b2s_handle* h, b2s_submap* sm, const b2s_feature_params* params, b2s_cloud* sparse_out,
                                     b2s_feature* feature_out);
 
+/* ---- loop-closure proposal: [O3D] RegistrationRANSACBasedOnFeatureMatching as PlaceRecognition::buildLoopClosureConstraints
+ *      calls it (src/PlaceRecognition.cpp:81-86): mutual filter, TransformationEstimationPointToPoint(false), the distance and
+ *      edge-length checkers, RANSACConvergenceCriteria(max_iteration, confidence).  The exact semantics, including the
+ *      counter-based hypothesis stream that replaces std::random_device and the sequential best / stop rule that makes a run
+ *      independent of how the device batches it, are DESIGN.md row K-ransac.
+ * b2s_default_ransac_params gives the Lua values (parameter_structure_definitions.lua:156-161): mutual 1, ransac_n 3,
+ * max_correspondence_distance 0.75, checker_distance 0.8, checker_edge_length 0.6, max_iteration 10 000 000, confidence 0.999.
+ * The C++ struct PlaceRecognitionParameters (Parameters.hpp:123-129) defaults differ: ransacNumIter_ 1 000 000, ransacProbability_
+ * 0.99, correspondenceCheckerDistance_ 0.75, correspondenceCheckerEdgeLength_ 0.5. */
+#define B2S_RANSAC_MAX_N 8
+typedef struct b2s_ransac_params {
+  int32_t mutual_filter;                /* mutual_filter (true at PlaceRecognition.cpp:82) */
+  int32_t ransac_n;                     /* ransacModelSize_ (3 <= n <= B2S_RANSAC_MAX_N; n < 3 gives the empty result) */
+  double max_correspondence_distance;   /* ransacMaxCorrespondenceDistance_ (validation radius) */
+  double checker_distance;              /* correspondenceCheckerDistance_ */
+  double checker_edge_length;           /* correspondenceCheckerEdgeLength_ */
+  int64_t max_iteration;                /* ransacNumIter_ */
+  double confidence;                    /* ransacProbability_, in (0, 1) */
+  uint64_t seed;                        /* replaces std::random_device: the hypothesis stream of DESIGN.md row K-ransac */
+} b2s_ransac_params;
+void b2s_default_ransac_params(b2s_ransac_params* p);
+typedef struct b2s_ransac_result {
+  b2s_result result;                    /* T, fitness, inlier_rmse, n_corr = inliers (correspondence_set_.size(), :86); iters = 0 */
+  int64_t hypotheses;                   /* the h the sequential loop stopped at */
+  int64_t validations;                  /* hypotheses that passed both checkers and were validated by that loop */
+  int64_t best_hypothesis;              /* the h of the result (-1 = the empty result) */
+  int32_t n_feature_corr;               /* size of the feature correspondence set RANSAC drew from */
+  int32_t used_mutual;                  /* 1 when that set is the mutual one */
+} b2s_ransac_result;
+/* One source (its sparse cloud and FPFH) against n_targets candidates, the loop of PlaceRecognition.cpp:71 in one call; out[k]
+ * belongs to target k and does not depend on the other targets.  Errors: a feature whose size differs from its cloud's, an object
+ * of another handle, n_targets < 0, confidence outside (0, 1) or max_iteration < 0 -> B2S_E_INVALID; ransac_n > B2S_RANSAC_MAX_N ->
+ * B2S_E_UNSUPPORTED.  ransac_n < 3, max_correspondence_distance <= 0, an empty cloud or a correspondence set smaller than ransac_n
+ * give the empty result (T = I, zeros) with B2S_OK.  Synchronises once per batch of hypotheses (B2S_RANSAC_BATCH, DESIGN.md 5). */
+int32_t b2s_ransac_feature_matching(b2s_handle* h, const b2s_cloud* source_sparse, const b2s_feature* source_feature, int32_t n_targets,
+                                    const b2s_cloud* const* target_sparses, const b2s_feature* const* target_features,
+                                    const b2s_ransac_params* params, b2s_ransac_result* out);
+/* The two exact nearest-feature arrays RANSAC's correspondence set is built from: src_to_tgt[i] = argmin_j d2(i, j),
+ * tgt_to_src[j] = argmin_i d2(i, j), d2 summed over the 33 bins in ascending order, ties to the lower index; -1 when the other
+ * feature is empty.  Host arrays hold the capacities given (>= the feature sizes, else B2S_E_CAPACITY).  Synchronises. */
+int32_t b2s_feature_correspondences(b2s_handle* h, const b2s_feature* source_feature, const b2s_feature* target_feature, int32_t* src_to_tgt,
+                                    size_t src_capacity, int32_t* tgt_to_src, size_t tgt_capacity);
+
 /* ---- device-to-device hand-over of a cloud's arrays (SURVEY.md section 8e: a submap that is the registration target on
  *      several GPUs is built once by its owner and broadcast over NVLink by the host side -- torch.distributed / NCCL own
  *      the transfer, this library only copies between its cloud and the caller's device buffers on the handle's stream).

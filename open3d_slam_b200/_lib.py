@@ -58,6 +58,17 @@ class FeatureParams(C.Structure):
                 ("feature_radius", C.c_double), ("feature_knn", C.c_int32)]
 
 
+class RansacParams(C.Structure):
+    _fields_ = [("mutual_filter", C.c_int32), ("ransac_n", C.c_int32), ("max_correspondence_distance", C.c_double),
+                ("checker_distance", C.c_double), ("checker_edge_length", C.c_double), ("max_iteration", C.c_int64),
+                ("confidence", C.c_double), ("seed", C.c_uint64)]
+
+
+class RansacResult(C.Structure):
+    _fields_ = [("result", Result), ("hypotheses", C.c_int64), ("validations", C.c_int64), ("best_hypothesis", C.c_int64), ("n_feature_corr", C.c_int32),
+                ("used_mutual", C.c_int32)]
+
+
 class MapperCounters(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("steps", "accepted", "inserted_map", "inserted_dense", "carve_runs", "carved_points_total",
                                          "dense_carve_runs", "carved_voxels_total")]
@@ -80,6 +91,7 @@ SYMBOLS = [
     "b2s_cloud_export_device", "b2s_cloud_import_device", "b2s_submap_to_cloud", "b2s_nearest_neighbors",
     "b2s_feature_create", "b2s_feature_destroy", "b2s_feature_size", "b2s_feature_download", "b2s_feature_upload", "b2s_compute_fpfh",
     "b2s_default_feature_params", "b2s_submap_compute_features",
+    "b2s_default_ransac_params", "b2s_ransac_feature_matching", "b2s_feature_correspondences",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 PROFILE_KINDS = ["icp", "normals", "radix_sort", "nn_grid_build", "voxel", "fuse", "select", "crop"]
@@ -112,6 +124,7 @@ def lib():
         L.b2s_default_config.restype = None
         L.b2s_default_mapper_options.restype = None
         L.b2s_default_feature_params.restype = None
+        L.b2s_default_ransac_params.restype = None
         L.b2s_destroy.argtypes = [C.c_void_p]
         L.b2s_cloud_destroy.argtypes = [C.c_void_p]
         L.b2s_submap_destroy.argtypes = [C.c_void_p]

@@ -1162,4 +1162,55 @@ int32_t b2s_submap_compute_features(b2s_handle* h, b2s_submap* sm, const b2s_fea
   return op_compute_fpfh(h, sparse, (size_t)n, p->feature_radius, p->feature_knn, f);
 }
 
+// ---- loop-closure proposal (PlaceRecognition.cpp:81-86) --------------------------------------------------------------------
+void b2s_default_ransac_params(b2s_ransac_params* p) {   // parameter_structure_definitions.lua:156-161
+  memset(p, 0, sizeof(*p));
+  p->mutual_filter = 1; p->ransac_n = 3; p->max_correspondence_distance = 0.75; p->checker_distance = 0.8; p->checker_edge_length = 0.6;
+  p->max_iteration = 10000000; p->confidence = 0.999; p->seed = 1;
+}
+
+// RegistrationRANSACBasedOnFeatureMatching(sourceSparse, targetSparse, sourceFeature, targetFeature, true, ...) for every candidate
+// of PlaceRecognition.cpp:71 in one call.  Synchronises for the cloud sizes, then once per batch of hypotheses.
+int32_t b2s_ransac_feature_matching(b2s_handle* h, const b2s_cloud* src, const b2s_feature* src_f, int32_t n, const b2s_cloud* const* tgts,
+                                    const b2s_feature* const* tgt_fs, const b2s_ransac_params* p, b2s_ransac_result* out) {
+  B2S_REQUIRE(n >= 0, B2S_E_INVALID, "n_targets must be >= 0");
+  B2S_REQUIRE(h && src && src_f && p && (n == 0 || (tgts && tgt_fs && out)), B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(p->confidence > 0.0 && p->confidence < 1.0, B2S_E_INVALID, "RANSACConvergenceCriteria: confidence must be in (0, 1)");
+  B2S_REQUIRE(p->max_iteration >= 0, B2S_E_INVALID, "RANSACConvergenceCriteria: max_iteration must be >= 0");
+  B2S_REQUIRE(p->ransac_n <= B2S_RANSAC_MAX_N, B2S_E_UNSUPPORTED, "ransac_n %d > %d is not supported", p->ransac_n, B2S_RANSAC_MAX_N);
+  B2S_REQUIRE(src->h == h && src_f->h == h, B2S_E_INVALID, "the source belongs to another handle");
+  for (int32_t k = 0; k < n; ++k) {
+    B2S_REQUIRE(tgts[k] && tgt_fs[k], B2S_E_INVALID, "null target %d", k);
+    B2S_REQUIRE(tgts[k]->h == h && tgt_fs[k]->h == h, B2S_E_INVALID, "target %d belongs to another handle", k);
+  }
+  LOCK(h);
+  size_t ns = 0;
+  B2S_TRY(cloud_count_sync(h, src, &ns));
+  B2S_REQUIRE(ns == src_f->n, B2S_E_INVALID, "the source feature has %zu points, its cloud %zu", src_f->n, ns);
+  std::vector<size_t> nts((size_t)n);
+  for (int32_t k = 0; k < n; ++k) {
+    B2S_TRY(cloud_count_sync(h, tgts[k], &nts[k]));
+    B2S_REQUIRE(nts[k] == tgt_fs[k]->n, B2S_E_INVALID, "target %d: the feature has %zu points, its cloud %zu", k, tgt_fs[k]->n, nts[k]);
+  }
+  if (n == 0) return B2S_OK;
+  B2S_TRY(op_ransac(h, src, ns, src_f, n, tgts, nts.data(), tgt_fs, *p, out));
+  return check_status(h);
+}
+
+int32_t b2s_feature_correspondences(b2s_handle* h, const b2s_feature* src_f, const b2s_feature* tgt_f, int32_t* s2t, size_t s_cap, int32_t* t2s,
+                                    size_t t_cap) {
+  B2S_REQUIRE(h && src_f && tgt_f && (s2t || src_f->n == 0) && (t2s || tgt_f->n == 0), B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(src_f->h == h && tgt_f->h == h, B2S_E_INVALID, "the feature belongs to another handle");
+  B2S_REQUIRE(src_f->n <= s_cap && tgt_f->n <= t_cap, B2S_E_CAPACITY, "output arrays hold %zu / %zu entries, the features have %zu / %zu points",
+              s_cap, t_cap, src_f->n, tgt_f->n);
+  LOCK(h);
+  B2S_TRY(h->tmp_i32.ensure((src_f->n + tgt_f->n + 1) * 4, h->stream));
+  int32_t* d_s2t = h->tmp_i32.as<int32_t>();
+  int32_t* d_t2s = d_s2t + src_f->n;
+  B2S_TRY(op_feature_correspondences(h, src_f, 1, &tgt_f, &d_s2t, &d_t2s));
+  if (src_f->n) B2S_CUDA(cudaMemcpyAsync(s2t, d_s2t, src_f->n * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (tgt_f->n) B2S_CUDA(cudaMemcpyAsync(t2s, d_t2s, tgt_f->n * 4, cudaMemcpyDeviceToHost, h->stream));
+  return check_status(h);
+}
+
 }  // extern "C"

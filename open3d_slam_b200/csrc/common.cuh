@@ -274,6 +274,7 @@ struct b2s_handle {
   std::vector<std::unique_ptr<b2s::GridIndex>> batch_grids;
   b2s::DevBuf batch_jobs;             // GridJob + ScanJob tables and the scan tile states of a batched index build
   std::vector<unsigned char> batch_jobs_host;
+  b2s::DevBuf lc;                     // K-ransac scratch (ransac.cu owns its layout)
 };
 
 // every entry point that touches a handle's stream or buffers holds its lock and works on its device
@@ -397,6 +398,12 @@ int32_t op_overlap(b2s_handle* h, const b2s_cloud* source, const b2s_cloud* targ
                    b2s_cloud* source_overlap, b2s_cloud* target_overlap);
 // K-fpfh (features.cu): [O3D] ComputeFPFHFeature of the n points of c (normals required, 1 <= knn <= B2S_FEATURE_MAX_KNN)
 int32_t op_compute_fpfh(b2s_handle* h, const b2s_cloud* c, size_t n, double radius, int knn, b2s_feature* f);
+// K-ransac (ransac.cu): exact feature correspondences of one source feature against n target features (device outputs; s2t[k] / t2s[k]
+// hold the source size / target k's size entries), and RegistrationRANSACBasedOnFeatureMatching of one source against n targets
+int32_t op_feature_correspondences(b2s_handle* h, const b2s_feature* src, int n, const b2s_feature* const* tgts, int32_t* const* s2t,
+                                   int32_t* const* t2s);
+int32_t op_ransac(b2s_handle* h, const b2s_cloud* src, size_t ns, const b2s_feature* src_f, int n, const b2s_cloud* const* tgts, const size_t* nts,
+                  const b2s_feature* const* tgt_fs, const b2s_ransac_params& p, b2s_ransac_result* out);
 // C1 space carving of the sparse map (carve.cu); removed_dev (optional) receives the number of removed points
 int32_t op_submap_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan, const double* T_dev, const CropDev& crop,
                         const b2s_carving_params& prm, int32_t* removed_dev, const int32_t* enable_dev = nullptr);
@@ -510,6 +517,59 @@ __device__ __forceinline__ double warp_max(double v) {
 __device__ __forceinline__ double dist2_exact(double ax, double ay, double az, double bx, double by, double bz) {
   double dx = __dsub_rn(ax, bx), dy = __dsub_rn(ay, by), dz = __dsub_rn(az, bz);
   return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
+// 3x3 SVD by one-sided Jacobi (Hestenes), singular values sorted descending like Eigen's JacobiSVD (the rotation that
+// umeyama builds from it is unique for rank >= 2, so the SVD algorithm itself need not be Eigen's).  One thread, a few
+// hundred flops per registration iteration (icp.cu) or RANSAC hypothesis (ransac.cu).
+static __device__ void svd3_dev(const double* A, double* U, double* S, double* V) {
+  double W[9], Vm[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  for (int i = 0; i < 9; i++) W[i] = A[i];
+  for (int sweep = 0; sweep < 60; sweep++) {
+    bool rotated = false;
+    for (int p = 0; p < 2; p++)
+      for (int q = p + 1; q < 3; q++) {
+        double alpha = 0, beta = 0, gamma = 0;
+        for (int i = 0; i < 3; i++) { alpha += W[3 * i + p] * W[3 * i + p]; beta += W[3 * i + q] * W[3 * i + q]; gamma += W[3 * i + p] * W[3 * i + q]; }
+        if (gamma == 0.0 || fabs(gamma) <= 1e-16 * sqrt(alpha * beta)) continue;
+        rotated = true;
+        const double zeta = (beta - alpha) / (2.0 * gamma);
+        const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+        const double c = 1.0 / sqrt(1.0 + t * t), sn = c * t;
+        for (int i = 0; i < 3; i++) {
+          const double wp = W[3 * i + p], wq = W[3 * i + q];
+          W[3 * i + p] = c * wp - sn * wq; W[3 * i + q] = sn * wp + c * wq;
+          const double vp = Vm[3 * i + p], vq = Vm[3 * i + q];
+          Vm[3 * i + p] = c * vp - sn * vq; Vm[3 * i + q] = sn * vp + c * vq;
+        }
+      }
+    if (!rotated) break;
+  }
+  double sv[3]; int ord[3] = {0, 1, 2};
+  for (int j = 0; j < 3; j++) sv[j] = sqrt(W[j] * W[j] + W[3 + j] * W[3 + j] + W[6 + j] * W[6 + j]);
+  for (int a = 0; a < 2; a++)
+    for (int b = 0; b < 2 - a; b++) if (sv[ord[b]] < sv[ord[b + 1]]) { const int t = ord[b]; ord[b] = ord[b + 1]; ord[b + 1] = t; }
+  const double tiny = 1e-300;
+  for (int j = 0; j < 3; j++) {
+    const int o = ord[j];
+    S[j] = sv[o];
+    for (int i = 0; i < 3; i++) { V[3 * i + j] = Vm[3 * i + o]; U[3 * i + j] = sv[o] > tiny ? W[3 * i + o] / sv[o] : 0.0; }
+  }
+  if (!(S[0] > tiny)) { for (int i = 0; i < 9; i++) U[i] = (i % 4 == 0) ? 1.0 : 0.0; return; }
+  if (!(S[1] > tiny)) {
+    const double u0[3] = {U[0], U[3], U[6]};
+    const int k = fabs(u0[0]) <= fabs(u0[1]) ? (fabs(u0[0]) <= fabs(u0[2]) ? 0 : 2) : (fabs(u0[1]) <= fabs(u0[2]) ? 1 : 2);
+    double e[3] = {0, 0, 0}; e[k] = 1.0;
+    const double d = e[0] * u0[0] + e[1] * u0[1] + e[2] * u0[2];
+    const double v[3] = {e[0] - d * u0[0], e[1] - d * u0[1], e[2] - d * u0[2]};
+    const double nv = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    U[1] = v[0] / nv; U[4] = v[1] / nv; U[7] = v[2] / nv;
+  }
+  if (!(S[2] > tiny)) { U[2] = U[3] * U[7] - U[6] * U[4]; U[5] = U[6] * U[1] - U[0] * U[7]; U[8] = U[0] * U[4] - U[3] * U[1]; }
+}
+
+__device__ __forceinline__ double det3_dev(const double* M) {
+  return M[0] * (M[4] * M[8] - M[5] * M[7]) - M[1] * (M[3] * M[8] - M[5] * M[6]) + M[2] * (M[3] * M[7] - M[4] * M[6]);
 }
 
 // reference croppers (core/src/croppers.cpp:121-165); only the translation of the pose is used

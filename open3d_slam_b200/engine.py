@@ -86,13 +86,28 @@ class CloudRegistrationParameters:
 
 @dataclass
 class PlaceRecognitionParameters:
-    """The fields of include/open3d_slam/Parameters.hpp:118-122 that Submap::computeFeatures reads.  Defaults = the Lua values
-    (parameter_structure_definitions.lua:155-159); the C++ struct's own defaults differ (normalEstimationRadius_ 1.0, normalKnn_ 10)."""
+    """The fields of include/open3d_slam/Parameters.hpp:118-129 that Submap::computeFeatures and the RANSAC proposal of
+    PlaceRecognition::buildLoopClosureConstraints read.  Defaults = the Lua values (parameter_structure_definitions.lua:151-162); the
+    C++ struct's own defaults differ (normalEstimationRadius_ 1.0, normalKnn_ 10, ransacNumIter_ 1e6, ransacProbability_ 0.99,
+    correspondenceCheckerDistance_ 0.75, correspondenceCheckerEdgeLength_ 0.5)."""
     featureVoxelSize: float = 0.5
     normalEstimationRadius: float = 2.0
     normalKnn: int = 20
     featureRadius: float = 2.5
     featureKnn: int = 100
+    ransacNumIter: int = 10_000_000
+    ransacProbability: float = 0.999
+    ransacModelSize: int = 3
+    ransacMaxCorrespondenceDistance: float = 0.75
+    correspondenceCheckerDistance: float = 0.8
+    correspondenceCheckerEdgeLength: float = 0.6
+    ransacMinCorrespondenceSetSize: int = 25
+    ransacSeed: int = 1            # replaces std::random_device of [O3D] RANSAC (DESIGN.md row K-ransac)
+
+    def ransac_c(self, mutual_filter: bool = True) -> L.RansacParams:
+        return L.RansacParams(int(mutual_filter), int(self.ransacModelSize), float(self.ransacMaxCorrespondenceDistance),
+                              float(self.correspondenceCheckerDistance), float(self.correspondenceCheckerEdgeLength), int(self.ransacNumIter),
+                              float(self.ransacProbability), int(self.ransacSeed))
 
     def to_c(self) -> L.FeatureParams:
         return L.FeatureParams(float(self.featureVoxelSize), float(self.normalEstimationRadius), int(self.normalKnn), float(self.featureRadius),
@@ -433,6 +448,54 @@ def computeFPFHFeature(eng: Engine, cloud: Cloud, radius: float, max_nn: int) ->
     f = Feature(eng)
     L.check(L.lib().b2s_compute_fpfh(eng._h, cloud._c, C.c_double(radius), C.c_int32(max_nn), f._f))
     return f
+
+
+@dataclass
+class RansacResult(RegistrationResult):
+    """RegistrationResult of RegistrationRANSACBasedOnFeatureMatching (n_corr = correspondence_set_.size() = inliers) plus how the
+    run went: the h the loop stopped at, the validated hypotheses, the size of the feature correspondence set and whether it is the
+    mutual one, and the h of the hypothesis the result comes from (-1 = none)."""
+    hypotheses: int = 0
+    validations: int = 0
+    best_hypothesis: int = -1
+    n_feature_corr: int = 0
+    used_mutual: bool = False
+
+
+def _ransac_res(r: L.RansacResult) -> RansacResult:
+    b = _res(r.result)
+    return RansacResult(b.transformation_, b.fitness_, b.inlier_rmse_, b.n_corr, b.iters, int(r.hypotheses), int(r.validations),
+                        int(r.best_hypothesis), int(r.n_feature_corr), bool(r.used_mutual))
+
+
+def registrationRANSACBasedOnFeatureMatchingBatch(eng: Engine, source: Cloud, targets, sourceFeature: Feature, targetFeatures,
+                                                  params: PlaceRecognitionParameters | None = None, mutual_filter: bool = True):
+    """[O3D] RegistrationRANSACBasedOnFeatureMatching of one source sparse cloud against every candidate, as
+    src/PlaceRecognition.cpp:71-84 loops over them, in one device call.  Returns one RansacResult per target."""
+    p = (params or PlaceRecognitionParameters()).ransac_c(mutual_filter)
+    n = len(targets)
+    assert len(targetFeatures) == n
+    tc = (C.c_void_p * max(n, 1))(*[t._c for t in targets])
+    tf = (C.c_void_p * max(n, 1))(*[f._f for f in targetFeatures])
+    out = (L.RansacResult * max(n, 1))()
+    L.check(L.lib().b2s_ransac_feature_matching(eng._h, source._c, sourceFeature._f, C.c_int32(n), tc, tf, C.byref(p), out))
+    return [_ransac_res(out[k]) for k in range(n)]
+
+
+def registrationRANSACBasedOnFeatureMatching(eng: Engine, source: Cloud, target: Cloud, sourceFeature: Feature, targetFeature: Feature,
+                                             params: PlaceRecognitionParameters | None = None, mutual_filter: bool = True) -> RansacResult:
+    """src/PlaceRecognition.cpp:81-84 for one candidate (mutual_filter = true there)."""
+    return registrationRANSACBasedOnFeatureMatchingBatch(eng, source, [target], sourceFeature, [targetFeature], params, mutual_filter)[0]
+
+
+def featureCorrespondences(eng: Engine, sourceFeature: Feature, targetFeature: Feature):
+    """The exact nearest-feature indices both ways (src_to_tgt, tgt_to_src) that the RANSAC correspondence set is built from;
+    -1 where the other feature is empty."""
+    ns, nt = sourceFeature.Num(), targetFeature.Num()
+    s2t = np.full(max(ns, 1), -1, dtype=np.int32); t2s = np.full(max(nt, 1), -1, dtype=np.int32)
+    L.check(L.lib().b2s_feature_correspondences(eng._h, sourceFeature._f, targetFeature._f, s2t.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                C.c_size_t(len(s2t)), t2s.ctypes.data_as(C.POINTER(C.c_int32)), C.c_size_t(len(t2s))))
+    return s2t[:ns], t2s[:nt]
 
 
 class CloudRegistration:

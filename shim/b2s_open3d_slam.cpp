@@ -395,4 +395,28 @@ void ScanToMapIcpB200::prepareInitialMap(PointCloud* map) const {
   map->normals_ = d.download()->normals_;
 }
 
+RansacResultB200 registrationRansacBasedOnFeatureMatchingB200(const SubmapB200& source, const SubmapB200& target,
+                                                              const PlaceRecognitionParameters& cfg, uint64_t seed) {
+  if (!source.feature() || !target.feature()) throw std::runtime_error("Feature ptr is nullptr");   // Submap.cpp:250
+  b2s_ransac_params rp;
+  b2s_default_ransac_params(&rp);
+  rp.mutual_filter = 1;                                                   // PlaceRecognition.cpp:82
+  rp.ransac_n = cfg.ransacModelSize_;
+  rp.max_correspondence_distance = cfg.ransacMaxCorrespondenceDistance_;
+  rp.checker_distance = cfg.correspondenceCheckerDistance_;               // :56-57
+  rp.checker_edge_length = cfg.correspondenceCheckerEdgeLength_;
+  rp.max_iteration = cfg.ransacNumIter_;
+  rp.confidence = cfg.ransacProbability_;
+  rp.seed = seed;
+  const b2s_cloud* tc = target.sparseCloud();
+  const b2s_feature* tf = target.feature();
+  b2s_ransac_result r;
+  const int32_t rc = b2s_ransac_feature_matching(source.engine(), source.sparseCloud(), source.feature(), 1, &tc, &tf, &rp, &r);
+  if (rc != B2S_OK) b2sThrow(rc);
+  RansacResultB200 out;
+  out.result = toResult(r.result);
+  out.numCorrespondences = (size_t)r.result.n_corr;
+  return out;
+}
+
 }  // namespace o3d_slam

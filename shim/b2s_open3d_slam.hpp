@@ -93,6 +93,8 @@ class SubmapB200 {
   const Feature& getFeatures() const;                       // throws before the first computeFeatures, like the reference
   b2s_submap* handle() const { return sm_; }
   b2s_handle* engine() const { return h_; }
+  b2s_cloud* sparseCloud() const { return sparse_; }        // device-resident sparse cloud / feature (null before computeFeatures)
+  b2s_feature* feature() const { return feature_; }
 
  private:
   b2s_config cfg_;
@@ -110,6 +112,19 @@ class SubmapB200 {
   mutable Feature featureCache_;
   mutable bool sparseValid_ = false, featureValid_ = false;
 };
+
+// PlaceRecognition::buildLoopClosureConstraints, src/PlaceRecognition.cpp:81-84: RegistrationRANSACBasedOnFeatureMatching(
+// sourceSparse, targetSparse, sourceFeature, targetFeature, true, cfg.ransacMaxCorrespondenceDistance_, PointToPoint(false),
+// cfg.ransacModelSize_, {distance, edge length checkers}, RANSACConvergenceCriteria(cfg.ransacNumIter_, cfg.ransacProbability_))
+// on the device, reading both SubmapB200s' device-resident sparse cloud and feature (computeFeatures must have run on both, on
+// the source's handle).  The proposal is deterministic for a given seed (DESIGN.md row K-ransac).  The device keeps the inlier
+// count, not the pairs: the gate at :86 reads numCorrespondences instead of correspondence_set_.size().
+struct RansacResultB200 {
+  RegistrationResult result;
+  size_t numCorrespondences = 0;
+};
+RansacResultB200 registrationRansacBasedOnFeatureMatchingB200(const SubmapB200& source, const SubmapB200& target,
+                                                              const PlaceRecognitionParameters& cfg, uint64_t seed = 1);
 
 class ScanToMapIcpB200 : public ScanToMapRegistration {
  public:

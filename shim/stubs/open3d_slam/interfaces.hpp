@@ -23,7 +23,9 @@ struct SpaceCarvingParameters { double voxelSize_ = 0.1, maxRaytracingLength_ = 
 struct MapBuilderParameters { double mapVoxelSize_ = 0.03; ScanCroppingParameters cropper_; SpaceCarvingParameters carving_; };
 enum class ScanToMapRegistrationType : int { PointToPlaneIcp, PointToPointIcp, GeneralizedIcp };   // Parameters.hpp:44-49
 struct ScanToMapRegistrationParameters { double minRefinementFitness_ = 0.7; IcpParameters icp_; ScanToMapRegistrationType scanToMapRegType_ = ScanToMapRegistrationType::PointToPlaneIcp; };
-struct PlaceRecognitionParameters { double normalEstimationRadius_ = 1.0, featureVoxelSize_ = 0.5, featureRadius_ = 2.5; int featureKnn_ = 100, normalKnn_ = 10; };   // Parameters.hpp:118-122
+struct PlaceRecognitionParameters { double normalEstimationRadius_ = 1.0, featureVoxelSize_ = 0.5, featureRadius_ = 2.5; int featureKnn_ = 100, normalKnn_ = 10;
+  int ransacNumIter_ = 1000000; double ransacProbability_ = 0.99; int ransacModelSize_ = 3; double ransacMaxCorrespondenceDistance_ = 0.75,
+  correspondenceCheckerDistance_ = 0.75, correspondenceCheckerEdgeLength_ = 0.5; int ransacMinCorrespondenceSetSize_ = 25; };   // Parameters.hpp:118-129
 struct MapperParameters { ScanToMapRegistrationParameters scanMatcher_; ScanProcessingParameters scanProcessing_; MapBuilderParameters mapBuilder_; MapBuilderParameters denseMapBuilder_; };
 class Submap;  // the shim only needs getMapPointCloud(); see b2s_open3d_slam.cpp
 class CloudRegistration {
