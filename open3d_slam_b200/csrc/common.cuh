@@ -187,6 +187,8 @@ struct b2s_submap {
   b2s::DevBuf stage_xyz, stage_nrm, stage_next, stage_in;   // the transformed scan of the insertion in flight
   b2s::DevBuf touched;       // int32 voxels (table slots) the insertion in flight touched
   b2s::DevBuf dups;          // int32 [2][FUSE_DUP_CAP] voxels holding more than one map point (ping-pong)
+  b2s::DevBuf wflag;         // int32 [capacity + 1] 1 = the slot is on K3's renormalisation worklist
+  b2s::DevBuf wlist;         // int32 [2][capacity + 1] the worklist (ping-pong): slots whose normal may not be a fixed point yet
   size_t vcap = 0;
   size_t stage_cap = 0;
   // Mapper / SubmapCollection wiring of the device chain (b2s_mapper_options) and its device-side state words (MS_*)
@@ -224,6 +226,8 @@ enum MapperStateWord {
   MS_NDUP = 20,       // [20], [21]: entries of the two halves
   MS_VUSED = 22,      // occupied slots of the voxel table
   MS_TICKET2 = 23,
+  MS_WSEL = 24,       // which half of `wlist` is current
+  MS_NW = 25,         // [25], [26]: entries of the two halves
   MS_WORDS = 32
 };
 // bumped by every DevBuf re-allocation: a captured graph holds raw pointers of the scratch buffers, so a graph captured
