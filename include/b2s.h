@@ -121,6 +121,9 @@ const char* b2s_version(void);
 int32_t b2s_device_count(void);
 /* number of kernels launched by this handle since creation ("gpu_launches" evidence for bench.py) */
 int64_t b2s_launch_count(const b2s_handle* h);
+/* number of CUDA graphs the per-scan chains of this handle captured since creation (b2s_mapper_graph_enable, b2s_slam_graph_enable):
+ * in steady state a replay adds launches but no capture */
+int64_t b2s_graph_capture_count(const b2s_handle* h);
 
 /* per-kernel-group device time, CUDA events on the handle's stream (the reference prints per-stage wall times with
  * o3d_slam::Timer, src/time.cpp:35-78).  kinds: 0 icp, 1 normals, 2 radix sort, 3 NN-grid build, 4 voxel keys+means,
@@ -312,6 +315,87 @@ typedef struct b2s_mapper_counters {
   int64_t carved_voxels_total;   /* dense voxels emptied */
 } b2s_mapper_counters;
 int32_t b2s_submap_get_mapper_counters(b2s_handle* h, const b2s_submap* sm, b2s_mapper_counters* out);
+
+/* ---- device-resident LidarOdometry (src/Odometry.cpp:19-110) and the combined per-scan step of SlamWrapper: odometry, then
+ *      Mapper::addRangeMeasurement with the prediction read from the odometry's TransformInterpolationBuffer on the device.
+ *      Every decision (initialise / ok / failed, the buffer, the prediction, the mapper gates) is taken on the device.
+ *      Timestamps are UniversalTimeScaleClock ticks (100 ns, include/open3d_slam/time.hpp:43-55).  They are host values, so the
+ *      order check stays on the host: a step whose t is not greater than the previous step's t on that odometry object returns
+ *      B2S_E_INVALID.  (Deliberate difference: the reference prints a warning and returns false, Odometry.cpp:41-44, Mapper.cpp:117-120.)
+ *      An odometry object belongs to the handle that created it: passing it with another handle -> B2S_E_INVALID. */
+/* OdometryParameters (Parameters.hpp:78-83): scanMatcher_ + scanProcessing_, plus the two constants the reference hard-codes */
+typedef struct b2s_odometry_params {
+  b2s_icp_params icp;            /* scanMatcher_ (reg_type, max_iter, max_corr_dist, knn, knn_radius, rel_*) */
+  double voxel_size;             /* scanProcessing_.voxelSize_ */
+  double downsampling_ratio;     /* scanProcessing_.downSamplingRatio_ */
+  uint32_t seed;                 /* replaces std::random_device in [O3D] RandomDownSample */
+  b2s_cropper cropper;           /* scanProcessing_.cropper_, applied in the sensor frame (Odometry.cpp:21,26) */
+  double min_fitness;            /* the "todo magic" 0.1 of Odometry.cpp:51: the registration succeeds iff fitness > min_fitness */
+  int32_t buffer_size;           /* size limit of odomToRangeSensorBuffer_: TransformInterpolationBuffer() = 2000; fixed at creation */
+} b2s_odometry_params;
+/* the Lua odometry block: the same scan-processing / ICP values as b2s_default_config, min_fitness 0.1, buffer_size 2000 */
+void b2s_default_odometry_params(b2s_odometry_params* p);
+enum { B2S_ODOM_INIT = 0, B2S_ODOM_OK = 1, B2S_ODOM_FAILED = 2, B2S_ODOM_FAILED_KEPT_PREV = 3 };
+typedef struct b2s_odometry b2s_odometry;
+/* capacity_points: the largest raw scan a step accepts (B2S_E_CAPACITY above it) */
+int32_t b2s_odometry_create(b2s_handle* h, const b2s_odometry_params* p, size_t capacity_points, b2s_odometry** out);
+void b2s_odometry_destroy(b2s_odometry* od);
+/* LidarOdometry::setParameters (Odometry.cpp:96-100); buffer_size must stay what the object was created with */
+int32_t b2s_odometry_set_params(b2s_handle* h, b2s_odometry* od, const b2s_odometry_params* p);
+/* LidarOdometry::setInitialTransform (Odometry.cpp:102-110): the cumulative pose becomes T now, and again (instead of the
+ * composition) at the next successful registration */
+int32_t b2s_odometry_set_initial_transform(b2s_handle* h, b2s_odometry* od, const double T[16]);
+/* LidarOdometry::addRangeScan(raw, t) (Odometry.cpp:32-79), enqueue only:
+ *   pre = RandomDownSample(normals(voxelize(crop(raw))))                        :25-30 (one crop, sensor frame)
+ *   cloudPrev_ empty          -> cloudPrev_ = pre, push (t, cumulative)         :33-39  outcome INIT
+ *   registerClouds(cloudPrev_, pre, I) with the object's own icp parameters    :48
+ *   fitness > min_fitness     -> cumulative = pending initial transform or cumulative * T^-1, cloudPrev_ = pre, push   outcome OK
+ *   otherwise                 -> cloudPrev_ = pre when pre is not empty, no push          outcome FAILED / FAILED_KEPT_PREV
+ * slot 0..255: where b2s_odometry_result_fetch finds the result.  The host may run at most 32 steps ahead of the device. */
+int32_t b2s_odometry_step_async(b2s_handle* h, b2s_odometry* od, const b2s_cloud* raw, int64_t t, int32_t slot);
+typedef struct b2s_odometry_result {
+  b2s_result registration;           /* registerClouds(cloudPrev_, pre, I); zeros on an initialising step */
+  double odom_to_range_sensor[16];   /* odomToRangeSensorCumulative_ after the step */
+  int32_t outcome;                   /* B2S_ODOM_* */
+  int32_t n_preprocessed;            /* points of pre */
+} b2s_odometry_result;
+int32_t b2s_odometry_result_fetch(b2s_handle* h, b2s_odometry* od, int32_t slot, b2s_odometry_result* out);   /* synchronises */
+/* getTransform(t, odomToRangeSensorBuffer_) and buffer.has(t) (TransformInterpolationBuffer.cpp:76-157, Transform.cpp:16-41):
+ * clamped to the earliest / latest entry, exact on an equal timestamp, else translation interpolated linearly and rotation by
+ * Eigen's slerp between the neighbours, factor = dt(t, start) / (dt(end, start) + 1e-6 s).  An empty buffer: has = 0, T = I.
+ * Synchronises. */
+int32_t b2s_odometry_lookup(b2s_handle* h, const b2s_odometry* od, int64_t t, double T[16], int32_t* has);
+/* LidarOdometry::getPreProcessedCloud (Odometry.cpp:84-86) = cloudPrev_, copied into out */
+int32_t b2s_odometry_preprocessed(b2s_handle* h, const b2s_odometry* od, b2s_cloud* out);
+
+/* One scan through SlamWrapper's two workers (odometryWorker + mappingWorker): b2s_odometry_step_async(raw, t), then
+ * Mapper::addRangeMeasurement(raw, t) on the submap (the steady-state branch of b2s_mapper_step_async) with
+ *   odom_used = buffer.has(t);  guess = pose * getTransform(t_last)^-1 * getTransform(t) if odom_used, else pose   Mapper.cpp:122-137
+ * t_last = lastMeasurementTimestamp_ of that mapper: Time() = 0 at first, set to t by every scan the fitness gate accepts (:164,178).
+ * It lives on the device with the odometry object (one robot's stream of scans), so a submap hand-over keeps it, as the
+ * reference's Mapper member does.  The submap must not be empty: the caller inserts the first scan (Mapper.cpp:105-114) and
+ * runs b2s_odometry_step_async on that scan and timestamp.  The mapper options, gates, carving, F1 and dense map follow
+ * unchanged; b2s_mapper_processed_scan returns this step's merge_ / match_. */
+typedef struct b2s_slam_result {
+  b2s_odometry_result odometry;
+  b2s_result mapper;
+  int32_t odom_used;                 /* the buffer had t (the prediction came from the odometry) */
+  int32_t mapper_accepted;           /* addRangeMeasurement returned true */
+} b2s_slam_result;
+int32_t b2s_slam_step_async(b2s_handle* h, b2s_submap* sm, b2s_odometry* od, const b2s_cloud* raw, int64_t t, double min_refinement_fitness,
+                            int32_t ignore_min_fitness, int32_t slot);
+int32_t b2s_slam_result_fetch(b2s_handle* h, b2s_odometry* od, int32_t slot, b2s_slam_result* out);   /* synchronises */
+/* the same with a float32 host scan (pinned memory keeps the copy asynchronous): upload, both chains and the copy of the result
+ * into *out_pinned (page-locked host memory, valid after the next b2s_synchronize) are only enqueued */
+int32_t b2s_slam_step_host_async(b2s_handle* h, b2s_submap* sm, b2s_odometry* od, const void* xyz_f32, size_t n, size_t stride_bytes, int64_t t,
+                                 double min_refinement_fitness, int32_t ignore_min_fitness, b2s_slam_result* out_pinned);
+/* CUDA-graph replay of b2s_slam_step_async: after two eager steps per submap the launches of one scan (odometry + mapper) are
+ * captured once and replayed with one cudaGraphLaunch.  The graphs are kept per submap on the odometry object, so a hand-over
+ * back to a submap seen before replays without a new capture (the graphs of destroyed submaps are released when the object next
+ * meets a submap it has no graph for); b2s_odometry_set_params, b2s_set_config and
+ * b2s_submap_set_mapper_options on that submap invalidate them.  Every scan must be uploaded or copied into the returned
+ * fixed-capacity staging cloud (one input stream per odometry object), which is then passed as raw. */
+int32_t b2s_slam_graph_enable(b2s_handle* h, b2s_odometry* od, size_t raw_capacity_points, b2s_cloud** staging_out);
 
 /* ---- F4  o3d_slam::VoxelMap (include/open3d_slam/Voxel.hpp:19-36, src/Voxel.cpp:123-160): voxel -> per-layer lists of point indices.
  *      Keys are getVoxelIdx(p, 1 / voxelSize) = floor(p * inv) per axis (VoxelHashMap.hpp:43-50).  Layers are integers

@@ -69,6 +69,22 @@ class RansacResult(C.Structure):
                 ("used_mutual", C.c_int32)]
 
 
+class OdometryParams(C.Structure):
+    _fields_ = [("icp", IcpParams), ("voxel_size", C.c_double), ("downsampling_ratio", C.c_double), ("seed", C.c_uint32), ("cropper", Cropper),
+                ("min_fitness", C.c_double), ("buffer_size", C.c_int32)]
+
+
+class OdometryResult(C.Structure):
+    _fields_ = [("registration", Result), ("odom_to_range_sensor", C.c_double * 16), ("outcome", C.c_int32), ("n_preprocessed", C.c_int32)]
+
+
+class SlamResult(C.Structure):
+    _fields_ = [("odometry", OdometryResult), ("mapper", Result), ("odom_used", C.c_int32), ("mapper_accepted", C.c_int32)]
+
+
+ODOM_INIT, ODOM_OK, ODOM_FAILED, ODOM_FAILED_KEPT_PREV = 0, 1, 2, 3
+
+
 class MapperCounters(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("steps", "accepted", "inserted_map", "inserted_dense", "carve_runs", "carved_points_total",
                                          "dense_carve_runs", "carved_voxels_total")]
@@ -77,7 +93,7 @@ class MapperCounters(C.Structure):
 # every symbol include/b2s.h declares (checked by tests/test_abi.py without needing a GPU)
 SYMBOLS = [
     "b2s_default_config", "b2s_create", "b2s_destroy", "b2s_set_config", "b2s_synchronize", "b2s_last_error", "b2s_version",
-    "b2s_device_count", "b2s_launch_count", "b2s_cloud_create", "b2s_cloud_destroy", "b2s_cloud_upload_f64", "b2s_cloud_upload_f32",
+    "b2s_device_count", "b2s_launch_count", "b2s_graph_capture_count", "b2s_cloud_create", "b2s_cloud_destroy", "b2s_cloud_upload_f64", "b2s_cloud_upload_f32",
     "b2s_cloud_size", "b2s_cloud_download", "b2s_cloud_copy", "b2s_crop", "b2s_voxel_down_sample", "b2s_estimate_normals",
     "b2s_random_down_sample", "b2s_transform", "b2s_process_scan", "b2s_register", "b2s_register_batch", "b2s_register_host",
     "b2s_submap_create", "b2s_submap_destroy", "b2s_submap_insert", "b2s_submap_insert_dense", "b2s_submap_size", "b2s_submap_download",
@@ -92,6 +108,9 @@ SYMBOLS = [
     "b2s_feature_create", "b2s_feature_destroy", "b2s_feature_size", "b2s_feature_download", "b2s_feature_upload", "b2s_compute_fpfh",
     "b2s_default_feature_params", "b2s_submap_compute_features",
     "b2s_default_ransac_params", "b2s_ransac_feature_matching", "b2s_feature_correspondences",
+    "b2s_default_odometry_params", "b2s_odometry_create", "b2s_odometry_destroy", "b2s_odometry_set_params", "b2s_odometry_set_initial_transform",
+    "b2s_odometry_step_async", "b2s_odometry_result_fetch", "b2s_odometry_lookup", "b2s_odometry_preprocessed",
+    "b2s_slam_step_async", "b2s_slam_result_fetch", "b2s_slam_step_host_async", "b2s_slam_graph_enable",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 PROFILE_KINDS = ["icp", "normals", "radix_sort", "nn_grid_build", "voxel", "fuse", "select", "crop"]
@@ -118,6 +137,8 @@ def lib():
         L.b2s_version.restype = C.c_char_p
         L.b2s_launch_count.restype = C.c_int64
         L.b2s_launch_count.argtypes = [C.c_void_p]
+        L.b2s_graph_capture_count.restype = C.c_int64
+        L.b2s_graph_capture_count.argtypes = [C.c_void_p]
         L.b2s_destroy.restype = None
         L.b2s_cloud_destroy.restype = None
         L.b2s_submap_destroy.restype = None
@@ -132,6 +153,9 @@ def lib():
         L.b2s_voxel_map_destroy.argtypes = [C.c_void_p]
         L.b2s_feature_destroy.restype = None
         L.b2s_feature_destroy.argtypes = [C.c_void_p]
+        L.b2s_odometry_destroy.restype = None
+        L.b2s_odometry_destroy.argtypes = [C.c_void_p]
+        L.b2s_default_odometry_params.restype = None
         _lib = L
     return _lib
 

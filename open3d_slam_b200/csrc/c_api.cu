@@ -7,11 +7,6 @@
 
 using namespace b2s;
 
-extern "C" {
-static int32_t register_to_submap_async(b2s_handle* h, const b2s_cloud* scan, const b2s_submap* sm, const double* sensor_pose_host,
-                                        const double* sensor_pose_dev, const double* init_host, const double* init_dev, b2s_result* out_dev);
-}
-
 namespace b2s {
 int32_t pose_to_device(b2s_handle* h, const double* T, double* dst);
 int32_t dense_init(b2s_handle* h, b2s_submap* sm, size_t cap, double voxel);
@@ -86,12 +81,12 @@ __global__ void mapper_post_kernel(int32_t* ms) {
   if (threadIdx.x == 0 && ms[MS_DENSE]) ms[MS_NDENSE] += 1;
 }
 
-static double nn_cell(const b2s_handle* h, double max_corr) {
+double nn_cell(const b2s_handle* h, double max_corr) {
   if (h->cfg.nn_cell_size > 0.0) return h->cfg.nn_cell_size;
   return max_corr * 0.25;   // box queries want cells of a few map voxels; the header kernel coarsens them if the box is huge
 }
 
-static int32_t check_icp_params(const b2s_icp_params& p) {
+int32_t check_icp_params(const b2s_icp_params& p) {
   B2S_REQUIRE(p.reg_type == B2S_REG_POINT_TO_PLANE || p.reg_type == B2S_REG_POINT_TO_POINT || p.reg_type == B2S_REG_GENERALIZED,
               B2S_E_UNSUPPORTED, "unknown registration type %d", (int)p.reg_type);
   B2S_REQUIRE(p.max_corr_dist > 0.0, B2S_E_INVALID, "[RegistrationICP] Invalid max_correspondence_distance.");
@@ -100,10 +95,10 @@ static int32_t check_icp_params(const b2s_icp_params& p) {
 }
 
 // global working copy of a source of n points (positions + per-point search state); only touched by sources too large for shared memory
-static inline size_t icp_work_bytes(size_t n) { return (n + 1) * 24 + (n + 1) * 4 + 16; }
+size_t icp_work_bytes(size_t n) { return (n + 1) * 24 + (n + 1) * 4 + 16; }
 
-static void fill_problem(b2s_handle* h, IcpProblem* P, const b2s_cloud* src, const GridIndex* g, const b2s_cloud* tgt, const double* init_host,
-                         const double* init_dev, double* work, b2s_result* out_dev) {
+void fill_problem(IcpProblem* P, const b2s_icp_params& icp, const b2s_cloud* src, const GridIndex* g, const b2s_cloud* tgt, const double* init_host,
+                  const double* init_dev, double* work, b2s_result* out_dev) {
   memset(P, 0, sizeof(*P));
   P->src_xyz = src->xyz.as<double>();
   P->src_n = src->dn.as<int32_t>();
@@ -115,40 +110,45 @@ static void fill_problem(b2s_handle* h, IcpProblem* P, const b2s_cloud* src, con
   P->work_prev = reinterpret_cast<int32_t*>(work + 3 * (src->n_max + 1));   // callers size the work buffer with icp_work_bytes()
   P->init_dev = init_dev;
   if (init_host) memcpy(P->init, init_host, 128);
-  P->max_corr = h->cfg.icp.max_corr_dist;
-  P->rel_fitness = h->cfg.icp.rel_fitness;
-  P->rel_rmse = h->cfg.icp.rel_rmse;
-  P->max_iter = h->cfg.icp.max_iter;
+  P->max_corr = icp.max_corr_dist;
+  P->rel_fitness = icp.rel_fitness;
+  P->rel_rmse = icp.rel_rmse;
+  P->max_iter = icp.max_iter;
   P->src_n_max = (int32_t)src->n_max;
-  P->estimator = h->cfg.icp.reg_type;
+  P->estimator = icp.reg_type;
   P->src_nrm = src->has_normals ? src->nrm.as<double>() : nullptr;
   P->gicp_eps = 1e-3;   // TransformationEstimationForGeneralizedICP() default, the object the reference holds (CloudRegistration.hpp)
   P->out = out_dev;
 }
 
-static int32_t process_scan_impl(b2s_handle* h, const b2s_cloud* raw, b2s_cloud* merge, b2s_cloud* match) {
-  const b2s_scan_params& sp = h->cfg.scan;
-  b2s_cropper c0 = sp.map_builder_cropper;
-  c0.center[0] = c0.center[1] = c0.center[2] = 0.0;   // ScanToMapIcp's own cropper never gets a pose: sensor frame
+int32_t preprocess_scan(b2s_handle* h, const b2s_cloud* raw, const b2s_cropper& cropper, double voxel_size, double ratio, uint32_t seed,
+                        const b2s_icp_params& icp, b2s_cloud* t0, b2s_cloud* out) {
+  b2s_cropper c0 = cropper;
+  c0.center[0] = c0.center[1] = c0.center[2] = 0.0;   // ScanToMapIcp's and LidarOdometry's own croppers never get a pose: sensor frame
   CropDev wide = make_crop(&c0);
   const bool has_crop = c0.kind != B2S_CROP_NONE || c0.invert;
-  b2s_cloud* t0 = h->t0.get();
-  if (sp.voxel_size > 0.0) B2S_TRY(op_voxel_down_sample(h, raw, has_crop ? &wide : nullptr, sp.voxel_size, t0));
+  if (voxel_size > 0.0) B2S_TRY(op_voxel_down_sample(h, raw, has_crop ? &wide : nullptr, voxel_size, t0));
   else if (has_crop) B2S_TRY(op_crop(h, raw, wide, t0));
   else B2S_TRY(op_voxel_down_sample(h, raw, nullptr, 0.0, t0));
   static const double cell_factor = getenv("B2S_NORMALS_CELL_FACTOR") ? atof(getenv("B2S_NORMALS_CELL_FACTOR")) : 4.0;   // tuning knob: index cell = factor x voxel
-  const double cell_hint = sp.voxel_size > 0.0 ? cell_factor * sp.voxel_size : 0.0;
-  if (sp.downsampling_ratio < 1.0) {
+  const double cell_hint = voxel_size > 0.0 ? cell_factor * voxel_size : 0.0;
+  if (ratio < 1.0) {
     // reference order: normals for every voxel point, then RandomDownSample.  The selection only depends on the point
     // positions, so select first and estimate normals for the survivors only (neighbours still from the full cloud).
-    B2S_REQUIRE(sp.downsampling_ratio >= 0.0, B2S_E_INVALID, "[RandomDownSample] sampling_ratio must be in [0, 1]");
-    B2S_TRY(select_flags(h, t0, sp.downsampling_ratio, sp.seed));
-    B2S_TRY(op_estimate_normals(h, t0, h->cfg.icp.knn, h->cfg.icp.knn_radius, cell_hint, h->flags.as<int32_t>()));
-    B2S_TRY(select_compact(h, t0, sp.downsampling_ratio, merge));
+    B2S_REQUIRE(ratio >= 0.0, B2S_E_INVALID, "[RandomDownSample] sampling_ratio must be in [0, 1]");
+    B2S_TRY(select_flags(h, t0, ratio, seed));
+    B2S_TRY(op_estimate_normals(h, t0, icp.knn, icp.knn_radius, cell_hint, h->flags.as<int32_t>()));
+    B2S_TRY(select_compact(h, t0, ratio, out));
   } else {
-    B2S_TRY(op_estimate_normals(h, t0, h->cfg.icp.knn, h->cfg.icp.knn_radius, cell_hint));
-    B2S_TRY(op_random_down_sample(h, t0, sp.downsampling_ratio, sp.seed, merge));
+    B2S_TRY(op_estimate_normals(h, t0, icp.knn, icp.knn_radius, cell_hint));
+    B2S_TRY(op_random_down_sample(h, t0, ratio, seed, out));
   }
+  return B2S_OK;
+}
+
+int32_t process_scan_impl(b2s_handle* h, const b2s_cloud* raw, b2s_cloud* merge, b2s_cloud* match) {
+  const b2s_scan_params& sp = h->cfg.scan;
+  B2S_TRY(preprocess_scan(h, raw, sp.map_builder_cropper, sp.voxel_size, sp.downsampling_ratio, sp.seed, h->cfg.icp, h->t0.get(), merge));
   b2s_cropper c1 = sp.scan_matcher_cropper;
   c1.center[0] = c1.center[1] = c1.center[2] = 0.0;   // ScanToMapRegistration.cpp:47 setPose(Identity)
   B2S_TRY(op_crop(h, merge, make_crop(&c1), match));
@@ -171,8 +171,8 @@ __global__ void graph_begin_kernel(const double* __restrict__ ring, int32_t* gst
 }
 
 // what follows the registration in every variant of the chain: gates, [carving], F1, [dense map]
-static int32_t mapper_chain_tail(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan, const b2s_cloud* merge, const b2s_result* res,
-                                 double min_fitness, int ignore_fitness, b2s_result* slots, const int32_t* gstate) {
+int32_t mapper_chain_tail(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan, const b2s_cloud* merge, const b2s_result* res,
+                          double min_fitness, int ignore_fitness, b2s_result* slots, const int32_t* gstate) {
   const b2s_mapper_options& o = sm->opts;
   double* pose_state = sm->pose.as<double>();
   int32_t* ms = sm->mstate.as<int32_t>();
@@ -202,7 +202,9 @@ static int32_t mapper_chain_tail(b2s_handle* h, b2s_submap* sm, const b2s_cloud*
   return B2S_OK;
 }
 
-static int32_t mapper_chain_graphable(b2s_handle* h, b2s_submap* sm) {
+static int32_t mapper_chain_graphable(void* ctx) {
+  b2s_submap* sm = static_cast<b2s_submap*>(ctx);
+  b2s_handle* h = sm->h;
   double* pose_state = sm->pose.as<double>();
   double* odom = pose_state + 32;
   double* guess = pose_state + 48;
@@ -215,18 +217,69 @@ static int32_t mapper_chain_graphable(b2s_handle* h, b2s_submap* sm) {
   B2S_TRY(process_scan_impl(h, sm->staging.get(), h->t1.get(), h->t2.get()));
   launch_pdl(compose_kernel, 1, 32, 0, h->stream, pose_state, odom, guess);
   h->launches++;
-  B2S_TRY(::register_to_submap_async(h, h->t2.get(), sm, nullptr, pose_state, nullptr, guess, res));
+  B2S_TRY(register_to_submap_async(h, h->t2.get(), sm, nullptr, pose_state, nullptr, guess, res));
   return mapper_chain_tail(h, sm, sm->staging.get(), h->t1.get(), res, sm->g_min_fitness, sm->g_ignore_fitness, h->slots.as<b2s_result>(), gstate);
 }
 
-// A captured chain bakes in buffer addresses, the configuration and the mapper options: once one of them changes it is
-// destroyed, the next step runs eagerly and the one after re-captures.
-static int32_t drop_graph(b2s_handle* h, b2s_submap* sm) {
-  if (!sm->gexec) return B2S_OK;
+static std::mutex g_live_mu;
+static std::unordered_set<unsigned long long> g_live_submaps;
+void submap_register(unsigned long long uid) { std::lock_guard<std::mutex> lk(g_live_mu); g_live_submaps.insert(uid); }
+void submap_forget(unsigned long long uid) { std::lock_guard<std::mutex> lk(g_live_mu); g_live_submaps.erase(uid); }
+bool submap_alive(unsigned long long uid) { std::lock_guard<std::mutex> lk(g_live_mu); return g_live_submaps.count(uid) != 0; }
+
+int32_t graph_drop(b2s_handle* h, GraphCache* g) {
+  if (!g->exec) return B2S_OK;
   B2S_CUDA(cudaStreamSynchronize(h->stream));
-  cudaGraphExecDestroy(sm->gexec);
-  sm->gexec = nullptr;
-  sm->graph_warm = 1;
+  cudaGraphExecDestroy(g->exec);
+  g->exec = nullptr;
+  g->warm = 1;
+  return B2S_OK;
+}
+
+int32_t graph_step(b2s_handle* h, GraphCache* g, unsigned long long key, int32_t (*chain)(void*), void* ctx) {
+  // a device buffer was re-allocated since the capture (any call that grows a scratch buffer): the graph holds the old
+  // address -- or b2s_set_config / the owner's options changed what the captured launches were built from.  This step runs
+  // eagerly (which also re-sizes the scratch).
+  if (g->alloc_gen != __atomic_load_n(&g_alloc_generation, __ATOMIC_RELAXED) || g->cfg_gen != h->cfg_gen || g->key != key) B2S_TRY(graph_drop(h, g));
+  if (g->exec) {
+    B2S_CUDA(cudaGraphLaunch(g->exec, h->stream));
+    h->launches += g->kernels;
+    return B2S_OK;
+  }
+  if (g->warm > 0) {   // eager steps size every scratch buffer (no allocation may happen during capture)
+    g->warm--;
+    return chain(ctx);
+  }
+  // capture this step's chain, instantiate, replay it
+  const int64_t l0 = h->launches;
+  g_capturing = true; g_capture_broken = false;
+  cudaError_t ce = cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal);
+  int32_t rc = B2S_E_CUDA;
+  cudaGraph_t graph = nullptr;
+  if (ce == cudaSuccess) {
+    rc = chain(ctx);
+    ce = cudaStreamEndCapture(h->stream, &graph);
+  }
+  g_capturing = false;
+  const int64_t captured_kernels = h->launches - l0;
+  h->launches = l0;
+  if (ce != cudaSuccess || rc != B2S_OK || g_capture_broken || !graph) {
+    // not capturable (e.g. an unbounded cropper needs a host round trip): stay eager for good
+    if (graph) cudaGraphDestroy(graph);
+    cudaGetLastError();
+    g->warm = 1 << 30;
+    return chain(ctx);
+  }
+  ce = cudaGraphInstantiate(&g->exec, graph, 0);
+  cudaGraphDestroy(graph);
+  if (ce != cudaSuccess) { g->exec = nullptr; g->warm = 1 << 30; cudaGetLastError(); return chain(ctx); }
+  g->kernels = captured_kernels;
+  h->captures++;
+  g->alloc_gen = __atomic_load_n(&g_alloc_generation, __ATOMIC_RELAXED);
+  g->cfg_gen = h->cfg_gen;
+  g->key = key;
+  B2S_CUDA(cudaGraphLaunch(g->exec, h->stream));
+  h->launches += g->kernels;
   return B2S_OK;
 }
 
@@ -238,47 +291,7 @@ static int32_t mapper_step_graph(b2s_handle* h, b2s_submap* sm, const b2s_cloud*
   if ((sm->host_step & 31) == 0) B2S_CUDA(cudaStreamSynchronize(h->stream));
   memcpy(sm->odom_ring.as<double>() + (sm->host_step & 63) * 16, odometry_motion, 128);   // read by graph_begin_kernel of this step
   sm->host_step++;
-  // a device buffer was re-allocated since the capture (any call that grows a scratch buffer): the graph holds the old
-  // address -- or b2s_set_config changed what the captured launches were built from.  This step runs eagerly (which also re-sizes the scratch).
-  if (sm->graph_alloc_gen != __atomic_load_n(&g_alloc_generation, __ATOMIC_RELAXED) || sm->graph_cfg_gen != h->cfg_gen) B2S_TRY(drop_graph(h, sm));
-  if (sm->gexec) {
-    B2S_CUDA(cudaGraphLaunch(sm->gexec, h->stream));
-    h->launches += sm->graph_kernels;
-    return B2S_OK;
-  }
-  if (sm->graph_warm > 0) {   // eager steps size every scratch buffer (no allocation may happen during capture)
-    sm->graph_warm--;
-    return mapper_chain_graphable(h, sm);
-  }
-  // capture this step's chain, instantiate, replay it
-  const int64_t l0 = h->launches;
-  g_capturing = true; g_capture_broken = false;
-  cudaError_t ce = cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal);
-  int32_t rc = B2S_E_CUDA;
-  cudaGraph_t graph = nullptr;
-  if (ce == cudaSuccess) {
-    rc = mapper_chain_graphable(h, sm);
-    ce = cudaStreamEndCapture(h->stream, &graph);
-  }
-  g_capturing = false;
-  const int64_t captured_kernels = h->launches - l0;
-  h->launches = l0;
-  if (ce != cudaSuccess || rc != B2S_OK || g_capture_broken || !graph) {
-    // not capturable (e.g. an unbounded cropper needs a host round trip): stay eager for good
-    if (graph) cudaGraphDestroy(graph);
-    cudaGetLastError();
-    sm->graph_warm = 1 << 30;
-    return mapper_chain_graphable(h, sm);
-  }
-  ce = cudaGraphInstantiate(&sm->gexec, graph, 0);
-  cudaGraphDestroy(graph);
-  if (ce != cudaSuccess) { sm->gexec = nullptr; sm->graph_warm = 1 << 30; cudaGetLastError(); return mapper_chain_graphable(h, sm); }
-  sm->graph_kernels = captured_kernels;
-  sm->graph_alloc_gen = __atomic_load_n(&g_alloc_generation, __ATOMIC_RELAXED);
-  sm->graph_cfg_gen = h->cfg_gen;
-  B2S_CUDA(cudaGraphLaunch(sm->gexec, h->stream));
-  h->launches += sm->graph_kernels;
-  return B2S_OK;
+  return graph_step(h, &sm->graph, 0, mapper_chain_graphable, sm);
 }
 
 // A cloud of `capacity` points and count 0 on h's device.  normals: allocate the normals too.  fixed: n_max stays at the capacity
@@ -294,7 +307,7 @@ static int32_t make_cloud(b2s_handle* h, size_t capacity, bool normals, bool fix
   });
 }
 // the same for a cloud the handle or a submap owns (tracked: its buffers may be captured in a graph)
-static int32_t make_cloud(b2s_handle* h, size_t capacity, bool normals, bool fixed, std::unique_ptr<b2s_cloud>* out) {
+int32_t make_cloud(b2s_handle* h, size_t capacity, bool normals, bool fixed, std::unique_ptr<b2s_cloud>* out) {
   b2s_cloud* c = nullptr;
   B2S_TRY(make_cloud(h, capacity, normals, fixed, true, &c));
   out->reset(c);
@@ -327,6 +340,7 @@ const char* b2s_last_error(void) { return get_error(); }
 const char* b2s_version(void) { return "b2s 0.1 (sm_90a, fp64)"; }
 int32_t b2s_device_count(void) { int n = 0; if (cudaGetDeviceCount(&n) != cudaSuccess) return 0; return n; }
 int64_t b2s_launch_count(const b2s_handle* h) { return h ? h->launches : 0; }
+int64_t b2s_graph_capture_count(const b2s_handle* h) { return h ? h->captures : 0; }
 
 int32_t b2s_create(const b2s_config* cfg, int32_t device, void* cuda_stream_or_null, b2s_handle** out) {
   B2S_REQUIRE(out != nullptr, B2S_E_INVALID, "b2s_create: out is null");
@@ -564,7 +578,7 @@ int32_t b2s_register(b2s_handle* h, const b2s_cloud* source, const b2s_cloud* ta
   B2S_TRY(h->problems.ensure(sizeof(IcpProblem), h->stream));
   B2S_TRY(h->results.ensure(sizeof(b2s_result), h->stream));
   IcpProblem P;
-  fill_problem(h, &P, source, &h->grid_a, target, init, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
+  fill_problem(&P, h->cfg.icp, source, &h->grid_a, target, init, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
   B2S_TRY(icp_launch(h, &P, nullptr, 1, source->n_max));
   B2S_CUDA(cudaMemcpyAsync(out, h->results.p, sizeof(b2s_result), cudaMemcpyDeviceToHost, h->stream));
   return check_status(h);
@@ -605,7 +619,7 @@ int32_t b2s_register_batch(b2s_handle* h, int32_t n, const b2s_cloud* const* sou
   B2S_TRY(h->results.ensure(sizeof(b2s_result) * (size_t)n, h->stream));
   size_t woff = 0;
   for (int i = 0; i < n; i++) {
-    fill_problem(h, &probs[i], sources[i], grids[grid_of[i]], targets[i], inits + 16 * (size_t)i, nullptr, h->work_xyz.as<double>() + woff,
+    fill_problem(&probs[i], h->cfg.icp, sources[i], grids[grid_of[i]], targets[i], inits + 16 * (size_t)i, nullptr, h->work_xyz.as<double>() + woff,
                  h->results.as<b2s_result>() + i);
     woff += (icp_work_bytes(sources[i]->n_max) + 7) / 8;
   }
@@ -697,7 +711,7 @@ int32_t b2s_information_matrix(b2s_handle* h, const b2s_cloud* source, const b2s
   B2S_TRY(h->work_xyz.ensure(icp_work_bytes(source->n_max), h->stream));
   B2S_TRY(h->results.ensure(sizeof(b2s_result) + 36 * 8 + 64, h->stream));
   IcpProblem P;
-  fill_problem(h, &P, source, &h->grid_a, target, T, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
+  fill_problem(&P, h->cfg.icp, source, &h->grid_a, target, T, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
   P.max_corr = max_corr;
   P.max_iter = 0;
   P.estimator = EST_INFORMATION;
@@ -730,7 +744,7 @@ int32_t b2s_nearest_neighbors(b2s_handle* h, const b2s_cloud* queries, const b2s
     launch_pdl(write_i32_kernel, 1, 1, 0, h->stream, d_cnt, (int32_t)cnt);
     h->launches++;
     IcpProblem P;
-    fill_problem(h, &P, queries, &h->grid_a, target, T ? T : I, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
+    fill_problem(&P, h->cfg.icp, queries, &h->grid_a, target, T ? T : I, nullptr, h->work_xyz.as<double>(), h->results.as<b2s_result>());
     P.src_xyz = queries->xyz.as<double>() + 3 * off;
     P.work_prev = reinterpret_cast<int32_t*>(h->work_xyz.as<double>() + 3 * (CHUNK + 1));   // the work buffer is sized for a chunk, not for the cloud
     P.src_n = d_cnt;
@@ -763,9 +777,12 @@ int32_t b2s_register_host(b2s_handle* h, const double* src_xyz, size_t n_src, co
 int32_t b2s_submap_create(b2s_handle* h, size_t capacity_points, b2s_submap** out) {
   B2S_REQUIRE(h && out && capacity_points > 0, B2S_E_INVALID, "bad argument");
   LOCK(h);
+  static unsigned long long next_uid = 0;
   return create_object(out, [&](b2s_submap* sm) -> int32_t {
     sm->h = h;
     sm->device = h->device;
+    sm->uid = __atomic_add_fetch(&next_uid, 1ull, __ATOMIC_RELAXED);
+    submap_register(sm->uid);
     sm->capacity = capacity_points;
     for (std::unique_ptr<b2s_cloud>& c : sm->cloud) {
       B2S_TRY(make_cloud(h, capacity_points, true, false, &c));
@@ -918,8 +935,10 @@ int32_t b2s_submap_set_cloud(b2s_handle* h, b2s_submap* sm, const b2s_cloud* clo
   return fuse_rehash(h, sm);
 }
 
-static int32_t register_to_submap_async(b2s_handle* h, const b2s_cloud* scan, const b2s_submap* sm, const double* sensor_pose_host,
-                                        const double* sensor_pose_dev, const double* init_host, const double* init_dev, b2s_result* out_dev) {
+}  // extern "C"
+
+int32_t b2s::register_to_submap_async(b2s_handle* h, const b2s_cloud* scan, const b2s_submap* sm, const double* sensor_pose_host,
+                                      const double* sensor_pose_dev, const double* init_host, const double* init_dev, b2s_result* out_dev) {
   B2S_TRY(check_icp_params(h->cfg.icp));
   B2S_REQUIRE(scan->has_normals || h->cfg.icp.reg_type != B2S_REG_GENERALIZED, B2S_E_NO_NORMALS, "GeneralizedIcp: the scan has no normals");
   const b2s_cloud* map = sm->cloud[0].get();
@@ -930,9 +949,11 @@ static int32_t register_to_submap_async(b2s_handle* h, const b2s_cloud* scan, co
   B2S_TRY(h->work_xyz.ensure(icp_work_bytes(scan->n_max), h->stream));
   B2S_TRY(h->problems.ensure(sizeof(IcpProblem), h->stream));
   IcpProblem P;
-  fill_problem(h, &P, scan, &h->grid_a, map, init_host, init_dev, h->work_xyz.as<double>(), out_dev);
+  fill_problem(&P, h->cfg.icp, scan, &h->grid_a, map, init_host, init_dev, h->work_xyz.as<double>(), out_dev);
   return icp_launch(h, &P, nullptr, 1, scan->n_max);
 }
+
+extern "C" {
 
 int32_t b2s_register_to_submap(b2s_handle* h, const b2s_cloud* scan, const b2s_submap* sm, const double map_to_sensor[16],
                                const double init[16], b2s_result* out) {
@@ -984,7 +1005,8 @@ int32_t b2s_submap_set_mapper_options(b2s_handle* h, b2s_submap* sm, const b2s_m
   B2S_REQUIRE(o->dense_carve_every_n_scans >= 0 && o->min_movement_between_mapping_steps >= 0.0, B2S_E_INVALID, "invalid mapper options");
   LOCK(h);
   sm->opts = *o;
-  return drop_graph(h, sm);
+  sm->opts_gen++;
+  return graph_drop(h, &sm->graph);
 }
 
 int32_t b2s_submap_get_mapper_counters(b2s_handle* h, const b2s_submap* sm, b2s_mapper_counters* out) {
@@ -1013,11 +1035,12 @@ int32_t b2s_mapper_graph_enable(b2s_handle* h, b2s_submap* sm, size_t raw_capaci
     B2S_TRY(gstate.ensure(64, h->stream));
     sm->staging = std::move(staging); sm->odom_ring = std::move(ring); sm->gstate = std::move(gstate);
   }
-  B2S_TRY(drop_graph(h, sm));
+  B2S_TRY(graph_drop(h, &sm->graph));
   sm->g_min_fitness = min_refinement_fitness;
   sm->g_ignore_fitness = ignore_min_fitness;
   sm->graph_mode = true;
-  sm->graph_warm = 2;
+  sm->fixed_launch = true;
+  sm->graph.warm = 2;
   sm->host_step = 0;
   B2S_CUDA(cudaMemsetAsync(sm->gstate.p, 0, 64, h->stream));
   *staging_out = sm->staging.get();

@@ -159,7 +159,7 @@ int32_t op_submap_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan
   b2s_cloud* map = sm->cloud[0].get();
   b2s_cloud* tmp = sm->cloud[1].get();
   // graph replay: constant launch dimensions (the map's host-side bound moves from scan to scan)
-  const size_t n_max = sm->graph_mode ? sm->capacity : (map->n_max > 0 ? map->n_max : 1);
+  const size_t n_max = sm->fixed_launch ? sm->capacity : (map->n_max > 0 ? map->n_max : 1);
   size_t cap = 1024;
   while (cap < 2 * n_max) cap <<= 1;
   B2S_TRY(h->keys.ensure(cap * 8, h->stream));                    // packed voxel keys
@@ -183,7 +183,7 @@ int32_t op_submap_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan
       cap - 1, prm.voxel_size, inv, prm.max_raytracing_length, prm.truncation_distance, prm.min_dot_product_with_normal, keep, enable_dev);
   h->launches += 3;
   const size_t keep_n_max = map->n_max;
-  if (sm->graph_mode) map->n_max = n_max;
+  if (sm->fixed_launch) map->n_max = n_max;
   const int32_t rc = compact_cloud(h, map, keep, tmp, n_eff);   // order-preserving (removeByIds = SelectByIndex(invert))
   map->n_max = keep_n_max;
   B2S_TRY(rc);

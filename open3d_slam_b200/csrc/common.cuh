@@ -6,6 +6,7 @@
 #include <string.h>
 #include <memory>
 #include <mutex>
+#include <unordered_set>
 #include <new>
 #include <string>
 #include <utility>
@@ -131,6 +132,28 @@ struct SortScratch {
   DevBuf keys_alt, vals_alt;
 };
 
+// process-wide registry of the submaps alive (by b2s_submap::uid): caches of graphs captured for a submap elsewhere drop the entries of
+// submaps that are gone
+void submap_register(unsigned long long uid);
+void submap_forget(unsigned long long uid);
+bool submap_alive(unsigned long long uid);
+
+// A captured per-scan chain (CUDA graph) and what it was captured under.  Its launches bake in buffer addresses, the handle's
+// configuration and the owner's options (key): once one of them changes the graph is destroyed, the next step runs eagerly and
+// the one after re-captures.
+struct GraphCache {
+  cudaGraphExec_t exec = nullptr;
+  int warm = 2;                       // eager steps still to run before the capture (sizes every scratch buffer)
+  int64_t kernels = 0;                // kernels per replay (for the launch counter)
+  unsigned long long alloc_gen = 0;   // value of b2s::g_alloc_generation when the graph was captured
+  unsigned long long cfg_gen = 0;     // value of b2s_handle::cfg_gen when the graph was captured
+  unsigned long long key = 0;         // the owner's options generation when the graph was captured
+  GraphCache() = default;
+  GraphCache(const GraphCache&) = delete;
+  GraphCache& operator=(const GraphCache&) = delete;
+  ~GraphCache() { if (exec) cudaGraphExecDestroy(exec); }
+};
+
 }  // namespace b2s
 
 struct b2s_cloud {
@@ -146,9 +169,10 @@ struct b2s_cloud {
 };
 
 struct b2s_submap {
-  ~b2s_submap() { if (gexec) cudaGraphExecDestroy(gexec); if (cnt_ev) cudaEventDestroy(cnt_ev); }   // the buffers and clouds free themselves
+  ~b2s_submap() { if (cnt_ev) cudaEventDestroy(cnt_ev); if (uid) b2s::submap_forget(uid); }   // the buffers, clouds and the graph free themselves
   b2s_handle* h = nullptr;
   int device = 0;
+  unsigned long long uid = 0;         // unique over the process: graphs captured for this submap elsewhere are keyed by it
   std::unique_ptr<b2s_cloud> cloud[2];  // ping-pong map cloud (mapCloud_)
   int cur = 0;
   size_t capacity = 0;
@@ -169,9 +193,8 @@ struct b2s_submap {
   // CUDA-graph replay of the per-scan chain (b2s_mapper_graph_enable): every launch dimension is derived from fixed
   // capacities, the per-step inputs (odometry motion, result slot) come from a ring indexed by a device-side counter
   bool graph_mode = false;
-  int graph_warm = 0;                 // eager steps still to run before the capture (sizes every scratch buffer)
-  cudaGraphExec_t gexec = nullptr;
-  int64_t graph_kernels = 0;          // kernels per replay (for the launch counter)
+  bool fixed_launch = false;           // a captured chain runs on this submap (either graph mode): launch dimensions from the capacity, no host read-backs
+  b2s::GraphCache graph;
   std::unique_ptr<b2s_cloud> staging; // fixed-capacity input cloud the caller uploads each scan into
   b2s::PinnedBuf odom_ring;           // device-mapped: 64 x (4x4 f64) odometry motions
   long long host_step = 0;
@@ -193,9 +216,8 @@ struct b2s_submap {
   size_t stage_cap = 0;
   // Mapper / SubmapCollection wiring of the device chain (b2s_mapper_options) and its device-side state words (MS_*)
   b2s_mapper_options opts;
+  unsigned long long opts_gen = 1;    // bumped by b2s_submap_set_mapper_options: graphs of other objects that run this chain compare it
   b2s::DevBuf mstate;                 // int32 [MS_WORDS]: gates and counters of the chain, see the MS_* indices below
-  unsigned long long graph_alloc_gen = 0;   // value of b2s::g_alloc_generation when the graph was captured
-  unsigned long long graph_cfg_gen = 0;     // value of b2s_handle::cfg_gen when the graph was captured
 };
 
 struct b2s_feature {
@@ -261,6 +283,7 @@ struct b2s_handle {
   b2s_config cfg;
   unsigned long long cfg_gen = 1;     // bumped by b2s_set_config: captured graphs bake the configuration in
   int64_t launches = 0;
+  int64_t captures = 0;               // CUDA graphs captured by this handle's per-scan chains (b2s_graph_capture_count)
 
   b2s::DevBuf status;                 // uint32 [16]: [0] device status word, the rest scratch words (b2s::SW_*)
   b2s::ScanScratch scan;
@@ -414,6 +437,26 @@ int32_t op_submap_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan
 // T_dev != nullptr: device-resident pose (T_host ignored)
 int32_t op_dense_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw, const double* T_host, const double* T_dev, const b2s_cropper* crop,
                         const int32_t* enable_dev = nullptr);
+
+// ---- pieces of the per-scan chains (c_api.cu) shared with the odometry chain (odometry.cu) ----
+int32_t check_icp_params(const b2s_icp_params& p);
+double nn_cell(const b2s_handle* h, double max_corr);
+size_t icp_work_bytes(size_t n);
+void fill_problem(IcpProblem* P, const b2s_icp_params& icp, const b2s_cloud* src, const GridIndex* g, const b2s_cloud* tgt, const double* init_host,
+                  const double* init_dev, double* work, b2s_result* out_dev);
+// crop (sensor frame) -> voxelize -> normals (icp.knn, icp.knn_radius) -> RandomDownSample; scratch receives the voxelized cloud
+int32_t preprocess_scan(b2s_handle* h, const b2s_cloud* raw, const b2s_cropper& cropper, double voxel_size, double ratio, uint32_t seed,
+                        const b2s_icp_params& icp, b2s_cloud* scratch, b2s_cloud* out);
+int32_t process_scan_impl(b2s_handle* h, const b2s_cloud* raw, b2s_cloud* merge, b2s_cloud* match);
+int32_t register_to_submap_async(b2s_handle* h, const b2s_cloud* scan, const b2s_submap* sm, const double* sensor_pose_host,
+                                 const double* sensor_pose_dev, const double* init_host, const double* init_dev, b2s_result* out_dev);
+int32_t mapper_chain_tail(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_scan, const b2s_cloud* merge, const b2s_result* res,
+                          double min_fitness, int ignore_fitness, b2s_result* slots, const int32_t* gstate);
+int32_t make_cloud(b2s_handle* h, size_t capacity, bool normals, bool fixed, std::unique_ptr<b2s_cloud>* out);
+// one step of a graph-replayable chain: replays the captured graph, or runs chain(ctx) eagerly while warming up, or captures it.
+// key: the owner's options generation (a different key drops the graph like a re-allocation or b2s_set_config does)
+int32_t graph_step(b2s_handle* h, GraphCache* g, unsigned long long key, int32_t (*chain)(void*), void* ctx);
+int32_t graph_drop(b2s_handle* h, GraphCache* g);
 
 // SMs of the current device (132 on an H100 SXM), queried once per device: the grid sizes below are multiples of it
 int device_sms();

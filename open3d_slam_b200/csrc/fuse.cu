@@ -428,7 +428,7 @@ int32_t fuse_reserve(b2s_handle* h, b2s_submap* sm) {
 int32_t fuse_rehash(b2s_handle* h, b2s_submap* sm, const int32_t* enable_dev) {
   B2S_TRY(fuse_reserve(h, sm));
   b2s_cloud* map = sm->cloud[0].get();
-  const size_t n_max = sm->graph_mode ? sm->capacity : (map->n_max > 0 ? map->n_max : 1);
+  const size_t n_max = sm->fixed_launch ? sm->capacity : (map->n_max > 0 ? map->n_max : 1);
   int32_t* ms = sm->mstate.as<int32_t>();
   ProfScope prof(h, PK_FUSE);
   launch_pdl(fuse_table_clear_kernel, 4 * device_sms(), 256, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vstamp.as<int32_t>(), sm->vcap,
@@ -472,13 +472,13 @@ int32_t op_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, c
   B2S_TRY(fuse_reserve(h, sm));
   // host-side upper bound of the map size.  The exact size is read back asynchronously after an insertion (pinned
   // host word + event); once that copy has landed the bound becomes exact-size + what was appended since.
-  if (sm->cnt_pending && cudaEventQuery(sm->cnt_ev) == cudaSuccess) {
+  if (sm->cnt_pending && !g_capturing && cudaEventQuery(sm->cnt_ev) == cudaSuccess) {   // (no event query inside a capture)
     map->n_max = (size_t)sm->pinned_cnt.as<int32_t>()[0] + sm->adds_after_readback;
     sm->cnt_pending = false;
   }
   const size_t m_max = 2 * (scan->n_max > 0 ? scan->n_max : 1);   // the duplication quirk doubles the scan
   size_t tot_max = map->n_max + m_max;
-  if (sm->graph_mode) tot_max = sm->capacity;   // graph replay: constant launch dimensions, overflow is caught on the device
+  if (sm->fixed_launch) tot_max = sm->capacity;   // graph replay: constant launch dimensions, overflow is caught on the device
   if (tot_max > sm->capacity) {
     int32_t n = 0;
     B2S_CUDA(cudaMemcpyAsync(&n, map->dn.p, 4, cudaMemcpyDeviceToHost, h->stream));
@@ -530,7 +530,7 @@ int32_t op_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, c
   map->n_known = -1;
   map->has_normals = true;
   B2S_CUDA(cudaGetLastError());
-  if (!sm->graph_mode) {
+  if (!sm->fixed_launch) {
     if (!sm->cnt_ev) {
       B2S_TRY(sm->pinned_cnt.alloc(64));
       B2S_CUDA(cudaEventCreateWithFlags(&sm->cnt_ev, cudaEventDisableTiming));

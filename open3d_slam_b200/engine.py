@@ -206,6 +206,11 @@ class Engine:
     def launches(self) -> int:
         return int(L.lib().b2s_launch_count(self._h))
 
+    @property
+    def graphCaptures(self) -> int:
+        """CUDA graphs the per-scan chains of this handle have captured (a replay adds launches, not captures)"""
+        return int(L.lib().b2s_graph_capture_count(self._h))
+
     def profile_enable(self, on: bool = True):
         L.check(L.lib().b2s_profile_enable(self._h, C.c_int32(int(on))))
 
@@ -884,6 +889,25 @@ class OdometryParameters:
     scanMatcher: CloudRegistrationParameters = field(default_factory=CloudRegistrationParameters)
     scanProcessing: ScanProcessingParameters = field(default_factory=ScanProcessingParameters)
     seed: int = 0
+    minFitness: float = 0.1        # the "todo magic" of Odometry.cpp:51
+    bufferSize: int = 2000         # odomToRangeSensorBuffer_ size limit (TransformInterpolationBuffer())
+
+    def to_c(self) -> L.OdometryParams:
+        types = {"PointToPlaneIcp": L.REG_POINT_TO_PLANE, "PointToPointIcp": L.REG_POINT_TO_POINT, "GeneralizedIcp": L.REG_GENERALIZED}
+        if self.scanMatcher.regType not in types:
+            raise L.B2SError(L.E_UNSUPPORTED, f"unknown registration type {self.scanMatcher.regType}")
+        p = L.OdometryParams()
+        L.lib().b2s_default_odometry_params(C.byref(p))
+        ic = self.scanMatcher.icp
+        p.icp.reg_type = types[self.scanMatcher.regType]
+        p.icp.max_iter, p.icp.max_corr_dist, p.icp.knn, p.icp.knn_radius = int(ic.maxNumIter), float(ic.maxCorrespondenceDistance), int(ic.knn), float(ic.maxDistanceKnn)
+        p.voxel_size = float(self.scanProcessing.voxelSize)
+        p.downsampling_ratio = float(self.scanProcessing.downSamplingRatio)
+        p.seed = int(self.seed)
+        p.cropper = self.scanProcessing.cropper.to_c()
+        p.min_fitness = float(self.minFitness)
+        p.buffer_size = int(self.bufferSize)
+        return p
 
 
 class LidarOdometry:
@@ -930,6 +954,119 @@ class LidarOdometry:
 
     def getOdomToRangeSensor(self) -> np.ndarray:
         return self.odomToRangeSensorCumulative_.copy()
+
+
+@dataclass
+class OdometryStepResult:
+    """b2s_odometry_result: the registration of the step (zeros when it initialised), the cumulative pose after it, the outcome"""
+    registration: RegistrationResult
+    odomToRangeSensor: np.ndarray
+    outcome: int
+    nPreprocessed: int
+
+
+def _odo_res(r: L.OdometryResult) -> OdometryStepResult:
+    return OdometryStepResult(_res(r.registration), np.array(r.odom_to_range_sensor, dtype=np.float64).reshape(4, 4), int(r.outcome),
+                              int(r.n_preprocessed))
+
+
+@dataclass
+class SlamStepResult:
+    """b2s_slam_result: the odometry step, the scan-to-map registration, whether the prediction came from the odometry buffer and
+    whether the mapper accepted the scan"""
+    odometry: OdometryStepResult
+    mapper: RegistrationResult
+    odomUsed: bool
+    mapperAccepted: bool
+
+
+def _slam_res(r: L.SlamResult) -> SlamStepResult:
+    return SlamStepResult(_odo_res(r.odometry), _res(r.mapper), bool(r.odom_used), bool(r.mapper_accepted))
+
+
+class _OdometryBuffer:
+    """LidarOdometry::getBuffer() as far as callers read it: has(t)"""
+
+    def __init__(self, odo: "DeviceLidarOdometry"):
+        self.odo = odo
+
+    def has(self, t: int) -> bool:
+        return self.odo._lookup(t)[1]
+
+
+class DeviceLidarOdometry:
+    """src/Odometry.cpp:19-110 on the device (b2s_odometry): its own parameters, cloudPrev_, cumulative pose and
+    TransformInterpolationBuffer.  addRangeScan only enqueues; fetchResult reads the outcome of a step.  Timestamps are
+    UniversalTimeScaleClock ticks (100 ns) and must increase from call to call."""
+
+    def __init__(self, eng: Engine, params: OdometryParameters | None = None, capacity_points: int = 200_000):
+        self.eng = eng
+        self.params_ = params or OdometryParameters()
+        self._o = C.c_void_p()
+        p = self.params_.to_c()
+        L.check(L.lib().b2s_odometry_create(eng._h, C.byref(p), C.c_size_t(capacity_points), C.byref(self._o)))
+
+    def setParameters(self, params: OdometryParameters):
+        p = params.to_c()
+        L.check(L.lib().b2s_odometry_set_params(self.eng._h, self._o, C.byref(p)))
+        self.params_ = params
+
+    def setInitialTransform(self, T):
+        M = _mat(T)
+        L.check(L.lib().b2s_odometry_set_initial_transform(self.eng._h, self._o, _pd(M)))
+
+    def addRangeScan(self, cloud: Cloud, t: int, slot: int = 0) -> int:
+        L.check(L.lib().b2s_odometry_step_async(self.eng._h, self._o, cloud._c, C.c_int64(int(t)), C.c_int32(slot)))
+        return slot
+
+    def fetchResult(self, slot: int = 0) -> OdometryStepResult:
+        r = L.OdometryResult()
+        L.check(L.lib().b2s_odometry_result_fetch(self.eng._h, self._o, C.c_int32(slot), C.byref(r)))
+        return _odo_res(r)
+
+    def _lookup(self, t: int):
+        T = np.zeros(16, dtype=np.float64)
+        has = C.c_int32()
+        L.check(L.lib().b2s_odometry_lookup(self.eng._h, self._o, C.c_int64(int(t)), _pd(T), C.byref(has)))
+        return T.reshape(4, 4), bool(has.value)
+
+    def getOdomToRangeSensor(self, t: int) -> np.ndarray:
+        """getTransform(t, odomToRangeSensorBuffer_)"""
+        return self._lookup(t)[0]
+
+    def getBuffer(self) -> _OdometryBuffer:
+        return _OdometryBuffer(self)
+
+    def getPreProcessedCloud(self) -> Cloud:
+        c = Cloud(self.eng)
+        L.check(L.lib().b2s_odometry_preprocessed(self.eng._h, self._o, c._c))
+        return c
+
+    def enableGraph(self, raw_capacity_points: int = 65536) -> Cloud:
+        """Replay the combined odometry + mapper step as CUDA graphs (one per submap).  Returns the staging cloud every scan
+        must be uploaded / copied into."""
+        st = C.c_void_p()
+        L.check(L.lib().b2s_slam_graph_enable(self.eng._h, self._o, C.c_size_t(raw_capacity_points), C.byref(st)))
+        c = Cloud.__new__(Cloud)
+        c.eng = self.eng; c._c = st; c._borrowed = True
+        self._staging = c
+        return c
+
+    def fetchSlamResult(self, slot: int = 0) -> SlamStepResult:
+        r = L.SlamResult()
+        L.check(L.lib().b2s_slam_result_fetch(self.eng._h, self._o, C.c_int32(slot), C.byref(r)))
+        return _slam_res(r)
+
+    def free(self):
+        if getattr(self, "_o", None) and self._o.value:
+            L.lib().b2s_odometry_destroy(self._o)
+            self._o = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
 
 
 class Mapper:
@@ -1028,3 +1165,20 @@ class Mapper:
         r = L.Result()
         L.check(L.lib().b2s_scan_result_fetch(self.eng._h, C.c_int32(slot), C.byref(r)))
         return _res(r)
+
+    # ---- odometry + mapper for the same scan, the prediction read from the odometry's buffer on the device --------------------
+    def addRangeMeasurementWithOdometry(self, odometry: DeviceLidarOdometry, rawScan: Cloud, t: int, slot: int = 0) -> int:
+        """odometry.addRangeScan(rawScan, t), then addRangeMeasurement(rawScan, t) on the active submap (b2s_slam_step_async): only
+        enqueues; odometry.fetchSlamResult(slot) reads the result.  After odometry.enableGraph() rawScan must be its staging cloud."""
+        L.check(L.lib().b2s_slam_step_async(self.eng._h, self.submap._s, odometry._o, rawScan._c, C.c_int64(int(t)),
+                                            C.c_double(self.params_.minRefinementFitness), C.c_int32(int(self.params_.isIgnoreMinRefinementFitness)),
+                                            C.c_int32(slot)))
+        return slot
+
+    def addRangeMeasurementWithOdometryHostAsync(self, odometry: DeviceLidarOdometry, xyz_f32_ptr: int, n: int, t: int, out_pinned_ptr: int,
+                                                 stride: int = 12) -> None:
+        """The same from a float32 host scan: upload, both chains and the copy of the b2s_slam_result to out_pinned_ptr (page-locked
+        host memory, ctypes layout _lib.SlamResult, valid once the engine's stream has been synchronised) are only enqueued."""
+        L.check(L.lib().b2s_slam_step_host_async(self.eng._h, self.submap._s, odometry._o, C.c_void_p(xyz_f32_ptr), C.c_size_t(n), C.c_size_t(stride),
+                                                 C.c_int64(int(t)), C.c_double(self.params_.minRefinementFitness),
+                                                 C.c_int32(int(self.params_.isIgnoreMinRefinementFitness)), C.c_void_p(out_pinned_ptr)))

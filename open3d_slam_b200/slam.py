@@ -18,10 +18,12 @@ replays the captured CUDA graph of the chain S1 -> S2 -> gates -> [carving] -> F
 from __future__ import annotations
 
 import collections
+import ctypes as C
 from dataclasses import dataclass, field
 
 import numpy as np
 
+from . import _lib as L
 from . import engine as E
 
 
@@ -190,6 +192,27 @@ class SegmentMapper:
             return None
         active = sc.getActiveSubmap()
         res, inserted = self.backend.step(active.handle, rawScanF32, odometryMotion)
+        return self._after_step(k, res, inserted)
+
+    def addRangeScan(self, rawScanF32: np.ndarray, t: int):
+        """One scan of SlamWrapper's odometry and mapping workers from the raw scan and its timestamp alone (UniversalTimeScaleClock
+        ticks, increasing): the backend runs the scan-to-scan odometry and the scan-to-map step with the prediction read from the
+        odometry's buffer (DeviceBackend: one b2s_slam_step_host_async).  The first scan initialises both."""
+        sc = self.submaps
+        k = self._k
+        self._k += 1
+        if not sc.submaps:
+            sc.createNewSubmap(self.mapToRangeSensor)
+            self.backend.first_scan_with_odometry(sc.getActiveSubmap().handle, rawScanF32, t)
+            sc.numScansMergedInActiveSubmap += 1
+            self.poses.append(self.mapToRangeSensor.copy())
+            self.results.append(None)
+            return None
+        res, inserted = self.backend.step_with_odometry(sc.getActiveSubmap().handle, rawScanF32, t)
+        return self._after_step(k, res, inserted)
+
+    def _after_step(self, k: int, res, inserted: bool):
+        sc = self.submaps
         self.results.append(res)
         if inserted:
             self.mapToRangeSensor = np.array(res.transformation_, dtype=np.float64)
@@ -328,8 +351,11 @@ class DeviceBackend:
     """All arithmetic on libb2s.so (one handle / one CUDA stream = one robot)."""
 
     def __init__(self, params: E.MapperParameters | None = None, device: int = 0, cuda_stream: int | None = None, submap_capacity: int = 900_000,
-                 carving: bool = True, dense: bool = True, graph: bool = True, raw_capacity: int = 65536):
+                 carving: bool = True, dense: bool = True, graph: bool = True, raw_capacity: int = 65536,
+                 odometry: E.OdometryParameters | None = None):
         self.params = params or E.MapperParameters()
+        self.odometry_params = odometry or E.OdometryParameters()   # the device odometry of SegmentMapper.addRangeScan
+        self._odo = None
         self.eng = E.Engine(self.params, device=device, cuda_stream=cuda_stream)
         self.mapper = E.Mapper(self.eng, 1024)     # its own first submap is a placeholder: submaps are created by new_submap()
         self.mapper.submap.free()
@@ -381,6 +407,34 @@ class DeviceBackend:
         p = self.params
         accepted = p.isIgnoreMinRefinementFitness or not (res.fitness_ < p.minRefinementFitness)
         return res, bool(accepted)     # minMovementBetweenMappingSteps = 0 in every preset: accepted scans are inserted
+
+    # -- scan-to-scan odometry on the device, feeding the mapper step its prediction (SegmentMapper.addRangeScan)
+    def odometry(self) -> E.DeviceLidarOdometry:
+        if self._odo is None:
+            import torch
+            self._odo = E.DeviceLidarOdometry(self.eng, self.odometry_params, self.raw_capacity)
+            if self.graph:
+                self._odo.enableGraph(self.raw_capacity)
+            self._slam_pin = torch.empty(C.sizeof(L.SlamResult), dtype=torch.uint8).pin_memory()
+            self._slam_out = L.SlamResult.from_address(self._slam_pin.data_ptr())
+        return self._odo
+
+    def first_scan_with_odometry(self, sm, raw: np.ndarray, t: int):
+        """Mapper.cpp:109-112 for the map and LidarOdometry::addRangeScan for the odometry, on the same scan and timestamp"""
+        merge = self.first_scan(sm, raw)
+        c = self.eng.cloud(np.ascontiguousarray(raw, dtype=np.float32))
+        self.odometry().addRangeScan(c, t)
+        c.free()
+        return merge
+
+    def step_with_odometry(self, sm, raw: np.ndarray, t: int):
+        odo = self.odometry()
+        self.mapper.submap = sm
+        ptr, n = self._pinned(raw)
+        self.mapper.addRangeMeasurementWithOdometryHostAsync(odo, ptr, n, t, C.addressof(self._slam_out))
+        self.eng.synchronize()
+        self.last_slam_result = E._slam_res(self._slam_out)
+        return self.last_slam_result.mapper, self.last_slam_result.mapperAccepted
 
     def last_merge_cloud(self):
         # ring of pre-allocated clouds (no cudaMalloc per scan); longer than SubmapCollection's overlap buffer, so a buffered cloud is
