@@ -397,6 +397,56 @@ int32_t b2s_slam_step_host_async(b2s_handle* h, b2s_submap* sm, b2s_odometry* od
  * fixed-capacity staging cloud (one input stream per odometry object), which is then passed as raw. */
 int32_t b2s_slam_graph_enable(b2s_handle* h, b2s_odometry* od, size_t raw_capacity_points, b2s_cloud** staging_out);
 
+/* D2  motion compensation (de-skew) inside the device step, SlamWrapper::loadParametersAndInitialize (src/SlamWrapper.cpp:195-200):
+ *     with enabled set, every step of b2s_odometry_step_async / b2s_slam_step_async / _host_async de-skews the raw scan twice, as
+ *     odometryWorker (:266-268) and mappingWorker (:298-304) do, each with ConstantVelocityMotionCompensation::undistortInputPointCloud
+ *     (src/MotionCompensation.cpp:64-139, the per-point arithmetic of b2s_undistort):
+ *       - the odometry's input: velocities from the odometry buffer as it is before this scan's odometry step;
+ *       - the mapper's input:   velocities from the mapper's buffer (mapToRangeSensorBuffer_) as it is before this scan's mapper
+ *                               step.  That cloud is the raw scan of everything downstream: pre-processing, ICP, carving, F1 and
+ *                               the dense map (Mapper.cpp:139,174, SlamWrapper.cpp:322).
+ *     The velocity estimate, at the step's timestamp t with offset = num_poses_velocity_estimation (:32-57):
+ *       size <= offset -> v = w = 0;   latest_time < t -> dT = start^-1 * finish with finish = the latest entry and start the entry
+ *       `offset` before it, dt = toSeconds(finish.t - start.t), v = dT.translation / (dt + 1e-6),
+ *       w = toRPY(Quaterniond(dT.rotation).normalized()) / (dt + 1e-6) (src/math.cpp:39-46);   otherwise v = w = 0.
+ *     The mapper's buffer lives on the odometry object (one robot's Mapper), so a submap hand-over keeps it.  Its size limit is the
+ *     object's buffer_size.  Every step the mapper's fitness gate accepts pushes (t, mapToRangeSensor) into it, before the minimum-
+ *     motion gate (Mapper.cpp:160), whether or not de-skew is enabled; loop-closure corrections never touch it.  A push earlier than
+ *     the earliest or the latest entry is ignored, an equal time is accepted (TransformInterpolationBuffer.cpp:21-43).
+ *     Disabled (the default), the steps issue exactly the launches they issue without this feature. */
+typedef struct b2s_motion_compensation_params {
+  int32_t enabled;                        /* motion_compensation.is_undistort_scan (isUndistortInputCloud_), default 0 */
+  int32_t spinning_clockwise;             /* isSpinningClockwise_, default 1 */
+  double scan_duration;                   /* scanDuration_ [s], default 0.1; must be > 0 (assert_gt, MotionCompensation.cpp:61) */
+  int32_t num_poses_velocity_estimation;  /* numPosesVelocityEstimation_, default 3; must be >= 1 */
+} b2s_motion_compensation_params;
+/* the Lua defaults of parameter_structure_definitions.lua:33-36 (Parameters.hpp:192-197) */
+void b2s_default_motion_compensation_params(b2s_motion_compensation_params* p);
+/* SlamWrapper.cpp:195-200 (both ConstantVelocityMotionCompensation objects).  scan_duration <= 0 or num_poses_velocity_estimation < 1
+ * -> B2S_E_INVALID and nothing changes.  The first call with enabled set allocates the two de-skewed clouds (the object's capacity).
+ * Drops the captured combined graphs of this object (they bake the parameters in). */
+int32_t b2s_odometry_set_motion_compensation(b2s_handle* h, b2s_odometry* od, const b2s_motion_compensation_params* p);
+/* mapToRangeSensorBuffer_.push(t, T) for the pushes the caller's host code makes: the first scan (Mapper.cpp:112) and a new initial
+ * value (:145).  Enqueued on the handle's stream. */
+int32_t b2s_slam_map_pose_push(b2s_handle* h, b2s_odometry* od, int64_t t, const double T[16]);
+/* Mapper::getMapToRangeSensor(t) = getTransform(t, mapToRangeSensorBuffer_) with the semantics of b2s_odometry_lookup (has = 0,
+ * T = I on an empty buffer).  Synchronises. */
+int32_t b2s_slam_map_lookup(b2s_handle* h, const b2s_odometry* od, int64_t t, double T[16], int32_t* has);
+/* the velocities each de-skew of the step written to `slot` used, and whether they were not all zero.  Written by the de-skew
+ * kernels only: a half whose de-skew did not run in that step keeps what it held.  Synchronises. */
+typedef struct b2s_motion_compensation_result {
+  double odometry_linear_velocity[3];
+  double odometry_angular_velocity_rpy[3];
+  double map_linear_velocity[3];
+  double map_angular_velocity_rpy[3];
+  int32_t odometry_applied;               /* the odometry's de-skew moved the points (a velocity was non-zero) */
+  int32_t map_applied;                    /* the mapper's de-skew did */
+} b2s_motion_compensation_result;
+int32_t b2s_slam_motion_fetch(b2s_handle* h, b2s_odometry* od, int32_t slot, b2s_motion_compensation_result* out);
+/* device copies of the last de-skewed clouds: the odometry's input (odo_out) and the mapper's (map_out); either may be NULL.
+ * B2S_E_INVALID when de-skew was never enabled on this object. */
+int32_t b2s_slam_undistorted(b2s_handle* h, const b2s_odometry* od, b2s_cloud* odo_out, b2s_cloud* map_out);
+
 /* ---- F4  o3d_slam::VoxelMap (include/open3d_slam/Voxel.hpp:19-36, src/Voxel.cpp:123-160): voxel -> per-layer lists of point indices.
  *      Keys are getVoxelIdx(p, 1 / voxelSize) = floor(p * inv) per axis (VoxelHashMap.hpp:43-50).  Layers are integers
  *      0..B2S_VOXEL_MAP_LAYERS-1 (the shim maps the reference's layer names, e.g. Submap::voxelMapLayer).  The users on this path:

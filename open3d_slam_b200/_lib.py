@@ -82,6 +82,17 @@ class SlamResult(C.Structure):
     _fields_ = [("odometry", OdometryResult), ("mapper", Result), ("odom_used", C.c_int32), ("mapper_accepted", C.c_int32)]
 
 
+class MotionCompensationParams(C.Structure):
+    _fields_ = [("enabled", C.c_int32), ("spinning_clockwise", C.c_int32), ("scan_duration", C.c_double),
+                ("num_poses_velocity_estimation", C.c_int32)]
+
+
+class MotionCompensationResult(C.Structure):
+    _fields_ = [("odometry_linear_velocity", C.c_double * 3), ("odometry_angular_velocity_rpy", C.c_double * 3),
+                ("map_linear_velocity", C.c_double * 3), ("map_angular_velocity_rpy", C.c_double * 3),
+                ("odometry_applied", C.c_int32), ("map_applied", C.c_int32)]
+
+
 ODOM_INIT, ODOM_OK, ODOM_FAILED, ODOM_FAILED_KEPT_PREV = 0, 1, 2, 3
 
 
@@ -111,6 +122,8 @@ SYMBOLS = [
     "b2s_default_odometry_params", "b2s_odometry_create", "b2s_odometry_destroy", "b2s_odometry_set_params", "b2s_odometry_set_initial_transform",
     "b2s_odometry_step_async", "b2s_odometry_result_fetch", "b2s_odometry_lookup", "b2s_odometry_preprocessed",
     "b2s_slam_step_async", "b2s_slam_result_fetch", "b2s_slam_step_host_async", "b2s_slam_graph_enable",
+    "b2s_default_motion_compensation_params", "b2s_odometry_set_motion_compensation", "b2s_slam_map_pose_push", "b2s_slam_map_lookup",
+    "b2s_slam_motion_fetch", "b2s_slam_undistorted",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 PROFILE_KINDS = ["icp", "normals", "radix_sort", "nn_grid_build", "voxel", "fuse", "select", "crop"]
@@ -156,6 +169,7 @@ def lib():
         L.b2s_odometry_destroy.restype = None
         L.b2s_odometry_destroy.argtypes = [C.c_void_p]
         L.b2s_default_odometry_params.restype = None
+        L.b2s_default_motion_compensation_params.restype = None
         _lib = L
     return _lib
 

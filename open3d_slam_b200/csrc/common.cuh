@@ -658,5 +658,39 @@ __device__ __forceinline__ uint64_t morton_part21(uint64_t x) {
   return x;
 }
 
+// ConstantVelocityMotionCompensation::undistortInputPointCloud / computePhase (core/src/MotionCompensation.cpp:82-100,120-139) for one
+// point: p' = R(q) p + t with t = phase * scanDuration * v, q = fromRPY(phase * scanDuration * w).normalized() = qz * qy * qx
+// (core/src/math.cpp:32-37), R(q) as Eigen::Quaternion::toRotationMatrix.  Shared by b2s_undistort (voxel.cu) and the de-skew of the
+// combined chain (odometry.cu), so both give the same bits for the same velocities.
+__device__ __forceinline__ void undistort_point(double px, double py, double pz, double vx, double vy, double vz, double wr, double wp,
+                                                double wy, double duration, int clockwise, double* out) {
+  const double two_pi = 2.0 * 3.14159265358979323846;
+  const double angle = atan2(py, px);
+  const double wrapped = angle < 0.0 ? (angle + two_pi) : angle;
+  double phase = 0.0;
+  if (wrapped != 0.0) phase = clockwise ? 1.0 - wrapped / two_pi : wrapped / two_pi;
+  const double s = phase * duration;
+  const double tx_ = s * vx, ty_ = s * vy, tz_ = s * vz;
+  const double r = s * wr, pi_ = s * wp, yw = s * wy;
+  double sr, cr, sp, cp, sy, cy;
+  sincos(0.5 * r, &sr, &cr); sincos(0.5 * pi_, &sp, &cp); sincos(0.5 * yw, &sy, &cy);
+  // qzy = qz * qy with qz = (cy,0,0,sy), qy = (cp,0,sp,0);  q = qzy * qx with qx = (cr,sr,0,0)   (Eigen's product, all terms kept)
+  const double a0 = cy * cp - 0.0 * 0.0 - 0.0 * sp - sy * 0.0;
+  const double a1 = cy * 0.0 + 0.0 * cp + 0.0 * 0.0 - sy * sp;
+  const double a2 = cy * sp + 0.0 * cp + sy * 0.0 - 0.0 * 0.0;
+  const double a3 = cy * 0.0 + sy * cp + 0.0 * sp - 0.0 * 0.0;
+  double w = a0 * cr - a1 * sr - a2 * 0.0 - a3 * 0.0;
+  double x = a0 * sr + a1 * cr + a2 * 0.0 - a3 * 0.0;
+  double y = a0 * 0.0 + a2 * cr + a3 * sr - a1 * 0.0;
+  double z = a0 * 0.0 + a3 * cr + a1 * 0.0 - a2 * sr;
+  const double n2 = w * w + x * x + y * y + z * z;
+  if (n2 > 0.0) { const double nn = sqrt(n2); w /= nn; x /= nn; y /= nn; z /= nn; }
+  const double tx = 2 * x, ty = 2 * y, tz = 2 * z, twx = tx * w, twy = ty * w, twz = tz * w, txx = tx * x, txy = ty * x, txz = tz * x,
+               tyy = ty * y, tyz = tz * y, tzz = tz * z;
+  out[0] = ((1 - (tyy + tzz)) * px + (txy - twz) * py + (txz + twy) * pz) + tx_;
+  out[1] = ((txy + twz) * px + (1 - (txx + tzz)) * py + (tyz - twx) * pz) + ty_;
+  out[2] = ((txz - twy) * px + (tyz + twx) * py + (1 - (txx + tyy)) * pz) + tz_;
+}
+
 }  // namespace b2s
 #endif

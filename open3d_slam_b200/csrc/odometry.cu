@@ -23,6 +23,7 @@ struct OdoState {
   int32_t head, count;        // buffer ring: physical index of the earliest entry, entries held
   int32_t odom_used;          // the step's prediction came from the buffer
   int32_t pad;
+  int32_t map_head, map_count;   // the mapper's mapToRangeSensorBuffer_ ring (map_t / map_T), same layout
 };
 
 struct OdoStepInput {         // what the host hands each step (pinned, device-mapped ring of 64)
@@ -50,7 +51,12 @@ struct b2s_odometry {
   b2s::GridIndex grid;                 // target index of the registration (the current scan, rebuilt every step)
   b2s::DevBuf state;                   // OdoState
   b2s::DevBuf ring_t, ring_T;          // odomToRangeSensorBuffer_: buffer_size x (int64 time, 4x4)
-  b2s::DevBuf res;                     // b2s_result [2]: the odometry registration, the mapper registration of the step in flight
+  b2s::DevBuf map_t, map_T;            // the mapper's mapToRangeSensorBuffer_: buffer_size x (int64 time, 4x4)
+  b2s_motion_compensation_params mc;   // de-skew of both inputs (b2s_odometry_set_motion_compensation)
+  std::unique_ptr<b2s_cloud> odo_in;   // de-skewed input of the odometry (allocated when de-skew is first enabled)
+  std::unique_ptr<b2s_cloud> map_in;   // de-skewed input of the mapper
+  b2s::DevBuf motion;                  // b2s_motion_compensation_result [256], written by the de-skew kernels
+  b2s::DevBuf res;                    // b2s_result [2]: the odometry registration, the mapper registration of the step in flight
   b2s::DevBuf odo_slots, slam_slots;   // 256 result slots of each kind
   b2s::DevBuf lookup;                  // b2s_odometry_lookup: 4x4 + has
   b2s::PinnedBuf inputs;               // OdoStepInput ring, device-mapped
@@ -163,19 +169,52 @@ struct BufferView {
   __device__ long long time(int i) const { return t[phys(i)]; }
   __device__ const double* tf(int i) const { return T + 16 * phys(i); }
   __device__ bool has(long long q) const { return count > 0 && time(0) <= q && q <= time(count - 1); }
-  // getTransform(q, buffer) (TransformInterpolationBuffer.cpp:149-157 -> lookup :83-109); Identity for an empty buffer
+  // getTransform(q, buffer) (TransformInterpolationBuffer.cpp:149-157 -> lookup :83-109); Identity for an empty buffer.  The times
+  // never decrease (the mapper's buffer accepts an equal time): the first entry with q <= time is the one std::find_if returns
   __device__ void get(long long q, double* out) const {
     if (count == 0) { mat_identity(out); return; }
-    int i;
-    if (q <= time(0)) i = 0;
-    else if (q >= time(count - 1)) i = count - 1;
-    else {
-      int lo = 1, hi = count - 1;   // first entry with q <= time (the times are strictly increasing)
+    int i = 0;
+    if (count > 1) {
+      if (q < time(0)) q = time(0);
+      if (q > time(count - 1)) q = time(count - 1);
+      int lo = 0, hi = count - 1;
       while (lo < hi) { const int mid = (lo + hi) / 2; if (q <= time(mid)) hi = mid; else lo = mid + 1; }
       if (time(lo) != q) { interpolate_dev(tf(lo - 1), time(lo - 1), tf(lo), time(lo), q, out); return; }
       i = lo;
     }
     for (int k = 0; k < 16; k++) out[k] = tf(i)[k];
+  }
+  // push (TransformInterpolationBuffer.cpp:21-43, 111-115): a time earlier than the earliest or the latest entry is ignored, then
+  // push_back and pop_front while the size exceeds the limit.  Updates head / count of the caller's state.
+  __device__ static void push(long long* rt, double* rT, int cap, int32_t* head, int32_t* count, long long t, const double* T) {
+    if (*count > 0 && (t < rt[*head] || t < rt[(*head + *count - 1) % cap])) return;
+    int idx;
+    if (*count < cap) { idx = (*head + *count) % cap; *count += 1; }
+    else { idx = *head; *head = (*head + 1) % cap; }
+    rt[idx] = t;
+    for (int i = 0; i < 16; i++) rT[16 * idx + i] = T[i];
+  }
+  // ConstantVelocityMotionCompensation::estimateLinearAndAngularVelocity (MotionCompensation.cpp:32-57) at time q
+  __device__ void velocity(long long q, int offset, double* v, double* w) const {
+    for (int k = 0; k < 3; k++) v[k] = w[k] = 0.0;
+    if (count <= offset || !(time(count - 1) < q)) return;   // too few poses / "buffer has this already": zeros
+    const int fi = count - 1, si = count - 1 - offset;
+    double Si[16], dT[16];
+    iso_inv(tf(si), Si);
+    iso_mul(Si, tf(fi), dT);
+    const double dt = (double)(time(fi) - time(si)) / 1e7;
+    double qq[4];
+    quat_from_rot(dT, qq);
+    for (int pass = 0; pass < 2; pass++) {   // Quaterniond(...).normalized(), then toRPY's own normalize() (math.cpp:39-41)
+      const double z = qq[0] * qq[0] + qq[1] * qq[1] + qq[2] * qq[2] + qq[3] * qq[3];
+      if (z > 0.0) { const double n = sqrt(z); for (int k = 0; k < 4; k++) qq[k] /= n; }
+    }
+    const double x = qq[0], y = qq[1], z = qq[2], ww = qq[3];
+    const double den = dt + 1e-6;
+    for (int k = 0; k < 3; k++) v[k] = dT[4 * k + 3] / den;
+    w[0] = atan2(2 * (ww * x + y * z), 1 - 2 * (x * x + y * y)) / den;   // getRollFromQuat (math.hpp:30-42)
+    w[1] = asin(2 * (ww * y - x * z)) / den;
+    w[2] = atan2(2 * (ww * z + x * y), 1 - 2 * (y * y + z * z)) / den;
   }
 };
 
@@ -183,6 +222,51 @@ __device__ BufferView buffer_view(const OdoState* s, const long long* rt, const 
   BufferView b;
   b.t = rt; b.T = rT; b.cap = cap; b.head = s->head; b.count = s->count;
   return b;
+}
+// the mapper's mapToRangeSensorBuffer_
+__device__ BufferView map_view(const OdoState* s, const long long* rt, const double* rT, int cap) {
+  BufferView b;
+  b.t = rt; b.T = rT; b.cap = cap; b.head = s->map_head; b.count = s->map_count;
+  return b;
+}
+
+constexpr int DESKEW_THREADS = 256;
+
+// D2: one de-skew of the step in flight.  Thread 0 of every CTA estimates the velocities from the buffer (odometry's or mapper's) at
+// the step's timestamp and shares them; every thread then moves its points with undistort_point.  CTA 0 records the velocities in the
+// step's result slot.  The count is read on the device, the launch is sized by the caller's bound, so the launch can be captured.
+__global__ void __launch_bounds__(DESKEW_THREADS) deskew_kernel(const double* __restrict__ xyz, const int32_t* __restrict__ d_n, const OdoState* s,
+                                                                const long long* __restrict__ rt, const double* __restrict__ rT, int cap, int map,
+                                                                double duration, int clockwise, int offset, double* __restrict__ out, int32_t* out_n,
+                                                                b2s_motion_compensation_result* rec) {
+  pdl_wait();
+  __shared__ double vel[6];
+  if (threadIdx.x == 0) {
+    const BufferView b = map ? map_view(s, rt, rT, cap) : buffer_view(s, rt, rT, cap);
+    b.velocity(s->t_cur, offset, vel, vel + 3);
+    if (blockIdx.x == 0) {
+      b2s_motion_compensation_result* o = rec + s->slot;
+      double* v = map ? o->map_linear_velocity : o->odometry_linear_velocity;
+      double* w = map ? o->map_angular_velocity_rpy : o->odometry_angular_velocity_rpy;
+      int applied = 0;
+      for (int k = 0; k < 3; k++) {
+        v[k] = vel[k]; w[k] = vel[3 + k];
+        applied |= vel[k] != 0.0 || vel[3 + k] != 0.0;
+      }
+      if (map) o->map_applied = applied; else o->odometry_applied = applied;
+      *out_n = *d_n;
+    }
+  }
+  __syncthreads();
+  const int n = *d_n;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    undistort_point(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], vel[0], vel[1], vel[2], vel[3], vel[4], vel[5], duration, clockwise, out + 3 * i);
+}
+
+__global__ void map_pose_push_kernel(OdoState* s, long long* map_t, double* map_T, int cap, long long t, Mat16 T) {
+  pdl_wait();
+  if (threadIdx.x != 0) return;
+  BufferView::push(map_t, map_T, cap, &s->map_head, &s->map_count, t, T.v);
 }
 
 // first node of every odometry step: this step's timestamp and result slot from the host ring
@@ -280,13 +364,18 @@ __global__ void odometry_prediction_kernel(OdoState* s, const long long* __restr
   s->odom_used = used;
 }
 
-// after the mapper's gate: lastMeasurementTimestamp_ = t for an accepted scan (Mapper.cpp:164,178), and the combined result slot
+// after the mapper's gate: for an accepted scan mapToRangeSensorBuffer_.push(t, mapToRangeSensor_) (Mapper.cpp:160, pose[0..15] is
+// the registration result by now) and lastMeasurementTimestamp_ = t (:164,178); then the combined result slot
 __global__ void slam_post_kernel(OdoState* s, const int32_t* __restrict__ ms, const b2s_result* __restrict__ mres,
-                                 const b2s_odometry_result* __restrict__ odo_slots, b2s_slam_result* slam_slots) {
+                                 const b2s_odometry_result* __restrict__ odo_slots, b2s_slam_result* slam_slots, const double* __restrict__ pose,
+                                 long long* map_t, double* map_T, int cap) {
   pdl_wait();
   if (threadIdx.x != 0) return;
   const int accepted = ms[MS_ACCEPT];
-  if (accepted) s->t_last = s->t_cur;
+  if (accepted) {
+    BufferView::push(map_t, map_T, cap, &s->map_head, &s->map_count, s->t_cur, pose);
+    s->t_last = s->t_cur;
+  }
   b2s_slam_result* o = slam_slots + s->slot;
   o->odometry = odo_slots[s->slot];
   o->mapper = *mres;
@@ -301,10 +390,10 @@ __global__ void odometry_set_initial_kernel(OdoState* s, Mat16 T) {
 }
 
 __global__ void odometry_lookup_kernel(const OdoState* s, const long long* __restrict__ ring_t, const double* __restrict__ ring_T, int cap, long long t,
-                                       double* out) {
+                                       double* out, int map) {
   pdl_wait();
   if (threadIdx.x != 0) return;
-  const BufferView b = buffer_view(s, ring_t, ring_T, cap);
+  const BufferView b = map ? map_view(s, ring_t, ring_T, cap) : buffer_view(s, ring_t, ring_T, cap);
   b.get(t, out);
   out[16] = b.has(t) ? 1.0 : 0.0;
 }
@@ -331,7 +420,24 @@ static int32_t odometry_push_input(b2s_handle* h, b2s_odometry* od, long long t,
   return B2S_OK;
 }
 
-// Odometry.cpp:25-79 on the device, reading the step's inputs from the host ring
+// D2: raw -> out de-skewed with the velocities of the odometry's buffer (map = false) or the mapper's (map = true), one launch sized by
+// raw's bound (the staging capacity in graph mode)
+static int32_t deskew(b2s_handle* h, b2s_odometry* od, const b2s_cloud* raw, bool map, b2s_cloud* out) {
+  const b2s_motion_compensation_params& mc = od->mc;
+  out->fixed_cap = raw->fixed_cap;   // downstream sizing sees what it would see on raw: a staging cloud's bound, never its last count
+  out->n_max = raw->n_max;
+  out->n_known = raw->n_known;
+  out->has_normals = false;   // the reference copies the input cloud and rewrites points_ only
+  launch_pdl(deskew_kernel, grid_for(raw->n_max, DESKEW_THREADS), DESKEW_THREADS, 0, h->stream, raw->xyz.as<double>(), raw->dn.as<int32_t>(),
+             od->state.as<OdoState>(), (map ? od->map_t : od->ring_t).as<long long>(), (map ? od->map_T : od->ring_T).as<double>(),
+             od->params.buffer_size, map ? 1 : 0, mc.scan_duration, mc.spinning_clockwise ? 1 : 0, mc.num_poses_velocity_estimation,
+             out->xyz.as<double>(), out->dn.as<int32_t>(), od->motion.as<b2s_motion_compensation_result>());
+  h->launches++;
+  return B2S_OK;
+}
+
+// Odometry.cpp:25-79 on the device, reading the step's inputs from the host ring; with de-skew enabled the odometry works on the scan
+// de-skewed from its own buffer (SlamWrapper.cpp:266-268)
 static int32_t odometry_chain(b2s_handle* h, b2s_odometry* od, const b2s_cloud* raw) {
   const b2s_odometry_params& p = od->params;
   OdoState* s = od->state.as<OdoState>();
@@ -339,6 +445,10 @@ static int32_t odometry_chain(b2s_handle* h, b2s_odometry* od, const b2s_cloud* 
   B2S_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&inputs_dev), od->inputs.p, 0));
   launch_pdl(odometry_begin_kernel, 1, 32, 0, h->stream, inputs_dev, s);
   h->launches++;
+  if (od->mc.enabled) {
+    B2S_TRY(deskew(h, od, raw, false, od->odo_in.get()));
+    raw = od->odo_in.get();
+  }
   b2s_cloud* pre = od->pre.get();
   b2s_cloud* prev = od->prev.get();
   B2S_TRY(preprocess_scan(h, raw, p.cropper, p.voxel_size, p.downsampling_ratio, p.seed, p.icp, od->scratch.get(), pre));   // :25-30
@@ -364,7 +474,9 @@ struct SlamCtx {
   b2s_handle* h; b2s_submap* sm; b2s_odometry* od; const b2s_cloud* raw; double min_fitness; int ignore_fitness;
 };
 
-// odometry, the prediction from its buffer, then the mapper chain (S1 -> S2 -> gates -> [carving] -> F1 -> [dense map]) and t_last
+// odometry, the prediction from its buffer, then the mapper chain (S1 -> S2 -> gates -> [carving] -> F1 -> [dense map]), the mapper's
+// pose buffer and t_last.  With de-skew enabled the mapper chain works on the scan de-skewed from the mapper's buffer
+// (SlamWrapper.cpp:298-304): it is the raw scan of pre-processing, ICP, carving and the dense map
 static int32_t slam_chain(void* ctx) {
   const SlamCtx& c = *static_cast<const SlamCtx*>(ctx);
   b2s_handle* h = c.h;
@@ -374,14 +486,20 @@ static int32_t slam_chain(void* ctx) {
   OdoState* s = od->state.as<OdoState>();
   double* pose_state = sm->pose.as<double>();
   b2s_result* mres = od->res.as<b2s_result>() + 1;
+  const b2s_cloud* raw = c.raw;
+  if (od->mc.enabled) {
+    B2S_TRY(deskew(h, od, raw, true, od->map_in.get()));
+    raw = od->map_in.get();
+  }
   launch_pdl(odometry_prediction_kernel, 1, 32, 0, h->stream, s, od->ring_t.as<long long>(), od->ring_T.as<double>(), od->params.buffer_size,
              pose_state);
   h->launches++;
-  B2S_TRY(process_scan_impl(h, c.raw, h->t1.get(), h->t2.get()));                                                 // Mapper.cpp:139
+  B2S_TRY(process_scan_impl(h, raw, h->t1.get(), h->t2.get()));                                                   // Mapper.cpp:139
   B2S_TRY(register_to_submap_async(h, h->t2.get(), sm, nullptr, pose_state, nullptr, pose_state + 48, mres));   // Mapper.cpp:140-141
-  B2S_TRY(mapper_chain_tail(h, sm, c.raw, h->t1.get(), mres, c.min_fitness, c.ignore_fitness, nullptr, nullptr));   // Mapper.cpp:151-177
+  B2S_TRY(mapper_chain_tail(h, sm, raw, h->t1.get(), mres, c.min_fitness, c.ignore_fitness, nullptr, nullptr));   // Mapper.cpp:151-177
   launch_pdl(slam_post_kernel, 1, 32, 0, h->stream, s, sm->mstate.as<int32_t>(), mres, od->odo_slots.as<b2s_odometry_result>(),
-             od->slam_slots.as<b2s_slam_result>());
+             od->slam_slots.as<b2s_slam_result>(), static_cast<const double*>(pose_state), od->map_t.as<long long>(), od->map_T.as<double>(),
+             od->params.buffer_size);
   h->launches++;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;
@@ -390,6 +508,19 @@ static int32_t slam_chain(void* ctx) {
 static int32_t check_raw(const b2s_odometry* od, const b2s_cloud* raw) {
   B2S_REQUIRE(raw->h == od->h, B2S_E_INVALID, "the scan belongs to another handle");
   B2S_REQUIRE(raw->n_max <= od->capacity, B2S_E_CAPACITY, "scan of up to %zu points, the odometry holds %zu", raw->n_max, od->capacity);
+  return B2S_OK;
+}
+
+// getTransform(t) / has(t) of the odometry's buffer or the mapper's; the caller holds the lock
+static int32_t buffer_lookup(b2s_handle* h, const b2s_odometry* od, bool map, long long t, double T[16], int32_t* has) {
+  launch_pdl(odometry_lookup_kernel, 1, 32, 0, h->stream, od->state.as<OdoState>(), (map ? od->map_t : od->ring_t).as<long long>(),
+             (map ? od->map_T : od->ring_T).as<double>(), od->params.buffer_size, t, od->lookup.as<double>(), map ? 1 : 0);
+  h->launches++;
+  B2S_CUDA(cudaGetLastError());
+  double v[17];
+  B2S_TRY(read_back(h, {{v, od->lookup.p, sizeof(v)}}));
+  memcpy(T, v, 128);
+  if (has) *has = v[16] != 0.0;
   return B2S_OK;
 }
 
@@ -431,6 +562,9 @@ int32_t b2s_odometry_create(b2s_handle* h, const b2s_odometry_params* p, size_t 
     B2S_TRY(pose_to_device(h, I, od->state.as<OdoState>()->cum));
     B2S_TRY(od->ring_t.ensure((size_t)p->buffer_size * 8, h->stream));
     B2S_TRY(od->ring_T.ensure((size_t)p->buffer_size * 128, h->stream));
+    B2S_TRY(od->map_t.ensure((size_t)p->buffer_size * 8, h->stream));
+    B2S_TRY(od->map_T.ensure((size_t)p->buffer_size * 128, h->stream));
+    b2s_default_motion_compensation_params(&od->mc);
     B2S_TRY(od->res.ensure(2 * sizeof(b2s_result), h->stream));
     B2S_CUDA(cudaMemsetAsync(od->res.p, 0, 2 * sizeof(b2s_result), h->stream));
     B2S_TRY(od->odo_slots.ensure(256 * sizeof(b2s_odometry_result), h->stream));
@@ -491,15 +625,7 @@ int32_t b2s_odometry_lookup(b2s_handle* h, const b2s_odometry* od, int64_t t, do
   B2S_REQUIRE(h && od && T, B2S_E_INVALID, "null argument");
   B2S_REQUIRE(od->h == h, B2S_E_INVALID, "the odometry belongs to another handle");
   LOCK(h);
-  launch_pdl(odometry_lookup_kernel, 1, 32, 0, h->stream, od->state.as<OdoState>(), od->ring_t.as<long long>(), od->ring_T.as<double>(),
-             od->params.buffer_size, (long long)t, od->lookup.as<double>());
-  h->launches++;
-  B2S_CUDA(cudaGetLastError());
-  double v[17];
-  B2S_TRY(read_back(h, {{v, od->lookup.p, sizeof(v)}}));
-  memcpy(T, v, 128);
-  if (has) *has = v[16] != 0.0;
-  return B2S_OK;
+  return buffer_lookup(h, od, false, t, T, has);
 }
 
 int32_t b2s_odometry_preprocessed(b2s_handle* h, const b2s_odometry* od, b2s_cloud* out) {
@@ -574,6 +700,78 @@ int32_t b2s_slam_graph_enable(b2s_handle* h, b2s_odometry* od, size_t raw_capaci
               od->staging->fixed_cap);
   od->graph_mode = true;
   *staging_out = od->staging.get();
+  return B2S_OK;
+}
+
+void b2s_default_motion_compensation_params(b2s_motion_compensation_params* p) {
+  memset(p, 0, sizeof(*p));
+  p->enabled = 0;
+  p->spinning_clockwise = 1;
+  p->scan_duration = 0.1;
+  p->num_poses_velocity_estimation = 3;
+}
+
+int32_t b2s_odometry_set_motion_compensation(b2s_handle* h, b2s_odometry* od, const b2s_motion_compensation_params* p) {
+  B2S_REQUIRE(h && od && p, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(od->h == h, B2S_E_INVALID, "the odometry belongs to another handle");
+  B2S_REQUIRE(p->scan_duration > 0.0, B2S_E_INVALID, "lidar scanDuration_: must be > 0");   // assert_gt at MotionCompensation.cpp:61
+  B2S_REQUIRE(p->num_poses_velocity_estimation >= 1, B2S_E_INVALID, "num_poses_velocity_estimation must be >= 1");
+  LOCK(h);
+  if (p->enabled && !od->odo_in) {
+    std::unique_ptr<b2s_cloud> a, b;
+    B2S_TRY(make_cloud(h, od->capacity, false, false, &a));
+    B2S_TRY(make_cloud(h, od->capacity, false, false, &b));
+    B2S_TRY(od->motion.ensure(256 * sizeof(b2s_motion_compensation_result), h->stream));
+    B2S_CUDA(cudaMemsetAsync(od->motion.p, 0, 256 * sizeof(b2s_motion_compensation_result), h->stream));
+    od->odo_in = std::move(a);
+    od->map_in = std::move(b);
+  }
+  od->mc = *p;
+  od->params_gen++;   // the captured combined graphs bake the parameters in
+  return B2S_OK;
+}
+
+int32_t b2s_slam_map_pose_push(b2s_handle* h, b2s_odometry* od, int64_t t, const double T[16]) {
+  B2S_REQUIRE(h && od && T, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(od->h == h, B2S_E_INVALID, "the odometry belongs to another handle");
+  LOCK(h);
+  Mat16 m;
+  memcpy(m.v, T, sizeof(m.v));
+  launch_pdl(map_pose_push_kernel, 1, 32, 0, h->stream, od->state.as<OdoState>(), od->map_t.as<long long>(), od->map_T.as<double>(),
+             od->params.buffer_size, (long long)t, m);
+  h->launches++;
+  B2S_CUDA(cudaGetLastError());
+  return B2S_OK;
+}
+
+int32_t b2s_slam_map_lookup(b2s_handle* h, const b2s_odometry* od, int64_t t, double T[16], int32_t* has) {
+  B2S_REQUIRE(h && od && T, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(od->h == h, B2S_E_INVALID, "the odometry belongs to another handle");
+  LOCK(h);
+  return buffer_lookup(h, od, true, t, T, has);
+}
+
+int32_t b2s_slam_motion_fetch(b2s_handle* h, b2s_odometry* od, int32_t slot, b2s_motion_compensation_result* out) {
+  B2S_REQUIRE(h && od && out && slot >= 0 && slot < 256, B2S_E_INVALID, "bad argument");
+  B2S_REQUIRE(od->h == h, B2S_E_INVALID, "the odometry belongs to another handle");
+  LOCK(h);   // b2s_odometry_set_motion_compensation allocates the records under the lock
+  B2S_REQUIRE(od->motion.p, B2S_E_INVALID, "motion compensation was never enabled on this odometry");
+  return read_back(h, {{out, od->motion.as<b2s_motion_compensation_result>() + slot, sizeof(b2s_motion_compensation_result)}});
+}
+
+int32_t b2s_slam_undistorted(b2s_handle* h, const b2s_odometry* od, b2s_cloud* odo_out, b2s_cloud* map_out) {
+  B2S_REQUIRE(h && od, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(od->h == h && (!odo_out || odo_out->h == h) && (!map_out || map_out->h == h), B2S_E_INVALID,
+              "the odometry or a cloud belongs to another handle");
+  LOCK(h);
+  B2S_REQUIRE(od->odo_in, B2S_E_INVALID, "motion compensation was never enabled on this odometry");
+  const b2s_cloud* src[2] = {od->odo_in.get(), od->map_in.get()};
+  b2s_cloud* dst[2] = {odo_out, map_out};
+  for (int i = 0; i < 2; i++) {
+    if (!dst[i]) continue;
+    B2S_TRY(op_voxel_down_sample(h, src[i], nullptr, 0.0, dst[i]));   // voxel <= 0: plain device copy
+    dst[i]->n_known = -1;   // a replayed graph updates only the device count: the host-side one may be that of the captured step
+  }
   return B2S_OK;
 }
 

@@ -910,6 +910,35 @@ class OdometryParameters:
         return p
 
 
+@dataclass
+class ConstantVelocityMotionCompensationParameters:
+    """include/open3d_slam/Parameters.hpp:192-197; defaults = parameter_structure_definitions.lua:33-36 (de-skew off)"""
+    isUndistortInputCloud: bool = False      # motion_compensation.is_undistort_scan
+    isSpinningClockwise: bool = True
+    scanDuration: float = 0.1                # seconds
+    numPosesVelocityEstimation: int = 3
+
+    def to_c(self) -> L.MotionCompensationParams:
+        p = L.MotionCompensationParams()
+        L.lib().b2s_default_motion_compensation_params(C.byref(p))
+        p.enabled = int(bool(self.isUndistortInputCloud))
+        p.spinning_clockwise = int(bool(self.isSpinningClockwise))
+        p.scan_duration = float(self.scanDuration)
+        p.num_poses_velocity_estimation = int(self.numPosesVelocityEstimation)
+        return p
+
+
+@dataclass
+class MotionCompensationStepResult:
+    """b2s_motion_compensation_result: the velocities each de-skew of a step used and whether they moved the points"""
+    odometryLinearVelocity: np.ndarray
+    odometryAngularVelocityRpy: np.ndarray
+    mapLinearVelocity: np.ndarray
+    mapAngularVelocityRpy: np.ndarray
+    odometryApplied: bool
+    mapApplied: bool
+
+
 class LidarOdometry:
     """src/Odometry.cpp:19-79 -- scan-to-scan odometry: preprocess = crop -> voxelize -> estimateNormalsOrCovariancesIfNeeded ->
     RandomDownSample; addRangeScan registers the PREVIOUS pre-processed cloud (source) against the new one (target) from Identity
@@ -1056,6 +1085,39 @@ class DeviceLidarOdometry:
         r = L.SlamResult()
         L.check(L.lib().b2s_slam_result_fetch(self.eng._h, self._o, C.c_int32(slot), C.byref(r)))
         return _slam_res(r)
+
+    # -- motion compensation (de-skew) of both inputs of a step, SlamWrapper.cpp:195-200,266-268,298-304
+    def setMotionCompensation(self, params: ConstantVelocityMotionCompensationParameters):
+        p = params.to_c()
+        L.check(L.lib().b2s_odometry_set_motion_compensation(self.eng._h, self._o, C.byref(p)))
+
+    def pushMapToRangeSensor(self, t: int, T):
+        """mapToRangeSensorBuffer_.push(t, T) (Mapper.cpp:112,145); the combined step pushes every accepted scan itself"""
+        M = _mat(T)
+        L.check(L.lib().b2s_slam_map_pose_push(self.eng._h, self._o, C.c_int64(int(t)), _pd(M)))
+
+    def _map_lookup(self, t: int):
+        T = np.zeros(16, dtype=np.float64)
+        has = C.c_int32()
+        L.check(L.lib().b2s_slam_map_lookup(self.eng._h, self._o, C.c_int64(int(t)), _pd(T), C.byref(has)))
+        return T.reshape(4, 4), bool(has.value)
+
+    def getMapToRangeSensor(self, t: int) -> np.ndarray:
+        """Mapper::getMapToRangeSensor(t) = getTransform(t, mapToRangeSensorBuffer_)"""
+        return self._map_lookup(t)[0]
+
+    def fetchMotionCompensation(self, slot: int = 0) -> MotionCompensationStepResult:
+        r = L.MotionCompensationResult()
+        L.check(L.lib().b2s_slam_motion_fetch(self.eng._h, self._o, C.c_int32(slot), C.byref(r)))
+        v = lambda a: np.array(a, dtype=np.float64)   # noqa: E731
+        return MotionCompensationStepResult(v(r.odometry_linear_velocity), v(r.odometry_angular_velocity_rpy), v(r.map_linear_velocity),
+                                            v(r.map_angular_velocity_rpy), bool(r.odometry_applied), bool(r.map_applied))
+
+    def undistortedScans(self) -> tuple[Cloud, Cloud]:
+        """device copies of the last step's de-skewed odometry input and mapper input"""
+        a, b = Cloud(self.eng), Cloud(self.eng)
+        L.check(L.lib().b2s_slam_undistorted(self.eng._h, self._o, a._c, b._c))
+        return a, b
 
     def free(self):
         if getattr(self, "_o", None) and self._o.value:

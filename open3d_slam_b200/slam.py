@@ -352,9 +352,10 @@ class DeviceBackend:
 
     def __init__(self, params: E.MapperParameters | None = None, device: int = 0, cuda_stream: int | None = None, submap_capacity: int = 900_000,
                  carving: bool = True, dense: bool = True, graph: bool = True, raw_capacity: int = 65536,
-                 odometry: E.OdometryParameters | None = None):
+                 odometry: E.OdometryParameters | None = None, motionCompensation: E.ConstantVelocityMotionCompensationParameters | None = None):
         self.params = params or E.MapperParameters()
         self.odometry_params = odometry or E.OdometryParameters()   # the device odometry of SegmentMapper.addRangeScan
+        self.motion_compensation = motionCompensation                # de-skew of both inputs of SegmentMapper.addRangeScan (None: off)
         self._odo = None
         self.eng = E.Engine(self.params, device=device, cuda_stream=cuda_stream)
         self.mapper = E.Mapper(self.eng, 1024)     # its own first submap is a placeholder: submaps are created by new_submap()
@@ -413,6 +414,8 @@ class DeviceBackend:
         if self._odo is None:
             import torch
             self._odo = E.DeviceLidarOdometry(self.eng, self.odometry_params, self.raw_capacity)
+            if self.motion_compensation is not None:
+                self._odo.setMotionCompensation(self.motion_compensation)
             if self.graph:
                 self._odo.enableGraph(self.raw_capacity)
             self._slam_pin = torch.empty(C.sizeof(L.SlamResult), dtype=torch.uint8).pin_memory()
@@ -420,10 +423,13 @@ class DeviceBackend:
         return self._odo
 
     def first_scan_with_odometry(self, sm, raw: np.ndarray, t: int):
-        """Mapper.cpp:109-112 for the map and LidarOdometry::addRangeScan for the odometry, on the same scan and timestamp"""
+        """Mapper.cpp:109-112 for the map, with mapToRangeSensorBuffer_.push(t, mapToRangeSensor_ = I), and LidarOdometry::addRangeScan
+        for the odometry, on the same scan and timestamp.  Both buffers are empty here, so a de-skew would leave the scan as it is."""
         merge = self.first_scan(sm, raw)
         c = self.eng.cloud(np.ascontiguousarray(raw, dtype=np.float32))
-        self.odometry().addRangeScan(c, t)
+        odo = self.odometry()
+        odo.addRangeScan(c, t)
+        odo.pushMapToRangeSensor(t, np.eye(4))
         c.free()
         return merge
 

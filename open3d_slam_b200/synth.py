@@ -77,6 +77,17 @@ def lidar_scan(scene: Scene, pose: np.ndarray, n_beams=64, n_az=1024, max_range=
     dl = _ray_dirs(n_beams, n_az)
     R = pose[:3, :3]; o = pose[:3, 3]
     d = dl @ R.T
+    t_best = _hit_distances(scene, d, o)
+    hit = np.isfinite(t_best) & (t_best <= max_range)
+    rng = np.random.default_rng(seed)
+    rr = t_best[hit] + (rng.normal(0.0, noise, size=int(hit.sum())) if noise > 0 else 0.0)
+    pts = dl[hit] * rr[:, None]
+    return np.ascontiguousarray(pts.astype(dtype))
+
+
+def _hit_distances(scene: Scene, d: np.ndarray, o) -> np.ndarray:
+    """distance along every map-frame ray direction d[i] to the first surface (inf: none); o = the rays' origin, (x, y, z) as
+    scalars (one sensor pose) or as per-ray arrays (lidar_cast_moving): the arithmetic per ray is the same either way"""
     t_best = np.full(len(d), np.inf)
     # ground
     with np.errstate(divide="ignore", invalid="ignore"):
@@ -109,11 +120,7 @@ def lidar_scan(scene: Scene, pose: np.ndarray, n_beams=64, n_az=1024, max_range=
         hz = o[2] + t * d[:, 2]
         ok = np.isfinite(t) & (t > 0) & (hz >= scene.ground_z) & (hz <= scene.ground_z + scene.wall_h)
         t_best = np.minimum(t_best, np.where(ok, t, np.inf))
-    hit = np.isfinite(t_best) & (t_best <= max_range)
-    rng = np.random.default_rng(seed)
-    rr = t_best[hit] + (rng.normal(0.0, noise, size=int(hit.sum())) if noise > 0 else 0.0)
-    pts = dl[hit] * rr[:, None]
-    return np.ascontiguousarray(pts.astype(dtype))
+    return t_best
 
 
 def _loop_path(half=8.0, corner_r=3.0):
@@ -156,6 +163,35 @@ def loop_trajectory(n_scans=600, step=0.5, half=8.0, corner_r=3.0, z=0.0):
 def lidar_cast(scene: Scene, pose: np.ndarray, n_beams=64, n_az=1024, max_range=60.0):
     """Noise-free part of lidar_scan(): returns (unit directions in the sensor frame of the rays that hit, ranges)."""
     clean = lidar_scan(scene, pose, n_beams, n_az, max_range, noise=0.0, seed=0, dtype=np.float64)
+    r = np.linalg.norm(clean, axis=1)
+    return clean / r[:, None], r
+
+
+def scan_phase(az: np.ndarray, clockwise: bool = True) -> np.ndarray:
+    """ConstantVelocityMotionCompensation::computePhase (core/src/MotionCompensation.cpp:120-139) of azimuths in [0, 2 pi): the fraction
+    of the scan period after the scan's timestamp at which that azimuth is measured; 0 at az = 0"""
+    az = np.asarray(az, dtype=np.float64)
+    ph = 1.0 - az / (2 * np.pi) if clockwise else az / (2 * np.pi)
+    return np.where(az == 0.0, 0.0, ph)
+
+
+def lidar_cast_moving(scene: Scene, pose_at, n_beams=64, n_az=1024, max_range=60.0, clockwise=True):
+    """Rolling-shutter lidar_cast(): azimuth column j is cast from its own pose pose_at(phase_j) (map -> sensor), phase_j =
+    scan_phase(2 pi j / n_az).  Every return is expressed in the sensor frame of its own column, as a spinning sensor reports it.
+    Returns (unit directions, ranges) of the rays that hit, in lidar_cast's order; lidar_from_cast adds the noise.  With a constant
+    pose_at this is lidar_cast exactly."""
+    dl = _ray_dirs(n_beams, n_az)
+    az = np.linspace(0.0, 2 * np.pi, n_az, endpoint=False)
+    phases = scan_phase(az, clockwise)
+    d = np.empty_like(dl)
+    o = np.empty_like(dl)
+    for j, ph in enumerate(phases):          # rows of column j: beam * n_az + j
+        P = np.asarray(pose_at(float(ph)), dtype=np.float64)
+        d[j::n_az] = dl[j::n_az] @ P[:3, :3].T
+        o[j::n_az] = P[:3, 3]
+    t_best = _hit_distances(scene, d, (o[:, 0], o[:, 1], o[:, 2]))
+    hit = np.isfinite(t_best) & (t_best <= max_range)
+    clean = dl[hit] * (t_best[hit] + 0.0)[:, None]
     r = np.linalg.norm(clean, axis=1)
     return clean / r[:, None], r
 

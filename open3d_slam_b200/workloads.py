@@ -28,6 +28,7 @@ class ClosedLoop:
         self.poses = synth.loop_trajectory(self.L, step=self.step)
         self.noise = noise
         self._casts = {}
+        self._casts_moving = {}
         rng = np.random.default_rng(odom_seed)
         self._pert = [synth.se3(0.0, 0.0, rng.normal(0, 2e-3), rng.normal(0, 0.02, 3)) for _ in range(self.L)]   # stands in for the odometry error
 
@@ -43,6 +44,29 @@ class ClosedLoop:
     def scan(self, k: int, seed: int) -> np.ndarray:
         """float32 sensor-frame scan of lap position k % L with the noise realisation `seed`"""
         return synth.lidar_from_cast(self.cast(k), self.noise, seed=seed)
+
+    def pose_between(self, k: int, phase: float) -> np.ndarray:
+        """the sensor pose a fraction `phase` of the way from pose(k) to pose(k + 1): translation linear, yaw slerped (the loop is
+        planar, so the slerp of two yaw rotations is the yaw rotation by the interpolated angle)"""
+        A, B = self.pose(k), self.pose(k + 1)
+        if phase == 0.0:
+            return A.copy()
+        ya, yb = np.arctan2(A[1, 0], A[0, 0]), np.arctan2(B[1, 0], B[0, 0])
+        dy = (yb - ya + np.pi) % (2 * np.pi) - np.pi
+        return synth.se3(0.0, 0.0, ya + phase * dy, A[:3, 3] + phase * (B[:3, 3] - A[:3, 3]))
+
+    def cast_moving(self, k: int, clockwise: bool = True):
+        """rolling-shutter cast of scan k: the sensor moves from pose(k) to pose(k + 1) during the scan (one scan period = one
+        scan_duration), each azimuth column is measured at its computePhase"""
+        key = (k % self.L, bool(clockwise))
+        if key not in self._casts_moving:
+            self._casts_moving[key] = synth.lidar_cast_moving(self.scene, lambda ph: self.pose_between(k, ph), clockwise=clockwise)
+        return self._casts_moving[key]
+
+    def scan_moving(self, k: int, seed: int, clockwise: bool = True) -> np.ndarray:
+        """float32 scan of lap position k taken while moving on to k + 1 (noise realisation `seed`); its timestamp's ground truth
+        stays pose(k)"""
+        return synth.lidar_from_cast(self.cast_moving(k, clockwise), self.noise, seed=seed)
 
     def delta(self, k: int) -> np.ndarray:
         """odometry motion between scan k-1 and scan k (identity for k = 0)"""
