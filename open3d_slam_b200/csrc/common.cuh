@@ -612,7 +612,11 @@ static __device__ void svd3_dev(const double* A, double* U, double* S, double* V
     const double nv = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
     U[1] = v[0] / nv; U[4] = v[1] / nv; U[7] = v[2] / nv;
   }
-  if (!(S[2] > tiny)) { U[2] = U[3] * U[7] - U[6] * U[4]; U[5] = U[6] * U[1] - U[0] * U[7]; U[8] = U[0] * U[4] - U[3] * U[1]; }
+  // u2 = u0 x u1 also when the third column is rounding noise that is not orthogonal to the others: an exactly zero row of A keeps
+  // every column of W in a plane, so W's third column can never become orthogonal to the first two (rank-2 sets such as a level
+  // plane of points)
+  const double c[3] = {U[3] * U[7] - U[6] * U[4], U[6] * U[1] - U[0] * U[7], U[0] * U[4] - U[3] * U[1]};
+  if (!(fabs(c[0] * U[2] + c[1] * U[5] + c[2] * U[8]) > 0.5)) { U[2] = c[0]; U[5] = c[1]; U[8] = c[2]; }
 }
 
 __device__ __forceinline__ double det3_dev(const double* M) {

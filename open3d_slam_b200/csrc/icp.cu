@@ -451,15 +451,20 @@ __device__ __forceinline__ double warp_sum32_transposed(F val, int lane) {
   return (up ? d[1] : d[0]) + __shfl_xor_sync(FULL, up ? d[0] : d[1], 1);
 }
 
-// point-to-point ([O3D] TransformationEstimationPointToPoint = Eigen::umeyama): sums for the means and the cross moments
-//   acc[0..2] = sum source, acc[3..5] = sum target, acc[6 + 3a + b] = sum target_a * source_b
+// point-to-point ([O3D] TransformationEstimationPointToPoint = Eigen::umeyama): sums for the means and the cross moments, every
+// coordinate taken relative to a reference point c known before the pass (the centre of the target grid's box, in shared memory).
+// Raw moments E[t s^T] - mt ms^T cancel catastrophically far from the origin (a cloud 1e4 m out loses ~8 digits of the covariance);
+// moments about a point inside the target's box cancel only at the scale of the clouds' spread.
+//   acc[0..2] = sum (source - c), acc[3..5] = sum (target - c), acc[6 + 3a + b] = sum (target - c)_a * (source - c)_b
 template <bool LANE0>
-__device__ __forceinline__ void icp_contribute_p2p(double* wacc, const GridView& g, int slot, double px, double py, double pz, int lane) {
+__device__ __forceinline__ void icp_contribute_p2p(double* wacc, const GridView& g, const double* c, int slot, double px, double py, double pz,
+                                                   int lane) {
   const bool ok = slot >= 0;
   double4 q = make_double4(0, 0, 0, 0);
   if (ok) q = g.pts[slot];
-  if (!ok) { px = 0; py = 0; pz = 0; }
   const double d2 = ok ? dist2_exact(px, py, pz, q.x, q.y, q.z) : 0.0;
+  if (!ok) { px = 0; py = 0; pz = 0; }
+  else { q.x -= c[0]; q.y -= c[1]; q.z -= c[2]; px -= c[0]; py -= c[1]; pz -= c[2]; }
   wadd<LANE0>(wacc, 0, px, lane); wadd<LANE0>(wacc, 1, py, lane); wadd<LANE0>(wacc, 2, pz, lane);
   wadd<LANE0>(wacc, 3, q.x, lane); wadd<LANE0>(wacc, 4, q.y, lane); wadd<LANE0>(wacc, 5, q.z, lane);
   wadd<LANE0>(wacc, 6, q.x * px, lane); wadd<LANE0>(wacc, 7, q.x * py, lane); wadd<LANE0>(wacc, 8, q.x * pz, lane);
@@ -493,13 +498,16 @@ __device__ void info_from_moments(const double* t, double* G) {
     for (int b = 0; b < 6; b++) G[6 * a + b] = M[a][b];
 }
 
-// Eigen::umeyama without scaling from the accumulated moments (tot as filled by icp_contribute_p2p, tot[28] = n)
-__device__ void umeyama_from_moments(const double* tot, double* Upd) {
+// Eigen::umeyama without scaling from the accumulated moments (tot as filled by icp_contribute_p2p about the reference point c,
+// tot[28] = n, c the reference point of the sums): sigma = E[(t - c)(s - c)^T] - (mt - c)(ms - c)^T, the means are c + E[. - c].
+// Not inlined: one thread runs it once per evaluation, and inlined its SVD crowds the registers of the kernel's point loops.
+__device__ __noinline__ void umeyama_from_moments(const double* tot, const double* c, double* Upd) {
   const double one_over_n = 1.0 / tot[28];
   double ms[3], mt[3], sigma[9];
   for (int a = 0; a < 3; a++) { ms[a] = tot[a] * one_over_n; mt[a] = tot[3 + a] * one_over_n; }
   for (int a = 0; a < 3; a++)
     for (int b = 0; b < 3; b++) sigma[3 * a + b] = tot[6 + 3 * a + b] * one_over_n - mt[a] * ms[b];
+  for (int a = 0; a < 3; a++) { ms[a] += c[a]; mt[a] += c[a]; }
   double U[9], S[3], V[9];
   svd3_dev(sigma, U, S, V);
   const double sgn = det3_dev(U) * det3_dev(V) < 0 ? -1.0 : 1.0;
@@ -661,7 +669,7 @@ __global__ void __launch_bounds__(icp_threads(MODE), 1) icp_kernel(const __grid_
   double* s_tot = s_part + 2 * NACC;                    // [NACC]
   double* s_U = s_tot + NACC;                           // [16] update of the current iteration
   double* s_T = s_U + 16;                               // [16] accumulated transformation
-  double* s_misc = s_T + 16;                            // [0] prev fitness [1] prev rmse [2] done [3] apply
+  double* s_misc = s_T + 16;                            // [0] prev fitness [1] prev rmse [2] done [3] apply [4..6] point-to-point reference point
   double* s_A = s_misc + 8;                             // [36 + 6] the 6x6 system of the solve
   GridHeader* s_g = reinterpret_cast<GridHeader*>(smem_raw + icp_fixed_smem_doubles(THREADS) * 8);
   int* s_qn = reinterpret_cast<int*>(s_g + 1);          // phase-2 queue length (16 bytes reserved)
@@ -704,6 +712,7 @@ __global__ void __launch_bounds__(icp_threads(MODE), 1) icp_kernel(const __grid_
     for (int i = 0; i < 16; i++) { s_T[i] = init[i]; s_U[i] = init[i]; }
     s_misc[0] = 0.0; s_misc[1] = 0.0; s_misc[2] = 0.0;
     s_misc[3] = mat4_is_identity_dev(init) ? 0.0 : 1.0;  // [O3D]: if (!init.isIdentity()) pcd.Transform(init)
+    for (int a = 0; a < 3; a++) s_misc[4 + a] = s_g->origin[a] + 0.5 * (double)s_g->dims[a] * s_g->cell;   // centre of the target's box
     s_qn[0] = 0; s_qn[1] = 0;
     if (in_smem) { mbar_init(s_bar, 1); mbar_fence_init(); }
   }
@@ -867,7 +876,7 @@ __global__ void __launch_bounds__(icp_threads(MODE), 1) icp_kernel(const __grid_
         double px = 0.0, py = 0.0, pz = 0.0;
         if (i < cnt) { const int wi = widx(i); slot = prev[wi]; px = work[3 * wi]; py = work[3 * wi + 1]; pz = work[3 * wi + 2]; }   // queued points (<= -2) are phase 2's
         if (GICP) icp_contribute_gicp<false>(wacc, g, slot, px, py, pz, RT, P.src_nrm + 3 * (size_t)gidx_of(i < cnt ? i : 0, (int)crank), P.gicp_eps, lane);
-        else if (p2p) icp_contribute_p2p<false>(wacc, g, slot, px, py, pz, lane);
+        else if (p2p) icp_contribute_p2p<false>(wacc, g, s_misc + 4, slot, px, py, pz, lane);
         else if (info) icp_contribute_info<false>(wacc, g, slot, px, py, pz, lane);
         else icp_contribute_plane<false>(wacc, g, slot, px, py, pz, lane);
       }
@@ -924,7 +933,7 @@ __global__ void __launch_bounds__(icp_threads(MODE), 1) icp_kernel(const __grid_
           rp[i] = st.bslot;
           if (st.bslot >= 0) {
             if (GICP) icp_contribute_gicp<true>(wacc, g, st.bslot, px, py, pz, RT, P.src_nrm + 3 * (size_t)gidx_of(i, r), P.gicp_eps, 0);
-            else if (p2p) icp_contribute_p2p<true>(wacc, g, st.bslot, px, py, pz, 0);
+            else if (p2p) icp_contribute_p2p<true>(wacc, g, s_misc + 4, st.bslot, px, py, pz, 0);
             else if (info) icp_contribute_info<true>(wacc, g, st.bslot, px, py, pz, 0);
             else icp_contribute_plane<true>(wacc, g, st.bslot, px, py, pz, 0);
           }
@@ -985,7 +994,7 @@ __global__ void __launch_bounds__(icp_threads(MODE), 1) icp_kernel(const __grid_
       if (!done) {
         double Upd[16];
         if (c > 0.0 && p2p) {
-          umeyama_from_moments(s_tot, Upd);
+          umeyama_from_moments(s_tot, s_misc + 4, Upd);
         } else if (c > 0.0) {
           double x[6];
           {
