@@ -16,6 +16,7 @@ int orc_kdtree_search_hybrid(void* t, const double* q, double radius, int max_nn
 void orc_svd3(const double* A, double* U, double* S, double* V);
 
 #define MAX_N 8
+#define SUM_LANES 256   /* rule 6: the validation's sum d2 is reduced over this many strided partials (RV_THREADS of ransac.cu) */
 
 /* rule 1: exact argmin both ways, d2 summed over k ascending, ties to the lower index; -1 when the other side is empty */
 void or_feature_corr(const double* fs, int ns, const double* ft, int nt, int* s2t, int* t2s) {
@@ -118,14 +119,17 @@ void or_ransac(const double* sx, const double* sf, int ns, const double* tx, con
       if (norm3(Q[j][0] - p[0], Q[j][1] - p[1], Q[j][2] - p[2]) > checker_dist) ok = 0;
     }
     if (!ok) continue;
-    /* rule 6 */
+    /* rule 6: sum d2 in its fixed order, SUM_LANES strided partials in ascending i, then the halving tree */
     validations++;
-    int inl = 0; double sum = 0.0;
+    int inl = 0;
+    double part[SUM_LANES] = {0};
     for (int i = 0; i < ns; i++) {
       double q[3], d2; int idx;
       xform(T, sx + 3 * (size_t)i, q);
-      if (orc_kdtree_search_hybrid(tree, q, max_corr, 1, &d2, &idx) > 0) { inl++; sum += d2; }
+      if (orc_kdtree_search_hybrid(tree, q, max_corr, 1, &d2, &idx) > 0) { inl++; part[i % SUM_LANES] += d2; }
     }
+    for (int o = SUM_LANES / 2; o > 0; o >>= 1) for (int t = 0; t < o; t++) part[t] += part[t + o];
+    const double sum = part[0];
     /* rule 7 */
     if (inl > 0 && (inl > best_inl || (inl == best_inl && sum < best_sum))) {
       best_inl = inl; best_sum = sum; best_h = h; memcpy(best_T, T, sizeof(T));

@@ -149,6 +149,23 @@ def _umeyama(S, Q):
     return T
 
 
+SUM_LANES = 256
+
+
+def fixed_order_sum(v):
+    """rule 6's order of the validation's sum d2: point i goes into partial i mod 256 in ascending i, then partial t += partial t + o
+    for o = 128, 64, ..., 1 (adding the 0.0 of a point that is no inlier changes no partial)"""
+    part = np.zeros(SUM_LANES)
+    for k in range(0, len(v), SUM_LANES):
+        seg = v[k:k + SUM_LANES]
+        part[:len(seg)] = part[:len(seg)] + seg
+    o = SUM_LANES // 2
+    while o:
+        part[:o] = part[:o] + part[o:2 * o]
+        o //= 2
+    return float(part[0])
+
+
 def np_ransac(sx, sf, tx, tf, p: Params) -> Result:
     sx = np.asarray(sx, dtype=np.float64).reshape(-1, 3); tx = np.asarray(tx, dtype=np.float64).reshape(-1, 3)
     ns, nt, n = len(sx), len(tx), p.ransac_n
@@ -183,9 +200,7 @@ def np_ransac(sx, sf, tx, tf, p: Params) -> Result:
             dmin = d.min(axis=1)
             hit = dmin < r2
             inl = int(hit.sum())
-            s = 0.0
-            for v in dmin[hit]:                 # sequential, in point order
-                s += float(v)
+            s = fixed_order_sum(np.where(hit, dmin, 0.0))
             if inl > 0 and (inl > best[0] or (inl == best[0] and s < best[1])):
                 fitness = inl / ns
                 with np.errstate(divide="ignore"):      # fitness 1: log(0) = -inf, k_d = -0 (as in C)
