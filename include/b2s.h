@@ -557,6 +557,49 @@ int32_t b2s_ransac_feature_matching(b2s_handle* h, const b2s_cloud* source_spars
 int32_t b2s_feature_correspondences(b2s_handle* h, const b2s_feature* source_feature, const b2s_feature* target_feature, int32_t* src_to_tgt,
                                     size_t src_capacity, int32_t* tgt_to_src, size_t tgt_capacity);
 
+/* ---- odometry constraints between consecutive submaps: buildOdometryConstraint -> buildConstraint (src/constraint_builders.cpp:33-90),
+ *      as SubmapCollection::computeFeatures (src/SubmapCollection.cpp:238) and SlamWrapper::loopClosureWorker (src/SlamWrapper.cpp:427-428)
+ *      reach it through computeOdometryConstraints (src/constraint_builders.cpp:92-118).  For every pair k, on the maps where they live:
+ *   - source = sources[k] is the PARENT, target = targets[k] the CHILD: buildOdometryConstraint(parent, child)            :33, :100-102
+ *   - both clouds are the WHOLE map, getMapPointCloudCopy (the live map slots in map order), no cropper                   :46-47
+ *   - voxel = getMapVoxelSize(map_voxel_size, voxel_if_zero): |v| <= 1e-3 -> voxel_if_zero, else v (a negative v passes
+ *     through, as it does in the reference)                                                                              helpers.cpp:343-345
+ *   - overlap at the IDENTITY with edge overlap_factor x voxel and minNumPointsPerVoxel = min_points_per_voxel: the points of
+ *     either map whose voxel holds points of both, each map's survivors in map order (b2s_overlap's rule)               :51-58
+ *   - refine != 0 only: RegistrationICP(sourceOverlap, targetOverlap, r = icp_factor x voxel, Identity,
+ *     TransformationEstimationPointToPlane, max_iter / rel_fitness / rel_rmse) -- ALWAYS point-to-plane, whatever
+ *     b2s_config.icp.reg_type is: the reference calls raw [O3D] RegistrationICP here, not the mapper's cloudRegistration    :62-68
+ *   - the information matrix is always estimated: GetInformationMatrixFromPointClouds(sourceOverlap, targetOverlap, r, T) with
+ *     T = the ICP result, or the identity without refinement ([O3D]'s no-transform branch, as b2s_information_matrix)    :69-73
+ *   - sourceToTarget_ = T (identity unless refined); isOdometryConstraint_ = isInformationMatrixValid_ = true            :75-82
+ * Errors: a submap or an overlap cloud of another handle, a voxel <= 0 after the getMapVoxelSize rule, overlap_factor or icp_factor
+ * <= 0, min_points_per_voxel < 1, max_iter < 0, n_pairs < 0 -> B2S_E_INVALID; refine != 0 and a child map without normals (a
+ * point-to-point map, stored as NaN) -> B2S_E_NO_NORMALS.  n_pairs = 0 -> B2S_OK.  One call runs every pair in one set of launches
+ * and synchronises once.  source_overlaps_or_null / target_overlaps_or_null (each an array of n_pairs clouds, or NULL) receive the
+ * selected points, in map order.  Semantics and kernels: DESIGN.md row L2. */
+typedef struct b2s_odometry_constraint_params {   /* constraint_builders.cpp:33-41, magic.hpp, helpers.cpp:343-345 */
+  double map_voxel_size;          /* map_builder.map_voxel_size (0.1) */
+  double voxel_if_zero;           /* magic::voxelSizeCorrespondenceSearchIfMapVoxelSizeIsZero = 0.04 */
+  double overlap_factor;          /* magic::voxelExpansionFactorOverlapComputation = 20 */
+  double icp_factor;              /* magic::voxelExpansionFactorIcpCorrespondenceDistance = 1.5 */
+  int32_t min_points_per_voxel;   /* 1 */
+  int32_t refine;                 /* is_refine_odometry_constraints_between_submaps (false) */
+  int32_t max_iter;               /* magic::icpRunUntilConvergenceNumberOfIterations = 100 */
+  double rel_fitness, rel_rmse;   /* [O3D] ICPConvergenceCriteria defaults, 1e-6 */
+} b2s_odometry_constraint_params;
+typedef struct b2s_odometry_constraint {
+  double T[16];                   /* sourceToTarget_ (identity unless refined), row-major */
+  double information[36];         /* informationMatrix_, row-major */
+  int64_t n_source_overlap, n_target_overlap;
+  int32_t refined;                /* the ICP ran */
+  b2s_result icp;                 /* its RegistrationResult when refined, zeros otherwise */
+} b2s_odometry_constraint;
+void b2s_default_odometry_constraint_params(b2s_odometry_constraint_params* p);
+int32_t b2s_submap_odometry_constraints(b2s_handle* h, int32_t n_pairs, const b2s_submap* const* sources /* parent */,
+                                        const b2s_submap* const* targets /* child */, const b2s_odometry_constraint_params* p,
+                                        b2s_cloud* const* source_overlaps_or_null, b2s_cloud* const* target_overlaps_or_null,
+                                        b2s_odometry_constraint* out);
+
 /* ---- device-to-device hand-over of a cloud's arrays (SURVEY.md section 8e: a submap that is the registration target on
  *      several GPUs is built once by its owner and broadcast over NVLink by the host side -- torch.distributed / NCCL own
  *      the transfer, this library only copies between its cloud and the caller's device buffers on the handle's stream).

@@ -96,6 +96,17 @@ class MotionCompensationResult(C.Structure):
 ODOM_INIT, ODOM_OK, ODOM_FAILED, ODOM_FAILED_KEPT_PREV = 0, 1, 2, 3
 
 
+class OdometryConstraintParams(C.Structure):
+    _fields_ = [("map_voxel_size", C.c_double), ("voxel_if_zero", C.c_double), ("overlap_factor", C.c_double), ("icp_factor", C.c_double),
+                ("min_points_per_voxel", C.c_int32), ("refine", C.c_int32), ("max_iter", C.c_int32), ("rel_fitness", C.c_double),
+                ("rel_rmse", C.c_double)]
+
+
+class OdometryConstraint(C.Structure):
+    _fields_ = [("T", C.c_double * 16), ("information", C.c_double * 36), ("n_source_overlap", C.c_int64), ("n_target_overlap", C.c_int64),
+                ("refined", C.c_int32), ("icp", Result)]
+
+
 class MapperCounters(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("steps", "accepted", "inserted_map", "inserted_dense", "carve_runs", "carved_points_total",
                                          "dense_carve_runs", "carved_voxels_total")]
@@ -124,6 +135,7 @@ SYMBOLS = [
     "b2s_slam_step_async", "b2s_slam_result_fetch", "b2s_slam_step_host_async", "b2s_slam_graph_enable",
     "b2s_default_motion_compensation_params", "b2s_odometry_set_motion_compensation", "b2s_slam_map_pose_push", "b2s_slam_map_lookup",
     "b2s_slam_motion_fetch", "b2s_slam_undistorted",
+    "b2s_default_odometry_constraint_params", "b2s_submap_odometry_constraints",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 PROFILE_KINDS = ["icp", "normals", "radix_sort", "nn_grid_build", "voxel", "fuse", "select", "crop"]
@@ -170,6 +182,7 @@ def lib():
         L.b2s_odometry_destroy.argtypes = [C.c_void_p]
         L.b2s_default_odometry_params.restype = None
         L.b2s_default_motion_compensation_params.restype = None
+        L.b2s_default_odometry_constraint_params.restype = None
         _lib = L
     return _lib
 

@@ -930,6 +930,7 @@ int32_t b2s_submap_set_cloud(b2s_handle* h, b2s_submap* sm, const b2s_cloud* clo
   }
   B2S_CUDA(cudaMemcpyAsync(m->dn.p, cloud->dn.p, 4, cudaMemcpyDeviceToDevice, h->stream));
   m->n_max = cloud->n_max; m->n_known = cloud->n_known; m->has_normals = true;
+  sm->no_normals = !cloud->has_normals;
   sm->cnt_pending = false; sm->adds_after_readback = 0;
   B2S_CUDA(cudaMemsetAsync(sm->mstate.as<int32_t>() + MS_NDEAD, 0, 4, h->stream));
   return fuse_rehash(h, sm);
@@ -1234,6 +1235,41 @@ int32_t b2s_feature_correspondences(b2s_handle* h, const b2s_feature* src_f, con
   if (src_f->n) B2S_CUDA(cudaMemcpyAsync(s2t, d_s2t, src_f->n * 4, cudaMemcpyDeviceToHost, h->stream));
   if (tgt_f->n) B2S_CUDA(cudaMemcpyAsync(t2s, d_t2s, tgt_f->n * 4, cudaMemcpyDeviceToHost, h->stream));
   return check_status(h);
+}
+
+// ---- odometry constraints (src/constraint_builders.cpp:33-118) ---------------------------------------------------------------
+void b2s_default_odometry_constraint_params(b2s_odometry_constraint_params* p) {   // magic.hpp:12-15, Lua map_builder / mapper defaults
+  memset(p, 0, sizeof(*p));
+  p->map_voxel_size = 0.1; p->voxel_if_zero = 0.04; p->overlap_factor = 20.0; p->icp_factor = 1.5; p->min_points_per_voxel = 1;
+  p->refine = 0; p->max_iter = 100; p->rel_fitness = 1e-6; p->rel_rmse = 1e-6;
+}
+
+int32_t b2s_submap_odometry_constraints(b2s_handle* h, int32_t n, const b2s_submap* const* sources, const b2s_submap* const* targets,
+                                        const b2s_odometry_constraint_params* p, b2s_cloud* const* so, b2s_cloud* const* to,
+                                        b2s_odometry_constraint* out) {
+  B2S_REQUIRE(h && p && n >= 0, B2S_E_INVALID, "bad argument");
+  if (n == 0) return B2S_OK;
+  B2S_REQUIRE(sources && targets && out, B2S_E_INVALID, "null argument");
+  const double voxel = fabs(p->map_voxel_size) <= 1e-3 ? p->voxel_if_zero : p->map_voxel_size;   // getMapVoxelSize, helpers.cpp:343-345
+  B2S_REQUIRE(voxel > 0.0, B2S_E_INVALID, "map voxel size %g after getMapVoxelSize: must be > 0", voxel);
+  B2S_REQUIRE(p->overlap_factor > 0.0 && p->icp_factor > 0.0, B2S_E_INVALID, "overlap_factor and icp_factor must be > 0");
+  B2S_REQUIRE(p->min_points_per_voxel >= 1, B2S_E_INVALID, "minNumPointsPerVoxel must be >= 1");   // assert_ge at helpers.cpp:310
+  B2S_REQUIRE(p->max_iter >= 0, B2S_E_INVALID, "max_iter must be >= 0");
+  for (int32_t k = 0; k < n; k++) {
+    B2S_REQUIRE(sources[k] && targets[k], B2S_E_INVALID, "null submap in pair %d", k);
+    B2S_REQUIRE(sources[k]->h == h && targets[k]->h == h, B2S_E_INVALID, "pair %d: a submap belongs to another handle", k);
+    for (b2s_cloud* const* c : {so, to})
+      if (c) {
+        B2S_REQUIRE(c[k] && c[k]->h == h, B2S_E_INVALID, "pair %d: an overlap cloud is null or belongs to another handle", k);
+        B2S_REQUIRE(!c[k]->fixed_cap, B2S_E_INVALID, "pair %d: an overlap cloud must not be a fixed-capacity staging cloud", k);
+      }
+    B2S_REQUIRE(!so || !to || so[k] != to[k], B2S_E_INVALID, "pair %d: the two overlap clouds are the same object", k);
+  }
+  for (int32_t k = 0; k < n; k++)   // RegistrationICP's point-to-plane estimator needs the target's normals ([O3D] LogError)
+    B2S_REQUIRE(!p->refine || !targets[k]->no_normals, B2S_E_NO_NORMALS,
+                "[RegistrationICP] pair %d: TransformationEstimationPointToPlane requires target normals, the child map has none", k);
+  LOCK(h);
+  return op_odometry_constraints(h, n, sources, targets, *p, voxel, so, to, out);
 }
 
 }  // extern "C"

@@ -218,6 +218,9 @@ struct b2s_submap {
   b2s_mapper_options opts;
   unsigned long long opts_gen = 1;    // bumped by b2s_submap_set_mapper_options: graphs of other objects that run this chain compare it
   b2s::DevBuf mstate;                 // int32 [MS_WORDS]: gates and counters of the chain, see the MS_* indices below
+  // the map has no normals (stored as NaN): loaded without them, or fed a scan without them.  [O3D] PointCloud::operator+= drops a
+  // cloud's normals as soon as one part lacks them, so the reference's map stays without normals from then on, and so does this flag
+  bool no_normals = false;
 };
 
 struct b2s_feature {
@@ -302,6 +305,11 @@ struct b2s_handle {
   b2s::DevBuf batch_jobs;             // GridJob + ScanJob tables and the scan tile states of a batched index build
   std::vector<unsigned char> batch_jobs_host;
   b2s::DevBuf lc;                     // K-ransac scratch (ransac.cu owns its layout)
+  // b2s_submap_odometry_constraints (constraints.cu): the batched overlap's tables and per-slot arrays, K-info-wide's tables / tile
+  // partials / records, their page-locked staging, and the overlap clouds used when the caller passes none
+  b2s::DevBuf odo, odo_info;
+  b2s::PinnedBuf odo_stage;
+  std::vector<std::unique_ptr<b2s_cloud>> odo_clouds;
 };
 
 // every entry point that touches a handle's stream or buffers holds its lock and works on its device
@@ -397,8 +405,10 @@ struct IcpProblem {
 };
 constexpr int EST_INFORMATION = 3;   // internal estimator code: a single evaluation that outputs [O3D]'s information matrix
 constexpr int EST_CORRESPONDENCES = 4;   // a single evaluation whose only output is corr_index / corr_d2 (+ fitness, rmse)
-// single_host != nullptr: one registration, the problem travels as a kernel argument (no copy, no sync)
-int32_t icp_launch(b2s_handle* h, const IcpProblem* single_host, const IcpProblem* problems_dev, int n_problems, size_t max_src_points);
+// single_host != nullptr: one registration, the problem travels as a kernel argument (no copy, no sync).  A batch runs the estimator of
+// the handle's configuration unless batch_estimator >= 0 names one (the odometry constraints are always point-to-plane)
+int32_t icp_launch(b2s_handle* h, const IcpProblem* single_host, const IcpProblem* problems_dev, int n_problems, size_t max_src_points,
+                   int batch_estimator = -1);
 
 int32_t op_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, const double* T_dev, const int32_t* gate_dev);
 // K-fuse bookkeeping (fuse.cu): (re)build the persistent voxel hash from the map cloud (after set_cloud / carving / transform;
@@ -423,6 +433,11 @@ int32_t op_undistort(b2s_handle* h, const b2s_cloud* in, const double* lin_vel, 
 // L1 overlap selection in front of the loop-closure ICP (overlap.cu); T_dev = sourceToTarget (device, row-major)
 int32_t op_overlap(b2s_handle* h, const b2s_cloud* source, const b2s_cloud* target, const double* T_dev, double voxel, int min_pts,
                    b2s_cloud* source_overlap, b2s_cloud* target_overlap);
+// L2 odometry constraints of n (parent, child) submap pairs (constraints.cu); voxel = the map voxel after getMapVoxelSize; so_out /
+// to_out: the caller's overlap clouds or nullptr; out: host records.  Synchronises once.
+int32_t op_odometry_constraints(b2s_handle* h, int n, const b2s_submap* const* sources, const b2s_submap* const* targets,
+                                const b2s_odometry_constraint_params& p, double voxel, b2s_cloud* const* so_out, b2s_cloud* const* to_out,
+                                b2s_odometry_constraint* out);
 // K-fpfh (features.cu): [O3D] ComputeFPFHFeature of the n points of c (normals required, 1 <= knn <= B2S_FEATURE_MAX_KNN)
 int32_t op_compute_fpfh(b2s_handle* h, const b2s_cloud* c, size_t n, double radius, int knn, b2s_feature* f);
 // K-ransac (ransac.cu): exact feature correspondences of one source feature against n target features (device outputs; s2t[k] / t2s[k]

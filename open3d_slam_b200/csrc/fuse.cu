@@ -529,6 +529,7 @@ int32_t op_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, c
   map->n_max = tot_max;   // upper bound only; the exact count lives on the device
   map->n_known = -1;
   map->has_normals = true;
+  if (!scan->has_normals) sm->no_normals = true;
   B2S_CUDA(cudaGetLastError());
   if (!sm->fixed_launch) {
     if (!sm->cnt_ev) {

@@ -1086,7 +1086,8 @@ static cudaError_t icp_set_attrs() {
   return cudaFuncSetAttribute(icp_kernel<MODE>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
 }
 
-int32_t icp_launch(b2s_handle* h, const IcpProblem* single_host, const IcpProblem* problems_dev, int n_problems, size_t max_src_points) {
+int32_t icp_launch(b2s_handle* h, const IcpProblem* single_host, const IcpProblem* problems_dev, int n_problems, size_t max_src_points,
+                   int batch_estimator) {
   if (n_problems <= 0) return B2S_OK;
   IcpProblem single;
   memset(&single, 0, sizeof(single));
@@ -1102,7 +1103,7 @@ int32_t icp_launch(b2s_handle* h, const IcpProblem* single_host, const IcpProble
       g_icp_attr_set[d] = true;
     }
   }
-  const int estimator = single_host ? single_host->estimator : h->cfg.icp.reg_type;   // uniform over a batch
+  const int estimator = single_host ? single_host->estimator : (batch_estimator >= 0 ? batch_estimator : h->cfg.icp.reg_type);   // uniform over a batch
   int csize = 1;
   const int cmax = icp_max_cluster(h);
   long long* const dbg = h->icp_dbg.as<long long>();

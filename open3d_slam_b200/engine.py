@@ -392,6 +392,66 @@ def getInformationMatrixFromPointClouds(eng: Engine, source: Cloud, target: Clou
     return G
 
 
+@dataclass
+class OdometryConstraintParameters:
+    """What buildOdometryConstraint reads (src/constraint_builders.cpp:33-41): the map voxel and the magic constants (magic.hpp:12-15),
+    isRefineOdometryConstraintsBetweenSubmaps_ (default false) and the [O3D] ICPConvergenceCriteria of the refinement."""
+    mapVoxelSize: float = 0.1
+    voxelSizeIfMapVoxelSizeIsZero: float = 0.04                  # magic::voxelSizeCorrespondenceSearchIfMapVoxelSizeIsZero
+    voxelExpansionFactorOverlapComputation: float = 20.0
+    voxelExpansionFactorIcpCorrespondenceDistance: float = 1.5
+    minNumPointsPerVoxel: int = 1
+    isRefineOdometryConstraintsBetweenSubmaps: bool = False
+    maxNumIter: int = 100                                        # magic::icpRunUntilConvergenceNumberOfIterations
+    relativeFitness: float = 1e-6
+    relativeRmse: float = 1e-6
+
+    def to_c(self) -> L.OdometryConstraintParams:
+        return L.OdometryConstraintParams(float(self.mapVoxelSize), float(self.voxelSizeIfMapVoxelSizeIsZero), float(self.voxelExpansionFactorOverlapComputation),
+                                          float(self.voxelExpansionFactorIcpCorrespondenceDistance), int(self.minNumPointsPerVoxel),
+                                          int(self.isRefineOdometryConstraintsBetweenSubmaps), int(self.maxNumIter), float(self.relativeFitness),
+                                          float(self.relativeRmse))
+
+
+def getMapVoxelSize(mapVoxelSize: float, valueIfZero: float) -> float:
+    """src/helpers.cpp:343-345: |v| <= 1e-3 -> valueIfZero, else v (a negative v passes through)."""
+    return valueIfZero if abs(mapVoxelSize) <= 1e-3 else mapVoxelSize
+
+
+@dataclass
+class OdometryConstraintResult:
+    """buildOdometryConstraint's Constraint (sourceToTarget_, informationMatrix_) and the overlap sizes; icp is the refinement's
+    RegistrationResult (None when it did not run)."""
+    sourceToTarget_: np.ndarray
+    informationMatrix_: np.ndarray
+    nSourceOverlap: int
+    nTargetOverlap: int
+    icp: RegistrationResult | None = None
+
+
+def buildOdometryConstraintsBatch(eng: Engine, sources, targets, params: OdometryConstraintParameters | None = None, sourceOverlaps=None,
+                                  targetOverlaps=None) -> list[OdometryConstraintResult]:
+    """buildOdometryConstraint(parent, child) (src/constraint_builders.cpp:33-90) for every pair (sources[k] = parent Submap, targets[k]
+    = child Submap) in one device call on the resident maps.  sourceOverlaps / targetOverlaps (lists of Cloud, optional) receive the
+    overlap selections in map order."""
+    p = (params or OdometryConstraintParameters()).to_c()
+    n = len(sources)
+    assert len(targets) == n
+    arr = lambda objs: (C.c_void_p * max(n, 1))(*objs)
+    so = arr([c._c for c in sourceOverlaps]) if sourceOverlaps is not None else None
+    to = arr([c._c for c in targetOverlaps]) if targetOverlaps is not None else None
+    out = (L.OdometryConstraint * max(n, 1))()
+    L.check(L.lib().b2s_submap_odometry_constraints(eng._h, C.c_int32(n), arr([s._s for s in sources]), arr([t._s for t in targets]), C.byref(p),
+                                                    so, to, out))
+    return [OdometryConstraintResult(np.array(o.T, dtype=np.float64).reshape(4, 4), np.array(o.information, dtype=np.float64).reshape(6, 6),
+                                     int(o.n_source_overlap), int(o.n_target_overlap), _res(o.icp) if o.refined else None) for o in out[:n]]
+
+
+def buildOdometryConstraint(eng: Engine, source, target, params: OdometryConstraintParameters | None = None) -> OdometryConstraintResult:
+    """src/constraint_builders.cpp:33-41 for one (parent, child) pair of Submaps."""
+    return buildOdometryConstraintsBatch(eng, [source], [target], params)[0]
+
+
 def nearestNeighbors(eng: Engine, queries: Cloud, target: Cloud, maxCorrespondenceDistance: float, T=None):
     """The correspondence search of [O3D] RegistrationICP on its own (KDTreeFlann::SearchHybrid(q, r, 1) per query): index of the
     nearest target point with d^2 < r^2 (-1 = none), squared distance.  correspondence_set_ = this at the result's transformation."""

@@ -8,6 +8,8 @@ What stays on the host in the reference and is restated here as plain control fl
     Submap::computeSubmapCenter / computeFeatures (voxel map part) src/Submap.cpp:228-259
     PlaceRecognition::buildLoopClosureConstraints for given candidates: RANSAC proposal -> correspondence gate -> consistency
     check -> refinement (overlap -> ICP -> information matrix) -> consistency check      src/PlaceRecognition.cpp:50-229
+    computeOdometryConstraints / buildOdometryConstraint: the constraints between consecutive submaps, all missing pairs in one
+    batched device call                                           src/constraint_builders.cpp:23-118
 Every arithmetic step is a call into a *backend*: `DeviceBackend` (below) drives libb2s.so; the parity tests run the very
 same control flow over a CPU backend built on the oracle (tests/oracle_backend.py) -- the product never imports it.
 
@@ -344,6 +346,55 @@ def buildLoopClosureConstraints(backend, collection: SubmapCollection, sourceIdx
     return constraints, log
 
 
+def hasConstraint(sourceIdx: int, targetIdx: int, constraints) -> bool:
+    """src/constraint_builders.cpp:23-30"""
+    return any(c.sourceSubmapIdx == sourceIdx and c.targetSubmapIdx == targetIdx for c in constraints)
+
+
+def _odometry_constraint(collection: SubmapCollection, sourceIdx: int, targetIdx: int, r) -> Constraint:
+    """buildConstraint's record (src/constraint_builders.cpp:75-82) from a backend result (T, information, ...)"""
+    return Constraint(np.array(r.sourceToTarget_, dtype=np.float64), collection.submaps[sourceIdx].id, collection.submaps[targetIdx].id,
+                      np.array(r.informationMatrix_, dtype=np.float64), isInformationMatrixValid=True, isOdometryConstraint=True)
+
+
+def buildOdometryConstraint(backend, collection: SubmapCollection, sourceIdx: int, targetIdx: int,
+                            params: E.OdometryConstraintParameters | None = None) -> Constraint:
+    """buildOdometryConstraint(sourceIdx = parent, targetIdx = child, submaps) (src/constraint_builders.cpp:33-41): overlap of the two
+    whole maps at the identity, optional point-to-plane refinement, information matrix."""
+    params = params or E.OdometryConstraintParameters()
+    (r,) = backend.odometry_constraints([(collection.submaps[sourceIdx].handle, collection.submaps[targetIdx].handle)], params)
+    return _odometry_constraint(collection, sourceIdx, targetIdx, r)
+
+
+def computeOdometryConstraints(backend, collection: SubmapCollection, constraints: list, finishedIds=None,
+                               params: E.OdometryConstraintParameters | None = None) -> list:
+    """Both overloads of computeOdometryConstraints (src/constraint_builders.cpp:92-118), appending to `constraints`:
+        finishedIds given (SubmapCollection::computeFeatures, :92-106): every listed submap but submap 0, from its parent;
+        finishedIds None  (SlamWrapper::loopClosureWorker, :108-118): every submap 1.. from its parent, except pairs that touch the
+                          active submap.
+    A (parent, child) pair already in `constraints` is not rebuilt (hasConstraint).  The missing pairs go to the backend in ONE batched
+    call.  Returns the constraints added, in the reference's order."""
+    params = params or E.OdometryConstraintParameters()
+    active = collection.activeSubmapIdx
+    pairs = []
+    targets = finishedIds if finishedIds is not None else range(1, len(collection.submaps))
+    for t in targets:
+        if t < 1:
+            continue
+        s = collection.submaps[t].parent
+        if finishedIds is None and (s == active or t == active):
+            continue
+        if hasConstraint(s, t, constraints) or (s, t) in pairs:   # the pending ones count: the reference appends as it goes
+            continue
+        pairs.append((s, t))
+    if not pairs:
+        return []
+    res = backend.odometry_constraints([(collection.submaps[s].handle, collection.submaps[t].handle) for s, t in pairs], params)
+    added = [_odometry_constraint(collection, s, t, r) for (s, t), r in zip(pairs, res)]
+    constraints.extend(added)
+    return added
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # device backend
 # ----------------------------------------------------------------------------------------------------------------------
@@ -510,6 +561,10 @@ class DeviceBackend:
     def ransac(self, source_sparse, source_feature, target_sparses, target_features, params: E.PlaceRecognitionParameters):
         """RegistrationRANSACBasedOnFeatureMatching of the source against every candidate in one call (mutual filter on, :82)"""
         return E.registrationRANSACBasedOnFeatureMatchingBatch(self.eng, source_sparse, target_sparses, source_feature, target_features, params)
+
+    def odometry_constraints(self, pairs, params: E.OdometryConstraintParameters):
+        """buildOdometryConstraint for every (parent, child) pair of submaps in one b2s_submap_odometry_constraints call"""
+        return E.buildOdometryConstraintsBatch(self.eng, [s for s, _t in pairs], [t for _s, t in pairs], params)
 
     def cloud_size(self, c) -> int:
         return len(c)

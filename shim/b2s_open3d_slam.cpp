@@ -419,4 +419,43 @@ RansacResultB200 registrationRansacBasedOnFeatureMatchingB200(const SubmapB200& 
   return out;
 }
 
+void computeOdometryConstraintsB200(const std::vector<const SubmapB200*>& submaps, const std::vector<size_t>& parentIds, size_t activeSubmapIdx,
+                                    const std::vector<size_t>* candidates, const MapperParameters& p, Constraints* constraints) {
+  auto has = [&](size_t s, size_t t) {   // hasConstraint (:23-30), the pairs of this call included
+    for (const Constraint& c : *constraints) if (c.sourceSubmapIdx_ == s && c.targetSubmapIdx_ == t) return true;
+    return false;
+  };
+  std::vector<std::pair<size_t, size_t>> pairs;
+  auto consider = [&](size_t t, bool skipActive) {
+    if (t < 1) return;
+    const size_t s = parentIds.at(t);
+    if (skipActive && (s == activeSubmapIdx || t == activeSubmapIdx)) return;
+    for (const auto& q : pairs) if (q.first == s && q.second == t) return;
+    if (!has(s, t)) pairs.emplace_back(s, t);
+  };
+  if (candidates) { for (size_t t : *candidates) consider(t, false); }
+  else { for (size_t t = 1; t < submaps.size(); ++t) consider(t, true); }
+  if (pairs.empty()) return;
+  std::vector<const b2s_submap*> src, tgt;
+  for (const auto& q : pairs) { src.push_back(submaps.at(q.first)->handle()); tgt.push_back(submaps.at(q.second)->handle()); }
+  b2s_odometry_constraint_params prm;
+  b2s_default_odometry_constraint_params(&prm);
+  prm.map_voxel_size = p.mapBuilder_.mapVoxelSize_;                        // getMapVoxelSize is applied by the call
+  prm.refine = p.isRefineOdometryConstraintsBetweenSubmaps_ ? 1 : 0;
+  std::vector<b2s_odometry_constraint> out(pairs.size());
+  const int32_t rc = b2s_submap_odometry_constraints(submaps.at(pairs.front().second)->engine(), (int32_t)pairs.size(), src.data(), tgt.data(), &prm,
+                                                     nullptr, nullptr, out.data());
+  if (rc != B2S_OK) b2sThrow(rc);
+  for (size_t k = 0; k < pairs.size(); ++k) {
+    Constraint c;
+    c.sourceSubmapIdx_ = pairs[k].first;
+    c.targetSubmapIdx_ = pairs[k].second;
+    for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) c.sourceToTarget_.matrix()(i, j) = out[k].T[4 * i + j];
+    for (int i = 0; i < 6; i++) for (int j = 0; j < 6; j++) c.informationMatrix_(i, j) = out[k].information[6 * i + j];
+    c.isInformationMatrixValid_ = true;
+    c.isOdometryConstraint_ = true;
+    constraints->push_back(c);
+  }
+}
+
 }  // namespace o3d_slam

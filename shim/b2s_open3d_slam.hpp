@@ -126,6 +126,15 @@ struct RansacResultB200 {
 RansacResultB200 registrationRansacBasedOnFeatureMatchingB200(const SubmapB200& source, const SubmapB200& target,
                                                               const PlaceRecognitionParameters& cfg, uint64_t seed = 1);
 
+// computeOdometryConstraints (src/constraint_builders.cpp:92-118) over device-resident submaps: submaps[i] is the SubmapB200 of submap
+// id i and parentIds[i] its getParentId().  candidates = the finished submap ids (the overload of SubmapCollection::computeFeatures,
+// :92-106), or nullptr for every submap (the overload of SlamWrapper::loopClosureWorker, :108-118, which leaves out the pairs that touch
+// activeSubmapIdx).  Submap 0 and the pairs constraints already holds are skipped; every missing (parent, child) pair is built by
+// buildOdometryConstraint (:33-90) in ONE b2s_submap_odometry_constraints call on the resident maps (all SubmapB200s on one handle),
+// with p.mapBuilder_.mapVoxelSize_ and p.isRefineOdometryConstraintsBetweenSubmaps_, and appended in the reference's order.
+void computeOdometryConstraintsB200(const std::vector<const SubmapB200*>& submaps, const std::vector<size_t>& parentIds, size_t activeSubmapIdx,
+                                    const std::vector<size_t>* candidates, const MapperParameters& p, Constraints* constraints);
+
 class ScanToMapIcpB200 : public ScanToMapRegistration {
  public:
   explicit ScanToMapIcpB200(const MapperParameters& p);

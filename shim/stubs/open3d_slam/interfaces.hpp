@@ -2,12 +2,14 @@
 // signatures the shim overrides so that it can be type-checked without Open3D / Eigen / the reference tree:
 //   CloudRegistration          include/open3d_slam/CloudRegistration.hpp:19-27
 //   ScanToMapRegistration      include/open3d_slam/ScanToMapRegistration.hpp:24-38
-//   parameter structs          include/open3d_slam/Parameters.hpp:51-98,118-122,148-153
+//   parameter structs          include/open3d_slam/Parameters.hpp:51-98,118-122,148-153,172
+//   Constraint                 include/open3d_slam/Constraint.hpp:14-20
 // In a real build, include the reference's own headers instead (INTEGRATION.md).
 #pragma once
 #include <Eigen/Dense>
 #include <memory>
 #include <string>
+#include <vector>
 #include "open3d/geometry/PointCloud.h"
 #include "open3d/pipelines/registration/Registration.h"
 namespace o3d_slam {
@@ -26,7 +28,11 @@ struct ScanToMapRegistrationParameters { double minRefinementFitness_ = 0.7; Icp
 struct PlaceRecognitionParameters { double normalEstimationRadius_ = 1.0, featureVoxelSize_ = 0.5, featureRadius_ = 2.5; int featureKnn_ = 100, normalKnn_ = 10;
   int ransacNumIter_ = 1000000; double ransacProbability_ = 0.99; int ransacModelSize_ = 3; double ransacMaxCorrespondenceDistance_ = 0.75,
   correspondenceCheckerDistance_ = 0.75, correspondenceCheckerEdgeLength_ = 0.5; int ransacMinCorrespondenceSetSize_ = 25; };   // Parameters.hpp:118-129
-struct MapperParameters { ScanToMapRegistrationParameters scanMatcher_; ScanProcessingParameters scanProcessing_; MapBuilderParameters mapBuilder_; MapBuilderParameters denseMapBuilder_; };
+struct MapperParameters { ScanToMapRegistrationParameters scanMatcher_; ScanProcessingParameters scanProcessing_; MapBuilderParameters mapBuilder_; MapBuilderParameters denseMapBuilder_;
+  bool isRefineOdometryConstraintsBetweenSubmaps_ = false; };
+struct Constraint { Transform sourceToTarget_ = Transform::Identity(); size_t sourceSubmapIdx_ = 0, targetSubmapIdx_ = 0;
+  Eigen::Matrix6d informationMatrix_ = Eigen::Matrix6d::Identity(); bool isInformationMatrixValid_ = false, isOdometryConstraint_ = false; };
+using Constraints = std::vector<Constraint>;
 class Submap;  // the shim only needs getMapPointCloud(); see b2s_open3d_slam.cpp
 class CloudRegistration {
  public:
