@@ -121,8 +121,9 @@ const char* b2s_version(void);
 int32_t b2s_device_count(void);
 /* number of kernels launched by this handle since creation ("gpu_launches" evidence for bench.py) */
 int64_t b2s_launch_count(const b2s_handle* h);
-/* number of CUDA graphs the per-scan chains of this handle captured since creation (b2s_mapper_graph_enable, b2s_slam_graph_enable):
- * in steady state a replay adds launches but no capture */
+/* number of CUDA graphs the per-scan chains of this handle captured since creation (b2s_mapper_graph_enable, b2s_slam_graph_enable),
+ * and the LM tries of b2s_global_optimization (one capture per padded size and edge capacity): in steady state a replay adds
+ * launches but no capture */
 int64_t b2s_graph_capture_count(const b2s_handle* h);
 
 /* per-kernel-group device time, CUDA events on the handle's stream (the reference prints per-stage wall times with
@@ -235,6 +236,9 @@ int32_t b2s_dense_clear(b2s_handle* h, b2s_submap* sm);
  *     denseMap_.transform(T) (src/Voxel.cpp:49-64: applied to the voxel SUMS, keys unchanged -- kept as it is),
  *     mapToRangeSensor_ = mapToRangeSensor_ * T (the pose state of b2s_submap_set_pose / b2s_submap_get_pose). */
 int32_t b2s_submap_transform(b2s_handle* h, b2s_submap* sm, const double T[16]);
+/* [O3D] PointCloud::Transform of a cloud in place, points and normals (no duplication quirk): Submap::transform applies it to the
+ * submap's sparse feature cloud, sparseMapCloud_ (src/Submap.cpp:96), with the same kernel as the map */
+int32_t b2s_cloud_transform_inplace(b2s_handle* h, b2s_cloud* c, const double T[16]);
 /* Submap::getMapPointCloud (copy-out)                                       src/Submap.cpp:184-191 */
 int32_t b2s_submap_size(b2s_handle* h, const b2s_submap* sm, size_t* n);
 int32_t b2s_submap_download(b2s_handle* h, const b2s_submap* sm, double* xyz, double* normals, size_t capacity, size_t* n);
@@ -599,6 +603,65 @@ int32_t b2s_submap_odometry_constraints(b2s_handle* h, int32_t n_pairs, const b2
                                         const b2s_submap* const* targets /* child */, const b2s_odometry_constraint_params* p,
                                         b2s_cloud* const* source_overlaps_or_null, b2s_cloud* const* target_overlaps_or_null,
                                         b2s_odometry_constraint* out);
+
+/* ---- submap pose-graph optimisation: [O3D] GlobalOptimization with GlobalOptimizationLevenbergMarquardt, as
+ *      OptimizationProblem::solve (src/OptimizationProblem.cpp:25-44) calls it.  Restated semantics (DESIGN.md row G1):
+ *   - validation: every edge id in [0, n_nodes) (else B2S_E_INVALID); the graph connected from node 0 over all edges and over the
+ *     certain edges alone (BFS), else B2S_OK with the poses unchanged and stats[0].valid = stats[1].valid = 0
+ *   - lpw = preference_loop_closure * max_correspondence_distance^2 * mean_e information_e(5,5) (0 without edges)
+ *   - zeta_e = lin(X^-1 Tt^-1 Ts), lin(M) = ((M21-M12)/2, (M02-M20)/2, (M10-M01)/2, M03, M13, M23); inverses are the rigid ones
+ *   - uncertain edges: conf = (lpw / (lpw + zeta' Info zeta))^2; certain edges keep 1
+ *   - residual = sum_e conf zeta' Info zeta + lpw (sqrt(conf) - 1)^2; H, b: conf-weighted J' Info J, -conf J' Info zeta
+ *   - LM: lambda = 1e-5 max diag H, nu = 2; delta = (H + lambda I)^-1 b by an UNPIVOTED LDL' (|d| <= 1/DBL_MAX zeroes the
+ *     component); trial T_i <- V2M(delta_i) T_i; rho = (cur - new) / (delta.(lambda delta + b) + 1e-3); criteria of [O3D]
+ *   - two passes (all edges; then the certain edges and the uncertain edges with conf > edge_prune_threshold), then every pose is
+ *     left-multiplied by T_ref(input) T_ref(new)^-1 when reference_node is in range.
+ * The LM control flow runs on the host; every try runs one CUDA graph (H + lambda I, blocked LDL' on fp64 mma.sync, substitution,
+ * trial poses, trial residual) and reads back one record.  Results repeat bit for bit. */
+typedef struct b2s_pose_graph_edge {   /* [O3D] PoseGraphEdge */
+  int32_t source, target;              /* node ids */
+  int32_t uncertain;                   /* uncertain_: a loop closure (line process); odometry edges are certain */
+  int32_t reserved_;
+  double T[16];                        /* transformation_, row-major (the source-to-target measurement X) */
+  double information[36];              /* information_, row-major */
+} b2s_pose_graph_edge;
+typedef struct b2s_global_optimization_params {   /* GlobalOptimizationOption + GlobalOptimizationConvergenceCriteria */
+  double max_correspondence_distance;  /* 1000 (Lua, parameter_structure_definitions.lua:45-50; the C++ struct has 10) */
+  double edge_prune_threshold;         /* 0.2 */
+  double preference_loop_closure;      /* loop_closure_preference, 2.0 */
+  int32_t reference_node;              /* 0; out of range = no compensation */
+  int32_t max_iteration;               /* 100 */
+  double min_relative_increment;       /* 1e-6 */
+  double min_relative_residual_increment; /* 1e-6 */
+  double min_right_term;               /* 1e-6 */
+  double min_residual;                 /* 1e-6 */
+  int32_t max_iteration_lm;            /* 20 */
+  int32_t reserved_;
+  double upper_scale_factor;           /* 2/3 */
+  double lower_scale_factor;           /* 1/3 */
+} b2s_global_optimization_params;
+enum {   /* b2s_global_optimization_stats.stop_reason: the first criterion that stopped the pass */
+  B2S_LM_STOP_NONE = 0, B2S_LM_STOP_RIGHT_TERM = 1, B2S_LM_STOP_RELATIVE_INCREMENT = 2, B2S_LM_STOP_RELATIVE_RESIDUAL_INCREMENT = 3,
+  B2S_LM_STOP_MAX_ITERATION_LM = 4, B2S_LM_STOP_RESIDUAL = 5, B2S_LM_STOP_MAX_ITERATION = 6
+};
+typedef struct b2s_global_optimization_stats {   /* one per pass: [0] all edges, [1] the pruned graph */
+  int32_t valid;                       /* the graph passed validation (the pass ran) */
+  int32_t n_edges;                     /* edges of the pass */
+  int32_t outer_iterations;
+  int32_t lm_tries;                    /* solves of (H + lambda I) delta = b */
+  int32_t accepted_steps;              /* tries with rho > 0 */
+  int32_t stop_reason;                 /* B2S_LM_STOP_* */
+  double initial_residual, final_residual;   /* the pass's residual at its start, and of its last accepted poses */
+  double final_lambda;
+} b2s_global_optimization_stats;
+void b2s_default_global_optimization_params(b2s_global_optimization_params* p);
+/* node_poses: n_nodes row-major 4x4, optimised in place.  edge_kept_out (n_edges int32, optional): 1 = the edge survived the pruning.
+ * edge_confidence_out (n_edges, optional): the edge's confidence at the end (the second pass's for kept edges, the first pass's
+ * for pruned ones).  stats_out (2, optional).  Errors: n_nodes < 1, n_edges < 0, an id out of range, a non-positive tolerance or
+ * iteration limit -> B2S_E_INVALID.  n_edges = 0 -> B2S_OK, poses unchanged (valid = 1 for a single node, as the BFS finds). */
+int32_t b2s_global_optimization(b2s_handle* h, int32_t n_nodes, double* node_poses, int32_t n_edges, const b2s_pose_graph_edge* edges,
+                                const b2s_global_optimization_params* p, int32_t* edge_kept_out, double* edge_confidence_out,
+                                b2s_global_optimization_stats* stats_out);
 
 /* ---- device-to-device hand-over of a cloud's arrays (SURVEY.md section 8e: a submap that is the registration target on
  *      several GPUs is built once by its owner and broadcast over NVLink by the host side -- torch.distributed / NCCL own

@@ -107,6 +107,27 @@ class OdometryConstraint(C.Structure):
                 ("refined", C.c_int32), ("icp", Result)]
 
 
+class PoseGraphEdge(C.Structure):
+    _fields_ = [("source", C.c_int32), ("target", C.c_int32), ("uncertain", C.c_int32), ("reserved_", C.c_int32), ("T", C.c_double * 16),
+                ("information", C.c_double * 36)]
+
+
+class GlobalOptimizationParams(C.Structure):
+    _fields_ = [("max_correspondence_distance", C.c_double), ("edge_prune_threshold", C.c_double), ("preference_loop_closure", C.c_double),
+                ("reference_node", C.c_int32), ("max_iteration", C.c_int32), ("min_relative_increment", C.c_double),
+                ("min_relative_residual_increment", C.c_double), ("min_right_term", C.c_double), ("min_residual", C.c_double),
+                ("max_iteration_lm", C.c_int32), ("reserved_", C.c_int32), ("upper_scale_factor", C.c_double), ("lower_scale_factor", C.c_double)]
+
+
+class GlobalOptimizationStats(C.Structure):
+    _fields_ = [("valid", C.c_int32), ("n_edges", C.c_int32), ("outer_iterations", C.c_int32), ("lm_tries", C.c_int32), ("accepted_steps", C.c_int32),
+                ("stop_reason", C.c_int32), ("initial_residual", C.c_double), ("final_residual", C.c_double), ("final_lambda", C.c_double)]
+
+
+# b2s_global_optimization_stats.stop_reason (B2S_LM_STOP_*)
+LM_STOP_REASONS = ["none", "right_term", "relative_increment", "relative_residual_increment", "max_iteration_lm", "residual", "max_iteration"]
+
+
 class MapperCounters(C.Structure):
     _fields_ = [(n, C.c_int64) for n in ("steps", "accepted", "inserted_map", "inserted_dense", "carve_runs", "carved_points_total",
                                          "dense_carve_runs", "carved_voxels_total")]
@@ -136,6 +157,7 @@ SYMBOLS = [
     "b2s_default_motion_compensation_params", "b2s_odometry_set_motion_compensation", "b2s_slam_map_pose_push", "b2s_slam_map_lookup",
     "b2s_slam_motion_fetch", "b2s_slam_undistorted",
     "b2s_default_odometry_constraint_params", "b2s_submap_odometry_constraints",
+    "b2s_default_global_optimization_params", "b2s_global_optimization", "b2s_cloud_transform_inplace",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 PROFILE_KINDS = ["icp", "normals", "radix_sort", "nn_grid_build", "voxel", "fuse", "select", "crop"]
@@ -183,6 +205,7 @@ def lib():
         L.b2s_default_odometry_params.restype = None
         L.b2s_default_motion_compensation_params.restype = None
         L.b2s_default_odometry_constraint_params.restype = None
+        L.b2s_default_global_optimization_params.restype = None
         _lib = L
     return _lib
 

@@ -809,6 +809,13 @@ int32_t b2s_submap_set_pose(b2s_handle* h, b2s_submap* sm, const double T[16]) {
   return pose_to_device(h, T, sm->pose.as<double>());
 }
 
+int32_t b2s_cloud_transform_inplace(b2s_handle* h, b2s_cloud* c, const double T[16]) {
+  B2S_REQUIRE(h && c && T, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(c->h == h, B2S_E_INVALID, "the cloud belongs to another handle");
+  LOCK(h);
+  return op_cloud_transform(h, c, T);
+}
+
 int32_t b2s_submap_transform(b2s_handle* h, b2s_submap* sm, const double T[16]) {
   B2S_REQUIRE(h && sm && T, B2S_E_INVALID, "null argument");
   LOCK(h);
@@ -1270,6 +1277,30 @@ int32_t b2s_submap_odometry_constraints(b2s_handle* h, int32_t n, const b2s_subm
                 "[RegistrationICP] pair %d: TransformationEstimationPointToPlane requires target normals, the child map has none", k);
   LOCK(h);
   return op_odometry_constraints(h, n, sources, targets, *p, voxel, so, to, out);
+}
+
+// ---- pose-graph optimisation (src/OptimizationProblem.cpp:25-44 -> [O3D] GlobalOptimization, LM) -------------------------------
+void b2s_default_global_optimization_params(b2s_global_optimization_params* p) {   // parameter_structure_definitions.lua:45-50, [O3D] criteria
+  memset(p, 0, sizeof(*p));
+  p->max_correspondence_distance = 1000.0; p->edge_prune_threshold = 0.2; p->preference_loop_closure = 2.0; p->reference_node = 0;
+  p->max_iteration = 100; p->min_relative_increment = 1e-6; p->min_relative_residual_increment = 1e-6; p->min_right_term = 1e-6;
+  p->min_residual = 1e-6; p->max_iteration_lm = 20; p->upper_scale_factor = 2.0 / 3.0; p->lower_scale_factor = 1.0 / 3.0;
+}
+
+int32_t b2s_global_optimization(b2s_handle* h, int32_t n_nodes, double* node_poses, int32_t n_edges, const b2s_pose_graph_edge* edges,
+                                const b2s_global_optimization_params* p, int32_t* edge_kept_out, double* edge_confidence_out,
+                                b2s_global_optimization_stats* stats_out) {
+  B2S_REQUIRE(h && p && node_poses, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(n_nodes >= 1 && n_edges >= 0, B2S_E_INVALID, "n_nodes %d must be >= 1 and n_edges %d >= 0", (int)n_nodes, (int)n_edges);
+  B2S_REQUIRE(n_edges == 0 || edges, B2S_E_INVALID, "null edges");
+  B2S_REQUIRE(p->min_relative_increment > 0.0 && p->min_relative_residual_increment > 0.0 && p->min_right_term > 0.0 && p->min_residual > 0.0,
+              B2S_E_INVALID, "the convergence tolerances must be > 0");
+  B2S_REQUIRE(p->max_iteration >= 1 && p->max_iteration_lm >= 1, B2S_E_INVALID, "max_iteration and max_iteration_lm must be >= 1");
+  for (int32_t e = 0; e < n_edges; e++)   // ValidatePoseGraph's id check
+    B2S_REQUIRE(edges[e].source >= 0 && edges[e].source < n_nodes && edges[e].target >= 0 && edges[e].target < n_nodes, B2S_E_INVALID,
+                "edge %d: node ids (%d, %d) outside [0, %d)", (int)e, (int)edges[e].source, (int)edges[e].target, (int)n_nodes);
+  LOCK(h);
+  return op_global_optimization(h, n_nodes, node_poses, n_edges, edges, *p, edge_kept_out, edge_confidence_out, stats_out);
 }
 
 }  // extern "C"

@@ -310,6 +310,12 @@ struct b2s_handle {
   b2s::DevBuf odo, odo_info;
   b2s::PinnedBuf odo_stage;
   std::vector<std::unique_ptr<b2s_cloud>> odo_clouds;
+  // b2s_global_optimization (posegraph.cu owns the layouts): the dense system H and the factor of H + lambda I (padded to whole
+  // tiles), the panel, the vectors and try records, the node poses and trial poses, the edge records with their per-edge scratch
+  // and assembly lists, and the CUDA graph of one LM try
+  b2s::DevBuf pg_A, pg_F, pg_W, pg_vec, pg_nodes, pg_edges;
+  int32_t pg_edge_cap = 0;
+  b2s::GraphCache pg_graph;
 };
 
 // every entry point that touches a handle's stream or buffers holds its lock and works on its device
@@ -426,7 +432,8 @@ int32_t op_dense_count(b2s_handle* h, const b2s_submap* sm, int32_t* out_dev);
 // kernels return at once unless *enable_dev != 0 (device-side schedule of the mapper chain)
 int32_t op_dense_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, const double* sensor, const double* sensor_dev, double radius,
                        double trunc, double max_len, int32_t* removed_dev, const int32_t* enable_dev = nullptr);
-int32_t op_submap_transform(b2s_handle* h, b2s_submap* sm, const double* T_host);   // Submap::transform (voxel.cu)
+int32_t op_submap_transform(b2s_handle* h, b2s_submap* sm, const double* T_host);
+int32_t op_cloud_transform(b2s_handle* h, b2s_cloud* c, const double* T_host);     // [O3D] PointCloud::Transform in place (voxel.cu)   // Submap::transform (voxel.cu)
 // D1 constant-velocity de-skew (voxel.cu)
 int32_t op_undistort(b2s_handle* h, const b2s_cloud* in, const double* lin_vel, const double* ang_vel_rpy, double scan_duration, int clockwise,
                      b2s_cloud* out);
@@ -438,6 +445,9 @@ int32_t op_overlap(b2s_handle* h, const b2s_cloud* source, const b2s_cloud* targ
 int32_t op_odometry_constraints(b2s_handle* h, int n, const b2s_submap* const* sources, const b2s_submap* const* targets,
                                 const b2s_odometry_constraint_params& p, double voxel, b2s_cloud* const* so_out, b2s_cloud* const* to_out,
                                 b2s_odometry_constraint* out);
+// G1 (posegraph.cu): [O3D] GlobalOptimization (Levenberg-Marquardt) of a validated graph: ids in range, parameters checked
+int32_t op_global_optimization(b2s_handle* h, int n_nodes, double* poses, int n_edges, const b2s_pose_graph_edge* edges,
+                               const b2s_global_optimization_params& p, int32_t* kept_out, double* conf_out, b2s_global_optimization_stats* stats);
 // K-fpfh (features.cu): [O3D] ComputeFPFHFeature of the n points of c (normals required, 1 <= knn <= B2S_FEATURE_MAX_KNN)
 int32_t op_compute_fpfh(b2s_handle* h, const b2s_cloud* c, size_t n, double radius, int knn, b2s_feature* f);
 // K-ransac (ransac.cu): exact feature correspondences of one source feature against n target features (device outputs; s2t[k] / t2s[k]
@@ -571,6 +581,16 @@ __device__ __forceinline__ double warp_max(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// [O3D] TransformVector6dToMatrix4d: R = Rz(x2) Ry(x1) Rx(x0), t = x[3..5] (the ICP update and the pose-graph LM step)
+__device__ __forceinline__ void vec6_to_mat4_dev(const double (&x)[6], double* T) {
+  double sa, ca, sb, cb, sg, cgm;
+  sincos(x[0], &sa, &ca); sincos(x[1], &sb, &cb); sincos(x[2], &sg, &cgm);
+  T[0] = cgm * cb; T[1] = cgm * sb * sa - sg * ca; T[2] = cgm * sb * ca + sg * sa; T[3] = x[3];
+  T[4] = sg * cb;  T[5] = sg * sb * sa + cgm * ca; T[6] = sg * sb * ca - cgm * sa; T[7] = x[4];
+  T[8] = -sb;      T[9] = cb * sa;                 T[10] = cb * ca;                T[11] = x[5];
+  T[12] = 0; T[13] = 0; T[14] = 0; T[15] = 1;
 }
 
 // squared distance accumulated exactly like nanoflann's L2 adaptor and the oracle: (dx*dx + dy*dy) + dz*dz,

@@ -376,16 +376,6 @@ __device__ __forceinline__ void ldlt6_solve_smem(double* a, double* b) {
   }
 }
 
-// [O3D] TransformVector6dToMatrix4d: R = Rz(x2) Ry(x1) Rx(x0), t = x[3..5]
-__device__ __forceinline__ void vec6_to_mat4_dev(const double (&x)[6], double* T) {
-  double sa, ca, sb, cb, sg, cgm;
-  sincos(x[0], &sa, &ca); sincos(x[1], &sb, &cb); sincos(x[2], &sg, &cgm);
-  T[0] = cgm * cb; T[1] = cgm * sb * sa - sg * ca; T[2] = cgm * sb * ca + sg * sa; T[3] = x[3];
-  T[4] = sg * cb;  T[5] = sg * sb * sa + cgm * ca; T[6] = sg * sb * ca - cgm * sa; T[7] = x[4];
-  T[8] = -sb;      T[9] = cb * sa;                 T[10] = cb * ca;                T[11] = x[5];
-  T[12] = 0; T[13] = 0; T[14] = 0; T[15] = 1;
-}
-
 __device__ bool mat4_is_identity_dev(const double* T) {  // Eigen isIdentity(1e-12)
   const double prec = 1e-12;
   for (int i = 0; i < 4; i++)

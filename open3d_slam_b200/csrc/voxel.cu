@@ -606,6 +606,19 @@ __global__ void dense_transform_kernel(double* __restrict__ sums, const int32_t*
   }
 }
 
+// [O3D] PointCloud::Transform of a cloud in place (points and, when present, normals): the submap's sparse feature cloud follows a
+// loop-closure correction with the map's kernel
+int32_t op_cloud_transform(b2s_handle* h, b2s_cloud* c, const double* T_host) {
+  Mat4 M;
+  for (int i = 0; i < 16; i++) M.m[i] = T_host[i];
+  const size_t n_max = c->n_max > 0 ? c->n_max : 1;
+  launch_pdl(o3d_transform_inplace_kernel, grid_for(n_max, VX_THREADS), VX_THREADS, 0, h->stream, c->xyz.as<double>(),
+             c->has_normals ? c->nrm.as<double>() : nullptr, c->dn.as<int32_t>(), M);
+  h->launches++;
+  B2S_CUDA(cudaGetLastError());
+  return B2S_OK;
+}
+
 int32_t op_submap_transform(b2s_handle* h, b2s_submap* sm, const double* T_host) {
   Mat4 M;
   for (int i = 0; i < 16; i++) M.m[i] = T_host[i];

@@ -452,6 +452,111 @@ def buildOdometryConstraint(eng: Engine, source, target, params: OdometryConstra
     return buildOdometryConstraintsBatch(eng, [source], [target], params)[0]
 
 
+@dataclass
+class PoseGraphNode:
+    """[O3D] PoseGraphNode: pose_ (4x4)"""
+    pose_: np.ndarray = field(default_factory=lambda: np.eye(4))
+
+
+@dataclass
+class PoseGraphEdge:
+    """[O3D] PoseGraphEdge: the measurement transformation_ (source to target), information_, uncertain_, and confidence_ (1 until
+    globalOptimization writes the value it ended with)"""
+    source_node_id_: int
+    target_node_id_: int
+    transformation_: np.ndarray = field(default_factory=lambda: np.eye(4))
+    information_: np.ndarray = field(default_factory=lambda: np.eye(6))
+    uncertain_: bool = False
+    confidence_: float = 1.0
+
+
+@dataclass
+class PoseGraph:
+    """[O3D] PoseGraph: nodes_ and edges_"""
+    nodes_: list = field(default_factory=list)
+    edges_: list = field(default_factory=list)
+
+
+@dataclass
+class GlobalOptimizationOption:
+    """[O3D] GlobalOptimizationOption with the project's values (parameter_structure_definitions.lua:45-50): max_correspondence_distance
+    1000 (the C++ struct, Parameters.hpp:138-143, has 10), edge_prune_threshold 0.2, loop_closure_preference 2.0, reference_node 0"""
+    max_correspondence_distance_: float = 1000.0
+    edge_prune_threshold_: float = 0.2
+    preference_loop_closure_: float = 2.0
+    reference_node_: int = 0
+
+
+@dataclass
+class GlobalOptimizationConvergenceCriteria:
+    """[O3D] GlobalOptimizationConvergenceCriteria defaults"""
+    max_iteration_: int = 100
+    min_relative_increment_: float = 1e-6
+    min_relative_residual_increment_: float = 1e-6
+    min_right_term_: float = 1e-6
+    min_residual_: float = 1e-6
+    max_iteration_lm_: int = 20
+    upper_scale_factor_: float = 2.0 / 3.0
+    lower_scale_factor_: float = 1.0 / 3.0
+
+
+@dataclass
+class GlobalOptimizationPassStats:
+    """b2s_global_optimization_stats of one pass (0: all edges, 1: the pruned graph)"""
+    valid: bool
+    n_edges: int
+    outer_iterations: int
+    lm_tries: int
+    accepted_steps: int
+    stop_reason: str
+    initial_residual: float
+    final_residual: float
+    final_lambda: float
+
+
+def _go_params(criteria: GlobalOptimizationConvergenceCriteria, option: GlobalOptimizationOption) -> L.GlobalOptimizationParams:
+    p = L.GlobalOptimizationParams()
+    L.lib().b2s_default_global_optimization_params(C.byref(p))
+    p.max_correspondence_distance = float(option.max_correspondence_distance_); p.edge_prune_threshold = float(option.edge_prune_threshold_)
+    p.preference_loop_closure = float(option.preference_loop_closure_); p.reference_node = int(option.reference_node_)
+    p.max_iteration = int(criteria.max_iteration_); p.min_relative_increment = float(criteria.min_relative_increment_)
+    p.min_relative_residual_increment = float(criteria.min_relative_residual_increment_); p.min_right_term = float(criteria.min_right_term_)
+    p.min_residual = float(criteria.min_residual_); p.max_iteration_lm = int(criteria.max_iteration_lm_)
+    p.upper_scale_factor = float(criteria.upper_scale_factor_); p.lower_scale_factor = float(criteria.lower_scale_factor_)
+    return p
+
+
+def globalOptimization(eng: Engine, poseGraph: PoseGraph, criteria: GlobalOptimizationConvergenceCriteria | None = None,
+                       option: GlobalOptimizationOption | None = None) -> list[GlobalOptimizationPassStats]:
+    """[O3D] GlobalOptimization(pose_graph, GlobalOptimizationLevenbergMarquardt, criteria, option) on the device (one
+    b2s_global_optimization call).  Like [O3D], poseGraph is updated in place: the node poses, and edges_ becomes the surviving edge set
+    (with the confidences the optimisation ended with).  A graph that fails validation is left as it is.  Returns the two passes' stats."""
+    criteria = criteria or GlobalOptimizationConvergenceCriteria()
+    option = option or GlobalOptimizationOption()
+    p = _go_params(criteria, option)
+    n, ne = len(poseGraph.nodes_), len(poseGraph.edges_)
+    poses = np.ascontiguousarray(np.stack([np.asarray(nd.pose_, dtype=np.float64) for nd in poseGraph.nodes_]) if n else np.zeros((0, 4, 4)))
+    edges = (L.PoseGraphEdge * max(ne, 1))()
+    for k, e in enumerate(poseGraph.edges_):
+        edges[k].source, edges[k].target, edges[k].uncertain = int(e.source_node_id_), int(e.target_node_id_), int(bool(e.uncertain_))
+        edges[k].T[:] = np.asarray(e.transformation_, dtype=np.float64).ravel().tolist()
+        edges[k].information[:] = np.asarray(e.information_, dtype=np.float64).ravel().tolist()
+    kept = np.zeros(max(ne, 1), dtype=np.int32)
+    conf = np.zeros(max(ne, 1), dtype=np.float64)
+    stats = (L.GlobalOptimizationStats * 2)()
+    L.check(L.lib().b2s_global_optimization(eng._h, C.c_int32(n), _pd(poses), C.c_int32(ne), edges, C.byref(p), kept.ctypes.data_as(C.POINTER(C.c_int32)), _pd(conf), stats))
+    out = [GlobalOptimizationPassStats(bool(s.valid), int(s.n_edges), int(s.outer_iterations), int(s.lm_tries), int(s.accepted_steps),
+                                       L.LM_STOP_REASONS[s.stop_reason], float(s.initial_residual), float(s.final_residual), float(s.final_lambda))
+           for s in stats]
+    if ne > 0 and out[0].valid:
+        for nd, T in zip(poseGraph.nodes_, poses):
+            nd.pose_ = np.array(T)
+        for e, c in zip(poseGraph.edges_, conf):
+            e.confidence_ = float(c)
+        poseGraph.edges_ = [e for e, k in zip(poseGraph.edges_, kept) if k]
+    return out
+
+
 def nearestNeighbors(eng: Engine, queries: Cloud, target: Cloud, maxCorrespondenceDistance: float, T=None):
     """The correspondence search of [O3D] RegistrationICP on its own (KDTreeFlann::SearchHybrid(q, r, 1) per query): index of the
     nearest target point with d^2 < r^2 (-1 = none), squared distance.  correspondence_set_ = this at the result's transformation."""
@@ -777,6 +882,12 @@ class Submap:
         """Submap::transform (src/Submap.cpp:94-107): map cloud, dense map and mapToRangeSensor_ follow a loop-closure correction."""
         L.check(L.lib().b2s_submap_transform(self.eng._h, self._s, _pd(_mat(T))))
         self._cropperPose = self._cropperPose   # mapBuilderCropper_ keeps its pose in the reference as well
+
+    def transformSparseMapCloud(self, T) -> None:
+        """The sparseMapCloud_ line of Submap::transform (src/Submap.cpp:96): [O3D] PointCloud::Transform of the feature cloud in place
+        (a no-op before computeFeatures)."""
+        if self.sparseMapCloud_ is not None:
+            L.check(L.lib().b2s_cloud_transform_inplace(self.eng._h, self.sparseMapCloud_._c, _pd(_mat(T))))
 
     def setMapPointCloud(self, cloud: Cloud):
         L.check(L.lib().b2s_submap_set_cloud(self.eng._h, self._s, cloud._c))

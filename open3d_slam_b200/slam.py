@@ -20,6 +20,7 @@ replays the captured CUDA graph of the chain S1 -> S2 -> gates -> [carving] -> F
 from __future__ import annotations
 
 import collections
+import copy
 import ctypes as C
 from dataclasses import dataclass, field
 
@@ -81,6 +82,8 @@ class SubmapCollection:
         self.overlapScansBuffer = collections.deque(maxlen=params.numScansOverlap)   # CircularBuffer, :216
         self.finishedSubmapsIdxs: list[int] = []
         self.adjacency: set[tuple[int, int]] = set()
+        self.loopClosureSubmaps: set[int] = set()   # adjacencyMatrix_.markAsLoopClosureSubmap
+        self.odometryConstraints: list = []          # odometryConstraints_ (SubmapCollection::computeFeatures appends to it)
         self.events: list[tuple] = []   # (scan index, what, ...) -- compared between backends by the parity test
 
     # -- helpers
@@ -144,6 +147,50 @@ class SubmapCollection:
             rec = self.submaps[idx]
             rec.sparse, rec.feature = self.backend.compute_features(rec.handle, params)
         return list(self.finishedSubmapsIdxs)
+
+    def getOdometryConstraints(self) -> list:
+        return list(self.odometryConstraints)
+
+    def updateAdjacencyMatrix(self, loopClosureConstraints) -> None:   # :75-81
+        for c in loopClosureConstraints:
+            self.adjacency.add((min(c.sourceSubmapIdx, c.targetSubmapIdx), max(c.sourceSubmapIdx, c.targetSubmapIdx)))
+            self.loopClosureSubmaps.update((c.sourceSubmapIdx, c.targetSubmapIdx))
+
+    def transformSubmap(self, idx: int, T: np.ndarray) -> None:
+        """Submap::transform (src/Submap.cpp:94-107): the map, the dense map and the sparse feature cloud ([O3D] PointCloud::Transform),
+        mapToRangeSensor_ * T on the submap's pose, submapCenter_ = T * submapCenter_.  The revisit VoxelMap is not moved, as in the
+        reference.  A submap whose center has not been computed yet keeps using its origin (mapToSubmap_, which Submap::transform
+        leaves alone as well)."""
+        rec = self.submaps[idx]
+        T = np.asarray(T, dtype=np.float64)
+        self.backend.transform_submap(rec.handle, rec.sparse, T)
+        if rec.center is not None:
+            rec.center = T[:3, :3] @ rec.center + T[:3, 3]
+        self.events.append(("transform", idx))
+
+    def transform(self, transformIncrements) -> None:
+        """SubmapCollection::transform (src/SubmapCollection.cpp:284-335): every submap of the graph by its increment; every other
+        submap by the increment of its first ancestor that is in the graph; then the overlap buffer is flushed."""
+        optimized = []
+        for u in transformIncrements:
+            if u.submapId_ < len(self.submaps):
+                self.transformSubmap(u.submapId_, u.dT_)
+                optimized.append(u.submapId_)
+            else:   # the reference prints "This should not happen!" and goes on
+                self.events.append(("transform_out_of_range", u.submapId_))
+        toUpdate = sorted(set(range(len(self.submaps))) - set(optimized))
+        for idx in toUpdate:
+            if not transformIncrements:
+                break
+            cur = idx
+            while True:
+                cur = self.submaps[cur].parent
+                if cur not in toUpdate:   # the parent is in the pose graph
+                    self.transformSubmap(idx, transformIncrements[cur].dT_)
+                    break
+                if cur == self.submaps[cur].parent:
+                    raise RuntimeError("Stuck in a loop, this should not happen")
+        self.overlapScansBuffer.clear()
 
     # -- the call the mapper makes after an accepted registration (:172-207).  The scan itself has ALREADY been fused into the
     # submap that was active during the registration (with carving), because the device chain does that without a host
@@ -212,6 +259,15 @@ class SegmentMapper:
             return None
         res, inserted = self.backend.step_with_odometry(sc.getActiveSubmap().handle, rawScanF32, t)
         return self._after_step(k, res, inserted)
+
+    def loopClosureUpdate(self, loopClosureCorrection: np.ndarray) -> None:
+        """Mapper::loopClosureUpdate (src/Mapper.cpp:44-47): mapToRangeSensor_ = dT * mapToRangeSensor_.  The device keeps one pose
+        slot per submap for both the reference's Submap::mapToRangeSensor_ (which SubmapCollection.transform right-multiplies) and
+        Mapper::mapToRangeSensor_, and the next step predicts from it: after the update the active submap's slot holds dT * (the mapper
+        pose before the update).  The odometry's pose buffer is left alone, as in the reference."""
+        self.mapToRangeSensor = np.asarray(loopClosureCorrection, dtype=np.float64) @ self.mapToRangeSensor
+        if self.submaps.submaps:
+            self.backend.loop_closure_update(self.submaps.getActiveSubmap().handle, self.mapToRangeSensor)
 
     def _after_step(self, k: int, res, inserted: bool):
         sc = self.submaps
@@ -396,6 +452,143 @@ def computeOdometryConstraints(backend, collection: SubmapCollection, constraint
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# pose-graph optimisation and the loop-closure correction
+# ----------------------------------------------------------------------------------------------------------------------
+@dataclass
+class GlobalOptimizationParameters:
+    """Parameters.hpp:138-143 with the Lua values (parameter_structure_definitions.lua:45-50); the C++ struct's own
+    maxCorrespondenceDistance default is 10"""
+    edgePruneThreshold: float = 0.2
+    loopClosurePreference: float = 2.0
+    maxCorrespondenceDistance: float = 1000.0
+    referenceNode: int = 0
+
+    def option(self) -> E.GlobalOptimizationOption:
+        return E.GlobalOptimizationOption(self.maxCorrespondenceDistance, self.edgePruneThreshold, self.loopClosurePreference, self.referenceNode)
+
+
+@dataclass
+class OptimizedTransform:
+    """OptimizedTransform (OptimizationProblem.hpp): the increment dT_ of submap submapId_"""
+    dT_: np.ndarray
+    submapId_: int
+
+
+class OptimizationProblem:
+    """src/OptimizationProblem.cpp (without the mutexes, timers and JSON I/O).  The solve runs on the backend
+    (DeviceBackend.global_optimization: one b2s_global_optimization call)."""
+
+    def __init__(self, backend, params: GlobalOptimizationParameters | None = None):
+        self.backend = backend
+        self.params = params or GlobalOptimizationParameters()
+        self.odometryConstraints_: list = []
+        self.loopClosureConstraints_: list = []
+        self.poseGraph_ = E.PoseGraph()
+        self.poseGraphOptimized_ = E.PoseGraph()
+        self.poseGraphNonOptimized_ = E.PoseGraph()
+        self.numOdometryEdgesPrev_ = 0
+        self.numLoopClosuresPrev_ = 0
+        self.lastStats = None
+
+    def clearOdometryConstraints(self):
+        self.odometryConstraints_.clear()
+
+    def clearLoopClosureConstraints(self):
+        self.loopClosureConstraints_.clear()
+
+    def insertOdometryConstraints(self, cs):
+        self.odometryConstraints_.extend(cs)
+
+    def insertLoopClosureConstraints(self, cs):   # :177-189: a (source, target) pair already held is not inserted again
+        for c in cs:
+            if not any(c.sourceSubmapIdx == c2.sourceSubmapIdx and c.targetSubmapIdx == c2.targetSubmapIdx for c2 in self.loopClosureConstraints_):
+                self.loopClosureConstraints_.append(c)
+
+    def getLoopClosureConstraints(self) -> list:
+        return self.loopClosureConstraints_
+
+    def updateLoopClosureConstraint(self, idx: int, c) -> None:
+        self.loopClosureConstraints_[idx] = c
+
+    def buildOptimizationProblem(self) -> None:   # :49-61
+        self.poseGraph_.edges_ = []
+        self.setupOdometryEdgesAndPoseGraphNodes()
+        self.setupLoopClosureEdges()
+
+    def setupOdometryEdgesAndPoseGraphNodes(self) -> None:   # :63-95
+        # The reference sorts with `c1.sourceSubmapIdx_ < c2.targetSubmapIdx_`, which is not a strict weak ordering (std::sort's result
+        # is then unspecified); the intent, "sources in increasing order", is a stable sort by source.
+        self.odometryConstraints_.sort(key=lambda c: c.sourceSubmapIdx)
+        for c in self.odometryConstraints_:
+            if not c.targetSubmapIdx > c.sourceSubmapIdx:
+                raise RuntimeError("id_source should always be less than id_target for the odometry constraints")
+            self.poseGraph_.edges_.append(E.PoseGraphEdge(c.sourceSubmapIdx, c.targetSubmapIdx, np.array(c.sourceToTarget), np.array(c.informationMatrix), False))
+        if len(self.poseGraphOptimized_.edges_) > 0:
+            odometry = np.linalg.inv(self.poseGraphOptimized_.nodes_[-1].pose_)
+        else:
+            self.poseGraph_.nodes_.append(E.PoseGraphNode(np.eye(4)))
+            odometry = np.eye(4)
+        for i in range(self.numOdometryEdgesPrev_, len(self.odometryConstraints_)):
+            odometry = np.asarray(self.odometryConstraints_[i].sourceToTarget) @ odometry
+            self.poseGraph_.nodes_.append(E.PoseGraphNode(np.linalg.inv(odometry)))
+        self.numOdometryEdgesPrev_ = len(self.odometryConstraints_)
+
+    def setupLoopClosureEdges(self) -> None:   # :97-120
+        self.numLoopClosuresPrev_ = len(self.loopClosureConstraints_)
+        for c in self.loopClosureConstraints_:
+            if not c.isInformationMatrixValid:
+                raise RuntimeError(f"Invalid information matrix between: {c.sourceSubmapIdx} and {c.targetSubmapIdx}")
+            if not c.sourceSubmapIdx > c.targetSubmapIdx:
+                raise RuntimeError("Optimization problem, loop closure constraints: ")
+            self.poseGraph_.edges_.append(E.PoseGraphEdge(c.sourceSubmapIdx, c.targetSubmapIdx, np.array(c.sourceToTarget), np.array(c.informationMatrix), True))
+
+    def solve(self) -> None:   # :25-44 with [O3D]'s default criteria
+        self.poseGraphNonOptimized_ = copy.deepcopy(self.poseGraph_)
+        self.lastStats = self.backend.global_optimization(self.poseGraph_, E.GlobalOptimizationConvergenceCriteria(), self.params.option())
+        self.poseGraphOptimized_ = copy.deepcopy(self.poseGraph_)
+
+    def getOptimizedTransformIncrements(self) -> list:   # :191-202: the increment is the optimised node pose itself
+        if len(self.poseGraphOptimized_.nodes_) != len(self.poseGraph_.nodes_):
+            raise RuntimeError("Graphs are not of same size, did you run the optimization?")
+        return [OptimizedTransform(np.array(n.pose_), i) for i, n in enumerate(self.poseGraphOptimized_.nodes_)]
+
+
+def updateSubmapsAndTrajectory(mapper: "SegmentMapper", problem: OptimizationProblem, lastLoopClosureConstraints) -> np.ndarray:
+    """SlamWrapper::updateSubmapsAndTrajectory (src/SlamWrapper.cpp:450-485).  The latest loop closure is the last one in
+    lastLoopClosureConstraints (the caller appends them in time order; the timestamps stay with the caller).  Returns its dT."""
+    inc = problem.getOptimizedTransformIncrements()
+    mapper.submaps.transform(inc)
+    latest = lastLoopClosureConstraints[-1]
+    if not latest.sourceSubmapIdx > latest.targetSubmapIdx:
+        raise RuntimeError("Wrapper ros, update submaps and trajectory: ")
+    dT = inc[latest.sourceSubmapIdx].dT_
+    mapper.loopClosureUpdate(dT)
+    lcs = problem.getLoopClosureConstraints()
+    for i, old in enumerate(list(lcs)):
+        c = copy.copy(old)
+        c.sourceToTarget = np.eye(4)
+        problem.updateLoopClosureConstraint(i, c)
+    mapper.submaps.updateAdjacencyMatrix(problem.getLoopClosureConstraints())
+    return dT
+
+
+def loopClosureCycle(backend, mapper: "SegmentMapper", problem: OptimizationProblem, loopClosureConstraints,
+                     odometryParams: E.OdometryConstraintParameters | None = None) -> np.ndarray:
+    """One loop closure of SlamWrapper (src/SlamWrapper.cpp:425-445, 450-485) for constraints the caller built
+    (buildLoopClosureConstraints): the missing odometry constraints (one batched device call), insert, build, solve, then the
+    correction of the submaps and of the mapper.  The mapper never calls this on its own.  Returns the dT applied to the mapper."""
+    sc = mapper.submaps
+    odometryConstraints = sc.getOdometryConstraints()
+    computeOdometryConstraints(backend, sc, odometryConstraints, None, odometryParams)
+    problem.clearOdometryConstraints()
+    problem.insertLoopClosureConstraints(loopClosureConstraints)
+    problem.insertOdometryConstraints(odometryConstraints)
+    problem.buildOptimizationProblem()
+    problem.solve()
+    return updateSubmapsAndTrajectory(mapper, problem, list(loopClosureConstraints))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # device backend
 # ----------------------------------------------------------------------------------------------------------------------
 class DeviceBackend:
@@ -565,6 +758,18 @@ class DeviceBackend:
     def odometry_constraints(self, pairs, params: E.OdometryConstraintParameters):
         """buildOdometryConstraint for every (parent, child) pair of submaps in one b2s_submap_odometry_constraints call"""
         return E.buildOdometryConstraintsBatch(self.eng, [s for s, _t in pairs], [t for _s, t in pairs], params)
+
+    def global_optimization(self, poseGraph, criteria, option):
+        """[O3D] GlobalOptimization on the device (b2s_global_optimization); poseGraph is updated in place"""
+        return E.globalOptimization(self.eng, poseGraph, criteria, option)
+
+    def transform_submap(self, sm, sparse, T):
+        """Submap::transform: map, dense map and pose slot (b2s_submap_transform), then the sparse feature cloud"""
+        sm.transform(T)
+        sm.transformSparseMapCloud(T)
+
+    def loop_closure_update(self, sm, mapToRangeSensor):
+        sm.setPose(mapToRangeSensor)
 
     def cloud_size(self, c) -> int:
         return len(c)
