@@ -320,6 +320,35 @@ typedef struct b2s_mapper_counters {
 } b2s_mapper_counters;
 int32_t b2s_submap_get_mapper_counters(b2s_handle* h, const b2s_submap* sm, b2s_mapper_counters* out);
 
+/* ---- localisation against a prior map (MapperParameters::isUseInitialMap_ / isMergeScansIntoMap_, Parameters.hpp:173-174) --------
+ * The reference's rules, with paths relative to open3d_slam/open3d_slam/:
+ *   1. initial map (SlamWrapper::setInitialMap, src/SlamWrapper.cpp:209-220): normals on the full map (prepareInitialMap: the caller runs
+ *      b2s_estimate_normals), then Submap::insertScan's initial branch, mapCloud_ = map; voxelize(mapVoxelSize) ([O3D] VoxelDownSample,
+ *      normals averaged, no carving, no fusion, src/Submap.cpp:47-52): b2s_submap_set_initial_map.
+ *   2. initial pose (SlamWrapper::setInitialTransform, :222-225): Mapper::setMapToRangeSensorInitial, mapToRangeSensor_ =
+ *      mapToRangeSensorPrev_ = T and isNewInitialValueSet_ = true (src/Mapper.cpp:87-91): b2s_submap_set_initial_transform.  The
+ *      odometry half is b2s_odometry_set_initial_transform.
+ *   3. the next step of b2s_mapper_step_* / b2s_slam_step_* (src/Mapper.cpp:130-149): the guess is the pose without odometry, the ICP
+ *      runs and its result is discarded, the pose stays T (the slam step pushes it into the map-pose buffer), no fitness gate, no
+ *      insertion, the step counts as accepted (the dense map is fed at T), lastMeasurementTimestamp_ is kept, and the step after it
+ *      predicts without odometry as well.
+ *   4. pure localisation (merge off, :163-167): an accepted scan moves the pose only -- no carving, no insertion, the pose of the last
+ *      insertion is kept.  The dense map is still fed.  b2s_submap_set_merge_scans(sm, 0); on is the default (mapping).
+ *   5. localisation with map building (merge on) merges as in mapping; the submap hand-over is host policy (SubmapCollection).
+ * Eager steps and graph replay follow the same rules; switching the merge flag drops a captured graph. */
+int32_t b2s_submap_set_initial_map(b2s_handle* h, b2s_submap* sm, const b2s_cloud* cloud, double map_voxel_size);
+int32_t b2s_submap_set_initial_transform(b2s_handle* h, b2s_submap* sm, const double map_to_sensor[16]);
+int32_t b2s_submap_set_merge_scans(b2s_handle* h, b2s_submap* sm, int32_t on);
+/* Static map patch.  While a submap's merge is off its map cannot change, so its slots are kept counting-sorted by a 2 m tile (built by
+ * the first registration after merge goes off), and every registration against it (the device chains and b2s_register_to_submap)
+ * gathers its patch from the tiles the cropper's box touches: the same indexed points, grid header and original indices as the full
+ * path, at O(points in the touched tiles) instead of O(map).  A cropper without a bounded extent (MIN_RADIUS, invert) uses the full
+ * path; b2s_submap_set_cloud / _set_initial_map / _insert / _carve / _transform and switching merge on drop the table (and a captured
+ * chain that reads it).  B2S_PATCH_FULL=1 in the environment forces the full path (read once per process).
+ * Debug aid: header {origin, cell}, {dims, ncell, n}, cell starts and original indices of the NN index the last registration built. */
+int32_t b2s_debug_nn_index(b2s_handle* h, double origin_cell[4], int32_t dims_n[5], int32_t* cell_start, size_t cap_cells, int32_t* orig,
+                           size_t cap_pts);
+
 /* ---- device-resident LidarOdometry (src/Odometry.cpp:19-110) and the combined per-scan step of SlamWrapper: odometry, then
  *      Mapper::addRangeMeasurement with the prediction read from the odometry's TransformInterpolationBuffer on the device.
  *      Every decision (initialise / ok / failed, the buffer, the prediction, the mapper gates) is taken on the device.

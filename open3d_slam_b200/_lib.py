@@ -158,6 +158,7 @@ SYMBOLS = [
     "b2s_slam_motion_fetch", "b2s_slam_undistorted",
     "b2s_default_odometry_constraint_params", "b2s_submap_odometry_constraints",
     "b2s_default_global_optimization_params", "b2s_global_optimization", "b2s_cloud_transform_inplace",
+    "b2s_submap_set_initial_map", "b2s_submap_set_initial_transform", "b2s_submap_set_merge_scans", "b2s_debug_nn_index",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 PROFILE_KINDS = ["icp", "normals", "radix_sort", "nn_grid_build", "voxel", "fuse", "select", "crop"]

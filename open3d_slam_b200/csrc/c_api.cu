@@ -30,14 +30,16 @@ __global__ void empty_check_kernel(const int32_t* a, const int32_t* b, uint32_t*
   if (*a <= 0 || *b <= 0) atomicOr(status, ST_EMPTY);
 }
 
-// guess = pose * odom ; (row-major 4x4)
-__global__ void compose_kernel(const double* __restrict__ A, const double* __restrict__ B, double* __restrict__ C) {
+// guess = pose * odom ; (row-major 4x4).  After a new initial value, and in the step that follows it, the guess is the pose
+// itself (Mapper.cpp:130-138: no odometry prediction while isNewInitialValueSet_ or isIgnoreOdometryPrediction_)
+__global__ void compose_kernel(const double* __restrict__ A, const double* __restrict__ B, double* __restrict__ C, const int32_t* __restrict__ ms) {
   pdl_wait();
   const int i = threadIdx.x >> 2, j = threadIdx.x & 3;
+  const bool hold = ms[MS_NEWINIT] || ms[MS_IGNODOM];
   if (threadIdx.x < 16) {
     double s = 0.0;
     for (int k = 0; k < 4; k++) s += A[4 * i + k] * B[4 * k + j];
-    C[4 * i + j] = s;
+    C[4 * i + j] = hold ? A[4 * i + j] : s;
   }
 }
 
@@ -46,19 +48,24 @@ __global__ void compose_kernel(const double* __restrict__ A, const double* __res
 //   minimum-motion gate (:170-176) sensorMotion = mapToRangeSensorLastScanInsertion_^-1 * mapToRangeSensor_ (pose slot 5)
 //   carving schedule               Submap::carve: map not empty and nScansInsertedMap_ % N == 1 (Submap.cpp:111)
 //   dense map                      fed with every accepted scan (SlamWrapper.cpp:318-327), carved when nScansInsertedDenseMap_ % N == 1
+//   new initial value (:143-149)   the first step after b2s_submap_set_initial_transform counts as accepted, keeps the pose (the ICP
+//                                  result is discarded), inserts nothing and makes the next step ignore the odometry prediction
+//   pure localisation (:163-167)   merge_on == 0: an accepted scan updates the pose only; no carving, no insertion
 // and the copy of the result into this step's slot of the result ring (slots == nullptr: the result already sits in its slot).
 struct GateArgs {
   double min_fitness, min_move;
-  int ignore_fitness, carve_on, carve_n, dense_on, dcarve_n, pad;
+  int ignore_fitness, carve_on, carve_n, dense_on, dcarve_n, merge_on;
 };
 __global__ void mapper_gate_kernel(const b2s_result* __restrict__ res, GateArgs a, double* pose, int32_t* ms, const int32_t* __restrict__ map_n,
                                    b2s_result* slots, const int32_t* __restrict__ gstate) {
   pdl_wait();
   if (threadIdx.x != 0) return;
-  const bool accepted = a.ignore_fitness || !(res->fitness < a.min_fitness);
-  if (accepted) for (int i = 0; i < 16; i++) pose[i] = res->T[i];
-  bool insert = accepted;
-  if (accepted && a.min_move > 0.0) {
+  const int init = ms[MS_NEWINIT];
+  ms[MS_NEWINIT] = 0; ms[MS_IGNODOM] = init; ms[MS_INITSTEP] = init;   // isIgnoreOdometryPrediction_ lasts exactly one step
+  const bool accepted = init || a.ignore_fitness || !(res->fitness < a.min_fitness);
+  if (accepted && !init) for (int i = 0; i < 16; i++) pose[i] = res->T[i];
+  bool insert = accepted && !init && a.merge_on;
+  if (insert && a.min_move > 0.0) {
     // Eigen: inverse of an isometry = (R^T, -(R^T t)); translation of the product A * B = A.linear() * B.translation() + A.translation()
     const double* L = pose + 5 * 16;
     const double* P = pose;
@@ -178,15 +185,18 @@ int32_t mapper_chain_tail(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_sc
   int32_t* ms = sm->mstate.as<int32_t>();
   GateArgs ga;
   ga.min_fitness = min_fitness; ga.min_move = o.min_movement_between_mapping_steps; ga.ignore_fitness = ignore_fitness;
-  ga.carve_on = o.carve_enabled; ga.carve_n = o.carve_every_n_scans; ga.dense_on = o.dense_enabled; ga.dcarve_n = o.dense_carve_every_n_scans; ga.pad = 0;
+  ga.carve_on = o.carve_enabled; ga.carve_n = o.carve_every_n_scans; ga.dense_on = o.dense_enabled; ga.dcarve_n = o.dense_carve_every_n_scans;
+  ga.merge_on = sm->merge_scans ? 1 : 0;
   launch_pdl(mapper_gate_kernel, 1, 32, 0, h->stream, res, ga, pose_state, ms, sm->cloud[0]->dn.as<int32_t>(), slots, gstate);
   h->launches++;
-  if (o.carve_enabled) {   // Submap::insertScan: carve BEFORE the scan is appended, cropper still at the pose of the last insertion
-    B2S_REQUIRE(o.carving.voxel_size > 0.0, B2S_E_INVALID, "carving voxel size must be > 0");
-    CropDev crop = make_crop(&h->cfg.scan.map_builder_cropper, pose_state + 5 * 16);
-    B2S_TRY(op_submap_carve(h, sm, raw_scan, pose_state, crop, o.carving, nullptr, ms + MS_CARVE));
+  if (sm->merge_scans) {   // pure localisation (merge off): the sparse map is never written, so neither kernel is launched
+    if (o.carve_enabled) {   // Submap::insertScan: carve BEFORE the scan is appended, cropper still at the pose of the last insertion
+      B2S_REQUIRE(o.carving.voxel_size > 0.0, B2S_E_INVALID, "carving voxel size must be > 0");
+      CropDev crop = make_crop(&h->cfg.scan.map_builder_cropper, pose_state + 5 * 16);
+      B2S_TRY(op_submap_carve(h, sm, raw_scan, pose_state, crop, o.carving, nullptr, ms + MS_CARVE));
+    }
+    B2S_TRY(op_submap_insert(h, sm, merge, pose_state, ms + MS_INSERT));                                // Mapper.cpp:174
   }
-  B2S_TRY(op_submap_insert(h, sm, merge, pose_state, ms + MS_INSERT));                                  // Mapper.cpp:174
   if (o.dense_enabled) {
     if (sm->dense_cap == 0) {
       B2S_REQUIRE(h->cfg.dense_voxel_size > 0.0, B2S_E_INVALID, "dense_voxel_size must be > 0");
@@ -215,7 +225,7 @@ static int32_t mapper_chain_graphable(void* ctx) {
   launch_pdl(graph_begin_kernel, 1, 32, 0, h->stream, ring_dev, gstate, odom);
   h->launches++;
   B2S_TRY(process_scan_impl(h, sm->staging.get(), h->t1.get(), h->t2.get()));
-  launch_pdl(compose_kernel, 1, 32, 0, h->stream, pose_state, odom, guess);
+  launch_pdl(compose_kernel, 1, 32, 0, h->stream, pose_state, odom, guess, static_cast<const int32_t*>(sm->mstate.as<int32_t>()));
   h->launches++;
   B2S_TRY(register_to_submap_async(h, h->t2.get(), sm, nullptr, pose_state, nullptr, guess, res));
   return mapper_chain_tail(h, sm, sm->staging.get(), h->t1.get(), res, sm->g_min_fitness, sm->g_ignore_fitness, h->slots.as<b2s_result>(), gstate);
@@ -819,6 +829,7 @@ int32_t b2s_cloud_transform_inplace(b2s_handle* h, b2s_cloud* c, const double T[
 int32_t b2s_submap_transform(b2s_handle* h, b2s_submap* sm, const double T[16]) {
   B2S_REQUIRE(h && sm && T, B2S_E_INVALID, "null argument");
   LOCK(h);
+  B2S_TRY(tile_drop(h, sm));
   return op_submap_transform(h, sm, T);
 }
 
@@ -832,6 +843,7 @@ int32_t b2s_submap_get_pose(b2s_handle* h, const b2s_submap* sm, double T[16]) {
 int32_t b2s_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, const double T[16]) {
   B2S_REQUIRE(h && sm && scan && T, B2S_E_INVALID, "null argument");
   LOCK(h);
+  B2S_TRY(tile_drop(h, sm));
   double* Td = sm->pose.as<double>() + 16;  // slot 1: pose used by this insertion
   B2S_TRY(pose_to_device(h, T, Td));
   return op_submap_insert(h, sm, scan, Td, nullptr);
@@ -842,6 +854,7 @@ int32_t b2s_submap_carve(b2s_handle* h, b2s_submap* sm, const b2s_cloud* raw_sca
   B2S_REQUIRE(h && sm && raw_scan && T && cropper_pose && prm, B2S_E_INVALID, "null argument");
   B2S_REQUIRE(prm->voxel_size > 0.0, B2S_E_INVALID, "carving voxel size must be > 0");
   LOCK(h);
+  B2S_TRY(tile_drop(h, sm));
   double* Td = sm->pose.as<double>() + 64;   // slot 4: pose of the carving scan
   B2S_TRY(pose_to_device(h, T, Td));
   b2s_cropper c = h->cfg.scan.map_builder_cropper;   // mapBuilderCropper_ at the pose of the previous insertion
@@ -929,6 +942,7 @@ int32_t b2s_submap_set_cloud(b2s_handle* h, b2s_submap* sm, const b2s_cloud* clo
   B2S_REQUIRE(cloud->has_normals || h->cfg.icp.reg_type == B2S_REG_POINT_TO_POINT, B2S_E_NO_NORMALS, "map cloud needs normals for this registration type");
   B2S_REQUIRE(cloud->n_max <= sm->capacity, B2S_E_CAPACITY, "cloud larger than the submap capacity");
   LOCK(h);
+  B2S_TRY(tile_drop(h, sm));
   b2s_cloud* m = sm->cloud[0].get();
   if (cloud->n_max) {
     B2S_CUDA(cudaMemcpyAsync(m->xyz.p, cloud->xyz.p, cloud->n_max * 24, cudaMemcpyDeviceToDevice, h->stream));
@@ -943,6 +957,48 @@ int32_t b2s_submap_set_cloud(b2s_handle* h, b2s_submap* sm, const b2s_cloud* clo
   return fuse_rehash(h, sm);
 }
 
+// Submap::insertScan's initial-map branch (src/Submap.cpp:47-52): mapCloud_ = cloud; voxelize(mapVoxelSize) -- [O3D] VoxelDownSample on
+// the data-dependent grid, normals averaged, no carving, no fusion; nScansInsertedMap_ is not counted.  voxelize returns early for a voxel
+// size <= 0 (helpers.cpp:107-113): the cloud is then loaded as it is.
+int32_t b2s_submap_set_initial_map(b2s_handle* h, b2s_submap* sm, const b2s_cloud* cloud, double map_voxel_size) {
+  B2S_REQUIRE(h && sm && cloud, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(sm->h == h && cloud->h == h, B2S_E_INVALID, "the submap or the cloud belongs to another handle");
+  LOCK(h);
+  b2s_cloud* v = h->t3.get();
+  {
+    WideGridScope wide(cloud->n_max);
+    B2S_TRY(op_voxel_down_sample(h, cloud, nullptr, map_voxel_size, v));   // voxel <= 0: plain device copy
+  }
+  size_t n = 0;
+  v->n_known = -1;
+  B2S_TRY(cloud_count_sync(h, v, &n));   // one-off load: the exact size bounds every later launch over the map
+  v->n_max = n;
+  return b2s_submap_set_cloud(h, sm, v);
+}
+
+// Mapper::setMapToRangeSensorInitial (src/Mapper.cpp:87-91): mapToRangeSensor_ = mapToRangeSensorPrev_ = T, isNewInitialValueSet_ = true.
+// The pose slot and the flag are device words the captured chains read, so a replayed graph picks both up.
+int32_t b2s_submap_set_initial_transform(b2s_handle* h, b2s_submap* sm, const double T[16]) {
+  B2S_REQUIRE(h && sm && T, B2S_E_INVALID, "null argument");
+  LOCK(h);
+  B2S_TRY(pose_to_device(h, T, sm->pose.as<double>()));
+  launch_pdl(write_i32_kernel, 1, 1, 0, h->stream, sm->mstate.as<int32_t>() + MS_NEWINIT, (int32_t)1);
+  h->launches++;
+  B2S_CUDA(cudaGetLastError());
+  return B2S_OK;
+}
+
+// MapperParameters::isMergeScansIntoMap_ for the chain on this submap (Mapper.cpp:163-167).  Off: accepted scans move the pose only.
+int32_t b2s_submap_set_merge_scans(b2s_handle* h, b2s_submap* sm, int32_t on) {
+  B2S_REQUIRE(h && sm, B2S_E_INVALID, "null argument");
+  LOCK(h);
+  if (sm->merge_scans == (on != 0)) return B2S_OK;
+  sm->merge_scans = on != 0;
+  if (on) B2S_TRY(tile_drop(h, sm));   // the chain writes the map again: the table would go stale
+  sm->opts_gen++;   // the combined chain's graphs compare it
+  return graph_drop(h, &sm->graph);
+}
+
 }  // extern "C"
 
 int32_t b2s::register_to_submap_async(b2s_handle* h, const b2s_cloud* scan, const b2s_submap* sm, const double* sensor_pose_host,
@@ -953,7 +1009,10 @@ int32_t b2s::register_to_submap_async(b2s_handle* h, const b2s_cloud* scan, cons
   b2s_cropper c = h->cfg.scan.scan_matcher_cropper;  // ScanToMapRegistration.cpp:58 setPose(mapToRangeSensor)
   if (sensor_pose_host) { c.center[0] = sensor_pose_host[3]; c.center[1] = sensor_pose_host[7]; c.center[2] = sensor_pose_host[11]; }
   CropDev patch = make_crop(&c, sensor_pose_dev);
-  B2S_TRY(grid_build(h, &h->grid_a, map, nn_cell(h, h->cfg.icp.max_corr_dist), &patch));
+  if (tile_patch_usable(sm, patch))   // frozen map: the patch from the tiles the cropper touches (K-patch, grid_index.cu)
+    B2S_TRY(tile_patch_build(h, const_cast<b2s_submap*>(sm), patch, nn_cell(h, h->cfg.icp.max_corr_dist), &h->grid_a));
+  else
+    B2S_TRY(grid_build(h, &h->grid_a, map, nn_cell(h, h->cfg.icp.max_corr_dist), &patch));
   B2S_TRY(h->work_xyz.ensure(icp_work_bytes(scan->n_max), h->stream));
   B2S_TRY(h->problems.ensure(sizeof(IcpProblem), h->stream));
   IcpProblem P;
@@ -990,7 +1049,7 @@ int32_t b2s_mapper_step_async(b2s_handle* h, b2s_submap* sm, const b2s_cloud* ra
   b2s_result* res = h->slots.as<b2s_result>() + slot;
   B2S_TRY(process_scan_impl(h, raw_scan, h->t1.get(), h->t2.get()));          // Mapper.cpp:139
   B2S_TRY(pose_to_device(h, odometry_motion, odom));
-  launch_pdl(compose_kernel, 1, 32, 0, h->stream, pose_state, odom, guess);           // Mapper.cpp:130-137
+  launch_pdl(compose_kernel, 1, 32, 0, h->stream, pose_state, odom, guess, static_cast<const int32_t*>(sm->mstate.as<int32_t>()));   // Mapper.cpp:130-138
   h->launches++;
   B2S_TRY(register_to_submap_async(h, h->t2.get(), sm, nullptr, pose_state, nullptr, guess, res));  // Mapper.cpp:140-141
   return mapper_chain_tail(h, sm, raw_scan, h->t1.get(), res, min_refinement_fitness, ignore_min_fitness, nullptr, nullptr);   // Mapper.cpp:151-177
@@ -1301,6 +1360,27 @@ int32_t b2s_global_optimization(b2s_handle* h, int32_t n_nodes, double* node_pos
                 "edge %d: node ids (%d, %d) outside [0, %d)", (int)e, (int)edges[e].source, (int)edges[e].target, (int)n_nodes);
   LOCK(h);
   return op_global_optimization(h, n_nodes, node_poses, n_edges, edges, *p, edge_kept_out, edge_confidence_out, stats_out);
+}
+
+// debug aid for tests: the header, cell starts and original indices of the NN index the last registration built (h->grid_a).
+// dims_n = {dims[0..2], ncell, n}; cell_start (ncell + 1 entries) and orig (n entries) are skipped when null or too small.
+int32_t b2s_debug_nn_index(b2s_handle* h, double origin_cell[4], int32_t dims_n[5], int32_t* cell_start, size_t cap_cells, int32_t* orig,
+                           size_t cap_pts) {
+  B2S_REQUIRE(h && origin_cell && dims_n, B2S_E_INVALID, "null argument");
+  LOCK(h);
+  B2S_REQUIRE(h->grid_a.hdr.p, B2S_E_INVALID, "no NN index has been built yet");
+  GridHeader gh;
+  B2S_TRY(read_back(h, {{&gh, h->grid_a.hdr.p, sizeof(gh)}}));
+  for (int d = 0; d < 3; d++) { origin_cell[d] = gh.origin[d]; dims_n[d] = gh.dims[d]; }
+  origin_cell[3] = gh.cell; dims_n[3] = gh.ncell; dims_n[4] = gh.n;
+  if (cell_start && cap_cells >= (size_t)gh.ncell + 1)
+    B2S_CUDA(cudaMemcpy(cell_start, grid_starts(&h->grid_a), ((size_t)gh.ncell + 1) * 4, cudaMemcpyDeviceToHost));
+  if (orig && cap_pts >= (size_t)gh.n && gh.n > 0) {
+    std::vector<double> p4((size_t)gh.n * 4);
+    B2S_CUDA(cudaMemcpy(p4.data(), h->grid_a.pts.p, p4.size() * 8, cudaMemcpyDeviceToHost));
+    for (int32_t k = 0; k < gh.n; k++) { long long v; memcpy(&v, &p4[4 * (size_t)k + 3], 8); orig[k] = (int32_t)v; }
+  }
+  return B2S_OK;
 }
 
 }  // extern "C"

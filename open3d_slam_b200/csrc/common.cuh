@@ -218,6 +218,16 @@ struct b2s_submap {
   b2s_mapper_options opts;
   unsigned long long opts_gen = 1;    // bumped by b2s_submap_set_mapper_options: graphs of other objects that run this chain compare it
   b2s::DevBuf mstate;                 // int32 [MS_WORDS]: gates and counters of the chain, see the MS_* indices below
+  // MapperParameters::isMergeScansIntoMap_ as the chain sees it (b2s_submap_set_merge_scans): off = pure localisation, the chain
+  // neither carves nor fuses (Mapper.cpp:163-167); part of the captured chain, so switching drops the graph like the options do
+  bool merge_scans = true;
+  // static map patch (grid_index.cu): while merge_scans is off the sparse map cannot change, so its slots are kept counting-sorted by a
+  // coarse tile cell (a GridIndex built with the tile edge and no cropper) and every registration gathers its patch from the tiles the
+  // cropper's box touches.  Built by the first registration after merge goes off; dropped by every call that writes the map.
+  b2s::GridIndex tile;
+  bool tile_valid = false;
+  std::unique_ptr<b2s_cloud> patch;   // the gathered patch points (sized like the map, so the NN grid gets the full path's cell budget) ...
+  b2s::DevBuf patch_idx;              // ... and each one's map slot, the original index the NN grid stores
   // the map has no normals (stored as NaN): loaded without them, or fed a scan without them.  [O3D] PointCloud::operator+= drops a
   // cloud's normals as soon as one part lacks them, so the reference's map stays without normals from then on, and so does this flag
   bool no_normals = false;
@@ -253,6 +263,9 @@ enum MapperStateWord {
   MS_TICKET2 = 23,
   MS_WSEL = 24,       // which half of `wlist` is current
   MS_NW = 25,         // [25], [26]: entries of the two halves
+  MS_NEWINIT = 27,    // Mapper::isNewInitialValueSet_: set by b2s_submap_set_initial_transform, cleared by the next step (Mapper.cpp:87-91,143-149)
+  MS_IGNODOM = 28,    // Mapper::isIgnoreOdometryPrediction_: the step after a new initial value predicts without odometry (Mapper.cpp:130-138)
+  MS_INITSTEP = 29,   // this step was the first after a new initial value: ICP result discarded, lastMeasurementTimestamp_ kept
   MS_WORDS = 32
 };
 // bumped by every DevBuf re-allocation: a captured graph holds raw pointers of the scratch buffers, so a graph captured
@@ -363,7 +376,18 @@ struct CropDev {      // cropper passed by value to kernels; centre may come fro
   const double* pose_dev;   // if non-null the centre is (pose[3], pose[7], pose[11])
 };
 CropDev make_crop(const b2s_cropper* c, const double* pose_dev = nullptr);
-int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch);
+// orig (optional): per point of cloud the original index the grid stores (default: the point's own index)
+int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch, const int32_t* orig = nullptr);
+// static map patch (grid_index.cu): true when sm's merge is off, the cropper is bounded and B2S_PATCH_FULL is not set
+bool tile_patch_usable(const b2s_submap* sm, const CropDev& crop);
+// builds the tile table if it is not valid, gathers the tiles the cropper touches, and builds g over the gathered points that pass
+// crop_within, each keeping its map slot as original index: the same indexed set, grid header and original indices as
+// grid_build(map, cell, &crop)
+int32_t tile_patch_build(b2s_handle* h, b2s_submap* sm, const CropDev& crop, double cell, GridIndex* g);
+// every call that writes a submap's map drops its tile table (and the captured chains that read it)
+int32_t tile_drop(b2s_handle* h, b2s_submap* sm);
+constexpr double TILE_EDGE = 2.0;        // tile edge of the static patch table (m)
+constexpr int TILE_MARGIN = 1;           // tiles added on every side of the cropper's box: rounding of the box and of crop_within
 // the same for n clouds at once (batched registration: every pair brings its own target), blockIdx.y = cloud
 int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* const* clouds, int n, double cell);
 

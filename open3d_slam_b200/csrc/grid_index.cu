@@ -10,6 +10,8 @@
 // Points outside the grid box are clamped into the border cells, which the search treats as semi-infinite.
 //
 // Build = bbox reduce -> header (1 thread) -> count (atomics, keeps the rank) -> look-back scan -> scatter.
+#include <stdlib.h>
+
 #include "common.cuh"
 
 namespace b2s {
@@ -121,7 +123,7 @@ __global__ void __launch_bounds__(GB_THREADS) grid_count_kernel(const double* __
 
 __device__ __forceinline__ void grid_scatter_body(const double* __restrict__ xyz, const int32_t* __restrict__ d_n, GridHeader* hdr,
                                                   const int32_t* __restrict__ cell_start, const int32_t* __restrict__ rank,
-                                                  double4* __restrict__ pts) {
+                                                  double4* __restrict__ pts, const int32_t* __restrict__ orig) {
   const int n = *d_n;
   __shared__ GridHeader g;
   if (threadIdx.x == 0) g = *hdr;
@@ -132,15 +134,16 @@ __device__ __forceinline__ void grid_scatter_body(const double* __restrict__ xyz
     if (r < 0) continue;
     double x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
     int slot = cell_start[grid_cell_of(g, x, y, z)] + r;
-    pts[slot] = make_double4(x, y, z, __longlong_as_double((long long)i));
+    pts[slot] = make_double4(x, y, z, __longlong_as_double((long long)(orig ? orig[i] : i)));
   }
 }
 
 __global__ void __launch_bounds__(GB_THREADS) grid_scatter_kernel(const double* __restrict__ xyz, const int32_t* __restrict__ d_n,
                                                                   GridHeader* hdr, const int32_t* __restrict__ cell_start,
-                                                                  const int32_t* __restrict__ rank, double4* __restrict__ pts) {
+                                                                  const int32_t* __restrict__ rank, double4* __restrict__ pts,
+                                                                  const int32_t* __restrict__ orig) {
   pdl_wait();
-  grid_scatter_body(xyz, d_n, hdr, cell_start, rank, pts);
+  grid_scatter_body(xyz, d_n, hdr, cell_start, rank, pts, orig);
 }
 
 // ---- batched build: blockIdx.y = job -------------------------------------------------------------------------------
@@ -183,7 +186,7 @@ __global__ void __launch_bounds__(GB_THREADS) gridb_count_kernel(const GridJob* 
 __global__ void __launch_bounds__(GB_THREADS) gridb_scatter_kernel(const GridJob* __restrict__ jobs) {
   pdl_wait();
   const GridJob j = jobs[blockIdx.y];
-  grid_scatter_body(j.xyz, j.d_n, j.hdr, j.starts, j.rank, j.pts);
+  grid_scatter_body(j.xyz, j.d_n, j.hdr, j.starts, j.rank, j.pts, nullptr);
 }
 
 CropDev make_crop(const b2s_cropper* c, const double* pose_dev) {
@@ -197,7 +200,7 @@ CropDev make_crop(const b2s_cropper* c, const double* pose_dev) {
   return d;
 }
 
-int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch) {
+int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch, const int32_t* orig) {
   B2S_REQUIRE(cell > 0.0, B2S_E_INVALID, "grid_build: cell size must be > 0");
   const size_t n_max = cloud->n_max > 0 ? cloud->n_max : 1;
   // buffers follow the ALLOCATION of the cloud, not its current size: a growing map never re-allocates its index
@@ -234,7 +237,7 @@ int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double c
   // scan over ncell (device-known) counts; launch sized for the capacity
   B2S_TRY(scan_exclusive_i32(h, counts, starts, &hdr->ncell, (size_t)g->cap_cells, nullptr));
   launch_pdl(grid_scatter_kernel, blocks, GB_THREADS, 0, h->stream, cloud->xyz.as<double>(), d_n, hdr, starts, g->rank.as<int32_t>(),
-             g->pts.as<double4>());
+             g->pts.as<double4>(), orig);
   h->launches++;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;
@@ -312,6 +315,106 @@ int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* co
   h->launches++;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;
+}
+
+// ---- K-patch: the static map patch of a submap whose map cannot change (merge off, pure localisation) -------------------------------
+// Tile table: the submap's GridIndex `tile`, built once over the map slots with cell = TILE_EDGE and no cropper (the K-index build:
+// bbox -> header -> count -> scan -> scatter), so the slots are counting-sorted by tile, x fastest, and a run of tiles along x is one
+// contiguous slot range.  The header doubles the edge when the map's box needs more than the cell budget, like every K-index build.
+// Per registration: tile_gather_kernel reads the sensor position from the device pose (or the host-given centre), takes the tiles the
+// cropper's box overlaps, grown by TILE_MARGIN tiles on every side (the box is computed in rounded arithmetic, and crop_within accepts a
+// point up to a few ulps outside it), and appends the points of those tiles that pass the unchanged crop_within, each with its map slot.
+// The NN grid is then built over exactly those points with the slot as original index: the same set, bbox, header and original indices
+// as the full path's crop inside the build, at O(points in the touched tiles) instead of O(map).  Why 2 m: a few map voxels, fine enough
+// that the cube of tiles around a 20-30 m cropper holds little beyond the sphere's own box, coarse enough that a site-sized map's table
+// stays within the cell budget.  Launches are sized from the map's bound (grid-stride over the device count): graph-capturable.
+__global__ void tile_zero_kernel(int32_t* n) {
+  pdl_wait();
+  if (threadIdx.x == 0) *n = 0;
+}
+
+// the tile box of the cropper: [lo, hi] per axis, clamped to the table; empty when lo > hi on an axis
+__device__ __forceinline__ void tile_box(const GridHeader& g, const CropDev& crop, int* box) {
+  double c[3] = {crop.cx, crop.cy, crop.cz};
+  if (crop.pose_dev) { c[0] = crop.pose_dev[3]; c[1] = crop.pose_dev[7]; c[2] = crop.pose_dev[11]; }
+  double lo[3], hi[3];
+  for (int d = 0; d < 3; d++) { lo[d] = c[d] - crop.rmax; hi[d] = c[d] + crop.rmax; }
+  if (crop.kind == B2S_CROP_CYLINDER) { lo[2] = crop.zmin; hi[2] = crop.zmax; }   // crop_within compares the absolute z
+  for (int d = 0; d < 3; d++) {
+    const double a = fmax(floor((lo[d] - g.origin[d]) * g.inv_cell) - TILE_MARGIN, 0.0);
+    const double b = fmin(floor((hi[d] - g.origin[d]) * g.inv_cell) + TILE_MARGIN, (double)(g.dims[d] - 1));
+    const bool ok = a <= b;   // false for NaN as well
+    box[d] = ok ? (int)a : 1;
+    box[3 + d] = ok ? (int)b : 0;
+  }
+}
+
+__global__ void __launch_bounds__(GB_THREADS) tile_gather_kernel(const GridHeader* __restrict__ thdr, const int32_t* __restrict__ tstart,
+                                                                 const double4* __restrict__ tpts, CropDev crop, double* __restrict__ out_xyz,
+                                                                 int32_t* __restrict__ out_idx, int32_t* __restrict__ out_n) {
+  pdl_wait();
+  __shared__ GridHeader g;
+  __shared__ int box[6];
+  if (threadIdx.x == 0) { g = *thdr; tile_box(g, crop, box); }
+  __syncthreads();
+  if (box[0] > box[3] || box[1] > box[4] || box[2] > box[5]) return;
+  const int ny = box[4] - box[1] + 1, nz = box[5] - box[2] + 1;
+  const int lane = threadIdx.x & 31;
+  for (int r = blockIdx.x; r < ny * nz; r += gridDim.x) {   // one (y, z) row of tiles per CTA
+    const int row = ((box[2] + r / ny) * g.dims[1] + (box[1] + r % ny)) * g.dims[0];
+    const int s0 = tstart[row + box[0]], s1 = tstart[row + box[3] + 1];
+    for (int j0 = s0; j0 < s1; j0 += blockDim.x) {   // uniform trip count over the CTA: every lane reaches the ballot
+      const int j = j0 + threadIdx.x;
+      double4 q = make_double4(0.0, 0.0, 0.0, 0.0);
+      bool pass = false;
+      if (j < s1) { q = tpts[j]; pass = crop_within(crop, q.x, q.y, q.z); }
+      const unsigned m = __ballot_sync(0xffffffffu, pass);
+      int base = 0;
+      if (lane == 0 && m) base = atomicAdd(out_n, __popc(m));
+      base = __shfl_sync(0xffffffffu, base, 0);
+      if (pass) {
+        const int o = base + __popc(m & ((1u << lane) - 1u));
+        out_xyz[3 * o] = q.x; out_xyz[3 * o + 1] = q.y; out_xyz[3 * o + 2] = q.z;
+        out_idx[o] = (int32_t)__double_as_longlong(q.w);
+      }
+    }
+  }
+}
+
+bool tile_patch_usable(const b2s_submap* sm, const CropDev& crop) {
+  // B2S_PATCH_FULL=1: every registration builds its patch from the whole map (A/B switch and test reference; read once per process)
+  static const bool full = getenv("B2S_PATCH_FULL") && atoi(getenv("B2S_PATCH_FULL")) != 0;
+  const bool bounded = !crop.invert && (crop.kind == B2S_CROP_MAX_RADIUS || crop.kind == B2S_CROP_MINMAX_RADIUS || crop.kind == B2S_CROP_CYLINDER);
+  return !full && !sm->merge_scans && bounded;
+}
+
+int32_t tile_drop(b2s_handle* h, b2s_submap* sm) {
+  if (!sm->tile_valid) return B2S_OK;
+  sm->tile_valid = false;
+  sm->opts_gen++;                      // the combined chain's graphs compare it
+  return graph_drop(h, &sm->graph);    // a captured chain reads the table: never replay it over a dropped one
+}
+
+int32_t tile_patch_build(b2s_handle* h, b2s_submap* sm, const CropDev& crop, double cell, GridIndex* g) {
+  const b2s_cloud* map = sm->cloud[0].get();
+  const size_t map_alloc = map->xyz.cap / 24;
+  if (!sm->patch) B2S_TRY(make_cloud(h, map_alloc, false, false, &sm->patch));
+  b2s_cloud* pc = sm->patch.get();
+  B2S_TRY(cloud_reserve(h, pc, map_alloc, false));   // the map's allocation: the NN grid's cell budget follows it
+  B2S_TRY(sm->patch_idx.ensure(map_alloc * 4 + 16, h->stream));
+  if (!sm->tile_valid) {
+    B2S_TRY(grid_build(h, &sm->tile, map, TILE_EDGE, nullptr));
+    sm->tile_valid = true;
+  }
+  pc->n_max = map->n_max; pc->n_known = -1; pc->has_normals = false;
+  {
+    launch_pdl(tile_zero_kernel, 1, 32, 0, h->stream, pc->dn.as<int32_t>());
+    launch_pdl(tile_gather_kernel, 2 * device_sms(), GB_THREADS, 0, h->stream, static_cast<const GridHeader*>(sm->tile.hdr.as<GridHeader>()),
+               grid_starts(&sm->tile), static_cast<const double4*>(sm->tile.pts.as<double4>()), crop, pc->xyz.as<double>(),
+               sm->patch_idx.as<int32_t>(), pc->dn.as<int32_t>());
+    h->launches += 2;
+  }
+  return grid_build(h, g, pc, cell, nullptr, sm->patch_idx.as<int32_t>());
 }
 
 }  // namespace b2s

@@ -338,9 +338,12 @@ __global__ void odometry_keep_kernel(const double* __restrict__ pre_xyz, const d
 
 // Mapper.cpp:122-137: odom_used = has(t); motion = getTransform(t_last)^-1 * getTransform(t); guess = pose * motion
 // (pose slots of the submap: [0] mapToRangeSensor_, [2] odometry motion, [3] guess)
-__global__ void odometry_prediction_kernel(OdoState* s, const long long* __restrict__ ring_t, const double* __restrict__ ring_T, int cap, double* pose) {
+// After a new initial value, and in the step after it, the guess is the pose itself (Mapper.cpp:130-138; ms: the submap's MS_* words)
+__global__ void odometry_prediction_kernel(OdoState* s, const long long* __restrict__ ring_t, const double* __restrict__ ring_T, int cap, double* pose,
+                                           const int32_t* __restrict__ ms) {
   pdl_wait();
   if (threadIdx.x != 0) return;
+  const bool hold = ms[MS_NEWINIT] || ms[MS_IGNODOM];
   const BufferView b = buffer_view(s, ring_t, ring_T, cap);
   const bool used = b.has(s->t_cur);
   double M[16];
@@ -358,14 +361,15 @@ __global__ void odometry_prediction_kernel(OdoState* s, const long long* __restr
     for (int j = 0; j < 4; j++) {
       double acc = 0.0;
       for (int k = 0; k < 4; k++) acc += pose[4 * i + k] * M[4 * k + j];
-      G[4 * i + j] = acc;
+      G[4 * i + j] = hold ? pose[4 * i + j] : acc;
     }
   for (int i = 0; i < 16; i++) pose[48 + i] = G[i];
   s->odom_used = used;
 }
 
 // after the mapper's gate: for an accepted scan mapToRangeSensorBuffer_.push(t, mapToRangeSensor_) (Mapper.cpp:160, pose[0..15] is
-// the registration result by now) and lastMeasurementTimestamp_ = t (:164,178); then the combined result slot
+// the registration result by now) and lastMeasurementTimestamp_ = t (:164,178); then the combined result slot.  The first step after a
+// new initial value pushes the pose it kept and leaves lastMeasurementTimestamp_ alone (:143-149)
 __global__ void slam_post_kernel(OdoState* s, const int32_t* __restrict__ ms, const b2s_result* __restrict__ mres,
                                  const b2s_odometry_result* __restrict__ odo_slots, b2s_slam_result* slam_slots, const double* __restrict__ pose,
                                  long long* map_t, double* map_T, int cap) {
@@ -374,7 +378,7 @@ __global__ void slam_post_kernel(OdoState* s, const int32_t* __restrict__ ms, co
   const int accepted = ms[MS_ACCEPT];
   if (accepted) {
     BufferView::push(map_t, map_T, cap, &s->map_head, &s->map_count, s->t_cur, pose);
-    s->t_last = s->t_cur;
+    if (!ms[MS_INITSTEP]) s->t_last = s->t_cur;
   }
   b2s_slam_result* o = slam_slots + s->slot;
   o->odometry = odo_slots[s->slot];
@@ -492,7 +496,7 @@ static int32_t slam_chain(void* ctx) {
     raw = od->map_in.get();
   }
   launch_pdl(odometry_prediction_kernel, 1, 32, 0, h->stream, s, od->ring_t.as<long long>(), od->ring_T.as<double>(), od->params.buffer_size,
-             pose_state);
+             pose_state, static_cast<const int32_t*>(sm->mstate.as<int32_t>()));
   h->launches++;
   B2S_TRY(process_scan_impl(h, raw, h->t1.get(), h->t2.get()));                                                   // Mapper.cpp:139
   B2S_TRY(register_to_submap_async(h, h->t2.get(), sm, nullptr, pose_state, nullptr, pose_state + 48, mres));   // Mapper.cpp:140-141

@@ -126,6 +126,10 @@ class MapperParameters:
     denseMapCarving: SpaceCarvingParameters = field(default_factory=SpaceCarvingParameters)       # denseMapBuilder_.carving_
     isIgnoreMinRefinementFitness: bool = False
     minMovementBetweenMappingSteps: float = 0.0
+    # localisation against a prior map (Parameters.hpp:173-174), both false as in Lua (is_use_map_initialization /
+    # is_merge_scans_into_map); the C++ struct defaults the merge flag to true.  The merge flag only matters with isUseInitialMap.
+    isUseInitialMap: bool = False
+    isMergeScansIntoMap: bool = False
     seed: int = 0            # replaces std::random_device of [O3D] RandomDownSample
     nnCellSize: float = 0.0  # engine knob: NN grid cell (0 = maxCorrespondenceDistance / 4)
     icpClusterCtas: int = 0  # engine knob: SMs one registration spreads over (0 = automatic; 8 = throughput, 16 = latency)
@@ -892,6 +896,19 @@ class Submap:
     def setMapPointCloud(self, cloud: Cloud):
         L.check(L.lib().b2s_submap_set_cloud(self.eng._h, self._s, cloud._c))
 
+    def setInitialMap(self, cloud: Cloud, mapVoxelSize: float) -> None:
+        """Submap::insertScan's initial-map branch (src/Submap.cpp:47-52): the map becomes VoxelDownSample(cloud, mapVoxelSize), normals
+        averaged, without carving or fusion; nScansInsertedMap_ is not counted.  cloud carries the normals prepareInitialMap estimated."""
+        L.check(L.lib().b2s_submap_set_initial_map(self.eng._h, self._s, cloud._c, C.c_double(float(mapVoxelSize))))
+
+    def setInitialTransform(self, T) -> None:
+        """Mapper::setMapToRangeSensorInitial (src/Mapper.cpp:87-91) on the device pose slot: the next step keeps T (see b2s.h)"""
+        L.check(L.lib().b2s_submap_set_initial_transform(self.eng._h, self._s, _pd(_mat(T))))
+
+    def setMergeScans(self, on: bool) -> None:
+        """isMergeScansIntoMap_ for the device chain on this submap: off = pure localisation (src/Mapper.cpp:163-167)"""
+        L.check(L.lib().b2s_submap_set_merge_scans(self.eng._h, self._s, C.c_int32(1 if on else 0)))
+
     def computeFeatures(self, params: PlaceRecognitionParameters | None = None) -> None:
         """The feature half of Submap::computeFeatures (src/Submap.cpp:239-244): sparse cloud (voxel down-sample of the map), its
         normals, their FPFH -- on the device, kept on this object.  Repeated calls reuse the same cloud and feature."""
@@ -1315,7 +1332,36 @@ class Mapper:
         self.mapToRangeSensorPrev_ = np.eye(4)
         self.mapToRangeSensorLastScanInsertion_ = np.eye(4)
         self._first = True
+        self.isNewInitialValueSet_ = False
+        self.isIgnoreOdometryPrediction_ = False
         self.lastResult = None
+        if self.params_.isUseInitialMap and not self.params_.isMergeScansIntoMap:
+            self.submap.setMergeScans(False)
+
+    def setInitialMap(self, mapCloud: Cloud) -> None:
+        """SlamWrapper::setInitialMap (src/SlamWrapper.cpp:209-220) with isUseInitialMap_: prepareInitialMap (normals on the full map),
+        then the first-scan branch of addRangeMeasurement (Mapper.cpp:106-108), which loads the map voxelized (Submap.cpp:47-52)."""
+        if not self.params_.isUseInitialMap:
+            raise RuntimeError("setInitialMap needs MapperParameters.isUseInitialMap")
+        self.scan2MapReg_.prepareInitialMap(mapCloud)
+        if not self.scan2MapReg_.isMergeScanValid(mapCloud):
+            raise RuntimeError("Init map invalid!!!!")   # assert_true at Mapper.cpp:107
+        self.submap.setInitialMap(mapCloud, self.params_.mapBuilder.mapVoxelSize)
+        self._first = False
+
+    def setMapToRangeSensorInitial(self, T) -> None:
+        """src/Mapper.cpp:87-91, on the host state and on the device pose slot the device chain reads"""
+        self.mapToRangeSensor_ = _mat(T).copy()
+        self.mapToRangeSensorPrev_ = self.mapToRangeSensor_.copy()
+        self.isNewInitialValueSet_ = True
+        if self.submap is not None:
+            self.submap.setInitialTransform(T)
+
+    def _deviceStep(self) -> None:
+        """a device step applied rules 3 / the ignore-once rule to the device words: the host copies follow, so that the host flow
+        and the device chain can be mixed on one Mapper"""
+        self.isIgnoreOdometryPrediction_ = self.isNewInitialValueSet_
+        self.isNewInitialValueSet_ = False
 
     def addRangeMeasurement(self, rawScan: Cloud, odometryMotion=None) -> bool:
         if self._first:  # Mapper.cpp:105-114
@@ -1323,13 +1369,23 @@ class Mapper:
             self.submap.insertScan(rawScan, processed.merge_, np.eye(4))
             self._first = False
             return True
-        estimate = self.mapToRangeSensorPrev_ if odometryMotion is None else self.mapToRangeSensorPrev_ @ _mat(odometryMotion)
+        predict = odometryMotion is not None and not self.isNewInitialValueSet_ and not self.isIgnoreOdometryPrediction_   # :130-137
+        estimate = self.mapToRangeSensorPrev_ @ _mat(odometryMotion) if predict else self.mapToRangeSensorPrev_
+        self.isIgnoreOdometryPrediction_ = False
         processed = self.scan2MapReg_.processForScanMatchingAndMerging(rawScan, self.mapToRangeSensor_)
         result = self.scan2MapReg_.scanToMapRegistration(processed.match_, self.submap, self.mapToRangeSensor_, estimate)
         self.lastResult = result
+        if self.isNewInitialValueSet_:   # :143-149: the result is discarded, the pose stays the initial value
+            self.mapToRangeSensorPrev_ = self.mapToRangeSensor_.copy()
+            self.isNewInitialValueSet_ = False
+            self.isIgnoreOdometryPrediction_ = True
+            return True
         if (not self.params_.isIgnoreMinRefinementFitness) and result.fitness_ < self.params_.minRefinementFitness:
             return False  # Mapper.cpp:151-156
         self.mapToRangeSensor_ = result.transformation_.copy()
+        if self.params_.isUseInitialMap and not self.params_.isMergeScansIntoMap:   # :163-167 pure localisation
+            self.mapToRangeSensorPrev_ = self.mapToRangeSensor_.copy()
+            return True
         motion = np.linalg.inv(self.mapToRangeSensorLastScanInsertion_) @ self.mapToRangeSensor_
         if not (np.linalg.norm(motion[:3, 3]) < self.params_.minMovementBetweenMappingSteps):
             self.submap.insertScan(rawScan, processed.merge_, self.mapToRangeSensor_)
@@ -1360,6 +1416,7 @@ class Mapper:
             slot = self._gstep % 256
             self._gstep += 1
         M = _mat(odometryMotion)
+        self._deviceStep()
         L.check(L.lib().b2s_mapper_step_async(self.eng._h, self.submap._s, rawScan._c, _pd(M), C.c_double(self.params_.minRefinementFitness),
                                               C.c_int32(int(self.params_.isIgnoreMinRefinementFitness)), C.c_int32(slot)))
         return slot
@@ -1368,6 +1425,7 @@ class Mapper:
         """End to end with host buffers: float32 scan (pinned host pointer) in, RegistrationResult out, one C call."""
         M = _mat(odometryMotion)
         r = L.Result()
+        self._deviceStep()
         L.check(L.lib().b2s_mapper_step_host(self.eng._h, self.submap._s, C.c_void_p(xyz_f32_ptr), C.c_size_t(n), C.c_size_t(stride), _pd(M),
                                              C.c_double(self.params_.minRefinementFitness),
                                              C.c_int32(int(self.params_.isIgnoreMinRefinementFitness)), C.byref(r)))
@@ -1379,6 +1437,7 @@ class Mapper:
         """Like addRangeMeasurementHost but only enqueues: the b2s_result lands at out_pinned_ptr (page-locked host memory,
         ctypes layout _lib.Result) once the engine's stream has been synchronised."""
         M = _mat(odometryMotion)
+        self._deviceStep()
         L.check(L.lib().b2s_mapper_step_host_async(self.eng._h, self.submap._s, C.c_void_p(xyz_f32_ptr), C.c_size_t(n), C.c_size_t(stride), _pd(M),
                                                    C.c_double(self.params_.minRefinementFitness),
                                                    C.c_int32(int(self.params_.isIgnoreMinRefinementFitness)), C.c_void_p(out_pinned_ptr)))
@@ -1403,6 +1462,7 @@ class Mapper:
     def addRangeMeasurementWithOdometry(self, odometry: DeviceLidarOdometry, rawScan: Cloud, t: int, slot: int = 0) -> int:
         """odometry.addRangeScan(rawScan, t), then addRangeMeasurement(rawScan, t) on the active submap (b2s_slam_step_async): only
         enqueues; odometry.fetchSlamResult(slot) reads the result.  After odometry.enableGraph() rawScan must be its staging cloud."""
+        self._deviceStep()
         L.check(L.lib().b2s_slam_step_async(self.eng._h, self.submap._s, odometry._o, rawScan._c, C.c_int64(int(t)),
                                             C.c_double(self.params_.minRefinementFitness), C.c_int32(int(self.params_.isIgnoreMinRefinementFitness)),
                                             C.c_int32(slot)))
@@ -1412,6 +1472,7 @@ class Mapper:
                                                  stride: int = 12) -> None:
         """The same from a float32 host scan: upload, both chains and the copy of the b2s_slam_result to out_pinned_ptr (page-locked
         host memory, ctypes layout _lib.SlamResult, valid once the engine's stream has been synchronised) are only enqueued."""
+        self._deviceStep()
         L.check(L.lib().b2s_slam_step_host_async(self.eng._h, self.submap._s, odometry._o, C.c_void_p(xyz_f32_ptr), C.c_size_t(n), C.c_size_t(stride),
                                                  C.c_int64(int(t)), C.c_double(self.params_.minRefinementFitness),
                                                  C.c_int32(int(self.params_.isIgnoreMinRefinementFitness)), C.c_void_p(out_pinned_ptr)))

@@ -84,6 +84,7 @@ class SubmapCollection:
         self.adjacency: set[tuple[int, int]] = set()
         self.loopClosureSubmaps: set[int] = set()   # adjacencyMatrix_.markAsLoopClosureSubmap
         self.odometryConstraints: list = []          # odometryConstraints_ (SubmapCollection::computeFeatures appends to it)
+        self.isUseInitialMap = False                 # MapperParameters::isUseInitialMap_: localisation mode never hands over (:105-107)
         self.events: list[tuple] = []   # (scan index, what, ...) -- compared between backends by the parity test
 
     # -- helpers
@@ -106,6 +107,8 @@ class SubmapCollection:
 
     def updateActiveSubmap(self, mapToRangeSensor: np.ndarray, scan) -> None:   # :94-131
         if self.numScansMergedInActiveSubmap < self.params.minNumRangeData:
+            return
+        if self.isUseInitialMap:   # "do not switch maps if we are doing in the localization mode"
             return
         closest = self.findClosestSubmap(mapToRangeSensor)
         closestSubmap, activeSubmap = self.submaps[closest], self.submaps[self.activeSubmapIdx]
@@ -226,6 +229,34 @@ class SegmentMapper:
         self.results: list = []
         self.poses: list[np.ndarray] = []
         self._k = 0
+        mp = getattr(backend, "params", None)   # MapperParameters (a backend without them maps)
+        self.isUseInitialMap = bool(mp is not None and mp.isUseInitialMap)
+        self.isMergeScansIntoMap = bool(mp is not None and mp.isMergeScansIntoMap)
+        self.submaps.isUseInitialMap = self.isUseInitialMap
+        self.isNewInitialValueSet = False   # Mapper::isNewInitialValueSet_ (the backend keeps the device's copy)
+
+    def setInitialMap(self, mapXyz: np.ndarray) -> None:
+        """SlamWrapper::setInitialMap (src/SlamWrapper.cpp:209-220) with isUseInitialMap_: the backend estimates the normals on the full
+        map (prepareInitialMap) and loads it voxelized (Submap.cpp:47-52); SubmapCollection::insertScan buffers it for the overlap,
+        keeps the active submap and counts one merged scan (SubmapCollection.cpp:172-207).  Nothing is pushed to the pose buffer."""
+        sc = self.submaps
+        if not self.isUseInitialMap:
+            raise RuntimeError("setInitialMap needs MapperParameters.isUseInitialMap")
+        if sc.submaps:
+            raise RuntimeError("setInitialMap: the map already holds scans")
+        sc.createNewSubmap(np.eye(4))
+        prepared = self.backend.initial_map(sc.getActiveSubmap().handle, mapXyz)
+        sc.overlapScansBuffer.append((prepared, np.eye(4)))
+        sc.numScansMergedInActiveSubmap += 1
+
+    def setInitialTransform(self, T: np.ndarray) -> None:
+        """SlamWrapper::setInitialTransform (src/SlamWrapper.cpp:222-225): the odometry's initial transform and
+        Mapper::setMapToRangeSensorInitial (Mapper.cpp:87-91).  The device pose slot lives in the submap: load the map first."""
+        if not self.submaps.submaps:
+            raise RuntimeError("setInitialTransform: no submap yet (call setInitialMap first)")
+        self.mapToRangeSensor = np.array(T, dtype=np.float64)
+        self.isNewInitialValueSet = True
+        self.backend.set_initial_transform(self.submaps.getActiveSubmap().handle, self.mapToRangeSensor)
 
     def addRangeMeasurement(self, rawScanF32: np.ndarray, odometryMotion: np.ndarray):
         sc = self.submaps
@@ -272,9 +303,12 @@ class SegmentMapper:
     def _after_step(self, k: int, res, inserted: bool):
         sc = self.submaps
         self.results.append(res)
-        if inserted:
+        if self.isNewInitialValueSet:   # Mapper.cpp:143-149: the result is discarded, the pose stays the initial value, nothing is inserted
+            self.isNewInitialValueSet = False
+        elif inserted:
             self.mapToRangeSensor = np.array(res.transformation_, dtype=np.float64)
-            sc.afterInsertion(k, self.backend.last_merge_cloud(), self.mapToRangeSensor)
+            if not (self.isUseInitialMap and not self.isMergeScansIntoMap):   # :163-167: pure localisation never inserts
+                sc.afterInsertion(k, self.backend.last_merge_cloud(), self.mapToRangeSensor)
         self.poses.append(self.mapToRangeSensor.copy())
         return res
 
@@ -601,6 +635,7 @@ class DeviceBackend:
         self.odometry_params = odometry or E.OdometryParameters()   # the device odometry of SegmentMapper.addRangeScan
         self.motion_compensation = motionCompensation                # de-skew of both inputs of SegmentMapper.addRangeScan (None: off)
         self._odo = None
+        self._odo_initial = None   # SlamWrapper::setInitialTransform's odometry half, applied when the odometry is created
         self.eng = E.Engine(self.params, device=device, cuda_stream=cuda_stream)
         self.mapper = E.Mapper(self.eng, 1024)     # its own first submap is a placeholder: submaps are created by new_submap()
         self.mapper.submap.free()
@@ -618,7 +653,25 @@ class DeviceBackend:
         sm.setMapperOptions(minMovement=p.minMovementBetweenMappingSteps, carving=p.mapBuilder.carving if self.carving else None,
                             dense=self.dense, denseCarving=p.denseMapCarving if (self.dense and self.carving) else None,
                             denseCropper=p.denseMapCropper)
+        if p.isUseInitialMap and not p.isMergeScansIntoMap:
+            sm.setMergeScans(False)    # pure localisation: the chain neither carves nor fuses
         return sm
+
+    # -- localisation against a prior map
+    def initial_map(self, sm, xyz: np.ndarray):
+        """prepareInitialMap (normals on the full map) and Submap::insertScan's initial branch (voxelized load); returns the prepared
+        cloud, which SubmapCollection keeps in its overlap buffer"""
+        c = self.eng.cloud(np.ascontiguousarray(xyz, dtype=np.float64))
+        self.mapper.scan2MapReg_.prepareInitialMap(c)
+        sm.setInitialMap(c, self.params.mapBuilder.mapVoxelSize)
+        return c
+
+    def set_initial_transform(self, sm, T):
+        """Mapper::setMapToRangeSensorInitial on the submap's device pose slot, and LidarOdometry's initial transform once it exists"""
+        sm.setInitialTransform(T)
+        self._odo_initial = np.array(T, dtype=np.float64)
+        if self._odo is not None:
+            self._odo.setInitialTransform(T)
 
     def _activate(self, sm):
         self.mapper.submap = sm
@@ -660,6 +713,8 @@ class DeviceBackend:
             self._odo = E.DeviceLidarOdometry(self.eng, self.odometry_params, self.raw_capacity)
             if self.motion_compensation is not None:
                 self._odo.setMotionCompensation(self.motion_compensation)
+            if self._odo_initial is not None:
+                self._odo.setInitialTransform(self._odo_initial)
             if self.graph:
                 self._odo.enableGraph(self.raw_capacity)
             self._slam_pin = torch.empty(C.sizeof(L.SlamResult), dtype=torch.uint8).pin_memory()

@@ -341,6 +341,11 @@ void SubmapB200::setMapPointCloud(const PointCloud& cloud) {
   cacheValid_ = false;
 }
 
+void SubmapB200::setMergeScans(bool on) {   // Mapper.cpp:163-167; off also keeps the static patch table (b2s.h)
+  const int32_t rc = b2s_submap_set_merge_scans(h_, sm_, on ? 1 : 0);
+  if (rc != B2S_OK) b2sThrow(rc);
+}
+
 void SubmapB200::computeFeatures(const PlaceRecognitionParameters& p) {
   int32_t rc = B2S_OK;
   if (!sparse_ && (rc = b2s_cloud_create(h_, &sparse_)) != B2S_OK) b2sThrow(rc);

@@ -88,6 +88,7 @@ class SubmapB200 {
   const PointCloud& getMapPointCloud() const;
   bool isEmpty() const;
   void setMapPointCloud(const PointCloud& cloud);           // initial map (SlamWrapper::setInitialMap)
+  void setMergeScans(bool on);                              // isMergeScansIntoMap_ for the device chain: false = pure localisation
   void computeFeatures(const PlaceRecognitionParameters& p);
   const PointCloud& getSparseMapPointCloud() const;
   const Feature& getFeatures() const;                       // throws before the first computeFeatures, like the reference
