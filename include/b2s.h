@@ -692,6 +692,32 @@ int32_t b2s_global_optimization(b2s_handle* h, int32_t n_nodes, double* node_pos
                                 const b2s_global_optimization_params* p, int32_t* edge_kept_out, double* edge_confidence_out,
                                 b2s_global_optimization_stats* stats_out);
 
+/* ---- the assembled map: Mapper::getAssembledMapPointCloud (src/Mapper.cpp:183-208), which SlamWrapper::saveMap (src/SlamWrapper.cpp:
+ *      242-247) writes and SlamWrapperRos::publishMaps (ros/open3d_slam_ros/src/SlamWrapperRos.cpp:222-244) voxelizes with
+ *      assembledMapVoxelSize_, and assembleColoredPointCloud (ros/open3d_slam_ros/src/helpers_ros.cpp:51-70), voxelized with
+ *      submapVoxelSize_ (Parameters.hpp:179-183).  Restated rules (DESIGN.md row A1):
+ *   - assembly: the live map points (fusion's tombstones skipped) of submaps[0], in map order, then those of submaps[1], ... -- exactly
+ *     what b2s_submap_to_cloud gives for each, with the normals                                                          Mapper.cpp:195-205
+ *   - normals: the output has normals only when every submap that contributes at least one point has them (a point-to-point map has
+ *     none).  Deliberate difference: with mixed inputs the reference pushes fewer normals than points, a malformed cloud whose [O3D]
+ *     HasNormals() is false; here that case returns no normals.  An empty output has no normals
+ *   - voxel_size > 0: [O3D] VoxelDownSample(voxel_size) of the assembly, as b2s_voxel_down_sample: members accumulated in input order,
+ *     the voxels in Morton order, a map wider than 2^21 voxels -> B2S_E_INVALID.  voxel_size <= 0: the assembly as it is     helpers.cpp:107-113
+ *   - coloured map: the points of the assembly without normals; a point of submaps[j] gets Color::getColor(j % 11 + 2), in order Gray
+ *     (.5,.5,.5), Red, Green, Blue, Yellow, Orange (1,.5,0), Purple (.5,0,1), Chartreuse (.5,1,0), Teal (0,1,1), Pink (1,0,.5), Magenta
+ *     (.78,0,.9), as float32 (std_msgs/ColorRGBA) promoted to double; VoxelDownSample averages the colours like the points.  rgb:
+ *     host n x 3 doubles in the order of `out` (NULL: not copied), capacity / n_out as b2s_submap_dense_download
+ *   - n_submaps = 0 or only empty submaps: an empty cloud, B2S_OK.  Errors: n_submaps < 0, a null submap, a submap or output of
+ *     another handle, a fixed-capacity staging cloud as output -> B2S_E_INVALID; more than (2^31 - 1) / 3 live points -> B2S_E_CAPACITY;
+ *     n_submaps > B2S_ASSEMBLY_MAX_SUBMAPS (one launch's job dimension) -> B2S_E_UNSUPPORTED.  The submaps are not modified; a
+ *     submap may appear more than once.
+ * One set of launches for every submap; synchronises once for the assembled count (and the voxel path's extent) and, on the voxel
+ * path, once for the voxel count; the colours are copied after that. */
+#define B2S_ASSEMBLY_MAX_SUBMAPS 65535
+int32_t b2s_assemble_map(b2s_handle* h, int32_t n_submaps, const b2s_submap* const* submaps, double voxel_size, b2s_cloud* out);
+int32_t b2s_assemble_colored_map(b2s_handle* h, int32_t n_submaps, const b2s_submap* const* submaps, double voxel_size, b2s_cloud* out,
+                                 double* rgb, size_t capacity, size_t* n_out);
+
 /* ---- device-to-device hand-over of a cloud's arrays (SURVEY.md section 8e: a submap that is the registration target on
  *      several GPUs is built once by its owner and broadcast over NVLink by the host side -- torch.distributed / NCCL own
  *      the transfer, this library only copies between its cloud and the caller's device buffers on the handle's stream).

@@ -1,0 +1,227 @@
+// assemble.cu -- A1: the global map assembled on the device, for saving and publishing it.
+//
+//   Mapper::getAssembledMapPointCloud                      core/src/Mapper.cpp:183-208 (SlamWrapper::saveMap, SlamWrapperRos::publishMaps)
+//   assembleColoredPointCloud                              ros/open3d_slam_ros/src/helpers_ros.cpp:51-70
+//   o3d_slam::voxelize -> [O3D] VoxelDownSample             core/src/helpers.cpp:107-113 (assembledMapVoxelSize_, submapVoxelSize_)
+//
+// K-assemble is one set of launches over every submap, whatever their number: a job table holds each submap's map slots, device count
+// and list position; a live flag per slot (fusion's tombstones are NaN) with blockIdx.y = job, the batched scan of the flags gives each
+// live point its offset within its submap, one CTA scans the per-submap totals into each submap's base, and a scatter writes points,
+// normals and, for the coloured map, the point's palette entry.  The voxel path is op_voxel_down_sample on the assembled cloud, with
+// the palette entries averaged beside the points.  Every buffer here is the assembly's own and untracked (AssemblyScratch).
+#include "common.cuh"
+
+namespace b2s {
+
+constexpr int AS_THREADS = 256;
+constexpr int AS_BASE_THREADS = 1024;                  // the base scan walks the jobs 1024 at a time
+constexpr long long AS_MAX_POINTS = 0x7fffffffLL / 3;   // the kernels downstream index 3 i in int32
+
+// Color::getColor(j % 11 + 2) (ros/open3d_slam_ros/include/open3d_slam_ros/Color.hpp:22-32): Gray, Red, Green, Blue, Yellow, Orange,
+// Purple, Chartreuse, Teal, Pink, Magenta.  std_msgs/ColorRGBA holds float32: the values are the float32 ones promoted to double.
+static const double kPalette[33] = {
+    (double)0.5f, (double)0.5f, (double)0.5f, 1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0, 1.0, 1.0, 0.0, 1.0, (double)0.5f, 0.0,
+    (double)0.5f, 0.0, 1.0, (double)0.5f, 1.0, 0.0, 0.0, 1.0, 1.0, 1.0, 0.0, (double)0.5f, (double)0.78f, 0.0, (double)0.9f};
+
+struct AsmJob {
+  const double* xyz; const double* nrm; const int32_t* d_n;   // the submap's map slots
+  int32_t* flags; int32_t* offs;                                 // per slot: live, offset of the live point within the submap
+  int32_t label;                                                 // palette entry: list position % 11
+  int32_t no_normals;                                            // the map has no normals (b2s_submap::no_normals)
+};
+
+__global__ void __launch_bounds__(AS_THREADS) asm_flags_kernel(const AsmJob* __restrict__ jobs) {
+  pdl_wait();
+  const AsmJob j = jobs[blockIdx.y];
+  const int n = *j.d_n;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const double x = j.xyz[3 * (size_t)i];
+    j.flags[i] = (x == x) ? 1 : 0;
+  }
+}
+
+// one CTA: base[k] = live points of the jobs before k (int64, job order); words[0] = the assembled count (0 above AS_MAX_POINTS, which
+// is reported as ST_CAPACITY), words[1] = a job that contributes a point has no normals
+__global__ void __launch_bounds__(AS_BASE_THREADS) asm_base_kernel(const AsmJob* __restrict__ jobs, int njobs, long long* __restrict__ base,
+                                                                   int32_t* out_n, int32_t* words, uint32_t* status) {
+  pdl_wait();
+  __shared__ long long s_warp[AS_BASE_THREADS / 32];
+  __shared__ long long s_carry;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) s_carry = 0;
+  int mixed = 0;
+  for (int r0 = 0; r0 < njobs; r0 += AS_BASE_THREADS) {
+    __syncthreads();
+    const int k = r0 + tid;
+    long long t = 0;
+    if (k < njobs) {
+      t = jobs[k].offs[*jobs[k].d_n];
+      if (t > 0 && jobs[k].no_normals) mixed = 1;
+    }
+    long long inc = t;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const long long v = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += v; }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    long long woff = 0, agg = 0;
+    for (int w = 0; w < AS_BASE_THREADS / 32; w++) { const long long v = s_warp[w]; if (w < warp) woff += v; agg += v; }
+    const long long carry = s_carry;
+    if (k < njobs) base[k] = carry + woff + inc - t;
+    __syncthreads();
+    if (tid == 0) s_carry = carry + agg;
+  }
+  mixed = __syncthreads_or(mixed);
+  if (tid == 0) {
+    const long long total = s_carry;
+    base[njobs] = total;
+    int32_t cnt = (int32_t)total;
+    if (total > AS_MAX_POINTS) { atomicOr(status, ST_CAPACITY); cnt = 0; }
+    *out_n = cnt;
+    words[0] = cnt;
+    words[1] = mixed;
+  }
+}
+
+// onrm / olabel / orgb optional: normals, the palette entry (voxel path), the colour itself (unvoxelized coloured map)
+__global__ void __launch_bounds__(AS_THREADS) asm_scatter_kernel(const AsmJob* __restrict__ jobs, const long long* __restrict__ base,
+                                                                 const int32_t* __restrict__ words, const double* __restrict__ palette,
+                                                                 double* __restrict__ oxyz, double* __restrict__ onrm, int32_t* __restrict__ olabel,
+                                                                 double* __restrict__ orgb) {
+  pdl_wait();
+  if (words[0] == 0) return;   // nothing to write, or more than AS_MAX_POINTS
+  const AsmJob j = jobs[blockIdx.y];
+  const int n = *j.d_n;
+  const long long b = base[blockIdx.y];
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (!j.flags[i]) continue;
+    const size_t o = (size_t)(b + j.offs[i]), s = (size_t)i;
+    oxyz[3 * o] = j.xyz[3 * s]; oxyz[3 * o + 1] = j.xyz[3 * s + 1]; oxyz[3 * o + 2] = j.xyz[3 * s + 2];
+    if (onrm) { onrm[3 * o] = j.nrm[3 * s]; onrm[3 * o + 1] = j.nrm[3 * s + 1]; onrm[3 * o + 2] = j.nrm[3 * s + 2]; }
+    if (olabel) olabel[o] = j.label;
+    if (orgb) { const double* c = palette + 3 * j.label; orgb[3 * o] = c[0]; orgb[3 * o + 1] = c[1]; orgb[3 * o + 2] = c[2]; }
+  }
+}
+
+int32_t op_assemble_map(b2s_handle* h, int n, const b2s_submap* const* submaps, double voxel, b2s_cloud* out, bool colored, double* rgb,
+                        size_t capacity, size_t* n_out) {
+  if (n == 0) {   // an empty cloud; [O3D] HasNormals() is false for it
+    B2S_TRY(cloud_reserve(h, out, 0, false));
+    B2S_TRY(cloud_set_count(h, out, 0));
+    out->has_normals = false;
+    if (n_out) *n_out = 0;
+    return B2S_OK;
+  }
+  AssemblyScratch& A = h->assembly;
+  A.cloud.h = h; A.cloud.device = h->device;
+  const bool vox = voxel > 0.0;   // helpers.cpp:108-110: voxelize() is a no-op for voxelSize <= 0
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  size_t bound = 0, max_n = 1, slot_bytes = 0;
+  for (int k = 0; k < n; k++) {
+    const size_t m = submaps[k]->cloud[0]->n_max > 0 ? submaps[k]->cloud[0]->n_max : 1;
+    bound += submaps[k]->cloud[0]->n_max;
+    if (m > max_n) max_n = m;
+    slot_bytes += al(scan_state_bytes(m)) + 2 * al((m + 2) * 4);
+  }
+  // a larger live total is refused on the device before anything is written, so the assembled cloud never needs more
+  if (bound > (size_t)AS_MAX_POINTS) bound = (size_t)AS_MAX_POINTS;
+  WideGridScope wide(bound);
+  b2s_cloud* dst = vox ? &A.cloud : out;
+  B2S_TRY(cloud_reserve(h, dst, bound, !colored));
+  if (colored && vox) B2S_TRY(A.labels.ensure((bound > 0 ? bound : 1) * 4, h->stream));
+  if (colored) B2S_TRY(A.rgb.ensure((bound > 0 ? bound : 1) * 24, h->stream));
+
+  // tables: [AsmJob x n][ScanJob x n][palette] staged from the host, then [base x (n + 1)][words] written on the device
+  const size_t t_jobs = al((size_t)n * sizeof(AsmJob)), t_scan = al((size_t)n * sizeof(ScanJob)), t_pal = al(sizeof(kPalette));
+  const size_t staged = t_jobs + t_scan + t_pal, t_base = al(((size_t)n + 1) * 8);
+  B2S_TRY(A.tables.ensure(staged + t_base + 256, h->stream));
+  B2S_TRY(A.slots.ensure(slot_bytes, h->stream));
+  if (A.stage.cap < staged) B2S_TRY(A.stage.alloc(2 * staged));   // every call ends with a synchronisation: the stage is free
+  unsigned char* st = A.stage.as<unsigned char>();
+  unsigned char* tab = A.tables.as<unsigned char>();
+  AsmJob* hj = reinterpret_cast<AsmJob*>(st);
+  ScanJob* hs = reinterpret_cast<ScanJob*>(st + t_jobs);
+  memcpy(st + t_jobs + t_scan, kPalette, sizeof(kPalette));
+  unsigned char* slots = A.slots.as<unsigned char>();
+  size_t off = 0;
+  for (int k = 0; k < n; k++) {   // tile states first: they are the region zeroed below
+    const size_t m = submaps[k]->cloud[0]->n_max > 0 ? submaps[k]->cloud[0]->n_max : 1;
+    unsigned long long* s = reinterpret_cast<unsigned long long*>(slots + off);
+    hs[k].state = s;
+    hs[k].counter = reinterpret_cast<int32_t*>(s + (scan_state_bytes(m) - 64) / 8);
+    off += al(scan_state_bytes(m));
+  }
+  const size_t state_bytes = off;
+  for (int k = 0; k < n; k++) {
+    const b2s_submap* sm = submaps[k];
+    const b2s_cloud* map = sm->cloud[0].get();
+    const size_t m = map->n_max > 0 ? map->n_max : 1;
+    AsmJob& J = hj[k];
+    J.xyz = map->xyz.as<double>(); J.nrm = map->nrm.as<double>(); J.d_n = map->dn.as<int32_t>();
+    J.flags = reinterpret_cast<int32_t*>(slots + off); off += al((m + 2) * 4);
+    J.offs = reinterpret_cast<int32_t*>(slots + off); off += al((m + 2) * 4);
+    J.label = k % 11;
+    J.no_normals = sm->no_normals ? 1 : 0;
+    hs[k].in = J.flags; hs[k].out = J.offs; hs[k].d_n = J.d_n;
+  }
+  B2S_CUDA(cudaMemcpyAsync(tab, st, staged, cudaMemcpyHostToDevice, h->stream));
+  B2S_CUDA(cudaMemsetAsync(slots, 0, state_bytes, h->stream));
+  const AsmJob* dj = reinterpret_cast<const AsmJob*>(tab);
+  const ScanJob* ds = reinterpret_cast<const ScanJob*>(tab + t_jobs);
+  const double* palette = reinterpret_cast<const double*>(tab + t_jobs + t_scan);
+  long long* base = reinterpret_cast<long long*>(tab + staged);
+  int32_t* words = reinterpret_cast<int32_t*>(tab + staged + t_base);
+
+  const int bx = grid_for(max_n, AS_THREADS, 2 * device_sms());   // x blocks per job (grid-stride); y = job
+  launch_pdl(asm_flags_kernel, dim3((unsigned)bx, (unsigned)n), AS_THREADS, 0, h->stream, dj);
+  h->launches++;
+  B2S_TRY(scan_exclusive_i32_batch(h, ds, n, max_n));
+  launch_pdl(asm_base_kernel, 1, AS_BASE_THREADS, 0, h->stream, dj, n, base, dst->dn.as<int32_t>(), words, h->status.as<uint32_t>());
+  launch_pdl(asm_scatter_kernel, dim3((unsigned)bx, (unsigned)n), AS_THREADS, 0, h->stream, dj, base, words, palette, dst->xyz.as<double>(),
+             colored ? nullptr : dst->nrm.as<double>(), colored && vox ? A.labels.as<int32_t>() : nullptr,
+             colored && !vox ? A.rgb.as<double>() : nullptr);
+  h->launches += 2;
+  B2S_CUDA(cudaGetLastError());
+
+  // synchronisation 1: the assembled count, the normals rule and (voxel path) the extent that sizes the voxel key
+  unsigned long long hb[6] = {0, 0, 0, 0, 0, 0};
+  int32_t hw[2] = {0, 0};
+  if (vox) {
+    B2S_TRY(h->misc.ensure(256, h->stream));
+    B2S_TRY(bbox_reduce(h, dst->xyz.as<double>(), dst->dn.as<int32_t>(), bound > 0 ? bound : 1, nullptr, h->misc.as<unsigned long long>()));
+    B2S_TRY(read_back(h, {{hw, words, 8}, {hb, h->misc.p, 48}}));
+  } else {
+    B2S_TRY(read_back(h, {{hw, words, 8}}));
+  }
+  size_t cnt = (size_t)hw[0];
+  const bool normals = !colored && cnt > 0 && hw[1] == 0;   // Mapper.cpp:201-203: a submap without normals pushes none
+  dst->has_normals = normals; dst->n_max = cnt; dst->n_known = (long long)cnt;
+  if (vox) {
+    if (cnt == 0) {
+      B2S_TRY(cloud_reserve(h, out, 0, false));
+      B2S_TRY(cloud_set_count(h, out, 0));
+      out->has_normals = false;
+    } else {
+      double ext = 0.0;
+      for (int d = 0; d < 3; d++) { const double e = ord_decode(hb[3 + d]) - ord_decode(hb[d]); if (e > ext) ext = e; }
+      const int bits = voxel_key_bits(ext, voxel);
+      B2S_REQUIRE(bits <= 21, B2S_E_INVALID, "[VoxelDownSample] voxel_size is too small for the extent of the assembled map");
+      B2S_TRY(op_voxel_down_sample(h, dst, nullptr, voxel, out, bits, &A.vox, colored ? A.labels.as<int32_t>() : nullptr, palette,
+                                   colored ? A.rgb.as<double>() : nullptr));
+      // synchronisation 2: the voxel count
+      int32_t nv = 0;
+      B2S_TRY(read_back(h, {{&nv, out->dn.p, 4}}));
+      cnt = (size_t)nv;
+      out->n_max = cnt; out->n_known = (long long)cnt;
+    }
+  }
+  if (n_out) *n_out = cnt;
+  if (!colored) return B2S_OK;
+  B2S_REQUIRE(cnt <= capacity, B2S_E_CAPACITY, "colour buffer too small: %zu points, capacity %zu", cnt, capacity);
+  if (cnt && rgb) {
+    B2S_CUDA(cudaMemcpyAsync(rgb, A.rgb.p, cnt * 24, cudaMemcpyDeviceToHost, h->stream));
+    B2S_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  return B2S_OK;
+}
+
+}  // namespace b2s

@@ -1362,6 +1362,34 @@ int32_t b2s_global_optimization(b2s_handle* h, int32_t n_nodes, double* node_pos
   return op_global_optimization(h, n_nodes, node_poses, n_edges, edges, *p, edge_kept_out, edge_confidence_out, stats_out);
 }
 
+// ---- the assembled map (Mapper.cpp:183-208, helpers_ros.cpp:51-70, SlamWrapperRos.cpp:222-244) ----------------------------------------
+static int32_t check_assembly_args(b2s_handle* h, int32_t n, const b2s_submap* const* submaps, const b2s_cloud* out) {
+  B2S_REQUIRE(h && out, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(n >= 0, B2S_E_INVALID, "n_submaps must be >= 0");
+  B2S_REQUIRE(n == 0 || submaps, B2S_E_INVALID, "null submap array");
+  B2S_REQUIRE(out->h == h, B2S_E_INVALID, "the output cloud belongs to another handle");
+  B2S_REQUIRE(!out->fixed_cap, B2S_E_INVALID, "the output cloud must not be a fixed-capacity staging cloud");
+  for (int32_t k = 0; k < n; k++) {
+    B2S_REQUIRE(submaps[k], B2S_E_INVALID, "null submap %d", k);
+    B2S_REQUIRE(submaps[k]->h == h, B2S_E_INVALID, "submap %d belongs to another handle", k);
+  }
+  B2S_REQUIRE(n <= B2S_ASSEMBLY_MAX_SUBMAPS, B2S_E_UNSUPPORTED, "%d submaps: one assembly takes at most %d", n, B2S_ASSEMBLY_MAX_SUBMAPS);
+  return B2S_OK;
+}
+
+int32_t b2s_assemble_map(b2s_handle* h, int32_t n, const b2s_submap* const* submaps, double voxel_size, b2s_cloud* out) {
+  B2S_TRY(check_assembly_args(h, n, submaps, out));
+  LOCK(h);
+  return op_assemble_map(h, n, submaps, voxel_size, out, false, nullptr, 0, nullptr);
+}
+
+int32_t b2s_assemble_colored_map(b2s_handle* h, int32_t n, const b2s_submap* const* submaps, double voxel_size, b2s_cloud* out, double* rgb,
+                                 size_t capacity, size_t* n_out) {
+  B2S_TRY(check_assembly_args(h, n, submaps, out));
+  LOCK(h);
+  return op_assemble_map(h, n, submaps, voxel_size, out, true, rgb, capacity, n_out);
+}
+
 // debug aid for tests: the header, cell starts and original indices of the NN index the last registration built (h->grid_a).
 // dims_n = {dims[0..2], ncell, n}; cell_start (ncell + 1 entries) and orig (n entries) are skipped when null or too small.
 int32_t b2s_debug_nn_index(b2s_handle* h, double origin_cell[4], int32_t dims_n[5], int32_t* cell_start, size_t cap_cells, int32_t* orig,

@@ -233,6 +233,27 @@ struct b2s_submap {
   bool no_normals = false;
 };
 
+namespace b2s {
+// Scratch of the operators that work on the whole map (b2s_assemble_map, assemble.cu).  Every buffer is sized to the assembled map and
+// grows with it, so none is tracked: no captured chain reads them, and their growth must not make the mapper chains re-capture.
+struct VoxelScratch {    // op_voxel_down_sample's own scratch instead of the handle's keys / vals / flags / offs, scan state and sort histogram
+  DevBuf keys, vals, flags, offs, scan_state, sort_hist;
+  VoxelScratch() { for (DevBuf* b : {&keys, &vals, &flags, &offs, &scan_state, &sort_hist}) b->tracked = false; }
+};
+struct AssemblyScratch {
+  DevBuf tables;         // AsmJob + ScanJob tables, the per-job base offsets and the palette
+  DevBuf slots;          // per map slot of every job: live flag, offset within the submap; the batched scan's tile states
+  DevBuf labels;         // int32 per assembled point: palette entry (coloured call, voxel path)
+  DevBuf rgb;            // 3 x f64 per output point (coloured call)
+  PinnedBuf stage;       // page-locked staging of the tables
+  b2s_cloud cloud;       // the assembled map in front of the voxel path
+  VoxelScratch vox;
+  AssemblyScratch() {
+    for (DevBuf* b : {&tables, &slots, &labels, &rgb, &cloud.xyz, &cloud.nrm, &cloud.dn}) b->tracked = false;
+  }
+};
+}  // namespace b2s
+
 struct b2s_feature {
   b2s_handle* h = nullptr;
   int device = 0;
@@ -329,6 +350,7 @@ struct b2s_handle {
   b2s::DevBuf pg_A, pg_F, pg_W, pg_vec, pg_nodes, pg_edges;
   int32_t pg_edge_cap = 0;
   b2s::GraphCache pg_graph;
+  b2s::AssemblyScratch assembly;      // b2s_assemble_map / b2s_assemble_colored_map (assemble.cu owns the layouts)
 };
 
 // every entry point that touches a handle's stream or buffers holds its lock and works on its device
@@ -355,17 +377,20 @@ struct ReadBack { void* dst; const void* src; size_t bytes; };   // host destina
 int32_t read_back(b2s_handle* h, std::initializer_list<ReadBack> copies);
 
 // ---- primitives (scan.cu / radix_sort.cu / grid_index.cu / ...) : all asynchronous on h->stream ----
-// exclusive scan of in[0..*d_n) into out[0..*d_n]; out[*d_n] and *d_total (optional) receive the total
-int32_t scan_exclusive_i32(b2s_handle* h, const int32_t* in, int32_t* out, const int32_t* d_n, size_t n_max, int32_t* d_total);
+// exclusive scan of in[0..*d_n) into out[0..*d_n]; out[*d_n] and *d_total (optional) receive the total.  state (optional): the tile
+// state buffer to use instead of the handle's
+int32_t scan_exclusive_i32(b2s_handle* h, const int32_t* in, int32_t* out, const int32_t* d_n, size_t n_max, int32_t* d_total,
+                           DevBuf* state = nullptr);
 // njobs independent scans in one launch; every job's tile state (scan_state_bytes(n_max), zeroed) is supplied by the caller
 size_t scan_state_bytes(size_t n_max);
 int32_t scan_exclusive_i32_batch(b2s_handle* h, const ScanJob* jobs_dev, int njobs, size_t n_max);
 // stable LSD radix sort of (key, value) pairs, key_bits low bits significant; result ends in keys/vals
-// (pointers are swapped so that keys/vals designate the sorted arrays on return, *_alt the scratch)
+// (pointers are swapped so that keys/vals designate the sorted arrays on return, *_alt the scratch).  own (optional): the histogram and
+// scan state of the multi-kernel sort come from it instead of the handle
 int32_t radix_sort_pairs_u32(b2s_handle* h, uint32_t*& keys, uint32_t*& vals, uint32_t*& keys_alt, uint32_t*& vals_alt,
-                             const int32_t* d_n, size_t n_max, int key_bits);
+                             const int32_t* d_n, size_t n_max, int key_bits, VoxelScratch* own = nullptr);
 int32_t radix_sort_pairs_u64(b2s_handle* h, uint64_t*& keys, uint32_t*& vals, uint64_t*& keys_alt, uint32_t*& vals_alt,
-                             const int32_t* d_n, size_t n_max, int key_bits);
+                             const int32_t* d_n, size_t n_max, int key_bits, VoxelScratch* own = nullptr);
 inline const int32_t* grid_starts(const GridIndex* g) { return g->cell_start.as<int32_t>() + g->cap_cells + 4; }
 
 // K-index: build the NN grid over cloud points (optionally only those inside `patch`, centre read from device pose)
@@ -399,7 +424,18 @@ int32_t cloud_set_count(b2s_handle* h, b2s_cloud* c, size_t n);
 int32_t op_crop(b2s_handle* h, const b2s_cloud* in, const CropDev& crop, b2s_cloud* out);
 // fixed_key_bits > 0: key width per axis given by the caller instead of measured (no synchronisation); a voxel index outside it
 // sets ST_KEY_OVERFLOW, reported by the next check_status
-int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, b2s_cloud* out, int fixed_key_bits = 0);
+// own (optional): every buffer sized to `in` comes from it instead of the handle.  labels / palette / rgb_out (optional, voxel > 0 and
+// no cropper): every point's colour is palette[3 labels[i] ..], averaged per voxel like the points into rgb_out (3 x f64 per voxel)
+int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, b2s_cloud* out, int fixed_key_bits = 0,
+                             VoxelScratch* own = nullptr, const int32_t* labels = nullptr, const double* palette = nullptr,
+                             double* rgb_out = nullptr);
+// key width per axis of the voxel down-sample for a cloud of the given extent (> 21: the extent is too wide for the voxel)
+int voxel_key_bits(double extent, double voxel);
+int32_t bbox_reduce(b2s_handle* h, const double* xyz, const int32_t* d_n, size_t n_max, const CropDev* crop, unsigned long long* bbox);
+// A1 (assemble.cu): Mapper::getAssembledMapPointCloud / assembleColoredPointCloud, optionally voxelized; rgb (coloured call): host
+// n x 3, capacity / n_out like b2s_submap_dense_download.  Validated arguments.
+int32_t op_assemble_map(b2s_handle* h, int n, const b2s_submap* const* submaps, double voxel, b2s_cloud* out, bool colored, double* rgb,
+                        size_t capacity, size_t* n_out);
 // flags (optional, one int per point of c): only flagged points get a normal.  with_prior: c's normals on entry are the priors of
 // [O3D] EstimateNormals on a cloud that has normals (keep the prior for a zero solver result, flip against it otherwise)
 int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius, double cell_hint, const int32_t* flags = nullptr,

@@ -273,12 +273,13 @@ int32_t scan_exclusive_i32_batch(b2s_handle* h, const ScanJob* jobs_dev, int njo
 }
 
 static int32_t scan_impl(b2s_handle* h, const int32_t* in, int32_t* out, const int32_t* d_n, int32_t n_host, size_t n_max,
-                         int32_t* d_total) {
+                         int32_t* d_total, DevBuf* state) {
   int ntiles = (int)((n_max + SCAN_TILE - 1) / SCAN_TILE);
   if (ntiles < 1) ntiles = 1;
-  B2S_TRY(h->scan.state.ensure((size_t)ntiles * 8 + 64, h->stream));
-  B2S_CUDA(cudaMemsetAsync(h->scan.state.p, 0, (size_t)ntiles * 8 + 64, h->stream));
-  unsigned long long* st = h->scan.state.as<unsigned long long>();
+  DevBuf& sb = state ? *state : h->scan.state;
+  B2S_TRY(sb.ensure((size_t)ntiles * 8 + 64, h->stream));
+  B2S_CUDA(cudaMemsetAsync(sb.p, 0, (size_t)ntiles * 8 + 64, h->stream));
+  unsigned long long* st = sb.as<unsigned long long>();
   int32_t* counter = reinterpret_cast<int32_t*>(st + ntiles);
   launch_pdl(scan_lookback_kernel, ntiles, SCAN_THREADS, 0, h->stream, in, out, d_n, n_host, st, counter, d_total);
   h->launches++;
@@ -286,8 +287,8 @@ static int32_t scan_impl(b2s_handle* h, const int32_t* in, int32_t* out, const i
   return B2S_OK;
 }
 
-int32_t scan_exclusive_i32(b2s_handle* h, const int32_t* in, int32_t* out, const int32_t* d_n, size_t n_max, int32_t* d_total) {
-  return scan_impl(h, in, out, d_n, (int32_t)n_max, n_max, d_total);
+int32_t scan_exclusive_i32(b2s_handle* h, const int32_t* in, int32_t* out, const int32_t* d_n, size_t n_max, int32_t* d_total, DevBuf* state) {
+  return scan_impl(h, in, out, d_n, (int32_t)n_max, n_max, d_total, state);
 }
 
 // =================================================================================================
@@ -511,14 +512,15 @@ static bool use_multi_kernel_sort() {
 // pointers swapped so that (keys, vals) always designate the sorted arrays afterwards
 template <typename K>
 static int32_t radix_sort_impl(b2s_handle* h, K*& keys, uint32_t*& vals, K*& keys_alt, uint32_t*& vals_alt, const int32_t* d_n,
-                               size_t n_max, int key_bits) {
+                               size_t n_max, int key_bits, VoxelScratch* own) {
   // one cluster (8 SMs) wins while the sort is launch-latency bound; from ~1e6 keys on the whole GPU has to work on it
   if (!use_multi_kernel_sort() && n_max <= ((size_t)3 << 18)) return cluster_sort_impl<K>(h, keys, vals, keys_alt, vals_alt, d_n, key_bits);
   int nblocks = (int)((n_max + RS_TILE - 1) / RS_TILE);
   if (nblocks < 1) nblocks = 1;
   size_t hist_n = (size_t)256 * nblocks;
-  B2S_TRY(h->sort.hist.ensure((hist_n + 8) * 4 * 2, h->stream));
-  int32_t* hist = h->sort.hist.as<int32_t>();
+  DevBuf& hb = own ? own->sort_hist : h->sort.hist;
+  B2S_TRY(hb.ensure((hist_n + 8) * 4 * 2, h->stream));
+  int32_t* hist = hb.as<int32_t>();
   int32_t* offs = hist + ((hist_n + 4) & ~(size_t)3);
   int passes = (key_bits + 7) / 8;
   if (passes < 1) passes = 1;
@@ -527,7 +529,7 @@ static int32_t radix_sort_impl(b2s_handle* h, K*& keys, uint32_t*& vals, K*& key
     int shift = 8 * p;
     launch_pdl(rs_hist_kernel<K>, nblocks, RS_THREADS, 0, h->stream, keys, d_n, shift, hist, nblocks);
     h->launches++;
-    B2S_TRY(scan_impl(h, hist, offs, nullptr, (int32_t)hist_n, hist_n, nullptr));
+    B2S_TRY(scan_impl(h, hist, offs, nullptr, (int32_t)hist_n, hist_n, nullptr, own ? &own->scan_state : nullptr));
     launch_pdl(rs_scatter_kernel<K>, nblocks, RS_THREADS, 0, h->stream, keys, vals, keys_alt, vals_alt, d_n, shift, offs, nblocks);
     h->launches++;
     K* tk = keys; keys = keys_alt; keys_alt = tk;
@@ -538,12 +540,12 @@ static int32_t radix_sort_impl(b2s_handle* h, K*& keys, uint32_t*& vals, K*& key
 }
 
 int32_t radix_sort_pairs_u32(b2s_handle* h, uint32_t*& keys, uint32_t*& vals, uint32_t*& keys_alt, uint32_t*& vals_alt,
-                             const int32_t* d_n, size_t n_max, int key_bits) {
-  return radix_sort_impl<uint32_t>(h, keys, vals, keys_alt, vals_alt, d_n, n_max, key_bits);
+                             const int32_t* d_n, size_t n_max, int key_bits, VoxelScratch* own) {
+  return radix_sort_impl<uint32_t>(h, keys, vals, keys_alt, vals_alt, d_n, n_max, key_bits, own);
 }
 int32_t radix_sort_pairs_u64(b2s_handle* h, uint64_t*& keys, uint32_t*& vals, uint64_t*& keys_alt, uint32_t*& vals_alt,
-                             const int32_t* d_n, size_t n_max, int key_bits) {
-  return radix_sort_impl<uint64_t>(h, keys, vals, keys_alt, vals_alt, d_n, n_max, key_bits);
+                             const int32_t* d_n, size_t n_max, int key_bits, VoxelScratch* own) {
+  return radix_sort_impl<uint64_t>(h, keys, vals, keys_alt, vals_alt, d_n, n_max, key_bits, own);
 }
 
 }  // namespace b2s

@@ -193,14 +193,15 @@ __global__ void __launch_bounds__(VX_THREADS) voxel_mean_kernel(const K* __restr
                                                                 const int32_t* __restrict__ d_n, const int32_t* __restrict__ head,
                                                                 const int32_t* __restrict__ offs, const double* __restrict__ xyz,
                                                                 const double* __restrict__ nrm, double* __restrict__ oxyz,
-                                                                double* __restrict__ onrm, int32_t* out_n) {
+                                                                double* __restrict__ onrm, int32_t* out_n, const int32_t* __restrict__ label,
+                                                                const double* __restrict__ palette, double* __restrict__ ocol) {
   pdl_wait();
   const int n = *d_n;
   if (blockIdx.x == 0 && threadIdx.x == 0) *out_n = offs[n];
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
     if (!head[j]) continue;
     const K k = keys[j];
-    double sx = 0, sy = 0, sz = 0, nx = 0, ny = 0, nz = 0;
+    double sx = 0, sy = 0, sz = 0, nx = 0, ny = 0, nz = 0, cr = 0, cg = 0, cb = 0;
     int cnt = 0;
     for (int t = j; t < n && keys[t] == k; ++t) {
       const uint32_t i = vals[t];
@@ -209,12 +210,17 @@ __global__ void __launch_bounds__(VX_THREADS) voxel_mean_kernel(const K* __restr
         const double a = nrm[3 * i], b = nrm[3 * i + 1], c = nrm[3 * i + 2];
         if (a == a && b == b && c == c) { nx = __dadd_rn(nx, a); ny = __dadd_rn(ny, b); nz = __dadd_rn(nz, c); }
       }
+      if (label) {   // AccumulatedPoint::AddPoint: color_ += colors_[index], in the same member order as the points
+        const double* pc = palette + 3 * label[i];
+        cr = __dadd_rn(cr, pc[0]); cg = __dadd_rn(cg, pc[1]); cb = __dadd_rn(cb, pc[2]);
+      }
       cnt++;
     }
     const int o = offs[j];
     const double c = (double)cnt;
     oxyz[3 * o] = __ddiv_rn(sx, c); oxyz[3 * o + 1] = __ddiv_rn(sy, c); oxyz[3 * o + 2] = __ddiv_rn(sz, c);
     if (nrm) { onrm[3 * o] = __ddiv_rn(nx, c); onrm[3 * o + 1] = __ddiv_rn(ny, c); onrm[3 * o + 2] = __ddiv_rn(nz, c); }
+    if (label) { ocol[3 * o] = __ddiv_rn(cr, c); ocol[3 * o + 1] = __ddiv_rn(cg, c); ocol[3 * o + 2] = __ddiv_rn(cb, c); }
   }
 }
 
@@ -224,17 +230,24 @@ static int bits_for(double extent, double voxel) {
   while ((double)(1u << b) < cells && b < 22) b++;
   return b;
 }
+int voxel_key_bits(double extent, double voxel) { return bits_for(extent, voxel); }
 
+// own: the buffers sized to `in` come from the caller's scratch instead of the handle's; labels / palette / rgb_out: see voxel_mean_kernel
 template <typename K>
-static int32_t voxel_impl(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, int bits, b2s_cloud* out) {
+static int32_t voxel_impl(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, int bits, b2s_cloud* out, VoxelScratch* own,
+                          const int32_t* labels, const double* palette, double* rgb_out) {
   const size_t n_max = in->n_max > 0 ? in->n_max : 1;
-  B2S_TRY(h->keys.ensure(n_max * sizeof(K) * 2, h->stream));
-  B2S_TRY(h->vals.ensure(n_max * 4 * 2, h->stream));
-  B2S_TRY(h->flags.ensure((n_max + 1) * 4, h->stream));
-  B2S_TRY(h->offs.ensure((n_max + 2) * 4, h->stream));
+  DevBuf& kb = own ? own->keys : h->keys;
+  DevBuf& vb = own ? own->vals : h->vals;
+  DevBuf& fb = own ? own->flags : h->flags;
+  DevBuf& ob = own ? own->offs : h->offs;
+  B2S_TRY(kb.ensure(n_max * sizeof(K) * 2, h->stream));
+  B2S_TRY(vb.ensure(n_max * 4 * 2, h->stream));
+  B2S_TRY(fb.ensure((n_max + 1) * 4, h->stream));
+  B2S_TRY(ob.ensure((n_max + 2) * 4, h->stream));
   B2S_TRY(cloud_reserve(h, out, n_max, in->has_normals));
-  K* keys = h->keys.as<K>(); K* keys_alt = keys + n_max;
-  uint32_t* vals = h->vals.as<uint32_t>(); uint32_t* vals_alt = vals + n_max;
+  K* keys = kb.as<K>(); K* keys_alt = keys + n_max;
+  uint32_t* vals = vb.as<uint32_t>(); uint32_t* vals_alt = vals + n_max;
   const int32_t* d_n = in->dn.as<int32_t>();
   const int blocks = grid_for(n_max, VX_THREADS);
   CropDev cd = crop ? *crop : make_crop(nullptr);
@@ -243,18 +256,18 @@ static int32_t voxel_impl(b2s_handle* h, const b2s_cloud* in, const CropDev* cro
                                                              voxel, bits, keys, vals, h->status.as<uint32_t>());
   h->launches++; }
   if constexpr (sizeof(K) == 4) {
-    B2S_TRY(radix_sort_pairs_u32(h, keys, vals, keys_alt, vals_alt, d_n, n_max, 3 * bits + 1));
+    B2S_TRY(radix_sort_pairs_u32(h, keys, vals, keys_alt, vals_alt, d_n, n_max, 3 * bits + 1, own));
   } else {
-    B2S_TRY(radix_sort_pairs_u64(h, keys, vals, keys_alt, vals_alt, d_n, n_max, 3 * bits + 1));
+    B2S_TRY(radix_sort_pairs_u64(h, keys, vals, keys_alt, vals_alt, d_n, n_max, 3 * bits + 1, own));
   }
   ProfScope prof2(h, PK_VOXEL);
-  launch_pdl(seg_head_kernel<K>, blocks, VX_THREADS, 0, h->stream, keys, d_n, bits, 0, h->flags.as<int32_t>());
+  launch_pdl(seg_head_kernel<K>, blocks, VX_THREADS, 0, h->stream, keys, d_n, bits, 0, fb.as<int32_t>());
   h->launches++;
-  B2S_TRY(scan_exclusive_i32(h, h->flags.as<int32_t>(), h->offs.as<int32_t>(), d_n, n_max, nullptr));
-  launch_pdl(voxel_mean_kernel<K>, blocks, VX_THREADS, 0, h->stream, keys, vals, d_n, h->flags.as<int32_t>(), h->offs.as<int32_t>(),
+  B2S_TRY(scan_exclusive_i32(h, fb.as<int32_t>(), ob.as<int32_t>(), d_n, n_max, nullptr, own ? &own->scan_state : nullptr));
+  launch_pdl(voxel_mean_kernel<K>, blocks, VX_THREADS, 0, h->stream, keys, vals, d_n, fb.as<int32_t>(), ob.as<int32_t>(),
                                                              in->xyz.as<double>(), in->has_normals ? in->nrm.as<double>() : nullptr,
                                                              out->xyz.as<double>(), in->has_normals ? out->nrm.as<double>() : nullptr,
-                                                             out->dn.as<int32_t>());
+                                                             out->dn.as<int32_t>(), labels, palette, rgb_out);
   h->launches++;
   out->has_normals = in->has_normals;
   out->n_max = in->n_max;
@@ -263,7 +276,8 @@ static int32_t voxel_impl(b2s_handle* h, const b2s_cloud* in, const CropDev* cro
   return B2S_OK;
 }
 
-int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, b2s_cloud* out, int fixed_key_bits) {
+int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* crop, double voxel, b2s_cloud* out, int fixed_key_bits,
+                             VoxelScratch* own, const int32_t* labels, const double* palette, double* rgb_out) {
   if (voxel <= 0.0) {  // helpers.cpp:108-110: voxelize() is a no-op for voxelSize <= 0 (the crop still applies)
     if (crop) return op_crop(h, in, *crop, out);
     B2S_TRY(cloud_reserve(h, out, in->n_max, in->has_normals));
@@ -292,8 +306,8 @@ int32_t op_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, const CropDev* 
     bits = bits_for(ext, voxel);
   }
   B2S_REQUIRE(bits <= 21, B2S_E_INVALID, "[VoxelDownSample] voxel_size is too small for the extent of the cloud");
-  if (bits <= 10) return voxel_impl<uint32_t>(h, in, crop, voxel, bits, out);
-  return voxel_impl<uint64_t>(h, in, crop, voxel, bits, out);
+  if (bits <= 10) return voxel_impl<uint32_t>(h, in, crop, voxel, bits, out, own, labels, palette, rgb_out);
+  return voxel_impl<uint64_t>(h, in, crop, voxel, bits, out, own, labels, palette, rgb_out);
 }
 
 // ---- P4: seeded random down-sample ------------------------------------------------------------------------------------

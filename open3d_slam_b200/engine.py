@@ -457,6 +457,40 @@ def buildOdometryConstraint(eng: Engine, source, target, params: OdometryConstra
 
 
 @dataclass
+class VisualizationParameters:
+    """include/open3d_slam/Parameters.hpp:179-183: the voxel sizes SlamWrapperRos::publishMaps applies to the assembled map and to the
+    coloured submap cloud, and how often it publishes them"""
+    assembledMapVoxelSize: float = 0.1
+    submapVoxelSize: float = 0.1
+    visualizeEveryNmsec: float = 250.0
+
+
+def _submap_array(submaps):
+    n = len(submaps)
+    return n, (C.c_void_p * max(n, 1))(*[s._s for s in submaps])
+
+
+def getAssembledMapPointCloud(eng: Engine, submaps, voxelSize: float = 0.0) -> Cloud:
+    """Mapper::getAssembledMapPointCloud (src/Mapper.cpp:183-208) over the given Submaps in list order, then o3d_slam::voxelize(voxelSize)
+    (a no-op for voxelSize <= 0), in one device call (b2s_assemble_map; rules in include/b2s.h)."""
+    n, arr = _submap_array(submaps)
+    out = Cloud(eng)
+    L.check(L.lib().b2s_assemble_map(eng._h, C.c_int32(n), arr, C.c_double(voxelSize), out._c))
+    return out
+
+
+def assembleColoredPointCloud(eng: Engine, submaps, voxelSize: float = 0.0):
+    """assembleColoredPointCloud (ros/open3d_slam_ros/src/helpers_ros.cpp:51-70), then voxelize(voxelSize): (Cloud without normals,
+    colours as an n x 3 float64 array in the cloud's order)."""
+    n, arr = _submap_array(submaps)
+    out = Cloud(eng)
+    cap = sum(int(s.capacity) for s in submaps)   # an upper bound of the live points; np.empty only commits the pages written
+    rgb = np.empty((max(cap, 1), 3)); m = C.c_size_t()
+    L.check(L.lib().b2s_assemble_colored_map(eng._h, C.c_int32(n), arr, C.c_double(voxelSize), out._c, _pd(rgb), C.c_size_t(cap), C.byref(m)))
+    return out, rgb[:m.value].copy()
+
+
+@dataclass
 class PoseGraphNode:
     """[O3D] PoseGraphNode: pose_ (4x4)"""
     pose_: np.ndarray = field(default_factory=lambda: np.eye(4))

@@ -154,6 +154,9 @@ class SubmapCollection:
     def getOdometryConstraints(self) -> list:
         return list(self.odometryConstraints)
 
+    def getTotalNumPoints(self) -> int:   # :69-73
+        return sum(self.backend.map_size(s.handle) for s in self.submaps)
+
     def updateAdjacencyMatrix(self, loopClosureConstraints) -> None:   # :75-81
         for c in loopClosureConstraints:
             self.adjacency.add((min(c.sourceSubmapIdx, c.targetSubmapIdx), max(c.sourceSubmapIdx, c.targetSubmapIdx)))
@@ -299,6 +302,16 @@ class SegmentMapper:
         self.mapToRangeSensor = np.asarray(loopClosureCorrection, dtype=np.float64) @ self.mapToRangeSensor
         if self.submaps.submaps:
             self.backend.loop_closure_update(self.submaps.getActiveSubmap().handle, self.mapToRangeSensor)
+
+    def getAssembledMapPointCloud(self, voxelSize: float = 0.0):
+        """Mapper::getAssembledMapPointCloud (src/Mapper.cpp:183-208): the maps of every submap in submap order, with normals, then
+        o3d_slam::voxelize(voxelSize) as SlamWrapperRos::publishMaps applies assembledMapVoxelSize_ (no-op for voxelSize <= 0;
+        SlamWrapper::saveMap keeps the plain assembly).  The mapper never calls it on its own."""
+        return self.backend.assembled_map([s.handle for s in self.submaps.submaps], voxelSize)
+
+    def assembleColoredPointCloud(self, voxelSize: float):
+        """assembleColoredPointCloud (ros/open3d_slam_ros/src/helpers_ros.cpp:51-70) + voxelize(submapVoxelSize_): (cloud, rgb)"""
+        return self.backend.assembled_colored_map([s.handle for s in self.submaps.submaps], voxelSize)
 
     def _after_step(self, k: int, res, inserted: bool):
         sc = self.submaps
@@ -759,6 +772,17 @@ class DeviceBackend:
 
     def map_cloud(self, sm):
         return sm.getMapPointCloud()
+
+    def map_size(self, sm) -> int:
+        return sm.size()
+
+    def assembled_map(self, sms, voxelSize: float):
+        """the assembled (and voxelized) map in one b2s_assemble_map call: a device Cloud"""
+        return E.getAssembledMapPointCloud(self.eng, sms, voxelSize)
+
+    def assembled_colored_map(self, sms, voxelSize: float):
+        """(device Cloud, host rgb) of one b2s_assemble_colored_map call"""
+        return E.assembleColoredPointCloud(self.eng, sms, voxelSize)
 
     def map_center(self, sm) -> np.ndarray:
         xyz, _ = sm.getMapPointCloud()

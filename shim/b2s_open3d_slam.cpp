@@ -463,4 +463,45 @@ void computeOdometryConstraintsB200(const std::vector<const SubmapB200*>& submap
   }
 }
 
+namespace {
+std::vector<const b2s_submap*> assemblyInputs(const std::vector<const SubmapB200*>& submaps, b2s_handle** h) {
+  std::vector<const b2s_submap*> sms;
+  for (const SubmapB200* s : submaps) { sms.push_back(s->handle()); *h = s->engine(); }
+  return sms;
+}
+}  // namespace
+
+PointCloud getAssembledMapPointCloudB200(const std::vector<const SubmapB200*>& submaps, double voxelSize) {
+  if (submaps.empty()) return PointCloud();
+  b2s_handle* h = nullptr;
+  const std::vector<const b2s_submap*> sms = assemblyInputs(submaps, &h);
+  DeviceCloud out(h);
+  const int32_t rc = b2s_assemble_map(h, (int32_t)sms.size(), sms.data(), voxelSize, out.c);
+  if (rc != B2S_OK) b2sThrow(rc);
+  return *out.download();
+}
+
+PointCloud assembleColoredPointCloudB200(const std::vector<const SubmapB200*>& submaps, double voxelSize) {
+  PointCloud cloud;
+  if (submaps.empty()) return cloud;   // helpers_ros.cpp:52-54
+  b2s_handle* h = nullptr;
+  const std::vector<const b2s_submap*> sms = assemblyInputs(submaps, &h);
+  size_t bound = 0;   // getTotalNumPoints: the colour buffer's capacity
+  for (const b2s_submap* s : sms) {
+    size_t n = 0;
+    const int32_t rc = b2s_submap_size(h, s, &n);
+    if (rc != B2S_OK) b2sThrow(rc);
+    bound += n;
+  }
+  DeviceCloud out(h);
+  std::vector<Eigen::Vector3d> rgb(bound);
+  size_t n = 0;
+  const int32_t rc = b2s_assemble_colored_map(h, (int32_t)sms.size(), sms.data(), voxelSize, out.c, bound ? rgb.front().data() : nullptr, bound, &n);
+  if (rc != B2S_OK) b2sThrow(rc);
+  cloud.points_ = std::move(out.download()->points_);
+  rgb.resize(n);
+  cloud.colors_ = std::move(rgb);
+  return cloud;
+}
+
 }  // namespace o3d_slam

@@ -136,6 +136,15 @@ RansacResultB200 registrationRansacBasedOnFeatureMatchingB200(const SubmapB200& 
 void computeOdometryConstraintsB200(const std::vector<const SubmapB200*>& submaps, const std::vector<size_t>& parentIds, size_t activeSubmapIdx,
                                     const std::vector<size_t>* candidates, const MapperParameters& p, Constraints* constraints);
 
+// Mapper::getAssembledMapPointCloud (src/Mapper.cpp:183-208) over device-resident submaps (all on one handle), in the order given, then
+// o3d_slam::voxelize(voxelSize) (a no-op for voxelSize <= 0): SlamWrapper::saveMap passes 0, SlamWrapperRos::publishMaps
+// assembledMapVoxelSize_.  One b2s_assemble_map call; points_ and normals_ (normals only when every submap that contributes a point has
+// them, DESIGN.md row A1).
+PointCloud getAssembledMapPointCloudB200(const std::vector<const SubmapB200*>& submaps, double voxelSize);
+// assembleColoredPointCloud (ros/open3d_slam_ros/src/helpers_ros.cpp:51-70) + voxelize(voxelSize) as publishMaps runs it with
+// submapVoxelSize_: points_ and colors_ (submap j in Color::getColor(j % 11 + 2)), no normals.  One b2s_assemble_colored_map call.
+PointCloud assembleColoredPointCloudB200(const std::vector<const SubmapB200*>& submaps, double voxelSize);
+
 class ScanToMapIcpB200 : public ScanToMapRegistration {
  public:
   explicit ScanToMapIcpB200(const MapperParameters& p);
