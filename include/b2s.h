@@ -691,6 +691,19 @@ void b2s_default_global_optimization_params(b2s_global_optimization_params* p);
 int32_t b2s_global_optimization(b2s_handle* h, int32_t n_nodes, double* node_poses, int32_t n_edges, const b2s_pose_graph_edge* edges,
                                 const b2s_global_optimization_params* p, int32_t* edge_kept_out, double* edge_confidence_out,
                                 b2s_global_optimization_stats* stats_out);
+/* Debug aids for tests: the production launches of one LM try and of one linearisation on host-given inputs (they use and may grow
+ * the handle's pose-graph scratch).  b2s_debug_pose_graph_solve: A is 6N x 6N row-major, only its lower triangle is read; runs the
+ * forming of A + lambda I, the blocked LDL' and both substitutions.  delta_out (6N) receives the step; d_out (6N, optional) the
+ * pivots D; L_out (6N x 6N row-major, optional) the unit lower factor (upper triangle 0).
+ * b2s_debug_pose_graph_linearize: poses n_nodes row-major 4x4, the line-process weight from p; the residual with conf_in, then the
+ * confidence update and the linear system, as the start of a pass runs them.  conf_out (n_edges), H_out (6N x 6N row-major, its
+ * lower triangle, upper 0), b_out (6N), rec_out {residual at conf_in, signed max b, max diag H, sum |TransformMatrix4dToVector6d|^2}.
+ * Errors: n_nodes < 1, n_edges < 0, a null array, an id out of range -> B2S_E_INVALID. */
+int32_t b2s_debug_pose_graph_solve(b2s_handle* h, int32_t n_nodes, const double* A, const double* b, double lambda, double* delta_out,
+                                   double* d_out, double* L_out);
+int32_t b2s_debug_pose_graph_linearize(b2s_handle* h, int32_t n_nodes, const double* poses, int32_t n_edges, const b2s_pose_graph_edge* edges,
+                                       const b2s_global_optimization_params* p, const double* conf_in, double* conf_out, double* H_out,
+                                       double* b_out, double rec_out[4]);
 
 /* ---- the assembled map: Mapper::getAssembledMapPointCloud (src/Mapper.cpp:183-208), which SlamWrapper::saveMap (src/SlamWrapper.cpp:
  *      242-247) writes and SlamWrapperRos::publishMaps (ros/open3d_slam_ros/src/SlamWrapperRos.cpp:222-244) voxelizes with

@@ -1362,6 +1362,27 @@ int32_t b2s_global_optimization(b2s_handle* h, int32_t n_nodes, double* node_pos
   return op_global_optimization(h, n_nodes, node_poses, n_edges, edges, *p, edge_kept_out, edge_confidence_out, stats_out);
 }
 
+int32_t b2s_debug_pose_graph_solve(b2s_handle* h, int32_t n_nodes, const double* A, const double* b, double lambda, double* delta_out,
+                                   double* d_out, double* L_out) {
+  B2S_REQUIRE(h && A && b && delta_out, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(n_nodes >= 1, B2S_E_INVALID, "n_nodes %d must be >= 1", (int)n_nodes);
+  LOCK(h);
+  return op_debug_pose_graph_solve(h, n_nodes, A, b, lambda, delta_out, d_out, L_out);
+}
+
+int32_t b2s_debug_pose_graph_linearize(b2s_handle* h, int32_t n_nodes, const double* poses, int32_t n_edges, const b2s_pose_graph_edge* edges,
+                                       const b2s_global_optimization_params* p, const double* conf_in, double* conf_out, double* H_out,
+                                       double* b_out, double rec_out[4]) {
+  B2S_REQUIRE(h && poses && p && H_out && b_out && rec_out, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(n_nodes >= 1 && n_edges >= 0, B2S_E_INVALID, "n_nodes %d must be >= 1 and n_edges %d >= 0", (int)n_nodes, (int)n_edges);
+  B2S_REQUIRE(n_edges == 0 || (edges && conf_in && conf_out), B2S_E_INVALID, "null edges or confidences");
+  for (int32_t e = 0; e < n_edges; e++)
+    B2S_REQUIRE(edges[e].source >= 0 && edges[e].source < n_nodes && edges[e].target >= 0 && edges[e].target < n_nodes, B2S_E_INVALID,
+                "edge %d: node ids (%d, %d) outside [0, %d)", (int)e, (int)edges[e].source, (int)edges[e].target, (int)n_nodes);
+  LOCK(h);
+  return op_debug_pose_graph_linearize(h, n_nodes, poses, n_edges, edges, *p, conf_in, conf_out, H_out, b_out, rec_out);
+}
+
 // ---- the assembled map (Mapper.cpp:183-208, helpers_ros.cpp:51-70, SlamWrapperRos.cpp:222-244) ----------------------------------------
 static int32_t check_assembly_args(b2s_handle* h, int32_t n, const b2s_submap* const* submaps, const b2s_cloud* out) {
   B2S_REQUIRE(h && out, B2S_E_INVALID, "null argument");

@@ -508,6 +508,12 @@ int32_t op_odometry_constraints(b2s_handle* h, int n, const b2s_submap* const* s
 // G1 (posegraph.cu): [O3D] GlobalOptimization (Levenberg-Marquardt) of a validated graph: ids in range, parameters checked
 int32_t op_global_optimization(b2s_handle* h, int n_nodes, double* poses, int n_edges, const b2s_pose_graph_edge* edges,
                                const b2s_global_optimization_params& p, int32_t* kept_out, double* conf_out, b2s_global_optimization_stats* stats);
+// its production launches on host-given inputs (b2s_debug_pose_graph_solve / _linearize)
+int32_t op_debug_pose_graph_solve(b2s_handle* h, int n_nodes, const double* A, const double* b, double lambda, double* delta_out, double* d_out,
+                                  double* L_out);
+int32_t op_debug_pose_graph_linearize(b2s_handle* h, int n_nodes, const double* poses, int n_edges, const b2s_pose_graph_edge* edges,
+                                      const b2s_global_optimization_params& p, const double* conf_in, double* conf_out, double* H_out,
+                                      double* b_out, double* rec_out);
 // K-fpfh (features.cu): [O3D] ComputeFPFHFeature of the n points of c (normals required, 1 <= knn <= B2S_FEATURE_MAX_KNN)
 int32_t op_compute_fpfh(b2s_handle* h, const b2s_cloud* c, size_t n, double radius, int knn, b2s_feature* f);
 // K-ransac (ransac.cu): exact feature correspondences of one source feature against n target features (device outputs; s2t[k] / t2s[k]

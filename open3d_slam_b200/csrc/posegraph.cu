@@ -21,7 +21,8 @@
 //   K-pg-update    trial poses V2M(delta_i) T_i; K-pg-edge (trial zeta and residual terms); K-pg-reduce-try (one record)
 // An accepted try adds K-pg-edge (linearise: confidences, per-edge blocks), K-pg-assemble (one CTA per nonzero node block: its
 // incident edges summed in edge order from host-built lists) and K-pg-reduce-lin.  Every sum has a fixed order and there are no
-// atomics: a repeated call is bit-identical.
+// atomics: a repeated call is bit-identical.  The test hooks b2s_debug_pose_graph_solve / _linearize run the same launch functions
+// (pg_factor_solve; pg_load, pg_eval and pg_linearize) on host-given inputs.
 #include "common.cuh"
 
 #include <algorithm>
@@ -513,10 +514,9 @@ int edge_grid(int ecap) { return (ecap + 127) / 128; }
 
 struct PgCtx { PgLayout L; b2s_handle* h; };
 
-// one LM try: H + lambda I -> LDL' -> delta -> trial poses -> trial residual; the record lands in L->rec
-int32_t pg_try_chain(void* ctx) {
-  const PgLayout& L = static_cast<const PgCtx*>(ctx)->L;
-  b2s_handle* h = static_cast<const PgCtx*>(ctx)->h;
+// H + lambda I -> blocked LDL' -> delta: K-pg-form, per tile column K-pg-diag, K-pg-panel and K-pg-trailing, then K-pg-fwd and
+// K-pg-bwd per tile.  Returns the number of launches
+int64_t pg_factor_solve(b2s_handle* h, const PgLayout& L) {
   const int M = L.M, nt = L.nt;
   int64_t n = 0;
   launch_pdl(pg_form_kernel, grid_for((size_t)M * M, 256, 4 * device_sms()), 256, 0, h->stream, (const double*)L.A, (const double*)L.b,
@@ -533,6 +533,14 @@ int32_t pg_try_chain(void* ctx) {
   }
   for (int K = 0; K < nt; K++) { launch_pdl(pg_fwd_kernel, nt - K, 256, 0, h->stream, (const double*)L.F, (const double*)L.D, L.rhs, L.z, K, M); n++; }
   for (int K = nt - 1; K >= 0; K--) { launch_pdl(pg_bwd_kernel, K + 1, 256, 0, h->stream, (const double*)L.F, L.z, L.delta, K, M); n++; }
+  return n;
+}
+
+// one LM try: H + lambda I -> LDL' -> delta -> trial poses -> trial residual; the record lands in L->rec
+int32_t pg_try_chain(void* ctx) {
+  const PgLayout& L = static_cast<const PgCtx*>(ctx)->L;
+  b2s_handle* h = static_cast<const PgCtx*>(ctx)->h;
+  int64_t n = pg_factor_solve(h, L);
   launch_pdl(pg_update_kernel, (L.N + 127) / 128, 128, 0, h->stream, (const double*)L.P, (const double*)L.delta, L.Pt, L.N);
   launch_pdl(pg_edge_kernel, edge_grid(L.ecap), 128, 0, h->stream, (const b2s_pose_graph_edge*)L.E, (const int32_t*)L.ne, (const double*)L.Pt,
              L.conf, (const double*)L.scal, 0, L.term, L.hss, L.gv);
@@ -567,14 +575,9 @@ int32_t pg_linearize(b2s_handle* h, const PgLayout& L, int ntasks) {
   return B2S_OK;
 }
 
-// GlobalOptimizationLevenbergMarquardt::OptimizePoseGraph over the edges E (the node poses are resident in L->P).  conf: the
-// edges' confidences, in and out
-int32_t pg_pass(b2s_handle* h, int N, const std::vector<b2s_pose_graph_edge>& E, std::vector<double>& conf, const b2s_global_optimization_params& p,
-                b2s_global_optimization_stats* st) {
+// the assembly lists: diagonal block of every node, then the off-diagonal blocks in (row, col) order; contributions in edge order
+void pg_assembly_lists(int N, const std::vector<b2s_pose_graph_edge>& E, std::vector<PgTask>& tasks, std::vector<int32_t>& contrib) {
   const int ne = (int)E.size();
-  // the assembly lists: diagonal block of every node, then the off-diagonal blocks in (row, col) order; contributions in edge order
-  std::vector<PgTask> tasks;
-  std::vector<int32_t> contrib;
   std::vector<std::vector<int32_t>> diag((size_t)N);
   std::vector<std::pair<std::pair<int, int>, int32_t>> off;
   for (int e = 0; e < ne; e++) {
@@ -598,8 +601,16 @@ int32_t pg_pass(b2s_handle* h, int N, const std::vector<b2s_pose_graph_edge>& E,
     contrib.push_back(off[k].second);
     tasks.back().end = (int32_t)contrib.size();
   }
-  PgLayout L;
-  B2S_TRY(pg_prepare(h, N, ne, (int)tasks.size(), (int)contrib.size(), &L));
+}
+
+// a pass's device state: the buffers (pg_prepare), the edges, their confidences, the assembly lists (built into tasks / contrib),
+// lambda = 0 and the line-process weight, a zeroed H and delta.  The node poses are the caller's
+int32_t pg_load(b2s_handle* h, int N, const std::vector<b2s_pose_graph_edge>& E, const std::vector<double>& conf, const b2s_global_optimization_params& p,
+                std::vector<PgTask>& tasks, std::vector<int32_t>& contrib, PgLayout* Lo) {
+  const int ne = (int)E.size();
+  pg_assembly_lists(N, E, tasks, contrib);
+  B2S_TRY(pg_prepare(h, N, ne, (int)tasks.size(), (int)contrib.size(), Lo));
+  const PgLayout& L = *Lo;
   double lpw = 0.0;   // ComputeLineProcessWeight
   for (const b2s_pose_graph_edge& e : E) lpw += e.information[35];
   if (ne > 0) lpw /= (double)ne;
@@ -612,10 +623,22 @@ int32_t pg_pass(b2s_handle* h, int N, const std::vector<b2s_pose_graph_edge>& E,
   B2S_CUDA(cudaMemcpyAsync(L.ne, &ne32, 4, cudaMemcpyHostToDevice, h->stream));
   B2S_CUDA(cudaMemcpyAsync(L.tasks, tasks.data(), sizeof(PgTask) * tasks.size(), cudaMemcpyHostToDevice, h->stream));
   if (!contrib.empty()) B2S_CUDA(cudaMemcpyAsync(L.contrib, contrib.data(), 4 * contrib.size(), cudaMemcpyHostToDevice, h->stream));
-  double scal[2] = {0.0, lpw};
+  const double scal[2] = {0.0, lpw};
   B2S_CUDA(cudaMemcpyAsync(L.scal, scal, sizeof(scal), cudaMemcpyHostToDevice, h->stream));
   B2S_CUDA(cudaMemsetAsync(L.A, 0, (size_t)L.M * L.M * 8, h->stream));
   B2S_CUDA(cudaMemsetAsync(L.delta, 0, (size_t)L.M * 8, h->stream));   // read (unused) by the first residual's reduction
+  return B2S_OK;
+}
+
+// GlobalOptimizationLevenbergMarquardt::OptimizePoseGraph over the edges E (the node poses are resident in L->P).  conf: the
+// edges' confidences, in and out
+int32_t pg_pass(b2s_handle* h, int N, const std::vector<b2s_pose_graph_edge>& E, std::vector<double>& conf, const b2s_global_optimization_params& p,
+                b2s_global_optimization_stats* st) {
+  const int ne = (int)E.size();
+  std::vector<PgTask> tasks;
+  std::vector<int32_t> contrib;
+  PgLayout L;
+  B2S_TRY(pg_load(h, N, E, conf, p, tasks, contrib, &L));
 
   double rec[PG_R_WORDS];
   auto fetch = [&]() { return read_back(h, {{rec, L.rec, sizeof(rec)}}); };
@@ -638,8 +661,7 @@ int32_t pg_pass(b2s_handle* h, int N, const std::vector<b2s_pose_graph_edge>& E,
     st->outer_iterations++;
     int lm_count = 0;
     do {
-      scal[0] = lambda;
-      B2S_CUDA(cudaMemcpyAsync(L.scal, scal, 8, cudaMemcpyHostToDevice, h->stream));
+      B2S_CUDA(cudaMemcpyAsync(L.scal + PG_S_LAMBDA, &lambda, 8, cudaMemcpyHostToDevice, h->stream));
       B2S_TRY(graph_step(h, &h->pg_graph, key, pg_try_chain, &ctx));
       B2S_TRY(fetch());
       st->lm_tries++;
@@ -736,6 +758,54 @@ int32_t op_global_optimization(b2s_handle* h, int N, double* poses, int ne, cons
   }
   memcpy(poses, out.data(), out.size() * 8);
   return finish();
+}
+
+int32_t op_debug_pose_graph_solve(b2s_handle* h, int N, const double* A, const double* b, double lambda, double* delta_out, double* d_out,
+                                  double* L_out) {
+  PgLayout L;
+  B2S_TRY(pg_prepare(h, N, 0, 0, 0, &L));
+  const size_t n6 = (size_t)L.n6, M = (size_t)L.M;
+  B2S_CUDA(cudaMemcpy2DAsync(L.A, M * 8, A, n6 * 8, n6 * 8, n6, cudaMemcpyHostToDevice, h->stream));
+  B2S_CUDA(cudaMemcpyAsync(L.b, b, n6 * 8, cudaMemcpyHostToDevice, h->stream));
+  B2S_CUDA(cudaMemcpyAsync(L.scal + PG_S_LAMBDA, &lambda, 8, cudaMemcpyHostToDevice, h->stream));
+  h->launches += pg_factor_solve(h, L);
+  B2S_CUDA(cudaGetLastError());
+  B2S_CUDA(cudaMemcpyAsync(delta_out, L.delta, n6 * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (d_out) B2S_CUDA(cudaMemcpyAsync(d_out, L.D, n6 * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (L_out) B2S_CUDA(cudaMemcpy2DAsync(L_out, n6 * 8, L.F, M * 8, n6 * 8, n6, cudaMemcpyDeviceToHost, h->stream));
+  B2S_TRY(check_status(h));
+  if (L_out)   // F holds the pivots on its diagonal and stale values above it
+    for (size_t r = 0; r < n6; r++) {
+      L_out[r * n6 + r] = 1.0;
+      for (size_t c = r + 1; c < n6; c++) L_out[r * n6 + c] = 0.0;
+    }
+  return B2S_OK;
+}
+
+int32_t op_debug_pose_graph_linearize(b2s_handle* h, int N, const double* poses, int ne, const b2s_pose_graph_edge* edges,
+                                      const b2s_global_optimization_params& p, const double* conf_in, double* conf_out, double* H_out,
+                                      double* b_out, double* rec_out) {
+  const std::vector<b2s_pose_graph_edge> E(edges, edges + ne);
+  const std::vector<double> conf(conf_in, conf_in + ne);
+  std::vector<PgTask> tasks;
+  std::vector<int32_t> contrib;
+  PgLayout L;
+  B2S_TRY(pg_load(h, N, E, conf, p, tasks, contrib, &L));
+  B2S_CUDA(cudaMemcpyAsync(L.P, poses, 16 * 8 * (size_t)N, cudaMemcpyHostToDevice, h->stream));
+  double rec[PG_R_WORDS];
+  B2S_TRY(pg_eval(h, L, L.P));   // as pg_pass: the residual with the incoming confidences, then the linear system
+  B2S_TRY(read_back(h, {{rec, L.rec, sizeof(rec)}}));
+  rec_out[0] = rec[PG_R_RES];
+  B2S_TRY(pg_linearize(h, L, (int)tasks.size()));
+  const size_t n6 = (size_t)L.n6, M = (size_t)L.M;
+  if (ne > 0) B2S_CUDA(cudaMemcpyAsync(conf_out, L.conf, 8 * (size_t)ne, cudaMemcpyDeviceToHost, h->stream));
+  B2S_CUDA(cudaMemcpy2DAsync(H_out, n6 * 8, L.A, M * 8, n6 * 8, n6, cudaMemcpyDeviceToHost, h->stream));
+  B2S_CUDA(cudaMemcpyAsync(b_out, L.b, n6 * 8, cudaMemcpyDeviceToHost, h->stream));
+  B2S_TRY(read_back(h, {{rec, L.rec, sizeof(rec)}}));
+  for (size_t r = 0; r < n6; r++)   // the factorisation reads the lower triangle; above it lie the diagonal blocks' upper halves
+    for (size_t c = r + 1; c < n6; c++) H_out[r * n6 + c] = 0.0;
+  rec_out[1] = rec[PG_R_MAXB]; rec_out[2] = rec[PG_R_MAXDIAG]; rec_out[3] = rec[PG_R_XX];
+  return B2S_OK;
 }
 
 }  // namespace b2s
