@@ -633,6 +633,51 @@ int32_t b2s_submap_odometry_constraints(b2s_handle* h, int32_t n_pairs, const b2
                                         b2s_cloud* const* source_overlaps_or_null, b2s_cloud* const* target_overlaps_or_null,
                                         b2s_odometry_constraint* out);
 
+/* ---- loop-closure refinement: the second half of PlaceRecognition::buildLoopClosureConstraints (src/PlaceRecognition.cpp:96-149)
+ *      for one finished (source) submap against the candidates whose RANSAC proposal passed its gates, on the maps where they live.
+ *      For every target k, with T0 = inits[16k .. 16k + 15] (row-major, the proposal's transformation_):
+ *   - source and target clouds are the WHOLE maps, getMapPointCloudCopy (the live map slots in map order)                  :64, :95
+ *   - voxel = getMapVoxelSize(map_voxel_size, voxel_if_zero): |v| <= 1e-3 -> voxel_if_zero, else v                       :98
+ *   - overlap at T0 with edge overlap_factor x voxel and minNumPointsPerVoxel = min_points_per_voxel: the source points are
+ *     keyed after T0 ([O3D] PointCloud::Transform), the selected points are the UNTRANSFORMED ones, each map's survivors in map
+ *     order (b2s_overlap's rule, SelectByIndex on the original clouds)                                                   :99-106
+ *   - RegistrationICP(sourceOverlap, targetOverlap, r = max_corr_dist, T0, TransformationEstimationPointToPlane,
+ *     max_iter / rel_fitness / rel_rmse) for every pair                                                                  :45-47, :110
+ *   - accepted = !(icp.fitness < min_refinement_fitness)                                                                  :118
+ *   - information = GetInformationMatrixFromPointClouds(sourceOverlap, targetOverlap, max_corr_dist, icp.T), for EVERY pair
+ *     (the reference computes it for the accepted ones; the others' matrix is there for the caller to ignore)           :148-149
+ *   The consistency check of icp.T (:124) stays with the caller, as does candidate selection and RANSAC.
+ * Deviations: the ICP is ALWAYS point-to-plane, whatever b2s_config.icp.reg_type is; the reference registers with the scan matcher's
+ * type (cloudRegistrationFactory, :47), point-to-plane in every shipped configuration.  The getMapVoxelSize rule is applied here,
+ * as the reference does; a caller that composes b2s_submap_to_cloud + b2s_overlap itself and passes map_voxel_size = 0 gets an
+ * error from b2s_overlap (voxel 0), while this call uses voxel_if_zero -- the one input where the two answer differently.
+ * Errors: a submap or an overlap cloud of another handle, a null init array for n_targets > 0, a voxel <= 0 after the getMapVoxelSize
+ * rule, overlap_factor <= 0, max_corr_dist <= 0, min_points_per_voxel < 1, max_iter < 0, n_targets < 0 -> B2S_E_INVALID; a target
+ * map without normals (a point-to-point map, stored as NaN) -> B2S_E_NO_NORMALS.  n_targets = 0 -> B2S_OK.  The same target may
+ * be listed more than once.  One call runs every pair in one set of launches and synchronises once; out[k] does not depend on the
+ * other targets.  source_overlaps_or_null / target_overlaps_or_null (each an array of n_targets clouds, or NULL) receive the
+ * selected points, in map order.  Scratch: the handle's odometry-constraint slots.  Semantics and kernels: DESIGN.md row L3. */
+typedef struct b2s_loop_closure_refinement_params {
+  double map_voxel_size, voxel_if_zero;  /* getMapVoxelSize(mapBuilder_, 0.04) (0.1, 0.04), PlaceRecognition.cpp:98 */
+  double overlap_factor;                 /* magic::voxelExpansionFactorOverlapComputation = 20, :100 */
+  int32_t min_points_per_voxel;          /* 1, :101 */
+  int32_t max_iter;                      /* magic::icpRunUntilConvergenceNumberOfIterations = 100, :45 */
+  double max_corr_dist;                  /* placeRecognition.maxIcpCorrespondenceDistance = 0.3: ICP and information radius, :46, :149 */
+  double rel_fitness, rel_rmse;          /* [O3D] ICPConvergenceCriteria defaults, 1e-6 */
+  double min_refinement_fitness;         /* placeRecognition.minRefinementFitness = 0.7, :118 */
+} b2s_loop_closure_refinement_params;
+typedef struct b2s_loop_closure_refinement {
+  b2s_result icp;                        /* RegistrationResult of the refinement */
+  double information[36];                /* row-major, at icp.T */
+  int64_t n_source_overlap, n_target_overlap;
+  int32_t accepted;                      /* the fitness gate */
+} b2s_loop_closure_refinement;
+void b2s_default_loop_closure_refinement_params(b2s_loop_closure_refinement_params* p);
+int32_t b2s_submap_loop_closure_refinement(b2s_handle* h, const b2s_submap* source, int32_t n_targets, const b2s_submap* const* targets,
+                                           const double* inits /* n_targets x 16 */, const b2s_loop_closure_refinement_params* p,
+                                           b2s_cloud* const* source_overlaps_or_null, b2s_cloud* const* target_overlaps_or_null,
+                                           b2s_loop_closure_refinement* out);
+
 /* ---- submap pose-graph optimisation: [O3D] GlobalOptimization with GlobalOptimizationLevenbergMarquardt, as
  *      OptimizationProblem::solve (src/OptimizationProblem.cpp:25-44) calls it.  Restated semantics (DESIGN.md row G1):
  *   - validation: every edge id in [0, n_nodes) (else B2S_E_INVALID); the graph connected from node 0 over all edges and over the

@@ -107,6 +107,17 @@ class OdometryConstraint(C.Structure):
                 ("refined", C.c_int32), ("icp", Result)]
 
 
+class LoopClosureRefinementParams(C.Structure):
+    _fields_ = [("map_voxel_size", C.c_double), ("voxel_if_zero", C.c_double), ("overlap_factor", C.c_double), ("min_points_per_voxel", C.c_int32),
+                ("max_iter", C.c_int32), ("max_corr_dist", C.c_double), ("rel_fitness", C.c_double), ("rel_rmse", C.c_double),
+                ("min_refinement_fitness", C.c_double)]
+
+
+class LoopClosureRefinement(C.Structure):
+    _fields_ = [("icp", Result), ("information", C.c_double * 36), ("n_source_overlap", C.c_int64), ("n_target_overlap", C.c_int64),
+                ("accepted", C.c_int32)]
+
+
 class PoseGraphEdge(C.Structure):
     _fields_ = [("source", C.c_int32), ("target", C.c_int32), ("uncertain", C.c_int32), ("reserved_", C.c_int32), ("T", C.c_double * 16),
                 ("information", C.c_double * 36)]
@@ -157,6 +168,7 @@ SYMBOLS = [
     "b2s_default_motion_compensation_params", "b2s_odometry_set_motion_compensation", "b2s_slam_map_pose_push", "b2s_slam_map_lookup",
     "b2s_slam_motion_fetch", "b2s_slam_undistorted",
     "b2s_default_odometry_constraint_params", "b2s_submap_odometry_constraints",
+    "b2s_default_loop_closure_refinement_params", "b2s_submap_loop_closure_refinement",
     "b2s_default_global_optimization_params", "b2s_global_optimization", "b2s_cloud_transform_inplace",
     "b2s_submap_set_initial_map", "b2s_submap_set_initial_transform", "b2s_submap_set_merge_scans", "b2s_debug_nn_index",
     "b2s_assemble_map", "b2s_assemble_colored_map", "b2s_debug_pose_graph_solve", "b2s_debug_pose_graph_linearize",
@@ -208,6 +220,7 @@ def lib():
         L.b2s_default_odometry_params.restype = None
         L.b2s_default_motion_compensation_params.restype = None
         L.b2s_default_odometry_constraint_params.restype = None
+        L.b2s_default_loop_closure_refinement_params.restype = None
         L.b2s_default_global_optimization_params.restype = None
         _lib = L
     return _lib

@@ -1338,6 +1338,43 @@ int32_t b2s_submap_odometry_constraints(b2s_handle* h, int32_t n, const b2s_subm
   return op_odometry_constraints(h, n, sources, targets, *p, voxel, so, to, out);
 }
 
+// ---- loop-closure refinement (src/PlaceRecognition.cpp:96-149) ----------------------------------------------------------------
+void b2s_default_loop_closure_refinement_params(b2s_loop_closure_refinement_params* p) {   // Parameters.hpp:130-131, magic.hpp, Lua mapper
+  memset(p, 0, sizeof(*p));
+  p->map_voxel_size = 0.1; p->voxel_if_zero = 0.04; p->overlap_factor = 20.0; p->min_points_per_voxel = 1; p->max_iter = 100;
+  p->max_corr_dist = 0.3; p->rel_fitness = 1e-6; p->rel_rmse = 1e-6; p->min_refinement_fitness = 0.7;
+}
+
+int32_t b2s_submap_loop_closure_refinement(b2s_handle* h, const b2s_submap* source, int32_t n, const b2s_submap* const* targets, const double* inits,
+                                           const b2s_loop_closure_refinement_params* p, b2s_cloud* const* so, b2s_cloud* const* to,
+                                           b2s_loop_closure_refinement* out) {
+  B2S_REQUIRE(h && source && p && n >= 0, B2S_E_INVALID, "bad argument");
+  B2S_REQUIRE(source->h == h, B2S_E_INVALID, "the source submap belongs to another handle");
+  if (n == 0) return B2S_OK;
+  B2S_REQUIRE(targets && inits && out, B2S_E_INVALID, "null argument");
+  const double voxel = fabs(p->map_voxel_size) <= 1e-3 ? p->voxel_if_zero : p->map_voxel_size;   // getMapVoxelSize, PlaceRecognition.cpp:98
+  B2S_REQUIRE(voxel > 0.0, B2S_E_INVALID, "map voxel size %g after getMapVoxelSize: must be > 0", voxel);
+  B2S_REQUIRE(p->overlap_factor > 0.0, B2S_E_INVALID, "overlap_factor must be > 0");
+  B2S_REQUIRE(p->max_corr_dist > 0.0, B2S_E_INVALID, "[RegistrationICP] Invalid max_correspondence_distance.");
+  B2S_REQUIRE(p->min_points_per_voxel >= 1, B2S_E_INVALID, "minNumPointsPerVoxel must be >= 1");   // assert_ge at helpers.cpp:310
+  B2S_REQUIRE(p->max_iter >= 0, B2S_E_INVALID, "max_iter must be >= 0");
+  for (int32_t k = 0; k < n; k++) {
+    B2S_REQUIRE(targets[k], B2S_E_INVALID, "null target submap %d", k);
+    B2S_REQUIRE(targets[k]->h == h, B2S_E_INVALID, "target %d belongs to another handle", k);
+    for (b2s_cloud* const* c : {so, to})
+      if (c) {
+        B2S_REQUIRE(c[k] && c[k]->h == h, B2S_E_INVALID, "target %d: an overlap cloud is null or belongs to another handle", k);
+        B2S_REQUIRE(!c[k]->fixed_cap, B2S_E_INVALID, "target %d: an overlap cloud must not be a fixed-capacity staging cloud", k);
+      }
+    B2S_REQUIRE(!so || !to || so[k] != to[k], B2S_E_INVALID, "target %d: the two overlap clouds are the same object", k);
+  }
+  for (int32_t k = 0; k < n; k++)   // RegistrationICP's point-to-plane estimator needs the target's normals ([O3D] LogError)
+    B2S_REQUIRE(!targets[k]->no_normals, B2S_E_NO_NORMALS,
+                "[RegistrationICP] target %d: TransformationEstimationPointToPlane requires target normals, the map has none", k);
+  LOCK(h);
+  return op_loop_closure_refinement(h, source, n, targets, inits, *p, voxel, so, to, out);
+}
+
 // ---- pose-graph optimisation (src/OptimizationProblem.cpp:25-44 -> [O3D] GlobalOptimization, LM) -------------------------------
 void b2s_default_global_optimization_params(b2s_global_optimization_params* p) {   // parameter_structure_definitions.lua:45-50, [O3D] criteria
   memset(p, 0, sizeof(*p));

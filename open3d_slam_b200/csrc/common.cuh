@@ -505,6 +505,11 @@ int32_t op_overlap(b2s_handle* h, const b2s_cloud* source, const b2s_cloud* targ
 int32_t op_odometry_constraints(b2s_handle* h, int n, const b2s_submap* const* sources, const b2s_submap* const* targets,
                                 const b2s_odometry_constraint_params& p, double voxel, b2s_cloud* const* so_out, b2s_cloud* const* to_out,
                                 b2s_odometry_constraint* out);
+// L3 loop-closure refinement of one source against n targets at the host-given sourceToTarget guesses inits (n x 16) (constraints.cu);
+// voxel = the map voxel after getMapVoxelSize.  Synchronises once.
+int32_t op_loop_closure_refinement(b2s_handle* h, const b2s_submap* source, int n, const b2s_submap* const* targets, const double* inits,
+                                   const b2s_loop_closure_refinement_params& p, double voxel, b2s_cloud* const* so_out, b2s_cloud* const* to_out,
+                                   b2s_loop_closure_refinement* out);
 // G1 (posegraph.cu): [O3D] GlobalOptimization (Levenberg-Marquardt) of a validated graph: ids in range, parameters checked
 int32_t op_global_optimization(b2s_handle* h, int n_nodes, double* poses, int n_edges, const b2s_pose_graph_edge* edges,
                                const b2s_global_optimization_params& p, int32_t* kept_out, double* conf_out, b2s_global_optimization_stats* stats);

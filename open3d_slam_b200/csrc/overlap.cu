@@ -105,16 +105,20 @@ int32_t op_overlap(b2s_handle* h, const b2s_cloud* source, const b2s_cloud* targ
   return B2S_OK;
 }
 
-// ---- batched, in place on the submaps: the overlap at the identity of n (parent, child) map pairs (odometry constraints) ------------
-// Every pair owns a segment of one hash (sized like op_overlap's table for the pair's two maps); job 2k reads pair k's parent map,
-// job 2k + 1 its child map, straight from the map slots: a tombstone (NaN, left by fusion) is skipped, so the compacted result is the
+// ---- batched, in place on the submaps: the overlap of n (source, target) map pairs (odometry constraints, loop-closure refinement) ----
+// Every pair owns a segment of one hash (sized like op_overlap's table for the pair's two maps); job 2k reads pair k's source map,
+// job 2k + 1 its target map, straight from the map slots: a tombstone (NaN, left by fusion) is skipped, so the compacted result is the
 // one b2s_submap_to_cloud + op_overlap give, cloud by cloud and in order.  Each kernel takes its job from blockIdx.y.
+// T: the source job's sourceToTarget (device, row-major), applied to the keys like ov_insert_kernel does ([O3D] PointCloud::Transform);
+// nullptr = the identity, the points as they are.  The compacted points are the untransformed ones either way (SelectByIndex on the
+// original source, PlaceRecognition.cpp:105).
 struct OvJob {
   const double* xyz; const double* nrm; const int32_t* d_n;   // map slots
   unsigned long long* keys; int32_t* cnt; size_t mask;          // the pair's hash segment
   int32_t* slot_of; int32_t* keep; int32_t* offs;               // per map slot
   double* oxyz; double* onrm; int32_t* out_n;                   // the overlap cloud
-  int32_t which, pad;                                           // 0 = parent (source), 1 = child (target)
+  const double* T;                                              // source jobs: sourceToTarget or nullptr; target jobs: nullptr
+  int32_t which, pad;                                           // 0 = source (parent), 1 = target (child)
 };
 
 __global__ void __launch_bounds__(OV_THREADS) ovb_init_kernel(const OvJob* __restrict__ jobs) {
@@ -130,9 +134,17 @@ __global__ void __launch_bounds__(OV_THREADS) ovb_insert_kernel(const OvJob* __r
   const OvJob j = jobs[blockIdx.y];
   const int n = *j.d_n;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double x = j.xyz[3 * (size_t)i], y = j.xyz[3 * (size_t)i + 1], z = j.xyz[3 * (size_t)i + 2];
+    double x = j.xyz[3 * (size_t)i], y = j.xyz[3 * (size_t)i + 1], z = j.xyz[3 * (size_t)i + 2];
     j.slot_of[i] = -1;
     if (!(x == x)) continue;   // tombstone
+    if (j.T) {                 // the arithmetic of ov_insert_kernel: row sums left to right, then the homogeneous divide
+      const double* T = j.T;
+      const double a = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], x), __dmul_rn(T[1], y)), __dmul_rn(T[2], z)), T[3]);
+      const double b = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], x), __dmul_rn(T[5], y)), __dmul_rn(T[6], z)), T[7]);
+      const double c = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], x), __dmul_rn(T[9], y)), __dmul_rn(T[10], z)), T[11]);
+      const double w = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[12], x), __dmul_rn(T[13], y)), __dmul_rn(T[14], z)), T[15]);
+      x = __ddiv_rn(a, w); y = __ddiv_rn(b, w); z = __ddiv_rn(c, w);
+    }
     const double fx = floor(x * inv), fy = floor(y * inv), fz = floor(z * inv);
     if (!(fabs(fx) < 1048575.0 && fabs(fy) < 1048575.0 && fabs(fz) < 1048575.0)) { atomicOr(status, ST_KEY_OVERFLOW); continue; }
     const unsigned long long key = ov_pack((int)fx, (int)fy, (int)fz);
@@ -167,15 +179,20 @@ __global__ void __launch_bounds__(OV_THREADS) ovb_compact_kernel(const OvJob* __
   }
 }
 
-// maps[2k], maps[2k + 1]: pair k's parent and child; outs[2k], outs[2k + 1]: their overlap clouds (reserved here).  The job tables and
-// the per-slot arrays live in h->odo; the tables are staged through host_stage (page-locked, op_overlap_batch_stage_bytes(n)) so that
-// nothing here waits for the device.
-size_t op_overlap_batch_stage_bytes(int n) { return (((size_t)2 * n * sizeof(OvJob) + 255) & ~(size_t)255) + (size_t)2 * n * sizeof(ScanJob); }
-int32_t op_overlap_batch(b2s_handle* h, int n, const b2s_submap* const* maps, double voxel, int min_pts, b2s_cloud* const* outs,
-                         unsigned char* host_stage) {
+// maps[2k], maps[2k + 1]: pair k's source and target; outs[2k], outs[2k + 1]: their overlap clouds (reserved here).  inits: n row-major
+// 4x4 sourceToTarget (host), or nullptr for the identity.  The job tables, the transforms and the per-slot arrays live in h->odo; the
+// tables and transforms are staged through host_stage (page-locked, op_overlap_batch_stage_bytes(n)) so that nothing here waits for
+// the device.
+size_t op_overlap_batch_stage_bytes(int n) {
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  return al((size_t)2 * n * sizeof(OvJob)) + al((size_t)2 * n * sizeof(ScanJob)) + (size_t)n * 16 * sizeof(double);
+}
+int32_t op_overlap_batch(b2s_handle* h, int n, const b2s_submap* const* maps, const double* inits, double voxel, int min_pts,
+                         b2s_cloud* const* outs, unsigned char* host_stage) {
   const int nj = 2 * n;
   auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-  size_t max_n = 1, bytes = al((size_t)nj * sizeof(OvJob)) + al((size_t)nj * sizeof(ScanJob));
+  const size_t tables = al((size_t)nj * sizeof(OvJob)) + al((size_t)nj * sizeof(ScanJob));
+  size_t max_n = 1, bytes = al(op_overlap_batch_stage_bytes(n));
   std::vector<size_t> caps((size_t)n);
   for (int k = 0; k < n; k++) {
     const size_t ns = maps[2 * k]->cloud[0]->n_max > 0 ? maps[2 * k]->cloud[0]->n_max : 1;
@@ -197,7 +214,9 @@ int32_t op_overlap_batch(b2s_handle* h, int n, const b2s_submap* const* maps, do
   unsigned char* dev = h->odo.as<unsigned char>();
   OvJob* oj = reinterpret_cast<OvJob*>(host_stage);
   ScanJob* sj = reinterpret_cast<ScanJob*>(host_stage + al((size_t)nj * sizeof(OvJob)));
-  size_t off = al((size_t)nj * sizeof(OvJob)) + al((size_t)nj * sizeof(ScanJob));
+  if (inits) memcpy(host_stage + tables, inits, (size_t)n * 16 * sizeof(double));
+  const double* dT = reinterpret_cast<const double*>(dev + tables);
+  size_t off = al(op_overlap_batch_stage_bytes(n));
   const size_t state_begin = off;
   for (int j = 0; j < nj; j++) {   // tile states first: they are the region zeroed below
     const size_t m = maps[j]->cloud[0]->n_max > 0 ? maps[j]->cloud[0]->n_max : 1;
@@ -221,11 +240,12 @@ int32_t op_overlap_batch(b2s_handle* h, int n, const b2s_submap* const* maps, do
       J.keep = reinterpret_cast<int32_t*>(dev + off); off += al((m + 2) * 4);
       J.offs = reinterpret_cast<int32_t*>(dev + off); off += al((m + 2) * 4);
       J.oxyz = outs[j]->xyz.as<double>(); J.onrm = outs[j]->nrm.as<double>(); J.out_n = outs[j]->dn.as<int32_t>();
+      J.T = (inits && w == 0) ? dT + 16 * (size_t)k : nullptr;
       J.which = w; J.pad = 0;
       sj[j].in = J.keep; sj[j].out = J.offs; sj[j].d_n = J.d_n;
     }
   }
-  B2S_CUDA(cudaMemcpyAsync(dev, host_stage, op_overlap_batch_stage_bytes(n), cudaMemcpyHostToDevice, h->stream));
+  B2S_CUDA(cudaMemcpyAsync(dev, host_stage, inits ? op_overlap_batch_stage_bytes(n) : tables, cudaMemcpyHostToDevice, h->stream));
   B2S_CUDA(cudaMemsetAsync(dev + state_begin, 0, state_end - state_begin, h->stream));
   const OvJob* dj = reinterpret_cast<const OvJob*>(dev);
   const ScanJob* ds = reinterpret_cast<const ScanJob*>(dev + al((size_t)nj * sizeof(OvJob)));

@@ -457,6 +457,57 @@ def buildOdometryConstraint(eng: Engine, source, target, params: OdometryConstra
 
 
 @dataclass
+class LoopClosureRefinementParameters:
+    """What the refinement half of PlaceRecognition::buildLoopClosureConstraints reads (src/PlaceRecognition.cpp:96-149): the map
+    voxel (getMapVoxelSize, :98), the magic constants (magic.hpp), placeRecognition.maxIcpCorrespondenceDistance_ /
+    minRefinementFitness_ (Parameters.hpp:130-131) and the [O3D] ICPConvergenceCriteria of the refinement."""
+    mapVoxelSize: float = 0.1
+    voxelSizeIfMapVoxelSizeIsZero: float = 0.04                  # magic::voxelSizeCorrespondenceSearchIfMapVoxelSizeIsZero
+    voxelExpansionFactorOverlapComputation: float = 20.0
+    minNumPointsPerVoxel: int = 1
+    maxNumIter: int = 100                                        # magic::icpRunUntilConvergenceNumberOfIterations
+    maxIcpCorrespondenceDistance: float = 0.3
+    relativeFitness: float = 1e-6
+    relativeRmse: float = 1e-6
+    minRefinementFitness: float = 0.7
+
+    def to_c(self) -> L.LoopClosureRefinementParams:
+        return L.LoopClosureRefinementParams(float(self.mapVoxelSize), float(self.voxelSizeIfMapVoxelSizeIsZero),
+                                             float(self.voxelExpansionFactorOverlapComputation), int(self.minNumPointsPerVoxel), int(self.maxNumIter),
+                                             float(self.maxIcpCorrespondenceDistance), float(self.relativeFitness), float(self.relativeRmse),
+                                             float(self.minRefinementFitness))
+
+
+@dataclass
+class LoopClosureRefinementResult:
+    """One candidate's refinement: the ICP's RegistrationResult, the information matrix at its T (computed for every candidate),
+    the fitness gate (:118) and the overlap sizes."""
+    result: RegistrationResult
+    information: np.ndarray
+    accepted: bool
+    nSourceOverlap: int
+    nTargetOverlap: int
+
+
+def refineLoopClosuresBatch(eng: Engine, sourceSubmap, targetSubmaps, inits, params: LoopClosureRefinementParameters | None = None,
+                            sourceOverlaps=None, targetOverlaps=None) -> list[LoopClosureRefinementResult]:
+    """src/PlaceRecognition.cpp:96-149 for one source Submap against every target Submap in one device call on the resident maps:
+    overlap at inits[k], point-to-plane ICP from inits[k], fitness gate, information matrix.  sourceOverlaps / targetOverlaps (lists
+    of Cloud, optional) receive the overlap selections in map order."""
+    p = (params or LoopClosureRefinementParameters()).to_c()
+    n = len(targetSubmaps)
+    T = np.ascontiguousarray(np.asarray(inits, dtype=np.float64).reshape(n, 16) if n else np.zeros((1, 16)))
+    arr = lambda objs: (C.c_void_p * max(n, 1))(*objs)
+    so = arr([c._c for c in sourceOverlaps]) if sourceOverlaps is not None else None
+    to = arr([c._c for c in targetOverlaps]) if targetOverlaps is not None else None
+    out = (L.LoopClosureRefinement * max(n, 1))()
+    L.check(L.lib().b2s_submap_loop_closure_refinement(eng._h, sourceSubmap._s, C.c_int32(n), arr([t._s for t in targetSubmaps]), _pd(T), C.byref(p),
+                                                       so, to, out))
+    return [LoopClosureRefinementResult(_res(o.icp), np.array(o.information, dtype=np.float64).reshape(6, 6), bool(o.accepted), int(o.n_source_overlap),
+                                        int(o.n_target_overlap)) for o in out[:n]]
+
+
+@dataclass
 class VisualizationParameters:
     """include/open3d_slam/Parameters.hpp:179-183: the voxel sizes SlamWrapperRos::publishMaps applies to the assembled map and to the
     coloured submap cloud, and how often it publishes them"""

@@ -424,6 +424,36 @@ RansacResultB200 registrationRansacBasedOnFeatureMatchingB200(const SubmapB200& 
   return out;
 }
 
+std::vector<LoopClosureRefinementB200> refineLoopClosuresB200(const SubmapB200& source, const std::vector<const SubmapB200*>& targets,
+                                                              const std::vector<Transform>& initialGuesses, const MapperParameters& cfg) {
+  if (initialGuesses.size() != targets.size()) throw std::runtime_error("one initial guess per target");
+  std::vector<LoopClosureRefinementB200> out(targets.size());
+  if (targets.empty()) return out;
+  std::vector<const b2s_submap*> tgt;
+  std::vector<double> inits(16 * targets.size());
+  for (size_t k = 0; k < targets.size(); ++k) {
+    tgt.push_back(targets[k]->handle());
+    toRowMajor(initialGuesses[k].matrix(), &inits[16 * k]);
+  }
+  b2s_loop_closure_refinement_params prm;
+  b2s_default_loop_closure_refinement_params(&prm);
+  prm.map_voxel_size = cfg.mapBuilder_.mapVoxelSize_;                     // getMapVoxelSize is applied by the call (:98)
+  prm.max_corr_dist = cfg.placeRecognition_.maxIcpCorrespondenceDistance_;   // :46, :149
+  prm.min_refinement_fitness = cfg.placeRecognition_.minRefinementFitness_;  // :118
+  std::vector<b2s_loop_closure_refinement> res(targets.size());
+  const int32_t rc = b2s_submap_loop_closure_refinement(source.engine(), source.handle(), (int32_t)targets.size(), tgt.data(), inits.data(), &prm,
+                                                        nullptr, nullptr, res.data());
+  if (rc != B2S_OK) b2sThrow(rc);
+  for (size_t k = 0; k < targets.size(); ++k) {
+    out[k].icpResult = toResult(res[k].icp);
+    for (int i = 0; i < 6; i++) for (int j = 0; j < 6; j++) out[k].informationMatrix(i, j) = res[k].information[6 * i + j];
+    out[k].isAccepted = res[k].accepted != 0;
+    out[k].numSourceOverlap = (size_t)res[k].n_source_overlap;
+    out[k].numTargetOverlap = (size_t)res[k].n_target_overlap;
+  }
+  return out;
+}
+
 void computeOdometryConstraintsB200(const std::vector<const SubmapB200*>& submaps, const std::vector<size_t>& parentIds, size_t activeSubmapIdx,
                                     const std::vector<size_t>* candidates, const MapperParameters& p, Constraints* constraints) {
   auto has = [&](size_t s, size_t t) {   // hasConstraint (:23-30), the pairs of this call included

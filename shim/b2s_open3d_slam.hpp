@@ -127,6 +127,21 @@ struct RansacResultB200 {
 RansacResultB200 registrationRansacBasedOnFeatureMatchingB200(const SubmapB200& source, const SubmapB200& target,
                                                               const PlaceRecognitionParameters& cfg, uint64_t seed = 1);
 
+// PlaceRecognition::buildLoopClosureConstraints, src/PlaceRecognition.cpp:96-149, for every candidate whose proposal passed the gates
+// at :86 and :92: overlap of the two whole maps at the proposal (20 x getMapVoxelSize(mapBuilder_, 0.04)), ICP of the overlaps from
+// the proposal with r = placeRecognition_.maxIcpCorrespondenceDistance_ and 100 iterations, the fitness gate of :118 and the
+// information matrix at the ICP's T (:148-149), all candidates in ONE b2s_submap_loop_closure_refinement call on the resident maps (all
+// SubmapB200s on one handle).  The ICP is point-to-plane; the reference uses the scan matcher's type (:47), point-to-plane in every
+// shipped configuration.  The consistency check of the ICP's T (:124) and the Constraint record (:140-150) stay with the caller.
+struct LoopClosureRefinementB200 {
+  RegistrationResult icpResult;                 // :110
+  Eigen::Matrix6d informationMatrix;            // :148-149, at icpResult.transformation_ (computed for every candidate)
+  bool isAccepted = false;                      // !(icpResult.fitness_ < minRefinementFitness_), :118
+  size_t numSourceOverlap = 0, numTargetOverlap = 0;
+};
+std::vector<LoopClosureRefinementB200> refineLoopClosuresB200(const SubmapB200& source, const std::vector<const SubmapB200*>& targets,
+                                                              const std::vector<Transform>& initialGuesses, const MapperParameters& cfg);
+
 // computeOdometryConstraints (src/constraint_builders.cpp:92-118) over device-resident submaps: submaps[i] is the SubmapB200 of submap
 // id i and parentIds[i] its getParentId().  candidates = the finished submap ids (the overload of SubmapCollection::computeFeatures,
 // :92-106), or nullptr for every submap (the overload of SlamWrapper::loopClosureWorker, :108-118, which leaves out the pairs that touch

@@ -27,9 +27,10 @@ enum class ScanToMapRegistrationType : int { PointToPlaneIcp, PointToPointIcp, G
 struct ScanToMapRegistrationParameters { double minRefinementFitness_ = 0.7; IcpParameters icp_; ScanToMapRegistrationType scanToMapRegType_ = ScanToMapRegistrationType::PointToPlaneIcp; };
 struct PlaceRecognitionParameters { double normalEstimationRadius_ = 1.0, featureVoxelSize_ = 0.5, featureRadius_ = 2.5; int featureKnn_ = 100, normalKnn_ = 10;
   int ransacNumIter_ = 1000000; double ransacProbability_ = 0.99; int ransacModelSize_ = 3; double ransacMaxCorrespondenceDistance_ = 0.75,
-  correspondenceCheckerDistance_ = 0.75, correspondenceCheckerEdgeLength_ = 0.5; int ransacMinCorrespondenceSetSize_ = 25; };   // Parameters.hpp:118-129
+  correspondenceCheckerDistance_ = 0.75, correspondenceCheckerEdgeLength_ = 0.5; int ransacMinCorrespondenceSetSize_ = 25;
+  double maxIcpCorrespondenceDistance_ = 0.3, minRefinementFitness_ = 0.7; };   // Parameters.hpp:118-131
 struct MapperParameters { ScanToMapRegistrationParameters scanMatcher_; ScanProcessingParameters scanProcessing_; MapBuilderParameters mapBuilder_; MapBuilderParameters denseMapBuilder_;
-  bool isRefineOdometryConstraintsBetweenSubmaps_ = false; };
+  PlaceRecognitionParameters placeRecognition_; bool isRefineOdometryConstraintsBetweenSubmaps_ = false; };
 struct Constraint { Transform sourceToTarget_ = Transform::Identity(); size_t sourceSubmapIdx_ = 0, targetSubmapIdx_ = 0;
   Eigen::Matrix6d informationMatrix_ = Eigen::Matrix6d::Identity(); bool isInformationMatrixValid_ = false, isOdometryConstraint_ = false; };
 using Constraints = std::vector<Constraint>;
