@@ -15,23 +15,7 @@
 
 namespace b2s {
 
-constexpr unsigned long long CV_EMPTY = ~0ull;
 constexpr int CV_THREADS = 256;
-
-__device__ __forceinline__ unsigned long long cv_pack(int x, int y, int z) {
-  return ((unsigned long long)(unsigned)(x + 1048576) << 42) | ((unsigned long long)(unsigned)(y + 1048576) << 21) |
-         (unsigned long long)(unsigned)(z + 1048576);
-}
-__device__ __forceinline__ unsigned long long cv_hash(unsigned long long k) {
-  k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
-  return k;
-}
-__device__ __forceinline__ bool cv_key_of(double x, double y, double z, double inv, unsigned long long* key) {
-  const double fx = floor(x * inv), fy = floor(y * inv), fz = floor(z * inv);
-  if (!(fabs(fx) < 1048575.0 && fabs(fy) < 1048575.0 && fabs(fz) < 1048575.0)) return false;   // also rejects NaN
-  *key = cv_pack((int)fx, (int)fy, (int)fz);
-  return true;
-}
 
 // enable (optional): device-side schedule of the mapper chain -- every kernel of the carving sequence returns at once unless
 // *enable != 0; n_eff (optional) receives the point count the compaction works on (0 when skipped)
@@ -42,7 +26,7 @@ __global__ void __launch_bounds__(CV_THREADS) carve_init_kernel(unsigned long lo
   const bool on = enable == nullptr || *enable != 0;
   if (n_eff && blockIdx.x == 0 && threadIdx.x == 0) *n_eff = on ? *d_nmap : 0;
   if (!on) return;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < cap; i += (size_t)gridDim.x * blockDim.x) { keys[i] = CV_EMPTY; head[i] = -1; }
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < cap; i += (size_t)gridDim.x * blockDim.x) { keys[i] = VOXEL_KEY_EMPTY; head[i] = -1; }
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_max; i += gridDim.x * blockDim.x) keep[i] = 1;
 }
 
@@ -59,12 +43,10 @@ __global__ void __launch_bounds__(CV_THREADS) carve_insert_kernel(const double* 
     if (!(x == x)) { keep[i] = 0; continue; }      // tombstone of the fusion (fuse.cu): dropped by the compaction below
     if (!crop_within(crop, x, y, z)) continue;     // getIndicesWithinVolume(*map): only these are candidates
     unsigned long long key;
-    if (!cv_key_of(x, y, z, inv, &key)) { atomicOr(status, ST_KEY_OVERFLOW); continue; }
-    size_t s = (size_t)cv_hash(key) & mask;
-    for (size_t probe = 0; probe <= mask; ++probe, s = (s + 1) & mask) {
-      const unsigned long long old = atomicCAS(&keys[s], CV_EMPTY, key);
-      if (old == CV_EMPTY || old == key) { next[i] = atomicExch(&head[s], i); break; }
-    }
+    if (!voxel_key_of(x, y, z, inv, inv, inv, &key)) { atomicOr(status, ST_KEY_OVERFLOW); continue; }
+    bool fresh;
+    const long long s = voxel_key_claim(keys, mask, key, &fresh);
+    if (s >= 0) next[i] = atomicExch(&head[s], i);
   }
 }
 
@@ -83,12 +65,8 @@ __global__ void __launch_bounds__(CV_THREADS) carve_march_kernel(const double* _
   for (int i = 0; i < 16; i++) T[i] = Tdev[i];
   const double sx = T[3], sy = T[7], sz = T[11];   // mapToRangeSensor.translation()
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double px = scan[3 * i], py = scan[3 * i + 1], pz = scan[3 * i + 2];
-    const double x = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], px), __dmul_rn(T[1], py)), __dmul_rn(T[2], pz)), T[3]);
-    const double y = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], px), __dmul_rn(T[5], py)), __dmul_rn(T[6], pz)), T[7]);
-    const double z = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], px), __dmul_rn(T[9], py)), __dmul_rn(T[10], pz)), T[11]);
-    const double w = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[12], px), __dmul_rn(T[13], py)), __dmul_rn(T[14], pz)), T[15]);
-    const double qx = __ddiv_rn(x, w), qy = __ddiv_rn(y, w), qz = __ddiv_rn(z, w);
+    double qx, qy, qz;
+    transform_point(T, scan[3 * i], scan[3 * i + 1], scan[3 * i + 2], &qx, &qy, &qz);
     const double dx = qx - sx, dy = qy - sy, dz = qz - sz;
     const double length = sqrt(dx * dx + dy * dy + dz * dz);
     const double ux = dx / length, uy = dy / length, uz = dz / length;
@@ -100,24 +78,16 @@ __global__ void __launch_bounds__(CV_THREADS) carve_march_kernel(const double* _
     while (distance < mp) {
       const double cx = distance * ux + sx, cy = distance * uy + sy, cz = distance * uz + sz;
       unsigned long long key;
-      if (cv_key_of(cx, cy, cz, inv, &key)) {
-        size_t s = (size_t)cv_hash(key) & mask;
-        for (size_t probe = 0; probe <= mask; ++probe, s = (s + 1) & mask) {
-          const unsigned long long k = keys[s];
-          if (k == CV_EMPTY) break;
-          if (k != key) continue;
-          for (int id = head[s]; id >= 0; id = next[id]) {
-            bool rm = true;
-            if (map_nrm) {
-              double nx = map_nrm[3 * (size_t)id], ny = map_nrm[3 * (size_t)id + 1], nz = map_nrm[3 * (size_t)id + 2];
-              const double nn = sqrt(nx * nx + ny * ny + nz * nz);
-              if (nn > 0.0) { nx /= nn; ny /= nn; nz /= nn; }   // Eigen normalized()
-              rm = fabs(ux * nx + uy * ny + uz * nz) > min_dot;
-            }
-            if (rm) keep[id] = 0;
-          }
-          break;
+      const long long s = voxel_key_of(cx, cy, cz, inv, inv, inv, &key) ? voxel_key_find(keys, mask, key) : -1;
+      for (int id = s >= 0 ? head[s] : -1; id >= 0; id = next[id]) {
+        bool rm = true;
+        if (map_nrm) {
+          double nx = map_nrm[3 * (size_t)id], ny = map_nrm[3 * (size_t)id + 1], nz = map_nrm[3 * (size_t)id + 2];
+          const double nn = sqrt(nx * nx + ny * ny + nz * nz);
+          if (nn > 0.0) { nx /= nn; ny /= nn; nz /= nn; }   // Eigen normalized()
+          rm = fabs(ux * nx + uy * ny + uz * nz) > min_dot;
         }
+        if (rm) keep[id] = 0;
       }
       distance += voxel;
     }

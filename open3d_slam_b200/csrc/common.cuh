@@ -802,5 +802,83 @@ __device__ __forceinline__ void undistort_point(double px, double py, double pz,
   out[2] = ((txz - twy) * px + (tyz + twx) * py + (1 - (txx + tyy)) * pz) + tz_;
 }
 
+// The map-side voxel hashes (fusion and dense map in fuse.cu, carve.cu, overlap.cu, voxelmap.cu) share one key and one probe: the
+// voxel index getVoxelIdx(p, inverseVoxelSize) = floor(p * inv) on the global-origin grid (VoxelHashMap.hpp:47-50), accepted while
+// |index| < 2^20 - 1 on every axis, packed as three 21-bit fields offset by 2^20, hashed by the murmur3 finalizer and probed linearly
+// over a power-of-two table (mask = slots - 1).  Each table keeps its own fill limit and occupancy count.  tests/voxel_hash.py restates
+// these rules.
+constexpr unsigned long long VOXEL_KEY_EMPTY = ~0ull;
+
+__device__ __forceinline__ unsigned long long voxel_key_pack(int x, int y, int z) {
+  return ((unsigned long long)(unsigned)(x + 1048576) << 42) | ((unsigned long long)(unsigned)(y + 1048576) << 21) |
+         (unsigned long long)(unsigned)(z + 1048576);
+}
+__device__ __forceinline__ void voxel_key_unpack(unsigned long long k, int* x, int* y, int* z) {
+  *x = (int)((k >> 42) & 0x1FFFFF) - 1048576; *y = (int)((k >> 21) & 0x1FFFFF) - 1048576; *z = (int)(k & 0x1FFFFF) - 1048576;
+}
+__device__ __forceinline__ unsigned long long voxel_key_hash(unsigned long long k) {
+  k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
+  return k;
+}
+// one inverse voxel size per axis (VoxelMap takes a Vector3d; every other table passes the same inverse three times)
+__device__ __forceinline__ bool voxel_key_of(double x, double y, double z, double ix, double iy, double iz, unsigned long long* key) {
+  const double fx = floor(__dmul_rn(x, ix)), fy = floor(__dmul_rn(y, iy)), fz = floor(__dmul_rn(z, iz));
+  if (!(fabs(fx) < 1048575.0 && fabs(fy) < 1048575.0 && fabs(fz) < 1048575.0)) return false;   // also rejects NaN
+  *key = voxel_key_pack((int)fx, (int)fy, (int)fz);
+  return true;
+}
+// slot of `key`, or -1 when it is absent
+__device__ __forceinline__ long long voxel_key_find(const unsigned long long* __restrict__ keys, size_t mask, unsigned long long key) {
+  size_t s = (size_t)voxel_key_hash(key) & mask;
+  for (size_t probe = 0; probe <= mask; ++probe, s = (s + 1) & mask) {
+    const unsigned long long k = keys[s];
+    if (k == VOXEL_KEY_EMPTY) return -1;
+    if (k == key) return (long long)s;
+  }
+  return -1;
+}
+// slot of `key`, inserting it when absent (-1: every slot of the probe run holds another key); *fresh: this thread claimed the slot
+__device__ __forceinline__ long long voxel_key_claim(unsigned long long* keys, size_t mask, unsigned long long key, bool* fresh) {
+  size_t s = (size_t)voxel_key_hash(key) & mask;
+  // written so that no caller needs more registers than it did with its own copy of the loop (ptxas reports)
+  for (size_t probe = 0;; s = (s + 1) & mask) {
+    const unsigned long long old = atomicCAS(&keys[s], VOXEL_KEY_EMPTY, key);
+    if (old == key) { *fresh = false; return (long long)s; }
+    if (old == VOXEL_KEY_EMPTY) { *fresh = true; return (long long)s; }
+    if (++probe > mask) { *fresh = false; return -1; }
+  }
+}
+
+// A row-major 4x4 T applied to one point or vector as the reference's Eigen code does it, every row summed left to right (the library
+// is built with -fmad=false, and the explicit round-to-nearest ops keep the order fixed): transform_point = o3d_slam::transform /
+// [O3D] TransformPoints, (T p).head3 / w; affine_point = R p + t; rotate_vector = R n ([O3D] TransformNormals).
+__device__ __forceinline__ void transform_point(const double* T, double x, double y, double z, double* ox, double* oy, double* oz) {
+  const double a = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], x), __dmul_rn(T[1], y)), __dmul_rn(T[2], z)), T[3]);
+  const double b = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], x), __dmul_rn(T[5], y)), __dmul_rn(T[6], z)), T[7]);
+  const double c = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], x), __dmul_rn(T[9], y)), __dmul_rn(T[10], z)), T[11]);
+  const double w = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[12], x), __dmul_rn(T[13], y)), __dmul_rn(T[14], z)), T[15]);
+  *ox = __ddiv_rn(a, w); *oy = __ddiv_rn(b, w); *oz = __ddiv_rn(c, w);
+}
+__device__ __forceinline__ void affine_point(const double* T, double x, double y, double z, double* ox, double* oy, double* oz) {
+  const double a = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], x), __dmul_rn(T[1], y)), __dmul_rn(T[2], z)), T[3]);
+  const double b = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], x), __dmul_rn(T[5], y)), __dmul_rn(T[6], z)), T[7]);
+  const double c = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], x), __dmul_rn(T[9], y)), __dmul_rn(T[10], z)), T[11]);
+  *ox = a; *oy = b; *oz = c;
+}
+__device__ __forceinline__ void rotate_vector(const double* T, double x, double y, double z, double* ox, double* oy, double* oz) {
+  const double a = __dadd_rn(__dadd_rn(__dmul_rn(T[0], x), __dmul_rn(T[1], y)), __dmul_rn(T[2], z));
+  const double b = __dadd_rn(__dadd_rn(__dmul_rn(T[4], x), __dmul_rn(T[5], y)), __dmul_rn(T[6], z));
+  const double c = __dadd_rn(__dadd_rn(__dmul_rn(T[8], x), __dmul_rn(T[9], y)), __dmul_rn(T[10], z));
+  *ox = a; *oy = b; *oz = c;
+}
+// o3d_slam::transform's near-identity test (helpers.cpp:275): max |T - I| < 1e-4 -> the untransformed cloud is copied first and every
+// transformed point appended as well
+__device__ __forceinline__ bool near_identity(const double* T) {
+  double mx = 0.0;
+#pragma unroll
+  for (int i = 0; i < 16; i++) mx = fmax(mx, fabs(T[i] - ((i % 5 == 0) ? 1.0 : 0.0)));
+  return mx < 1e-4;
+}
+
 }  // namespace b2s
 #endif

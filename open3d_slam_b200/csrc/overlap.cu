@@ -13,22 +13,12 @@
 
 namespace b2s {
 
-constexpr unsigned long long OV_EMPTY = ~0ull;
 constexpr int OV_THREADS = 256;
-
-__device__ __forceinline__ unsigned long long ov_pack(int x, int y, int z) {
-  return ((unsigned long long)(unsigned)(x + 1048576) << 42) | ((unsigned long long)(unsigned)(y + 1048576) << 21) |
-         (unsigned long long)(unsigned)(z + 1048576);
-}
-__device__ __forceinline__ unsigned long long ov_hash(unsigned long long k) {
-  k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
-  return k;
-}
 
 __global__ void __launch_bounds__(OV_THREADS) ov_init_kernel(unsigned long long* __restrict__ keys, int32_t* __restrict__ cnt, size_t cap) {
   pdl_wait();
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < cap; i += (size_t)gridDim.x * blockDim.x) {
-    keys[i] = OV_EMPTY; cnt[2 * i] = 0; cnt[2 * i + 1] = 0;
+    keys[i] = VOXEL_KEY_EMPTY; cnt[2 * i] = 0; cnt[2 * i + 1] = 0;
   }
 }
 
@@ -43,22 +33,13 @@ __global__ void __launch_bounds__(OV_THREADS) ov_insert_kernel(const double* __r
   for (int i = 0; i < 16; i++) T[i] = Tdev ? Tdev[i] : ((i % 5 == 0) ? 1.0 : 0.0);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     double x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
-    if (which == 0) {
-      const double a = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], x), __dmul_rn(T[1], y)), __dmul_rn(T[2], z)), T[3]);
-      const double b = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], x), __dmul_rn(T[5], y)), __dmul_rn(T[6], z)), T[7]);
-      const double c = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], x), __dmul_rn(T[9], y)), __dmul_rn(T[10], z)), T[11]);
-      const double w = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[12], x), __dmul_rn(T[13], y)), __dmul_rn(T[14], z)), T[15]);
-      x = __ddiv_rn(a, w); y = __ddiv_rn(b, w); z = __ddiv_rn(c, w);
-    }
-    const double fx = floor(x * inv), fy = floor(y * inv), fz = floor(z * inv);
+    if (which == 0) transform_point(T, x, y, z, &x, &y, &z);
     slot_of[i] = -1;
-    if (!(fabs(fx) < 1048575.0 && fabs(fy) < 1048575.0 && fabs(fz) < 1048575.0)) { atomicOr(status, ST_KEY_OVERFLOW); continue; }
-    const unsigned long long key = ov_pack((int)fx, (int)fy, (int)fz);
-    size_t s = (size_t)ov_hash(key) & mask;
-    for (size_t probe = 0; probe <= mask; ++probe, s = (s + 1) & mask) {
-      const unsigned long long old = atomicCAS(&keys[s], OV_EMPTY, key);
-      if (old == OV_EMPTY || old == key) { atomicAdd(&cnt[2 * s + which], 1); slot_of[i] = (int32_t)s; break; }
-    }
+    unsigned long long key;
+    if (!voxel_key_of(x, y, z, inv, inv, inv, &key)) { atomicOr(status, ST_KEY_OVERFLOW); continue; }
+    bool fresh;
+    const long long s = voxel_key_claim(keys, mask, key, &fresh);
+    if (s >= 0) { atomicAdd(&cnt[2 * s + which], 1); slot_of[i] = (int32_t)s; }
   }
 }
 
@@ -125,7 +106,7 @@ __global__ void __launch_bounds__(OV_THREADS) ovb_init_kernel(const OvJob* __res
   pdl_wait();
   const OvJob j = jobs[2 * blockIdx.y];
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i <= j.mask; i += (size_t)gridDim.x * blockDim.x) {
-    j.keys[i] = OV_EMPTY; j.cnt[2 * i] = 0; j.cnt[2 * i + 1] = 0;
+    j.keys[i] = VOXEL_KEY_EMPTY; j.cnt[2 * i] = 0; j.cnt[2 * i + 1] = 0;
   }
 }
 
@@ -137,22 +118,12 @@ __global__ void __launch_bounds__(OV_THREADS) ovb_insert_kernel(const OvJob* __r
     double x = j.xyz[3 * (size_t)i], y = j.xyz[3 * (size_t)i + 1], z = j.xyz[3 * (size_t)i + 2];
     j.slot_of[i] = -1;
     if (!(x == x)) continue;   // tombstone
-    if (j.T) {                 // the arithmetic of ov_insert_kernel: row sums left to right, then the homogeneous divide
-      const double* T = j.T;
-      const double a = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], x), __dmul_rn(T[1], y)), __dmul_rn(T[2], z)), T[3]);
-      const double b = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], x), __dmul_rn(T[5], y)), __dmul_rn(T[6], z)), T[7]);
-      const double c = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], x), __dmul_rn(T[9], y)), __dmul_rn(T[10], z)), T[11]);
-      const double w = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[12], x), __dmul_rn(T[13], y)), __dmul_rn(T[14], z)), T[15]);
-      x = __ddiv_rn(a, w); y = __ddiv_rn(b, w); z = __ddiv_rn(c, w);
-    }
-    const double fx = floor(x * inv), fy = floor(y * inv), fz = floor(z * inv);
-    if (!(fabs(fx) < 1048575.0 && fabs(fy) < 1048575.0 && fabs(fz) < 1048575.0)) { atomicOr(status, ST_KEY_OVERFLOW); continue; }
-    const unsigned long long key = ov_pack((int)fx, (int)fy, (int)fz);
-    size_t s = (size_t)ov_hash(key) & j.mask;
-    for (size_t probe = 0; probe <= j.mask; ++probe, s = (s + 1) & j.mask) {
-      const unsigned long long old = atomicCAS(&j.keys[s], OV_EMPTY, key);
-      if (old == OV_EMPTY || old == key) { atomicAdd(&j.cnt[2 * s + j.which], 1); j.slot_of[i] = (int32_t)s; break; }
-    }
+    if (j.T) transform_point(j.T, x, y, z, &x, &y, &z);
+    unsigned long long key;
+    if (!voxel_key_of(x, y, z, inv, inv, inv, &key)) { atomicOr(status, ST_KEY_OVERFLOW); continue; }
+    bool fresh;
+    const long long s = voxel_key_claim(j.keys, j.mask, key, &fresh);
+    if (s >= 0) { atomicAdd(&j.cnt[2 * s + j.which], 1); j.slot_of[i] = (int32_t)s; }
   }
 }
 

@@ -482,27 +482,18 @@ __global__ void __launch_bounds__(VX_THREADS) transform_kernel(const double* __r
   double T[16];
 #pragma unroll
   for (int i = 0; i < 16; i++) T[i] = Tdev[i];
-  double mx = 0.0;
-#pragma unroll
-  for (int i = 0; i < 16; i++) mx = fmax(mx, fabs(T[i] - ((i % 5 == 0) ? 1.0 : 0.0)));
-  const bool ident = mx < 1e-4;
+  const bool ident = near_identity(T);
   const int base = ident ? n : 0;
   if (blockIdx.x == 0 && threadIdx.x == 0) *out_n = base + n;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const double px = xyz[3 * i], py = xyz[3 * i + 1], pz = xyz[3 * i + 2];
     if (ident) { oxyz[3 * i] = px; oxyz[3 * i + 1] = py; oxyz[3 * i + 2] = pz; }
-    const double x = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], px), __dmul_rn(T[1], py)), __dmul_rn(T[2], pz)), T[3]);
-    const double y = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], px), __dmul_rn(T[5], py)), __dmul_rn(T[6], pz)), T[7]);
-    const double z = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], px), __dmul_rn(T[9], py)), __dmul_rn(T[10], pz)), T[11]);
-    const double w = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[12], px), __dmul_rn(T[13], py)), __dmul_rn(T[14], pz)), T[15]);
     const int o = base + i;
-    oxyz[3 * o] = __ddiv_rn(x, w); oxyz[3 * o + 1] = __ddiv_rn(y, w); oxyz[3 * o + 2] = __ddiv_rn(z, w);
+    transform_point(T, px, py, pz, &oxyz[3 * o], &oxyz[3 * o + 1], &oxyz[3 * o + 2]);
     if (nrm) {
       const double a = nrm[3 * i], b = nrm[3 * i + 1], c = nrm[3 * i + 2];
       if (ident) { onrm[3 * i] = a; onrm[3 * i + 1] = b; onrm[3 * i + 2] = c; }
-      onrm[3 * o] = __dadd_rn(__dadd_rn(__dmul_rn(T[0], a), __dmul_rn(T[1], b)), __dmul_rn(T[2], c));
-      onrm[3 * o + 1] = __dadd_rn(__dadd_rn(__dmul_rn(T[4], a), __dmul_rn(T[5], b)), __dmul_rn(T[6], c));
-      onrm[3 * o + 2] = __dadd_rn(__dadd_rn(__dmul_rn(T[8], a), __dmul_rn(T[9], b)), __dmul_rn(T[10], c));
+      rotate_vector(T, a, b, c, &onrm[3 * o], &onrm[3 * o + 1], &onrm[3 * o + 2]);
     }
   }
 }
@@ -580,18 +571,8 @@ __global__ void __launch_bounds__(VX_THREADS) o3d_transform_inplace_kernel(doubl
   const int n = *d_n;
   const double* T = M.m;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double px = xyz[3 * i], py = xyz[3 * i + 1], pz = xyz[3 * i + 2];
-    const double x = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], px), __dmul_rn(T[1], py)), __dmul_rn(T[2], pz)), T[3]);
-    const double y = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], px), __dmul_rn(T[5], py)), __dmul_rn(T[6], pz)), T[7]);
-    const double z = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], px), __dmul_rn(T[9], py)), __dmul_rn(T[10], pz)), T[11]);
-    const double w = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[12], px), __dmul_rn(T[13], py)), __dmul_rn(T[14], pz)), T[15]);
-    xyz[3 * i] = __ddiv_rn(x, w); xyz[3 * i + 1] = __ddiv_rn(y, w); xyz[3 * i + 2] = __ddiv_rn(z, w);
-    if (nrm) {
-      const double a = nrm[3 * i], b = nrm[3 * i + 1], c = nrm[3 * i + 2];
-      nrm[3 * i] = __dadd_rn(__dadd_rn(__dmul_rn(T[0], a), __dmul_rn(T[1], b)), __dmul_rn(T[2], c));
-      nrm[3 * i + 1] = __dadd_rn(__dadd_rn(__dmul_rn(T[4], a), __dmul_rn(T[5], b)), __dmul_rn(T[6], c));
-      nrm[3 * i + 2] = __dadd_rn(__dadd_rn(__dmul_rn(T[8], a), __dmul_rn(T[9], b)), __dmul_rn(T[10], c));
-    }
+    transform_point(T, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], &xyz[3 * i], &xyz[3 * i + 1], &xyz[3 * i + 2]);
+    if (nrm) rotate_vector(T, nrm[3 * i], nrm[3 * i + 1], nrm[3 * i + 2], &nrm[3 * i], &nrm[3 * i + 1], &nrm[3 * i + 2]);
   }
 }
 __global__ void pose_right_multiply_kernel(double* pose, Mat4 M) {
@@ -613,10 +594,7 @@ __global__ void dense_transform_kernel(double* __restrict__ sums, const int32_t*
   const double* T = M.m;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (size_t)gridDim.x * blockDim.x) {
     if (cnts[i] <= 0) continue;
-    const double a = sums[6 * i], b = sums[6 * i + 1], c = sums[6 * i + 2];
-    sums[6 * i] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], a), __dmul_rn(T[1], b)), __dmul_rn(T[2], c)), T[3]);
-    sums[6 * i + 1] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], a), __dmul_rn(T[5], b)), __dmul_rn(T[6], c)), T[7]);
-    sums[6 * i + 2] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], a), __dmul_rn(T[9], b)), __dmul_rn(T[10], c)), T[11]);
+    affine_point(T, sums[6 * i], sums[6 * i + 1], sums[6 * i + 2], &sums[6 * i], &sums[6 * i + 1], &sums[6 * i + 2]);
   }
 }
 

@@ -31,7 +31,6 @@ struct b2s_voxel_map {
 
 namespace b2s {
 
-constexpr unsigned long long VM_EMPTY = ~0ull;
 constexpr int VM_THREADS = 256;
 constexpr int VM_LAYERS = 4;
 
@@ -41,35 +40,10 @@ struct VmView {
   const unsigned long long* keys;
 };
 
-__device__ __forceinline__ unsigned long long vm_pack(int x, int y, int z) {
-  return ((unsigned long long)(unsigned)(x + 1048576) << 42) | ((unsigned long long)(unsigned)(y + 1048576) << 21) |
-         (unsigned long long)(unsigned)(z + 1048576);
-}
-__device__ __forceinline__ unsigned long long vm_hash(unsigned long long k) {
-  k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
-  return k;
-}
-// getVoxelIdx(p, inverseVoxelSize): int(floor(p[i] * inv[i]))   VoxelHashMap.hpp:47-50
-__device__ __forceinline__ bool vm_key(double x, double y, double z, double ix, double iy, double iz, unsigned long long* key) {
-  const double fx = floor(__dmul_rn(x, ix)), fy = floor(__dmul_rn(y, iy)), fz = floor(__dmul_rn(z, iz));
-  if (!(fabs(fx) < 1048575.0 && fabs(fy) < 1048575.0 && fabs(fz) < 1048575.0)) return false;   // also rejects NaN
-  *key = vm_pack((int)fx, (int)fy, (int)fz);
-  return true;
-}
-__device__ __forceinline__ long long vm_find(const unsigned long long* __restrict__ keys, size_t mask, unsigned long long key) {
-  size_t s = (size_t)vm_hash(key) & mask;
-  for (size_t probe = 0; probe <= mask; ++probe, s = (s + 1) & mask) {
-    const unsigned long long k = keys[s];
-    if (k == VM_EMPTY) return -1;
-    if (k == key) return (long long)s;
-  }
-  return -1;
-}
-
 __global__ void __launch_bounds__(VM_THREADS) vm_clear_kernel(unsigned long long* keys, int32_t* head, int32_t* cnt, size_t cap, int32_t* used) {
   pdl_wait();
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (size_t)gridDim.x * blockDim.x) {
-    keys[i] = VM_EMPTY;
+    keys[i] = VOXEL_KEY_EMPTY;
     for (int l = 0; l < VM_LAYERS; l++) { head[(size_t)l * cap + i] = -1; cnt[(size_t)l * cap + i] = 0; }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) { used[0] = 0; used[1] = 0; }
@@ -85,20 +59,16 @@ __global__ void __launch_bounds__(VM_THREADS) vm_insert_kernel(const double* __r
   const size_t mask = cap - 1;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     unsigned long long key;
-    if (!vm_key(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], ix, iy, iz, &key)) { atomicOr(status, ST_KEY_OVERFLOW); continue; }
-    size_t s = (size_t)vm_hash(key) & mask;
-    for (size_t probe = 0; probe <= mask; ++probe, s = (s + 1) & mask) {
-      const unsigned long long old = atomicCAS(&keys[s], VM_EMPTY, key);
-      if (old == VM_EMPTY) { if ((size_t)atomicAdd(&used[0], 1) + 1 > cap - cap / 8) atomicOr(status, ST_HASH_FULL); }
-      if (old == VM_EMPTY || old == key) {
-        const int e = atomicAdd(&used[1], 1);
-        if ((size_t)e >= entries_cap) { atomicOr(status, ST_CAPACITY); break; }
-        eidx[e] = i;
-        next[e] = atomicExch(&head[(size_t)layer * cap + s], e);
-        atomicAdd(&cnt[(size_t)layer * cap + s], 1);
-        break;
-      }
-    }
+    if (!voxel_key_of(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], ix, iy, iz, &key)) { atomicOr(status, ST_KEY_OVERFLOW); continue; }
+    bool fresh;
+    const long long s = voxel_key_claim(keys, mask, key, &fresh);
+    if (fresh) { if ((size_t)atomicAdd(&used[0], 1) + 1 > cap - cap / 8) atomicOr(status, ST_HASH_FULL); }
+    if (s < 0) continue;
+    const int e = atomicAdd(&used[1], 1);
+    if ((size_t)e >= entries_cap) { atomicOr(status, ST_CAPACITY); continue; }
+    eidx[e] = i;
+    next[e] = atomicExch(&head[(size_t)layer * cap + s], e);
+    atomicAdd(&cnt[(size_t)layer * cap + s], 1);
   }
 }
 
@@ -116,14 +86,9 @@ __global__ void __launch_bounds__(VM_THREADS) vm_has_kernel(const double* __rest
   int local = 0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     double x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
-    if (Tdev) {
-      const double a = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[0], x), __dmul_rn(T[1], y)), __dmul_rn(T[2], z)), T[3]);
-      const double b = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4], x), __dmul_rn(T[5], y)), __dmul_rn(T[6], z)), T[7]);
-      const double c = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[8], x), __dmul_rn(T[9], y)), __dmul_rn(T[10], z)), T[11]);
-      x = a; y = b; z = c;
-    }
+    if (Tdev) affine_point(T, x, y, z, &x, &y, &z);
     unsigned long long key;
-    const bool has = vm_key(x, y, z, v.ix, v.iy, v.iz, &key) && vm_find(v.keys, v.mask, key) >= 0;
+    const bool has = voxel_key_of(x, y, z, v.ix, v.iy, v.iz, &key) && voxel_key_find(v.keys, v.mask, key) >= 0;
     if (flags) flags[i] = has ? 1 : 0;
     local += has ? 1 : 0;
   }
@@ -139,8 +104,8 @@ __global__ void __launch_bounds__(VM_THREADS) vm_count_kernel(const double* __re
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     unsigned long long key;
     int c = 0;
-    if (vm_key(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], v.ix, v.iy, v.iz, &key)) {
-      const long long s = vm_find(v.keys, v.mask, key);
+    if (voxel_key_of(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], v.ix, v.iy, v.iz, &key)) {
+      const long long s = voxel_key_find(v.keys, v.mask, key);
       if (s >= 0) c = cnt[(size_t)layer * cap + (size_t)s];
     }
     out[i] = c;
@@ -155,8 +120,8 @@ __global__ void __launch_bounds__(VM_THREADS) vm_fill_kernel(const double* __res
   const int n = *d_n;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     unsigned long long key;
-    if (!vm_key(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], v.ix, v.iy, v.iz, &key)) continue;
-    const long long s = vm_find(v.keys, v.mask, key);
+    if (!voxel_key_of(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], v.ix, v.iy, v.iz, &key)) continue;
+    const long long s = voxel_key_find(v.keys, v.mask, key);
     if (s < 0) continue;
     int32_t* dst = out + offs[i];
     int m = 0;

@@ -11,8 +11,9 @@ offset by 2^20 in one 64-bit word, hashed by the murmur3 finalizer, linear probi
     voxel map       (voxelmap.cu)             1024 slots, doubled while < 2 x capacity_voxels; full past 7/8 of them
 
 A key index is accepted while |floor(p * (1/v))| < KEY_LIMIT on every axis.  The finalizer is a bijection, so fmix64_inv gives the
-keys whose home slot is any chosen slot.  test_voxel_hash_rules.py checks these constants against the CUDA sources, so a change
-there fails loudly instead of turning the collision tests into ordinary ones.
+keys whose home slot is any chosen slot.  The key, the hash and the probes are defined once, in open3d_slam_b200/csrc/common.cuh
+(voxel_key_*); the sizes and fill limits live with each table.  test_voxel_hash_rules.py checks these constants against the CUDA
+sources, so a change there fails loudly instead of turning the collision tests into ordinary ones.
 """
 from __future__ import annotations
 
