@@ -641,20 +641,30 @@ int32_t b2s_submap_odometry_constraints(b2s_handle* h, int32_t n_pairs, const b2
  *   - overlap at T0 with edge overlap_factor x voxel and minNumPointsPerVoxel = min_points_per_voxel: the source points are
  *     keyed after T0 ([O3D] PointCloud::Transform), the selected points are the UNTRANSFORMED ones, each map's survivors in map
  *     order (b2s_overlap's rule, SelectByIndex on the original clouds)                                                   :99-106
- *   - RegistrationICP(sourceOverlap, targetOverlap, r = max_corr_dist, T0, TransformationEstimationPointToPlane,
- *     max_iter / rel_fitness / rel_rmse) for every pair                                                                  :45-47, :110
+ *   - cloudRegistration->registerClouds(sourceOverlap, targetOverlap, T0) for every pair: the estimator p.reg_type (B2S_REG_*), with
+ *     r = max_corr_dist and max_iter / rel_fitness / rel_rmse -- RegistrationICP with TransformationEstimationPointToPlane or
+ *     ...PointToPoint, or RegistrationGeneralizedICP (epsilon 1e-3; the source's covariances are rotated by T0 before the first
+ *     iteration, as [O3D] transforms the source by init)                                                              :45-47, :110
  *   - accepted = !(icp.fitness < min_refinement_fitness)                                                                  :118
- *   - information = GetInformationMatrixFromPointClouds(sourceOverlap, targetOverlap, max_corr_dist, icp.T), for EVERY pair
- *     (the reference computes it for the accepted ones; the others' matrix is there for the caller to ignore)           :148-149
+ *   - information = GetInformationMatrixFromPointClouds(sourceOverlap, targetOverlap, max_corr_dist, icp.T), for EVERY pair and
+ *     every estimator (the reference computes it for the accepted ones; the others' matrix is there for the caller to ignore)
+ *                                                                                                                       :148-149
  *   The consistency check of icp.T (:124) stays with the caller, as does candidate selection and RANSAC.
- * Deviations: the ICP is ALWAYS point-to-plane, whatever b2s_config.icp.reg_type is; the reference registers with the scan matcher's
- * type (cloudRegistrationFactory, :47), point-to-plane in every shipped configuration.  The getMapVoxelSize rule is applied here,
- * as the reference does; a caller that composes b2s_submap_to_cloud + b2s_overlap itself and passes map_voxel_size = 0 gets an
- * error from b2s_overlap (voxel 0), while this call uses voxel_if_zero -- the one input where the two answer differently.
+ * The estimator: the reference refines with the scan matcher's type (PlaceRecognition::updateRegistrationAlgorithm, :44-48:
+ * cloudRegistrationFactory(toCloudRegistrationType(scanMatcher_)) with 100 iterations and maxIcpCorrespondenceDistance), which is
+ * GeneralizedIcp in every shipped Lua preset.  Here the caller chooses it: pass the scan matcher's b2s_config.icp.reg_type for the
+ * reference's behaviour.  A zeroed reg_type, and b2s_default_loop_closure_refinement_params, mean point-to-plane.  What each needs:
+ *     B2S_REG_POINT_TO_PLANE   every target map carries normals
+ *     B2S_REG_POINT_TO_POINT   no normals on either side (a point-to-point map refines here)
+ *     B2S_REG_GENERALIZED      the source map and every target map carry normals; [O3D] would estimate covariances for a cloud
+ *                              with neither, the device answers B2S_E_NO_NORMALS (as b2s_register does)
+ * Deviation: the getMapVoxelSize rule is applied here, as the reference does; a caller that composes b2s_submap_to_cloud +
+ * b2s_overlap itself and passes map_voxel_size = 0 gets an error from b2s_overlap (voxel 0), while this call uses voxel_if_zero --
+ * the one input where the two answer differently.
  * Errors: a submap or an overlap cloud of another handle, a null init array for n_targets > 0, a voxel <= 0 after the getMapVoxelSize
- * rule, overlap_factor <= 0, max_corr_dist <= 0, min_points_per_voxel < 1, max_iter < 0, n_targets < 0 -> B2S_E_INVALID; a target
- * map without normals (a point-to-point map, stored as NaN) -> B2S_E_NO_NORMALS.  n_targets = 0 -> B2S_OK.  The same target may
- * be listed more than once.  One call runs every pair in one set of launches and synchronises once; out[k] does not depend on the
+ * rule, overlap_factor <= 0, max_corr_dist <= 0, min_points_per_voxel < 1, max_iter < 0, n_targets < 0 -> B2S_E_INVALID; a reg_type
+ * that is none of B2S_REG_* -> B2S_E_UNSUPPORTED (as b2s_set_config); a map without the normals the estimator needs (a point-to-point
+ * map, stored as NaN) -> B2S_E_NO_NORMALS.  n_targets = 0 -> B2S_OK.  The same target may be listed more than once.  One call runs every pair in one set of launches and synchronises once; out[k] does not depend on the
  * other targets.  source_overlaps_or_null / target_overlaps_or_null (each an array of n_targets clouds, or NULL) receive the
  * selected points, in map order.  Scratch: the handle's odometry-constraint slots.  Semantics and kernels: DESIGN.md row L3. */
 typedef struct b2s_loop_closure_refinement_params {
@@ -665,6 +675,8 @@ typedef struct b2s_loop_closure_refinement_params {
   double max_corr_dist;                  /* placeRecognition.maxIcpCorrespondenceDistance = 0.3: ICP and information radius, :46, :149 */
   double rel_fitness, rel_rmse;          /* [O3D] ICPConvergenceCriteria defaults, 1e-6 */
   double min_refinement_fitness;         /* placeRecognition.minRefinementFitness = 0.7, :118 */
+  int32_t reg_type;                      /* B2S_REG_*: the refinement's estimator (B2S_REG_POINT_TO_PLANE); the reference: the scan
+                                            matcher's type, :47 */
 } b2s_loop_closure_refinement_params;
 typedef struct b2s_loop_closure_refinement {
   b2s_result icp;                        /* RegistrationResult of the refinement */

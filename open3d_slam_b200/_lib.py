@@ -110,7 +110,7 @@ class OdometryConstraint(C.Structure):
 class LoopClosureRefinementParams(C.Structure):
     _fields_ = [("map_voxel_size", C.c_double), ("voxel_if_zero", C.c_double), ("overlap_factor", C.c_double), ("min_points_per_voxel", C.c_int32),
                 ("max_iter", C.c_int32), ("max_corr_dist", C.c_double), ("rel_fitness", C.c_double), ("rel_rmse", C.c_double),
-                ("min_refinement_fitness", C.c_double)]
+                ("min_refinement_fitness", C.c_double), ("reg_type", C.c_int32)]
 
 
 class LoopClosureRefinement(C.Structure):

@@ -1343,6 +1343,7 @@ void b2s_default_loop_closure_refinement_params(b2s_loop_closure_refinement_para
   memset(p, 0, sizeof(*p));
   p->map_voxel_size = 0.1; p->voxel_if_zero = 0.04; p->overlap_factor = 20.0; p->min_points_per_voxel = 1; p->max_iter = 100;
   p->max_corr_dist = 0.3; p->rel_fitness = 1e-6; p->rel_rmse = 1e-6; p->min_refinement_fitness = 0.7;
+  p->reg_type = B2S_REG_POINT_TO_PLANE;
 }
 
 int32_t b2s_submap_loop_closure_refinement(b2s_handle* h, const b2s_submap* source, int32_t n, const b2s_submap* const* targets, const double* inits,
@@ -1368,9 +1369,16 @@ int32_t b2s_submap_loop_closure_refinement(b2s_handle* h, const b2s_submap* sour
       }
     B2S_REQUIRE(!so || !to || so[k] != to[k], B2S_E_INVALID, "target %d: the two overlap clouds are the same object", k);
   }
-  for (int32_t k = 0; k < n; k++)   // RegistrationICP's point-to-plane estimator needs the target's normals ([O3D] LogError)
-    B2S_REQUIRE(!targets[k]->no_normals, B2S_E_NO_NORMALS,
-                "[RegistrationICP] target %d: TransformationEstimationPointToPlane requires target normals, the map has none", k);
+  B2S_REQUIRE(p->reg_type == B2S_REG_POINT_TO_PLANE || p->reg_type == B2S_REG_POINT_TO_POINT || p->reg_type == B2S_REG_GENERALIZED,
+              B2S_E_UNSUPPORTED, "unknown registration type %d", (int)p->reg_type);
+  // the overlap clouds are marked as carrying normals whatever the maps hold, so the maps are checked here: point-to-plane needs the
+  // targets' ([O3D] LogError), generalized ICP derives both sides' covariances from normals, point-to-point reads none
+  B2S_REQUIRE(p->reg_type != B2S_REG_GENERALIZED || !source->no_normals, B2S_E_NO_NORMALS,
+              "GeneralizedIcp on the device derives the covariances from normals: the source map has none");
+  for (int32_t k = 0; k < n; k++)
+    B2S_REQUIRE(p->reg_type == B2S_REG_POINT_TO_POINT || !targets[k]->no_normals, B2S_E_NO_NORMALS,
+                "[RegistrationICP] target %d: the %s estimator requires target normals, the map has none", k,
+                p->reg_type == B2S_REG_GENERALIZED ? "GeneralizedIcp" : "TransformationEstimationPointToPlane");
   LOCK(h);
   return op_loop_closure_refinement(h, source, n, targets, inits, *p, voxel, so, to, out);
 }

@@ -6,7 +6,7 @@
 //
 //   overlap                    op_overlap_batch (overlap.cu): one set of launches for every pair, straight from the map slots
 //   target-overlap indexes     grid_build_batch (grid_index.cu): one build for all pairs, shared by the ICP and K-info-wide
-//   refinement                 the batched K-icp-iter launch with the point-to-plane estimator forced (icp.cu)
+//   refinement                 the batched K-icp-iter launch with the job's estimator (icp.cu): L2 point-to-plane, L3 the caller's
 //   information matrix         K-info-wide (below): [O3D] GetInformationMatrixFromPointClouds over ALL SMs
 //
 // K-info-wide.  b2s_information_matrix evaluates on K-icp-iter, one registration per 8-CTA cluster: sized for scans of ~10^4 points,
@@ -187,6 +187,7 @@ struct PairJob {
   double overlap_voxel;      // edge of the overlap's voxels
   int32_t min_pts;           // minNumPointsPerVoxel
   bool refine;               // run the ICP
+  int32_t estimator;         // B2S_REG_*: its estimator, one for the whole batch
   int32_t max_iter;
   double rel_fitness, rel_rmse;
   double radius;             // max_correspondence_distance of the ICP and of GetInformationMatrixFromPointClouds (equal in both kinds)
@@ -226,11 +227,11 @@ int32_t op_submap_constraints(b2s_handle* h, int n, const b2s_submap* const* sou
   for (int k = 0; k < n; k++) { grids[k] = h->batch_grids[k].get(); tclouds[k] = outs[2 * k + 1]; }
   B2S_TRY(grid_build_batch(h, grids.data(), tclouds.data(), n, J.grid_cell));
 
-  // refinement: RegistrationICP(sourceOverlap, targetOverlap, r, T0, PointToPlane, criteria) for every pair in one launch
+  // refinement: RegistrationICP / RegistrationGeneralizedICP(sourceOverlap, targetOverlap, r, T0, estimator, criteria) for every pair in one launch
   if (J.refine) {
     b2s_icp_params icp;
     memset(&icp, 0, sizeof(icp));
-    icp.reg_type = B2S_REG_POINT_TO_PLANE; icp.max_iter = J.max_iter; icp.max_corr_dist = J.radius; icp.rel_fitness = J.rel_fitness;
+    icp.reg_type = J.estimator; icp.max_iter = J.max_iter; icp.max_corr_dist = J.radius; icp.rel_fitness = J.rel_fitness;
     icp.rel_rmse = J.rel_rmse;
     size_t work_total = 0, max_src = 1;
     for (int k = 0; k < n; k++) {
@@ -249,7 +250,7 @@ int32_t op_submap_constraints(b2s_handle* h, int n, const b2s_submap* const* sou
       woff += (icp_work_bytes(outs[2 * k]->n_max) + 7) / 8;
     }
     B2S_CUDA(cudaMemcpyAsync(h->problems.p, probs, sizeof(IcpProblem) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
-    B2S_TRY(icp_launch(h, nullptr, h->problems.as<IcpProblem>(), n, max_src, B2S_REG_POINT_TO_PLANE));
+    B2S_TRY(icp_launch(h, nullptr, h->problems.as<IcpProblem>(), n, max_src, J.estimator));
   }
 
   // the information matrices: K-info-wide over the tiles of every pair, then one CTA per pair
@@ -292,6 +293,7 @@ int32_t op_odometry_constraints(b2s_handle* h, int n, const b2s_submap* const* s
   J.overlap_voxel = p.overlap_factor * voxel;
   J.min_pts = p.min_points_per_voxel;
   J.refine = p.refine != 0;
+  J.estimator = B2S_REG_POINT_TO_PLANE;               // raw RegistrationICP with TransformationEstimationPointToPlane (:62-68)
   J.max_iter = p.max_iter; J.rel_fitness = p.rel_fitness; J.rel_rmse = p.rel_rmse;
   J.radius = p.icp_factor * voxel;                     // icpMaxCorrespondenceDistance, also the information matrix's radius (:36, :71)
   J.grid_cell = 0.5 * J.radius;
@@ -308,6 +310,7 @@ int32_t op_loop_closure_refinement(b2s_handle* h, const b2s_submap* source, int 
   J.overlap_voxel = p.overlap_factor * voxel;          // :100
   J.min_pts = p.min_points_per_voxel;
   J.refine = true;
+  J.estimator = p.reg_type;                            // cloudRegistrationFactory(toCloudRegistrationType(scanMatcher_)) (:47)
   J.max_iter = p.max_iter; J.rel_fitness = p.rel_fitness; J.rel_rmse = p.rel_rmse;
   J.radius = p.max_corr_dist;                          // maxIcpCorrespondenceDistance_: the ICP's (:46) and the information's (:149)
   J.grid_cell = nn_cell(h, p.max_corr_dist);           // the cell b2s_register_batch indexes its targets at

@@ -24,6 +24,14 @@ from . import _lib as L
 # --------------------------------------------------------------------------------------------------------------------
 
 
+def regTypeOf(name: str) -> int:
+    """CloudRegistrationType by its Lua name (Parameters.hpp:37-49) -> B2S_REG_*; an unknown name is what the factories throw on"""
+    types = {"PointToPlaneIcp": L.REG_POINT_TO_PLANE, "PointToPointIcp": L.REG_POINT_TO_POINT, "GeneralizedIcp": L.REG_GENERALIZED}
+    if name not in types:
+        raise L.B2SError(L.E_UNSUPPORTED, f"unknown registration type {name}")
+    return types[name]
+
+
 @dataclass
 class ScanCroppingParameters:
     cropperName: str = "MinMaxRadius"
@@ -135,12 +143,10 @@ class MapperParameters:
     icpClusterCtas: int = 0  # engine knob: SMs one registration spreads over (0 = automatic; 8 = throughput, 16 = latency)
 
     def to_config(self) -> L.Config:
-        types = {"PointToPlaneIcp": L.REG_POINT_TO_PLANE, "PointToPointIcp": L.REG_POINT_TO_POINT, "GeneralizedIcp": L.REG_GENERALIZED}
-        if self.scanToMapRegType not in types:   # Parameters.hpp:37-49 ; unknown -> the factories throw
-            raise L.B2SError(L.E_UNSUPPORTED, f"unknown registration type {self.scanToMapRegType}")
+        reg_type = regTypeOf(self.scanToMapRegType)
         cfg = L.Config()
         L.lib().b2s_default_config(C.byref(cfg))
-        cfg.icp.reg_type = types[self.scanToMapRegType]
+        cfg.icp.reg_type = reg_type
         cfg.icp.max_iter = int(self.icp.maxNumIter)
         cfg.icp.max_corr_dist = float(self.icp.maxCorrespondenceDistance)
         cfg.icp.knn = int(self.icp.knn)
@@ -470,12 +476,13 @@ class LoopClosureRefinementParameters:
     relativeFitness: float = 1e-6
     relativeRmse: float = 1e-6
     minRefinementFitness: float = 0.7
+    regType: str = "PointToPlaneIcp"                             # the refinement's estimator; the reference's: the scan matcher's (:47)
 
     def to_c(self) -> L.LoopClosureRefinementParams:
         return L.LoopClosureRefinementParams(float(self.mapVoxelSize), float(self.voxelSizeIfMapVoxelSizeIsZero),
                                              float(self.voxelExpansionFactorOverlapComputation), int(self.minNumPointsPerVoxel), int(self.maxNumIter),
                                              float(self.maxIcpCorrespondenceDistance), float(self.relativeFitness), float(self.relativeRmse),
-                                             float(self.minRefinementFitness))
+                                             float(self.minRefinementFitness), regTypeOf(self.regType))
 
 
 @dataclass
@@ -492,7 +499,7 @@ class LoopClosureRefinementResult:
 def refineLoopClosuresBatch(eng: Engine, sourceSubmap, targetSubmaps, inits, params: LoopClosureRefinementParameters | None = None,
                             sourceOverlaps=None, targetOverlaps=None) -> list[LoopClosureRefinementResult]:
     """src/PlaceRecognition.cpp:96-149 for one source Submap against every target Submap in one device call on the resident maps:
-    overlap at inits[k], point-to-plane ICP from inits[k], fitness gate, information matrix.  sourceOverlaps / targetOverlaps (lists
+    overlap at inits[k], ICP with params.regType from inits[k], fitness gate, information matrix.  sourceOverlaps / targetOverlaps (lists
     of Cloud, optional) receive the overlap selections in map order."""
     p = (params or LoopClosureRefinementParameters()).to_c()
     n = len(targetSubmaps)
@@ -1166,13 +1173,11 @@ class OdometryParameters:
     bufferSize: int = 2000         # odomToRangeSensorBuffer_ size limit (TransformInterpolationBuffer())
 
     def to_c(self) -> L.OdometryParams:
-        types = {"PointToPlaneIcp": L.REG_POINT_TO_PLANE, "PointToPointIcp": L.REG_POINT_TO_POINT, "GeneralizedIcp": L.REG_GENERALIZED}
-        if self.scanMatcher.regType not in types:
-            raise L.B2SError(L.E_UNSUPPORTED, f"unknown registration type {self.scanMatcher.regType}")
+        reg_type = regTypeOf(self.scanMatcher.regType)
         p = L.OdometryParams()
         L.lib().b2s_default_odometry_params(C.byref(p))
         ic = self.scanMatcher.icp
-        p.icp.reg_type = types[self.scanMatcher.regType]
+        p.icp.reg_type = reg_type
         p.icp.max_iter, p.icp.max_corr_dist, p.icp.knn, p.icp.knn_radius = int(ic.maxNumIter), float(ic.maxCorrespondenceDistance), int(ic.knn), float(ic.maxDistanceKnn)
         p.voxel_size = float(self.scanProcessing.voxelSize)
         p.downsampling_ratio = float(self.scanProcessing.downSamplingRatio)

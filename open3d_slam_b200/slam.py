@@ -42,12 +42,25 @@ class SubmapParameters:
 
 @dataclass
 class LoopClosureParameters:
-    """the PlaceRecognitionParameters the refinement half reads (Parameters.hpp:132-135) + magic.hpp:14"""
+    """the PlaceRecognitionParameters the refinement half reads (Parameters.hpp:132-135) + magic.hpp:14, and the refinement's
+    estimator.  registrationType defaults to point-to-plane; the reference refines with the scan matcher's type, which
+    fromMapperParameters takes over."""
     maxIcpCorrespondenceDistance: float = 0.3
     minRefinementFitness: float = 0.7
     maxNumIter: int = 100                       # magic::icpRunUntilConvergenceNumberOfIterations
     voxelExpansionFactorOverlapComputation: float = 20.0
     minNumPointsPerVoxel: int = 1
+    registrationType: str = "PointToPlaneIcp"   # CloudRegistrationType of the refinement ICP
+
+    @classmethod
+    def fromMapperParameters(cls, mapperParams: E.MapperParameters, maxIcpCorrespondenceDistance: float = 0.3,
+                             minRefinementFitness: float = 0.7) -> "LoopClosureParameters":
+        """PlaceRecognition::updateRegistrationAlgorithm (src/PlaceRecognition.cpp:44-48): the loop-closure ICP is the scan matcher's
+        registration type with maxNumIter = magic::icpRunUntilConvergenceNumberOfIterations and maxCorrespondenceDistance =
+        placeRecognition.maxIcpCorrespondenceDistance (passed here with minRefinementFitness: MapperParameters does not hold them)."""
+        E.regTypeOf(mapperParams.scanToMapRegType)   # an unknown type throws, as cloudRegistrationFactory does
+        return cls(maxIcpCorrespondenceDistance=maxIcpCorrespondenceDistance, minRefinementFitness=minRefinementFitness, maxNumIter=100,
+                   registrationType=mapperParams.scanToMapRegType)
 
 
 VOXEL_EXPANSION_ADJACENCY_REVISITING = 2.5     # magic::voxelExpansionFactorAdjacencyBasedRevisiting
@@ -330,12 +343,16 @@ class SegmentMapper:
 def refineLoopClosures(backend, source_handle, target_handles, initial_guesses, mapVoxelSize: float, p: LoopClosureParameters | None = None):
     """The refinement half of PlaceRecognition::buildLoopClosureConstraints for one finished (source) submap against its
     candidate (target) submaps, src/PlaceRecognition.cpp:96-149: overlap selection with voxel = 20 x map voxel, ICP of the
-    overlapping parts from the proposal, fitness gate, information matrix.  The n registrations run as one batch.
-    Returns a list of dicts {overlap sizes, result, accepted, information}."""
+    overlapping parts from the proposal with p.registrationType, fitness gate, information matrix.  The n registrations run as one
+    batch.  Returns a list of dicts {overlap sizes, result, accepted, information}."""
     p = p or LoopClosureParameters()
     voxel = p.voxelExpansionFactorOverlapComputation * mapVoxelSize
     pairs = [backend.overlap(source_handle, t, T0, voxel, p.minNumPointsPerVoxel) for t, T0 in zip(target_handles, initial_guesses)]
-    results = backend.register_batch([so for so, _to in pairs], [to for _so, to in pairs], initial_guesses, p.maxIcpCorrespondenceDistance, p.maxNumIter)
+    # point-to-plane is what register_batch does without a regType, so a backend that only registers point-to-plane needs none;
+    # any other estimator is asked for by name, and a backend that cannot take it fails instead of registering point-to-plane
+    kw = {} if p.registrationType == "PointToPlaneIcp" else {"regType": p.registrationType}
+    results = backend.register_batch([so for so, _to in pairs], [to for _so, to in pairs], initial_guesses, p.maxIcpCorrespondenceDistance, p.maxNumIter,
+                                     **kw)
     out = []
     for (so, to), r in zip(pairs, results):
         acc = not (r.fitness_ < p.minRefinementFitness)
@@ -831,10 +848,10 @@ class DeviceBackend:
     def overlap(self, source, target, T0, voxel, min_pts):
         return E.computeOverlappingClouds(self.eng, source, target, T0, voxel, min_pts)
 
-    def register_batch(self, sources, targets, inits, max_corr, max_iter):
-        pc = E.CloudRegistrationParameters(icp=E.IcpParameters(maxNumIter=max_iter, maxCorrespondenceDistance=max_corr, knn=self.params.icp.knn,
-                                                              maxDistanceKnn=self.params.icp.maxDistanceKnn))
-        reg = E.RegistrationIcpPointToPlane(self.eng, pc)
+    def register_batch(self, sources, targets, inits, max_corr, max_iter, regType: str = "PointToPlaneIcp"):
+        pc = E.CloudRegistrationParameters(regType=regType, icp=E.IcpParameters(maxNumIter=max_iter, maxCorrespondenceDistance=max_corr,
+                                                                               knn=self.params.icp.knn, maxDistanceKnn=self.params.icp.maxDistanceKnn))
+        reg = E.cloudRegistrationFactory(self.eng, pc)
         out = reg.registerCloudsBatch(sources, targets, inits)
         self.eng.set_parameters(self.params)   # the scan-to-map chain keeps its own ICP parameters
         return out
@@ -849,7 +866,8 @@ class DeviceBackend:
         lc = lc or LoopClosureParameters()
         prm = E.LoopClosureRefinementParameters(mapVoxelSize=mapVoxelSize, voxelExpansionFactorOverlapComputation=lc.voxelExpansionFactorOverlapComputation,
                                                 minNumPointsPerVoxel=lc.minNumPointsPerVoxel, maxNumIter=lc.maxNumIter,
-                                                maxIcpCorrespondenceDistance=lc.maxIcpCorrespondenceDistance, minRefinementFitness=lc.minRefinementFitness)
+                                                maxIcpCorrespondenceDistance=lc.maxIcpCorrespondenceDistance, minRefinementFitness=lc.minRefinementFitness,
+                                                regType=lc.registrationType)
         res = E.refineLoopClosuresBatch(self.eng, source_sm, list(target_sms), inits, prm)
         return [{"n_source_overlap": r.nSourceOverlap, "n_target_overlap": r.nTargetOverlap, "result": r.result, "accepted": r.accepted,
                  "information": r.information} for r in res]

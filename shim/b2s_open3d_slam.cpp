@@ -425,7 +425,8 @@ RansacResultB200 registrationRansacBasedOnFeatureMatchingB200(const SubmapB200& 
 }
 
 std::vector<LoopClosureRefinementB200> refineLoopClosuresB200(const SubmapB200& source, const std::vector<const SubmapB200*>& targets,
-                                                              const std::vector<Transform>& initialGuesses, const MapperParameters& cfg) {
+                                                              const std::vector<Transform>& initialGuesses, const MapperParameters& cfg,
+                                                              CloudRegistrationType regType) {
   if (initialGuesses.size() != targets.size()) throw std::runtime_error("one initial guess per target");
   std::vector<LoopClosureRefinementB200> out(targets.size());
   if (targets.empty()) return out;
@@ -440,6 +441,11 @@ std::vector<LoopClosureRefinementB200> refineLoopClosuresB200(const SubmapB200& 
   prm.map_voxel_size = cfg.mapBuilder_.mapVoxelSize_;                     // getMapVoxelSize is applied by the call (:98)
   prm.max_corr_dist = cfg.placeRecognition_.maxIcpCorrespondenceDistance_;   // :46, :149
   prm.min_refinement_fitness = cfg.placeRecognition_.minRefinementFitness_;  // :118
+  switch (regType) {                                                        // cloudRegistrationFactory's estimator (:47)
+    case CloudRegistrationType::PointToPointIcp: prm.reg_type = B2S_REG_POINT_TO_POINT; break;
+    case CloudRegistrationType::GeneralizedIcp: prm.reg_type = B2S_REG_GENERALIZED; break;
+    default: prm.reg_type = B2S_REG_POINT_TO_PLANE; break;
+  }
   std::vector<b2s_loop_closure_refinement> res(targets.size());
   const int32_t rc = b2s_submap_loop_closure_refinement(source.engine(), source.handle(), (int32_t)targets.size(), tgt.data(), inits.data(), &prm,
                                                         nullptr, nullptr, res.data());

@@ -131,8 +131,10 @@ RansacResultB200 registrationRansacBasedOnFeatureMatchingB200(const SubmapB200& 
 // at :86 and :92: overlap of the two whole maps at the proposal (20 x getMapVoxelSize(mapBuilder_, 0.04)), ICP of the overlaps from
 // the proposal with r = placeRecognition_.maxIcpCorrespondenceDistance_ and 100 iterations, the fitness gate of :118 and the
 // information matrix at the ICP's T (:148-149), all candidates in ONE b2s_submap_loop_closure_refinement call on the resident maps (all
-// SubmapB200s on one handle).  The ICP is point-to-plane; the reference uses the scan matcher's type (:47), point-to-plane in every
-// shipped configuration.  The consistency check of the ICP's T (:124) and the Constraint record (:140-150) stay with the caller.
+// SubmapB200s on one handle).  regType is the refinement's estimator, point-to-plane unless given; the reference uses the scan matcher's
+// type (:47), so pass toCloudRegistrationType(cfg.scanMatcher_).regType_ for its behaviour (GeneralizedIcp in the shipped Lua presets).
+// Point-to-plane needs normals on every target map, GeneralizedIcp on the source and every target, PointToPointIcp none; a missing
+// one throws (B2S_E_NO_NORMALS).  The consistency check of the ICP's T (:124) and the Constraint record (:140-150) stay with the caller.
 struct LoopClosureRefinementB200 {
   RegistrationResult icpResult;                 // :110
   Eigen::Matrix6d informationMatrix;            // :148-149, at icpResult.transformation_ (computed for every candidate)
@@ -140,7 +142,8 @@ struct LoopClosureRefinementB200 {
   size_t numSourceOverlap = 0, numTargetOverlap = 0;
 };
 std::vector<LoopClosureRefinementB200> refineLoopClosuresB200(const SubmapB200& source, const std::vector<const SubmapB200*>& targets,
-                                                              const std::vector<Transform>& initialGuesses, const MapperParameters& cfg);
+                                                              const std::vector<Transform>& initialGuesses, const MapperParameters& cfg,
+                                                              CloudRegistrationType regType = CloudRegistrationType::PointToPlaneIcp);
 
 // computeOdometryConstraints (src/constraint_builders.cpp:92-118) over device-resident submaps: submaps[i] is the SubmapB200 of submap
 // id i and parentIds[i] its getParentId().  candidates = the finished submap ids (the overload of SubmapCollection::computeFeatures,

@@ -2,7 +2,7 @@
 // signatures the shim overrides so that it can be type-checked without Open3D / Eigen / the reference tree:
 //   CloudRegistration          include/open3d_slam/CloudRegistration.hpp:19-27
 //   ScanToMapRegistration      include/open3d_slam/ScanToMapRegistration.hpp:24-38
-//   parameter structs          include/open3d_slam/Parameters.hpp:51-98,118-122,148-153,172
+//   parameter structs          include/open3d_slam/Parameters.hpp:37,51-98,118-122,148-153,172
 //   Constraint                 include/open3d_slam/Constraint.hpp:14-20
 // In a real build, include the reference's own headers instead (INTEGRATION.md).
 #pragma once
@@ -20,7 +20,8 @@ using RegistrationResult = open3d::pipelines::registration::RegistrationResult;
 struct ScanCroppingParameters { double croppingMinZ_ = -10, croppingMaxZ_ = 10, croppingMinRadius_ = 0, croppingMaxRadius_ = 20; std::string cropperName_ = "MaxRadius"; };
 struct ScanProcessingParameters { double downSamplingRatio_ = 1.0, voxelSize_ = 0.03; ScanCroppingParameters cropper_; };
 struct IcpParameters { int maxNumIter_ = 50; double maxCorrespondenceDistance_ = 0.2; int knn_ = 5; double maxDistanceKnn_ = 10.0; };
-struct CloudRegistrationParameters { IcpParameters icp_; };
+enum class CloudRegistrationType : int { PointToPlaneIcp, PointToPointIcp, GeneralizedIcp };   // Parameters.hpp:37
+struct CloudRegistrationParameters { IcpParameters icp_; CloudRegistrationType regType_ = CloudRegistrationType::PointToPlaneIcp; };
 struct SpaceCarvingParameters { double voxelSize_ = 0.1, maxRaytracingLength_ = 20.0, truncationDistance_ = 0.1; int carveSpaceEveryNscans_ = 10; double minDotProductWithNormal_ = 0.5, neighborhoodRadiusDenseMap_ = 0.1; };
 struct MapBuilderParameters { double mapVoxelSize_ = 0.03; ScanCroppingParameters cropper_; SpaceCarvingParameters carving_; };
 enum class ScanToMapRegistrationType : int { PointToPlaneIcp, PointToPointIcp, GeneralizedIcp };   // Parameters.hpp:44-49
