@@ -153,6 +153,19 @@ int32_t b2s_crop(b2s_handle* h, const b2s_cloud* in, const b2s_cropper* cropper,
 int32_t b2s_voxel_down_sample(b2s_handle* h, const b2s_cloud* in, double voxel_size, b2s_cloud* out);
 /* P3  estimateNormalsOrCovariancesIfNeeded                    src/CloudRegistration.cpp:49-56 */
 int32_t b2s_estimate_normals(b2s_handle* h, b2s_cloud* cloud, int32_t knn, double radius);
+/* Debug aid for tests: the normal estimation of b2s_estimate_normals (same grid, cell rule and launches, normals written to the cloud)
+ * with cell_hint (<= 0: radius / 4; never below radius / 16), flags_host (nullable, one int per point: only flagged points get a normal)
+ * and with_prior (the cloud's normals on entry are the priors, as b2s_submap_compute_features runs it), recording per point how the
+ * kernels decided.  rec_out (n x 10): the nine cumulants sum x, y, z, xx, xy, xz, yy, yz, zz and the neighbour count exactly as the
+ * eigen-solver received them; NaN for a point that was not queried.  path_out (n): 1, 2 or 3 = resolved by the block gather at that
+ * block radius, 4 = by the block that covers the whole search radius, 5 = by the ring walk after a block held too many candidates,
+ * 6 = by the ring walk after the last block could not certify the k-th neighbour; 0 = not queried (or an A/B search variant chosen in
+ * the environment).  sel_out (n x 4, nullable): the block gather's selection at the last block it tried -- candidates inside the
+ * certified ball (over NS2_CAP = 256: the block went over capacity), the 32-bin d2 histogram bin of the k-th key (-1: at most k
+ * candidates, no histogram), that bin's member count, and the ball's squared radius lim2 the histogram spans; NaN where not queried.
+ * The kernels run in their debug instantiations (the production ones compile none of the recording).  Synchronises. */
+int32_t b2s_debug_estimate_normals(b2s_handle* h, b2s_cloud* cloud, int32_t knn, double radius, double cell_hint, const int32_t* flags_host,
+                                   int32_t with_prior, double* rec_out, int32_t* path_out, double* sel_out);
 /* P4  [O3D] RandomDownSample (seeded)                         src/ScanToMapRegistration.cpp:39 */
 int32_t b2s_random_down_sample(b2s_handle* h, const b2s_cloud* in, double ratio, uint32_t seed, b2s_cloud* out);
 /* F0  o3d_slam::transform (keeps the near-identity duplication quirk)   src/helpers.cpp:273-305 */

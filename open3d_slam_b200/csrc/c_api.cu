@@ -556,6 +556,46 @@ int32_t b2s_estimate_normals(b2s_handle* h, b2s_cloud* cloud, int32_t knn, doubl
   return op_estimate_normals(h, cloud, knn, radius, h->cfg.scan.voxel_size > 0.0 ? 4.0 * h->cfg.scan.voxel_size : 0.0);
 }
 
+// debug aid for tests: op_estimate_normals with its debug record switched on, i.e. the kDebug instantiations of its kernels (include/b2s.h)
+int32_t b2s_debug_estimate_normals(b2s_handle* h, b2s_cloud* cloud, int32_t knn, double radius, double cell_hint, const int32_t* flags_host,
+                                   int32_t with_prior, double* rec_out, int32_t* path_out, double* sel_out) {
+  B2S_REQUIRE(h && cloud && rec_out && path_out, B2S_E_INVALID, "null argument");
+  LOCK(h);
+  WideGridScope wide(cloud->n_max);
+  int32_t n = 0;
+  B2S_TRY(read_back(h, {{&n, cloud->dn.p, 4}}));
+  const size_t nb = n > 0 ? (size_t)n : 1;
+  DevBuf rec, path, sel, flags;   // the call's own buffers, freed on return
+  rec.tracked = path.tracked = sel.tracked = flags.tracked = false;
+  B2S_TRY(rec.ensure(nb * 80, h->stream));
+  B2S_TRY(path.ensure(nb * 4, h->stream));
+  B2S_TRY(sel.ensure(nb * 32, h->stream));
+  std::vector<double> rec_init(nb * 10, NAN);   // points that are not queried keep NaN
+  B2S_CUDA(cudaMemcpyAsync(rec.p, rec_init.data(), nb * 80, cudaMemcpyHostToDevice, h->stream));
+  B2S_CUDA(cudaMemcpyAsync(sel.p, rec_init.data(), nb * 32, cudaMemcpyHostToDevice, h->stream));
+  B2S_CUDA(cudaMemsetAsync(path.p, 0, nb * 4, h->stream));
+  if (flags_host) {
+    B2S_TRY(flags.ensure(nb * 4, h->stream));
+    B2S_CUDA(cudaMemcpyAsync(flags.p, flags_host, (size_t)n * 4, cudaMemcpyHostToDevice, h->stream));
+  }
+  const NormalsDebug dbg{rec.as<double>(), path.as<int32_t>(), sel.as<double>()};
+  B2S_TRY(op_estimate_normals(h, cloud, knn, radius, cell_hint, flags_host ? flags.as<int32_t>() : nullptr, with_prior != 0, &dbg));
+  // the path is recorded per grid slot: map it to the original index through the index's stored point bits
+  std::vector<int32_t> path_slot(nb);
+  std::vector<double> p4(nb * 4), sel_slot(nb * 4);
+  B2S_CUDA(cudaMemcpyAsync(rec_out, rec.p, (size_t)n * 80, cudaMemcpyDeviceToHost, h->stream));
+  B2S_CUDA(cudaMemcpyAsync(path_slot.data(), path.p, (size_t)n * 4, cudaMemcpyDeviceToHost, h->stream));
+  B2S_CUDA(cudaMemcpyAsync(sel_slot.data(), sel.p, (size_t)n * 32, cudaMemcpyDeviceToHost, h->stream));
+  B2S_CUDA(cudaMemcpyAsync(p4.data(), h->grid_b.pts.p, (size_t)n * 32, cudaMemcpyDeviceToHost, h->stream));
+  B2S_CUDA(cudaStreamSynchronize(h->stream));
+  for (int32_t k = 0; k < n; k++) {
+    long long v; memcpy(&v, &p4[4 * (size_t)k + 3], 8);
+    path_out[(int32_t)v] = path_slot[k];
+    if (sel_out) memcpy(sel_out + 4 * (size_t)v, &sel_slot[4 * (size_t)k], 32);
+  }
+  return B2S_OK;
+}
+
 int32_t b2s_random_down_sample(b2s_handle* h, const b2s_cloud* in, double ratio, uint32_t seed, b2s_cloud* out) {
   B2S_REQUIRE(h && in && out && in != out, B2S_E_INVALID, "bad argument");
   LOCK(h);

@@ -438,8 +438,12 @@ int32_t op_assemble_map(b2s_handle* h, int n, const b2s_submap* const* submaps, 
                         size_t capacity, size_t* n_out);
 // flags (optional, one int per point of c): only flagged points get a normal.  with_prior: c's normals on entry are the priors of
 // [O3D] EstimateNormals on a cloud that has normals (keep the prior for a zero solver result, flip against it otherwise)
+// dbg (b2s_debug_estimate_normals only; nullptr everywhere else): rec, 10 doubles per ORIGINAL point index, receives the nine cumulants
+// and the neighbour count finish_normal was given; path (one int) and sel (4 doubles) per GRID SLOT: how select2 resolved the query
+// (normals.cu NPATH_*) and its selection at the last block it tried (normals_select2_kernel)
+struct NormalsDebug { double* rec; int32_t* path; double* sel; };
 int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius, double cell_hint, const int32_t* flags = nullptr,
-                            bool with_prior = false);
+                            bool with_prior = false, const NormalsDebug* dbg = nullptr);
 int32_t select_flags(b2s_handle* h, const b2s_cloud* in, double ratio, uint32_t seed);
 int32_t select_compact(b2s_handle* h, const b2s_cloud* in, double ratio, b2s_cloud* out);
 int32_t op_random_down_sample(b2s_handle* h, const b2s_cloud* in, double ratio, uint32_t seed, b2s_cloud* out);

@@ -291,10 +291,11 @@ __global__ void __launch_bounds__(NK_THREADS) normals_kernel(const GridHeader* _
 // pruning test and the two dependent cell_start loads, the latency that dominates in empty space -- then the warp
 // walks the non-empty rows together: 32 candidates per step, the k best kept as a sorted list with one entry per lane
 // (k <= 32), a qualifying candidate inserted with a single shuffle-up step.
+template <bool kDebug>
 __global__ void __launch_bounds__(NK_THREADS) normals_phase2_kernel(const GridHeader* __restrict__ hdr, const int32_t* __restrict__ cs,
                                                                     const double4* __restrict__ pts, int knn, double radius,
                                                                     const int32_t* __restrict__ queue, const int32_t* __restrict__ queue_n,
-                                                                    const double* prior_nrm, double* out_nrm) {
+                                                                    const double* prior_nrm, double* out_nrm, double* __restrict__ dbg_rec) {
   pdl_wait();
   __shared__ GridHeader g;
   if (threadIdx.x == 0) g = *hdr;
@@ -396,6 +397,10 @@ __global__ void __launch_bounds__(NK_THREADS) normals_phase2_kernel(const GridHe
       c[6] = __dadd_rn(c[6], __dmul_rn(y, y)); c[7] = __dadd_rn(c[7], __dmul_rn(y, z)); c[8] = __dadd_rn(c[8], __dmul_rn(z, z));
     }
     if (lane == 0) {
+      if (kDebug) {   // debug record (b2s_debug_estimate_normals): what finish_normal receives
+        for (int t = 0; t < 9; t++) dbg_rec[10 * (size_t)qi + t] = c[t];
+        dbg_rec[10 * (size_t)qi + 9] = (double)kk;
+      }
       double nr[3];
       finish_normal(c, kk, qx, qy, qz, prior_nrm ? prior_nrm + 3 * (size_t)qi : nullptr, nr);
       out_nrm[3 * (size_t)qi] = nr[0]; out_nrm[3 * (size_t)qi + 1] = nr[1]; out_nrm[3 * (size_t)qi + 2] = nr[2];
@@ -634,12 +639,20 @@ constexpr int NS2_CAP = 256;
 constexpr int NS2_CHUNKS = NS2_CAP / 32;
 constexpr int NS2_RMAX = 3;
 constexpr int NS2_ROWS = 320;   // row-table entries per warp: (2 R + 1)^2 rows of the largest block, rounded up to 32 (R = 8 -> 289)
+// path codes of the debug record (b2s_debug_estimate_normals, include/b2s.h): 1..NS2_RMAX = select2 resolved the query at that block
+// radius, then the block that covers the whole radius, then the two ways a query goes to normals_phase2_kernel
+enum : int32_t { NPATH_FULL_BLOCK = NS2_RMAX + 1, NPATH_OVER_CAPACITY, NPATH_NOT_CERTIFIED };
 
+// kDebug (b2s_debug_estimate_normals only): per grid slot, the path code (dbg_path) and the selection at the last block tried (dbg_sel,
+// 4 doubles: candidates inside the certified ball nc, the histogram bin of the k-th key or -1 without a histogram, that bin's member count,
+// lim2).  The production instantiation (kDebug = false) compiles none of it.
+template <bool kDebug>
 __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2_kernel(const GridHeader* __restrict__ hdr, const int32_t* __restrict__ cs,
                                                                      const double4* __restrict__ pts, int knn, double radius,
                                                                      const int32_t* __restrict__ qlist, const int32_t* __restrict__ qcount,
                                                                      int32_t* __restrict__ queue, int32_t* queue_n,
-                                                                     double* __restrict__ cum) {
+                                                                     double* __restrict__ cum, int32_t* __restrict__ dbg_path,
+                                                                     double* __restrict__ dbg_sel) {
   pdl_wait();
   __shared__ GridHeader g;
   __shared__ double s_d[NK_THREADS / 32][NS2_CAP];
@@ -748,7 +761,13 @@ __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2
         nc += __popc(m);
       }
       __syncwarp();
-      if (nc > NS2_CAP) { if (lane == 0) atomicAdd(queue_n + 2, 1); break; }   // too dense for the buffer: general kernel
+      if (nc > NS2_CAP) {   // too dense for the buffer: general kernel
+        if (lane == 0) {
+          atomicAdd(queue_n + 2, 1);
+          if (kDebug) { dbg_path[s] = NPATH_OVER_CAPACITY; dbg_sel[4 * (size_t)s] = nc; dbg_sel[4 * (size_t)s + 1] = -1; dbg_sel[4 * (size_t)s + 2] = 0; dbg_sel[4 * (size_t)s + 3] = lim2; }
+        }
+        break;
+      }
       // ---- candidates -> registers (round-robin), statistics ----
       // nc is uniform over the warp, so is the number of 32-candidate chunks in use: every chunk loop below stops there
       // (the loops stay fully unrolled -- the register arrays need static indices -- but the unused tail is branched over)
@@ -766,6 +785,7 @@ __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2
       __syncwarp();
       need = min(knn, nc);
       double td = INFINITY; int ti = 0x7fffffff;
+      int dbg_bin = -1, dbg_nb = 0;   // debug record only
       if (nc > knn) {   // k-th smallest (d2, index) by counting: 32-bin histogram over d2, then arg-min rounds in one bin
         // every candidate kept lies below lim2 (finite: lim2 <= radius^2), so that is the histogram's range -- no maximum to reduce
         const double scale = lim2 > 0.0 ? 32.0 / lim2 : 0.0;
@@ -795,6 +815,7 @@ __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2
           nb += __popc(bm);
         }
         __syncwarp();
+        if (kDebug) { dbg_bin = B; dbg_nb = nb; }
         for (int base = 0; base < nb; base += 32) {
           const int t = base + lane;
           double md = INFINITY; int mi = 0x7fffffff, rank = -1;
@@ -811,7 +832,13 @@ __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2
       // ---- exact?  every candidate kept lies strictly inside the guaranteed ball (radius sqrt(lim2) <= distance to the
       // nearest block face), so k kept candidates contain the true k nearest; fewer than k is final only when the
       // block covers the whole search radius ----
-      if (!(nc >= knn || b2 > r2)) { if (last_try) break; continue; }   // grow the block
+      if (!(nc >= knn || b2 > r2)) {   // grow the block
+        if (last_try) {
+          if (kDebug && lane == 0) { dbg_path[s] = NPATH_NOT_CERTIFIED; dbg_sel[4 * (size_t)s] = nc; dbg_sel[4 * (size_t)s + 1] = dbg_bin; dbg_sel[4 * (size_t)s + 2] = dbg_nb; dbg_sel[4 * (size_t)s + 3] = lim2; }
+          break;
+        }
+        continue;
+      }
       // ---- cumulants of the selected candidates, butterfly sum over the warp ----
 #pragma unroll
       for (int c = 0; c < NS2_CHUNKS; c++) {
@@ -826,7 +853,10 @@ __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2
       }
       warp_sum9_transposed(c9, lane);   // lane l now holds the warp total of cumulant l >> 1 in c9[0] (l < 18)
       resolved = true;
-      if (lane == 0 && R > 1) atomicAdd(queue_n + 2 + min(R, 3), 1);   // statistics (B2S_DEBUG_NORMALS): resolved at R = 2 / at R >= 3
+      if (lane == 0) {
+        if (R > 1) atomicAdd(queue_n + 2 + min(R, 3), 1);   // statistics (B2S_DEBUG_NORMALS): resolved at R = 2 / at R >= 3
+        if (kDebug) { dbg_path[s] = R <= NS2_RMAX ? R : NPATH_FULL_BLOCK; dbg_sel[4 * (size_t)s] = nc; dbg_sel[4 * (size_t)s + 1] = dbg_bin; dbg_sel[4 * (size_t)s + 2] = dbg_nb; dbg_sel[4 * (size_t)s + 3] = lim2; }
+      }
     }
     if (!resolved) {
       if (lane == 0) { queue[atomicAdd(queue_n, 1)] = s; cum[10 * (size_t)tq + 9] = -1.0; }
@@ -841,9 +871,11 @@ __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2
 }
 
 // eigen-solver + normalise + orient for the queries the select kernel resolved: one THREAD per query
+template <bool kDebug>
 __global__ void __launch_bounds__(NK_THREADS) normals_finish_kernel(const GridHeader* __restrict__ hdr, const double4* __restrict__ pts,
                                                                     const int32_t* __restrict__ qlist, const int32_t* __restrict__ qcount,
-                                                                    const double* __restrict__ cum, const double* prior_nrm, double* out_nrm) {
+                                                                    const double* __restrict__ cum, const double* prior_nrm, double* out_nrm,
+                                                                    double* __restrict__ dbg_rec) {
   pdl_wait();
   const int nq = qlist ? *qcount : hdr->n;
   for (int tq = blockIdx.x * blockDim.x + threadIdx.x; tq < nq; tq += gridDim.x * blockDim.x) {
@@ -854,6 +886,11 @@ __global__ void __launch_bounds__(NK_THREADS) normals_finish_kernel(const GridHe
     for (int t = 0; t < 9; t++) c9[t] = cum[10 * (size_t)tq + t];
     const double4 qp = pts[qlist ? qlist[tq] : tq];
     const size_t qi = (size_t)(int)__double_as_longlong(qp.w);
+    if (kDebug) {   // debug record (b2s_debug_estimate_normals): what finish_normal receives
+#pragma unroll
+      for (int t = 0; t < 9; t++) dbg_rec[10 * qi + t] = c9[t];
+      dbg_rec[10 * qi + 9] = kkd;
+    }
     double nr[3];
     finish_normal(c9, (int)kkd, qp.x, qp.y, qp.z, prior_nrm ? prior_nrm + 3 * qi : nullptr, nr);
     out_nrm[3 * qi] = nr[0]; out_nrm[3 * qi + 1] = nr[1]; out_nrm[3 * qi + 2] = nr[2];
@@ -883,7 +920,8 @@ __global__ void __launch_bounds__(NK_THREADS) normals_qlist_kernel(const GridHea
   }
 }
 
-int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius, double cell_hint, const int32_t* flags, bool with_prior) {
+int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius, double cell_hint, const int32_t* flags, bool with_prior,
+                            const NormalsDebug* dbg) {
   B2S_REQUIRE(radius > 0.0, B2S_E_INVALID, "maxRadiusNormalEstimation_ must be > 0");  // CloudRegistration.cpp:50
   B2S_REQUIRE(knn > 0, B2S_E_INVALID, "knnNormalEstimation_ must be > 0");            // CloudRegistration.cpp:51
   B2S_REQUIRE(knn <= 32, B2S_E_UNSUPPORTED, "knn > 32 is not supported by the register-resident k-best list yet");
@@ -935,8 +973,12 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
     double* cum = h->tmp_f64.as<double>();
     static const bool use_v1 = getenv("B2S_NORMALS_SELECT_V1") != nullptr;   // A/B knob: fixed 3x3x3 block, register gather
     if (use_v1) launch_pdl(normals_select_kernel, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn, cum);
-    else launch_pdl(normals_select2_kernel, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn, cum);
-    launch_pdl(normals_finish_kernel, blocks, NK_THREADS, 0, h->stream, hdr, pts, qlist, qcount, cum, prior, out);
+    else if (dbg) launch_pdl(normals_select2_kernel<true>, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn,
+                             cum, dbg->path, dbg->sel);
+    else launch_pdl(normals_select2_kernel<false>, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn, cum,
+                    nullptr, nullptr);
+    if (dbg) launch_pdl(normals_finish_kernel<true>, blocks, NK_THREADS, 0, h->stream, hdr, pts, qlist, qcount, cum, prior, out, dbg->rec);
+    else launch_pdl(normals_finish_kernel<false>, blocks, NK_THREADS, 0, h->stream, hdr, pts, qlist, qcount, cum, prior, out, nullptr);
     h->launches++;
   } else if (knn == 20) launch_pdl(normals_kernel<20, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
   else if (knn == 10) launch_pdl(normals_kernel<10, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
@@ -954,7 +996,10 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
     fprintf(stderr, "[b2s normals] indexed %d queries %d fallback %d cell %.3f dims %dx%dx%d\n", gh.n, flags ? hq[1] : gh.n, hq[0], gh.cell,
             gh.dims[0], gh.dims[1], gh.dims[2]);
   }
-  launch_pdl(normals_phase2_kernel, 4 * device_sms(), NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, queue, qn, prior, out);
+  if (dbg) launch_pdl(normals_phase2_kernel<true>, 4 * device_sms(), NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, queue, qn, prior, out,
+                      dbg->rec);
+  else launch_pdl(normals_phase2_kernel<false>, 4 * device_sms(), NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, queue, qn, prior, out,
+                  nullptr);
   h->launches += 3;
   c->has_normals = true;
   B2S_CUDA(cudaGetLastError());

@@ -25,6 +25,7 @@ import sys
 import numpy as np
 import pytest
 
+import normals_checks as NC
 from oracle import oracle as O
 from open3d_slam_b200 import engine as E
 from open3d_slam_b200 import synth
@@ -385,11 +386,11 @@ def test_icp_phase2_on_every_cta(engine_factory, csize, n, ctas):
 # ----------------------------------------------------------------------------------------------------------------------
 # normals
 # ----------------------------------------------------------------------------------------------------------------------
-def assert_normals_match(got, ref):
-    dots = (got * ref).sum(axis=1)
-    assert np.abs(np.linalg.norm(got, axis=1) - 1.0).max() < 1e-12
-    assert (dots > 1.0 - 1e-10).mean() > 0.999, (dots < 1.0 - 1e-10).sum()
-    assert dots.min() > 1.0 - 1e-6, dots.min()
+def assert_normals_match(got, ref, xyz, knn, radius, queries=None):
+    """per point, within the gap-aware bound of tests/normals_checks.py (the two sides sum the cumulants in different orders); xyz is
+    the cloud the neighbours come from, queries the rows of xyz that got / ref belong to (default: all)"""
+    worst = NC.assert_normals_close(got, ref, xyz, knn, radius, queries)
+    print(f"normals: worst {worst:.3g} of the gap-aware bound")
 
 
 def _scan_voxels(eng):
@@ -410,7 +411,7 @@ def test_normals_knn_edges(engine_factory, knn, cloud):
     L.check(L.lib().b2s_estimate_normals(eng._h, cl._c, knn, C.c_double(radius)))
     _x, got = cl.download()
     assert np.array_equal(_x, xyz)
-    assert_normals_match(got, O.estimate_normals(xyz, knn, radius))
+    assert_normals_match(got, O.estimate_normals(xyz, knn, radius), xyz, knn, radius)
 
 
 def test_normals_knn_33_is_refused(engine_factory):
@@ -431,12 +432,16 @@ def _process_scan_matches(engine_factory, raw, p):
     (mx, mn), (ax, an) = O.process_scan(raw.astype(np.float64), _oracle_cropper(p.mapBuilder.cropper), _oracle_cropper(p.scanProcessing.cropper),
                                         p.scanProcessing.voxelSize, p.icp.knn, p.icp.maxDistanceKnn, p.scanProcessing.downSamplingRatio, p.seed)
     gx, gn = ps.merge_.download()
+    # the voxel cloud the normals were estimated on (merge_ is its selected subset), in the device's order: the map builder's cropper
+    # in the sensor frame, then the voxel down-sample; the oracle runs on that same cloud (equal d2 go to the lower index)
+    t0, _ = E.voxelize(eng, E.crop(eng, eng.cloud(raw), p.mapBuilder.cropper.to_c(center=(0.0, 0.0, 0.0))), p.scanProcessing.voxelSize).download()
+    idx = NC.rows_in(gx, t0)
     hx, _ = ps.match_.download()
     from scipy.spatial import cKDTree
     assert len(gx) == len(mx) and len(hx) == len(ax)
     d, j = cKDTree(mx).query(gx)
     assert d.max() == 0.0 and len(np.unique(j)) == len(mx)      # identical point sets (bit-exact voxel means)
-    assert_normals_match(gn, mn[j])
+    assert_normals_match(gn, O.estimate_normals(t0, p.icp.knn, p.icp.maxDistanceKnn)[idx], t0, p.icp.knn, p.icp.maxDistanceKnn, idx)
     d, j = cKDTree(ax).query(hx)
     assert d.max() == 0.0 and len(np.unique(j)) == len(ax)
 
@@ -490,7 +495,7 @@ def test_normals_select_exits_and_coarse_grid(engine_factory):
     L.check(L.lib().b2s_estimate_normals(eng._h, cl._c, 10, C.c_double(1.0)))
     _x, got = cl.download()
     nrm = O.estimate_normals(xyz, 10, 1.0)
-    assert_normals_match(got, nrm)
+    assert_normals_match(got, nrm, xyz, 10, 1.0)
     # ICP against the two-patch target (its grid coarsens as well)
     rng = np.random.default_rng(3)
     src = xyz[rng.integers(0, len(xyz) // 2, 2500)] + 0.005 * rng.standard_normal((2500, 3))
@@ -544,7 +549,7 @@ def test_wide_grid_switch_voxel_and_normals(engine_factory, n):
     cl = eng.cloud(xyz)
     L.check(L.lib().b2s_estimate_normals(eng._h, cl._c, 10, C.c_double(0.5)))
     _x, got = cl.download()
-    assert_normals_match(got, O.estimate_normals(xyz, 10, 0.5))
+    assert_normals_match(got, O.estimate_normals(xyz, 10, 0.5), xyz, 10, 0.5)
 
 
 def test_results_independent_of_grid_size(tmp_path):
@@ -558,13 +563,22 @@ def test_results_independent_of_grid_size(tmp_path):
         run_child(["ops", str(out)], env)
         runs[name] = dict(np.load(out))
     base = runs.pop("default")
+    # the clouds the three normal estimations of run_ops take their neighbours from, and their knn / radius
+    p = E.MapperParameters(seed=9)
+    p.scanProcessing.downSamplingRatio = 0.5
+    sc = p.mapBuilder.cropper
+    raw = synth.lidar_scan(synth.Scene(), synth.loop_trajectory(8)[0], seed=70).astype(np.float64)
+    t0, _ = O.voxel_down_sample(O.crop(O.cropper(sc.cropperName, sc.croppingMinRadius, sc.croppingMaxRadius, sc.croppingMinZ,
+                                               sc.croppingMaxZ), raw)[0], p.scanProcessing.voxelSize)
+    nbh = {"normals": (base["normals_xyz"], 20, 3.0, None), "merge_nrm": (t0, p.icp.knn, p.icp.maxDistanceKnn, NC.rows_in(base["merge_xyz"], t0)),
+           "match_nrm": (t0, p.icp.knn, p.icp.maxDistanceKnn, NC.rows_in(base["match_xyz"], t0))}
     for name, got in runs.items():
         assert set(got) == set(base)
         for k in ("crop", "voxel", "normals_xyz", "merge_xyz", "match_xyz", "carved"):
             assert got[k].shape == base[k].shape and np.array_equal(got[k], base[k]), f"{name}: {k} differs from the default grid"
         for k in ("normals", "merge_nrm", "match_nrm"):
             print(f"{name}: {k} max |difference| {np.abs(got[k] - base[k]).max():.3g}")
-            assert_normals_match(got[k], base[k])
+            assert_normals_match(got[k], base[k], *nbh[k])
         for k in ("reg", "step1", "step2", "step3"):
             assert np.array_equal(got[k][-2:], base[k][-2:]), f"{name}: {k} iterations / correspondences differ"
             assert np.abs(got[k][:-2] - base[k][:-2]).max() < 1e-10, f"{name}: {k} differs"

@@ -12,6 +12,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import normals_checks as NC
 from oracle import oracle as O
 from open3d_slam_b200 import engine as E
 from open3d_slam_b200 import synth
@@ -263,11 +264,10 @@ def test_estimate_normals(engine_factory, knn, radius):
     reg.estimateNormalsOrCovariancesIfNeeded(vx)
     _x, got = vx.download()
     ref = O.estimate_normals(xyz, knn, radius)
-    dots = (got * ref).sum(axis=1)
-    # same neighbour sets, same covariance arithmetic: agreement far below the 1e-6 rad of SURVEY 8c test 4
-    assert np.abs(np.linalg.norm(got, axis=1) - 1.0).max() < 1e-12
-    assert (dots > 1.0 - 1e-10).mean() > 0.999
-    assert dots.min() > 1.0 - 1e-6
+    # same neighbour sets, same covariance arithmetic, the cumulants summed in another order: per point within the gap-aware bound
+    # of tests/normals_checks.py (far below the 1e-6 rad of SURVEY 8c test 4 wherever the eigenproblem is well conditioned)
+    worst = NC.assert_normals_close(got, ref, xyz, knn, radius)
+    print(f"normals knn {knn} r {radius}: worst {worst:.3g} of the gap-aware bound")
 
 
 def test_normals_degenerate_few_neighbours(engine_factory):
