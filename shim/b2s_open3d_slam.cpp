@@ -499,6 +499,45 @@ void computeOdometryConstraintsB200(const std::vector<const SubmapB200*>& submap
   }
 }
 
+void globalOptimizationB200(b2s_handle* h, open3d::pipelines::registration::PoseGraph* poseGraph, const GlobalOptimizationParameters& p) {
+  auto& nodes = poseGraph->nodes_;
+  auto& edges = poseGraph->edges_;
+  if (nodes.empty()) return;   // nothing to optimise (b2s_global_optimization needs a node)
+  b2s_global_optimization_params prm;
+  b2s_default_global_optimization_params(&prm);   // [O3D] GlobalOptimizationConvergenceCriteria defaults
+  prm.max_correspondence_distance = p.maxCorrespondenceDistance_;
+  prm.edge_prune_threshold = p.edgePruneThreshold_;
+  prm.preference_loop_closure = p.loopClosurePreference_;
+  prm.reference_node = p.referenceNode_;
+  std::vector<double> poses(16 * nodes.size());
+  for (size_t n = 0; n < nodes.size(); ++n)
+    for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) poses[16 * n + 4 * i + j] = nodes[n].pose_(i, j);
+  std::vector<b2s_pose_graph_edge> in(edges.size());
+  for (size_t e = 0; e < edges.size(); ++e) {
+    in[e].source = edges[e].source_node_id_;
+    in[e].target = edges[e].target_node_id_;
+    in[e].uncertain = edges[e].uncertain_ ? 1 : 0;
+    in[e].reserved_ = 0;
+    for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) in[e].T[4 * i + j] = edges[e].transformation_(i, j);
+    for (int i = 0; i < 6; i++) for (int j = 0; j < 6; j++) in[e].information[6 * i + j] = edges[e].information_(i, j);
+  }
+  std::vector<int32_t> kept(edges.size());
+  std::vector<double> confidence(edges.size());
+  b2s_global_optimization_stats stats[2];
+  const int32_t rc = b2s_global_optimization(h, (int32_t)nodes.size(), poses.data(), (int32_t)edges.size(), in.data(), &prm, kept.data(),
+                                             confidence.data(), stats);
+  if (rc != B2S_OK) b2sThrow(rc);
+  if (edges.empty() || !stats[0].valid) return;
+  for (size_t n = 0; n < nodes.size(); ++n)
+    for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) nodes[n].pose_(i, j) = poses[16 * n + 4 * i + j];
+  std::vector<open3d::pipelines::registration::PoseGraphEdge> out;
+  for (size_t e = 0; e < edges.size(); ++e) {
+    edges[e].confidence_ = confidence[e];
+    if (kept[e]) out.push_back(edges[e]);
+  }
+  edges.swap(out);
+}
+
 namespace {
 std::vector<const b2s_submap*> assemblyInputs(const std::vector<const SubmapB200*>& submaps, b2s_handle** h) {
   std::vector<const b2s_submap*> sms;

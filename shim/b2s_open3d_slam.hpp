@@ -17,6 +17,7 @@
 #include <mutex>
 #include "b2s.h"
 #include "open3d/pipelines/registration/Feature.h"
+#include "open3d/pipelines/registration/PoseGraph.h"
 
 namespace o3d_slam {
 
@@ -162,6 +163,13 @@ PointCloud getAssembledMapPointCloudB200(const std::vector<const SubmapB200*>& s
 // assembleColoredPointCloud (ros/open3d_slam_ros/src/helpers_ros.cpp:51-70) + voxelize(voxelSize) as publishMaps runs it with
 // submapVoxelSize_: points_ and colors_ (submap j in Color::getColor(j % 11 + 2)), no normals.  One b2s_assemble_colored_map call.
 PointCloud assembleColoredPointCloudB200(const std::vector<const SubmapB200*>& submaps, double voxelSize);
+
+// OptimizationProblem::solve (src/OptimizationProblem.cpp:25-44): in place of GlobalOptimization(poseGraph_, LevenbergMarquardt, criteria,
+// option) at :40, with option from params_.globalOptimization_ and [O3D]'s default GlobalOptimizationConvergenceCriteria.  One
+// b2s_global_optimization call on h (any handle: the solve touches no submap; the mapping thread's, or b2sThreadHandle on the
+// loop-closure worker).  Like [O3D]: the node poses are optimised in place and edges_ becomes the kept edges with the confidences the
+// solve ended with; a graph that fails validation (not connected over all edges or over the certain ones) is left as it is.
+void globalOptimizationB200(b2s_handle* h, open3d::pipelines::registration::PoseGraph* poseGraph, const GlobalOptimizationParameters& p);
 
 class ScanToMapIcpB200 : public ScanToMapRegistration {
  public:

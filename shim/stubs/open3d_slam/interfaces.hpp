@@ -4,6 +4,7 @@
 //   ScanToMapRegistration      include/open3d_slam/ScanToMapRegistration.hpp:24-38
 //   parameter structs          include/open3d_slam/Parameters.hpp:37,51-98,118-122,148-153,172
 //   Constraint                 include/open3d_slam/Constraint.hpp:14-20
+//   GlobalOptimizationParameters include/open3d_slam/Parameters.hpp:138-143
 // In a real build, include the reference's own headers instead (INTEGRATION.md).
 #pragma once
 #include <Eigen/Dense>
@@ -32,6 +33,8 @@ struct PlaceRecognitionParameters { double normalEstimationRadius_ = 1.0, featur
   double maxIcpCorrespondenceDistance_ = 0.3, minRefinementFitness_ = 0.7; };   // Parameters.hpp:118-131
 struct MapperParameters { ScanToMapRegistrationParameters scanMatcher_; ScanProcessingParameters scanProcessing_; MapBuilderParameters mapBuilder_; MapBuilderParameters denseMapBuilder_;
   PlaceRecognitionParameters placeRecognition_; bool isRefineOdometryConstraintsBetweenSubmaps_ = false; };
+struct GlobalOptimizationParameters { double maxCorrespondenceDistance_ = 10.0, loopClosurePreference_ = 2.0, edgePruneThreshold_ = 0.2;
+  int referenceNode_ = 0; };   // Parameters.hpp:138-143
 struct Constraint { Transform sourceToTarget_ = Transform::Identity(); size_t sourceSubmapIdx_ = 0, targetSubmapIdx_ = 0;
   Eigen::Matrix6d informationMatrix_ = Eigen::Matrix6d::Identity(); bool isInformationMatrixValid_ = false, isOdometryConstraint_ = false; };
 using Constraints = std::vector<Constraint>;
