@@ -361,6 +361,10 @@ int32_t b2s_submap_set_merge_scans(b2s_handle* h, b2s_submap* sm, int32_t on);
  * Debug aid: header {origin, cell}, {dims, ncell, n}, cell starts and original indices of the NN index the last registration built. */
 int32_t b2s_debug_nn_index(b2s_handle* h, double origin_cell[4], int32_t dims_n[5], int32_t* cell_start, size_t cap_cells, int32_t* orig,
                            size_t cap_pts);
+/* Debug aid: the submap's bounding box {min x, y, z, max x, y, z} (it holds every live map slot, maybe more; the scan-to-map index takes
+ * its grid box from it).  The empty map gives min = +inf, max = -inf.  B2S_GRID_BBOX_PASS=1 in the environment makes that index measure
+ * its grid box with a pass over the map instead (read once per process). */
+int32_t b2s_debug_submap_bbox(b2s_handle* h, const b2s_submap* sm, double box[6]);
 
 /* ---- device-resident LidarOdometry (src/Odometry.cpp:19-110) and the combined per-scan step of SlamWrapper: odometry, then
  *      Mapper::addRangeMeasurement with the prediction read from the odometry's TransformInterpolationBuffer on the device.

@@ -172,7 +172,7 @@ SYMBOLS = [
     "b2s_default_global_optimization_params", "b2s_global_optimization", "b2s_cloud_transform_inplace",
     "b2s_submap_set_initial_map", "b2s_submap_set_initial_transform", "b2s_submap_set_merge_scans", "b2s_debug_nn_index",
     "b2s_assemble_map", "b2s_assemble_colored_map", "b2s_debug_pose_graph_solve", "b2s_debug_pose_graph_linearize",
-    "b2s_debug_estimate_normals",
+    "b2s_debug_estimate_normals", "b2s_debug_submap_bbox",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 ASSEMBLY_MAX_SUBMAPS = 65535             # B2S_ASSEMBLY_MAX_SUBMAPS

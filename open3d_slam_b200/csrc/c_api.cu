@@ -846,6 +846,8 @@ int32_t b2s_submap_create(b2s_handle* h, size_t capacity_points, b2s_submap** ou
     B2S_TRY(pose_to_device(h, I, sm->pose.as<double>() + 5 * 16));
     B2S_TRY(sm->mstate.ensure(MS_WORDS * 4, h->stream));
     B2S_CUDA(cudaMemsetAsync(sm->mstate.p, 0, MS_WORDS * 4, h->stream));
+    B2S_TRY(sm->bbox.ensure(6 * 8, h->stream));
+    B2S_TRY(box_reset(h, sm->bbox.as<unsigned long long>()));   // the empty map
     b2s_default_mapper_options(&sm->opts);
     return B2S_OK;
   });
@@ -1052,7 +1054,7 @@ int32_t b2s::register_to_submap_async(b2s_handle* h, const b2s_cloud* scan, cons
   if (tile_patch_usable(sm, patch))   // frozen map: the patch from the tiles the cropper touches (K-patch, grid_index.cu)
     B2S_TRY(tile_patch_build(h, const_cast<b2s_submap*>(sm), patch, nn_cell(h, h->cfg.icp.max_corr_dist), &h->grid_a));
   else
-    B2S_TRY(grid_build(h, &h->grid_a, map, nn_cell(h, h->cfg.icp.max_corr_dist), &patch));
+    B2S_TRY(grid_build(h, &h->grid_a, map, nn_cell(h, h->cfg.icp.max_corr_dist), &patch, nullptr, sm->bbox.as<unsigned long long>(), &patch));
   B2S_TRY(h->work_xyz.ensure(icp_work_bytes(scan->n_max), h->stream));
   B2S_TRY(h->problems.ensure(sizeof(IcpProblem), h->stream));
   IcpProblem P;
@@ -1466,6 +1468,16 @@ int32_t b2s_debug_pose_graph_linearize(b2s_handle* h, int32_t n_nodes, const dou
                 "edge %d: node ids (%d, %d) outside [0, %d)", (int)e, (int)edges[e].source, (int)edges[e].target, (int)n_nodes);
   LOCK(h);
   return op_debug_pose_graph_linearize(h, n_nodes, poses, n_edges, edges, *p, conf_in, conf_out, H_out, b_out, rec_out);
+}
+
+int32_t b2s_debug_submap_bbox(b2s_handle* h, const b2s_submap* sm, double box[6]) {
+  B2S_REQUIRE(h && sm && box, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(sm->h == h, B2S_E_INVALID, "the submap belongs to another handle");
+  LOCK(h);
+  unsigned long long w[6];
+  const int32_t rc = read_back(h, {{w, sm->bbox.p, sizeof(w)}});
+  for (int d = 0; d < 6; d++) box[d] = ord_decode(w[d]);
+  return rc;
 }
 
 // ---- the assembled map (Mapper.cpp:183-208, helpers_ros.cpp:51-70, SlamWrapperRos.cpp:222-244) ----------------------------------------

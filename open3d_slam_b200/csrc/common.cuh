@@ -212,6 +212,10 @@ struct b2s_submap {
   b2s::DevBuf dups;          // int32 [2][FUSE_DUP_CAP] voxels holding more than one map point (ping-pong)
   b2s::DevBuf wflag;         // int32 [capacity + 1] 1 = the slot is on K3's renormalisation worklist
   b2s::DevBuf wlist;         // int32 [2][capacity + 1] the worklist (ping-pong): slots whose normal may not be a fixed point yet
+  // uint64 [6] bounding box of the live map slots, ord_encode'd min xyz / max xyz like GridIndex::bbox.  It may hold more than the live
+  // slots, never less: K2 folds in every position it writes into a slot, fuse_rehash recomputes it exactly.  The map-index build takes
+  // its grid box from it (grid_build) instead of reading the whole map for one.
+  b2s::DevBuf bbox;
   size_t vcap = 0;
   size_t stage_cap = 0;
   // Mapper / SubmapCollection wiring of the device chain (b2s_mapper_options) and its device-side state words (MS_*)
@@ -401,8 +405,14 @@ struct CropDev {      // cropper passed by value to kernels; centre may come fro
   const double* pose_dev;   // if non-null the centre is (pose[3], pose[7], pose[11])
 };
 CropDev make_crop(const b2s_cropper* c, const double* pose_dev = nullptr);
-// orig (optional): per point of cloud the original index the grid stores (default: the point's own index)
-int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch, const int32_t* orig = nullptr);
+// orig (optional): per point of cloud the original index the grid stores (default: the point's own index).
+// map_box, map_crop (optional, together): a box holding every point of cloud (b2s_submap::bbox) and the cropper of the patch.  The grid
+// box is then map_box cut to map_crop's axis-aligned box, with no pass over the cloud for it.  B2S_GRID_BBOX_PASS=1 ignores them (A/B
+// switch and test reference).
+int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch, const int32_t* orig = nullptr,
+                   const unsigned long long* map_box = nullptr, const CropDev* map_crop = nullptr);
+// sets the six words of an ord_encode'd box (min xyz, max xyz) to the empty box
+int32_t box_reset(b2s_handle* h, unsigned long long* box);
 // static map patch (grid_index.cu): true when sm's merge is off, the cropper is bounded and B2S_PATCH_FULL is not set
 bool tile_patch_usable(const b2s_submap* sm, const CropDev& crop);
 // builds the tile table if it is not valid, gathers the tiles the cropper touches, and builds g over the gathered points that pass
@@ -656,6 +666,27 @@ __device__ __forceinline__ double warp_max(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// Folds every thread's box (mn / mx, +-INFINITY when empty) into the ord_encode'd words box[0..5] (min xyz, max xyz): reduced over the
+// block, then six atomics.  Every thread of the block must call it (it synchronises the block); THREADS = blockDim.x, a multiple of 32.
+template <int THREADS>
+__device__ __forceinline__ void box_fold_block(double (&mn)[3], double (&mx)[3], unsigned long long* box) {
+  constexpr int nwarps = THREADS / 32;
+  __shared__ double s[6][nwarps];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int d = 0; d < 3; d++) { mn[d] = warp_min(mn[d]); mx[d] = warp_max(mx[d]); }
+  if (lane == 0) { for (int d = 0; d < 3; d++) { s[d][warp] = mn[d]; s[3 + d][warp] = mx[d]; } }
+  __syncthreads();
+  if (threadIdx.x < 6) {
+    const int d = threadIdx.x;
+    double v = s[d][0];
+#pragma unroll 1
+    for (int w = 1; w < nwarps; w++) v = d < 3 ? fmin(v, s[d][w]) : fmax(v, s[d][w]);
+    if (d < 3) { if (v < INFINITY) atomicMin(&box[d], ord_encode(v)); }
+    else if (v > -INFINITY) atomicMax(&box[d], ord_encode(v));
+  }
 }
 
 // [O3D] TransformVector6dToMatrix4d: R = Rz(x2) Ry(x1) Rx(x0), t = x[3..5] (the ICP update and the pose-graph LM step)

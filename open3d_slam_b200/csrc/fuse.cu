@@ -64,6 +64,17 @@ __device__ __forceinline__ long long fv_find_or_insert(unsigned long long* keys,
   return -1;
 }
 
+// K2 writes a position into a map slot: the submap's box takes it.  An atomic only when the box grows, which it stops doing once the
+// map covers the place (a mean can still leave its members' box by the rounding of the sum and the division); a stale read of the
+// box only costs an atomic that changes nothing.
+__device__ __forceinline__ void box_fold_point(unsigned long long* box, const double* p) {
+  for (int d = 0; d < 3; d++) {
+    const unsigned long long e = ord_encode(p[d]);
+    if (e < box[d]) atomicMin(&box[d], e);
+    if (e > box[3 + d]) atomicMax(&box[3 + d], e);
+  }
+}
+
 struct FuseView {
   double* mxyz; double* mnrm; int32_t* vnext; int32_t* pstamp;
   const double* sxyz; const double* snrm; int32_t* snext; const int32_t* sin;
@@ -129,7 +140,7 @@ __global__ void __launch_bounds__(FZ_THREADS) fuse_stage_kernel(const double* __
 __global__ void __launch_bounds__(128) fuse_merge_kernel(const int32_t* __restrict__ gate, const int32_t* __restrict__ d_nscan, CropDev crop,
                                                          FuseView v, const unsigned long long* __restrict__ vkeys, double inv, int32_t* vhead,
                                                          int32_t* vstamp, const int32_t* __restrict__ touched, int32_t* dups, int32_t* d_nmap,
-                                                         size_t capacity, Worklist wl, int32_t* ms, uint32_t* status) {
+                                                         size_t capacity, Worklist wl, int32_t* ms, uint32_t* status, unsigned long long* box) {
   pdl_wait();
   if (!((gate == nullptr || *gate != 0) && *d_nscan > 0)) return;
   const int cur = ms[MS_STAMP] + 1;
@@ -197,6 +208,7 @@ __global__ void __launch_bounds__(128) fuse_merge_kernel(const int32_t* __restri
           if ((size_t)sl >= capacity) { atomicOr(status, ST_CAPACITY); atomicSub(d_nmap, 1); }
           else {
             for (int k = 0; k < 3; k++) { v.mxyz[3 * (size_t)sl + k] = v.sxyz[3 * (size_t)j + k]; v.mnrm[3 * (size_t)sl + k] = v.snrm[3 * (size_t)j + k]; }
+            box_fold_point(box, v.sxyz + 3 * (size_t)j);
             v.pstamp[sl] = cur;
             v.vnext[sl] = newhead; newhead = sl; survivors++;
             fv_worklist_join(wl, ms, sl);
@@ -226,6 +238,7 @@ __global__ void __launch_bounds__(128) fuse_merge_kernel(const int32_t* __restri
       fv_worklist_join(wl, ms, dest);   // also how K3 finds a mean marked below
       unsigned long long key;
       const double* m = v.mxyz + 3 * (size_t)dest;
+      box_fold_point(box, m);
       if (voxel_key_of(m[0], m[1], m[2], inv, inv, inv, &key) && key == vkeys[slot]) {
         v.pstamp[dest] = cur;
         v.vnext[dest] = newhead; newhead = dest; survivors++;
@@ -336,9 +349,10 @@ __global__ void __launch_bounds__(FZ_THREADS) fuse_renorm_commit_kernel(const in
 
 // ---- (re)build of the voxel hash from the map cloud --------------------------------------------------------------------------
 __global__ void fuse_table_clear_kernel(unsigned long long* vkeys, int32_t* vhead, int32_t* vstamp, size_t vcap, int32_t* __restrict__ wflag,
-                                        size_t wcap, int32_t* ms, const int32_t* __restrict__ enable) {
+                                        size_t wcap, int32_t* ms, const int32_t* __restrict__ enable, unsigned long long* box) {
   pdl_wait();
   if (enable != nullptr && *enable == 0) return;
+  if (blockIdx.x == 0 && threadIdx.x < 6) box[threadIdx.x] = threadIdx.x < 3 ? ord_encode(INFINITY) : ord_encode(-INFINITY);   // the link pass refills it
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < vcap; i += (size_t)gridDim.x * blockDim.x) { vkeys[i] = VOXEL_KEY_EMPTY; vhead[i] = -1; vstamp[i] = 0; }
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < wcap; i += (size_t)gridDim.x * blockDim.x) wflag[i] = 0;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -346,23 +360,32 @@ __global__ void fuse_table_clear_kernel(unsigned long long* vkeys, int32_t* vhea
     ms[MS_WSEL] = 0; ms[MS_NW] = 0; ms[MS_NW + 1] = 0;
   }
 }
-// relinks every map point and puts every slot on the renormalisation worklist (the normals may have been rewritten)
+// relinks every map point, puts every slot on the renormalisation worklist (the normals may have been rewritten) and measures the
+// submap's box
 __global__ void __launch_bounds__(FZ_THREADS) fuse_table_link_kernel(const double* __restrict__ mxyz, const int32_t* __restrict__ d_nmap, double inv,
                                                                      unsigned long long* vkeys, int32_t* vhead, size_t vmask, int32_t* __restrict__ vnext,
                                                                      int32_t* __restrict__ pstamp, int32_t* __restrict__ wflag, int32_t* __restrict__ wlist,
-                                                                     int32_t* ms, uint32_t* status, const int32_t* __restrict__ enable) {
+                                                                     int32_t* ms, uint32_t* status, const int32_t* __restrict__ enable,
+                                                                     unsigned long long* box) {
   pdl_wait();
   if (enable != nullptr && *enable == 0) return;
   const int n = *d_nmap;
   if (blockIdx.x == 0 && threadIdx.x == 0) ms[MS_NW] = n;   // half 0 (the clear kernel selected it)
+  double mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     vnext[i] = -1; pstamp[i] = 0;
     wflag[i] = 1; wlist[i] = i;
+    const double x = mxyz[3 * (size_t)i], y = mxyz[3 * (size_t)i + 1], z = mxyz[3 * (size_t)i + 2];
+    if (x == x && y == y && z == z) {   // every live slot, the far ones too
+      mn[0] = fmin(mn[0], x); mn[1] = fmin(mn[1], y); mn[2] = fmin(mn[2], z);
+      mx[0] = fmax(mx[0], x); mx[1] = fmax(mx[1], y); mx[2] = fmax(mx[2], z);
+    }
     unsigned long long key;
-    if (!voxel_key_of(mxyz[3 * (size_t)i], mxyz[3 * (size_t)i + 1], mxyz[3 * (size_t)i + 2], inv, inv, inv, &key)) continue;   // tombstones / far points stay unlinked
+    if (!voxel_key_of(x, y, z, inv, inv, inv, &key)) continue;   // tombstones / far points stay unlinked
     const long long s = fv_find_or_insert(vkeys, vmask, key, ms, status);
     if (s >= 0) vnext[i] = atomicExch(&vhead[s], i);
   }
+  box_fold_block<FZ_THREADS>(mn, mx, box);
 }
 // voxels whose chain holds more than one point, reported once (by the chain head)
 __global__ void __launch_bounds__(FZ_THREADS) fuse_table_dups_kernel(const unsigned long long* __restrict__ vkeys, const int32_t* __restrict__ vhead,
@@ -393,7 +416,8 @@ int32_t fuse_reserve(b2s_handle* h, b2s_submap* sm) {
   B2S_TRY(sm->wlist.ensure(2 * (sm->capacity + 1) * 4, h->stream));
   sm->vcap = vcap;
   launch_pdl(fuse_table_clear_kernel, 4 * device_sms(), 256, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vstamp.as<int32_t>(), vcap,
-                                                         sm->wflag.as<int32_t>(), sm->capacity + 1, sm->mstate.as<int32_t>(), nullptr);
+                                                         sm->wflag.as<int32_t>(), sm->capacity + 1, sm->mstate.as<int32_t>(), nullptr,
+                                                         sm->bbox.as<unsigned long long>());
   h->launches++;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;
@@ -406,12 +430,12 @@ int32_t fuse_rehash(b2s_handle* h, b2s_submap* sm, const int32_t* enable_dev) {
   int32_t* ms = sm->mstate.as<int32_t>();
   ProfScope prof(h, PK_FUSE);
   launch_pdl(fuse_table_clear_kernel, 4 * device_sms(), 256, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vstamp.as<int32_t>(), sm->vcap,
-                                                         sm->wflag.as<int32_t>(), sm->capacity + 1, ms, enable_dev);
+                                                         sm->wflag.as<int32_t>(), sm->capacity + 1, ms, enable_dev, sm->bbox.as<unsigned long long>());
   launch_pdl(fuse_table_link_kernel, grid_for(n_max, FZ_THREADS), FZ_THREADS, 0, h->stream, map->xyz.as<double>(), map->dn.as<int32_t>(),
                                                                                    1.0 / h->cfg.map_voxel_size, sm->vkeys.as<unsigned long long>(),
                                                                                    sm->vhead.as<int32_t>(), sm->vcap - 1, sm->vnext.as<int32_t>(),
                                                                                    sm->pstamp.as<int32_t>(), sm->wflag.as<int32_t>(), sm->wlist.as<int32_t>(),
-                                                                                   ms, h->status.as<uint32_t>(), enable_dev);
+                                                                                   ms, h->status.as<uint32_t>(), enable_dev, sm->bbox.as<unsigned long long>());
   launch_pdl(fuse_table_dups_kernel, 4 * device_sms(), FZ_THREADS, 0, h->stream, sm->vkeys.as<unsigned long long>(), sm->vhead.as<int32_t>(), sm->vcap,
                                                                sm->vnext.as<int32_t>(), sm->dups.as<int32_t>(), ms, h->status.as<uint32_t>(), enable_dev);
   h->launches += 3;
@@ -491,7 +515,8 @@ int32_t op_submap_insert(b2s_handle* h, b2s_submap* sm, const b2s_cloud* scan, c
     launch_pdl(fuse_merge_kernel, grid_for(m_max + 4096, 128), 128, 0, h->stream, gate_dev, scan->dn.as<int32_t>(), crop, fv,
                                                                          sm->vkeys.as<unsigned long long>(), inv, sm->vhead.as<int32_t>(),
                                                                          sm->vstamp.as<int32_t>(), sm->touched.as<int32_t>(), sm->dups.as<int32_t>(),
-                                                                         map->dn.as<int32_t>(), sm->capacity, wl, ms, h->status.as<uint32_t>());
+                                                                         map->dn.as<int32_t>(), sm->capacity, wl, ms, h->status.as<uint32_t>(),
+                                                                         sm->bbox.as<unsigned long long>());
     launch_pdl(fuse_renorm_commit_kernel, grid_for(k3_items, FZ_THREADS), FZ_THREADS, 0, h->stream, gate_dev, scan->dn.as<int32_t>(), crop, map->xyz.as<double>(),
                                                                                          map->nrm.as<double>(), sm->pstamp.as<int32_t>(),
                                                                                          map->dn.as<int32_t>(), inv, sm->vkeys.as<unsigned long long>(),

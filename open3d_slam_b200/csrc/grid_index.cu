@@ -9,7 +9,8 @@
 // neighbouring cells along x is ONE contiguous slot range, so a 3x3x3 neighbourhood is 9 ranges.
 // Points outside the grid box are clamped into the border cells, which the search treats as semi-infinite.
 //
-// Build = bbox reduce -> header (1 thread) -> count (atomics, keeps the rank) -> look-back scan -> scatter.
+// Build = bbox reduce -> header (1 thread) -> count (atomics, keeps the rank) -> look-back scan -> scatter.  The map index of a
+// registration against a submap has no bbox reduce: its header comes from the submap's box (grid_header_box_kernel).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -36,18 +37,7 @@ __device__ __forceinline__ void grid_bbox_body(const double* __restrict__ xyz, c
     mn[0] = fmin(mn[0], x); mn[1] = fmin(mn[1], y); mn[2] = fmin(mn[2], z);
     mx[0] = fmax(mx[0], x); mx[1] = fmax(mx[1], y); mx[2] = fmax(mx[2], z);
   }
-  __shared__ double s[6][GB_THREADS / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int d = 0; d < 3; d++) { mn[d] = warp_min(mn[d]); mx[d] = warp_max(mx[d]); }
-  if (lane == 0) { for (int d = 0; d < 3; d++) { s[d][warp] = mn[d]; s[3 + d][warp] = mx[d]; } }
-  __syncthreads();
-  if (threadIdx.x < 6) {
-    int d = threadIdx.x;
-    double v = s[d][0];
-    for (int w = 1; w < GB_THREADS / 32; w++) v = d < 3 ? fmin(v, s[d][w]) : fmax(v, s[d][w]);
-    if (d < 3) atomicMin(&bbox[d], ord_encode(v)); else atomicMax(&bbox[d], ord_encode(v));
-  }
+  box_fold_block<GB_THREADS>(mn, mx, bbox);
 }
 
 __global__ void __launch_bounds__(GB_THREADS) grid_bbox_kernel(const double* __restrict__ xyz, const int32_t* __restrict__ d_n,
@@ -56,10 +46,9 @@ __global__ void __launch_bounds__(GB_THREADS) grid_bbox_kernel(const double* __r
   grid_bbox_body(xyz, d_n, crop, use_crop, bbox);
 }
 
-__device__ void grid_header_body(const unsigned long long* bbox, double cell, int cap_cells, GridHeader* hdr) {
-  double mn[3], mx[3];
-  for (int d = 0; d < 3; d++) { mn[d] = ord_decode(bbox[d]); mx[d] = ord_decode(bbox[3 + d]); }
-  if (!(mn[0] <= mx[0])) { for (int d = 0; d < 3; d++) { mn[d] = 0.0; mx[d] = 0.0; } }  // empty set
+// the header of a grid over the box [mn, mx] (an empty box on any axis, or NaN: the empty set)
+__device__ void grid_header_of(double (&mn)[3], double (&mx)[3], double cell, int cap_cells, GridHeader* hdr) {
+  if (!(mn[0] <= mx[0] && mn[1] <= mx[1] && mn[2] <= mx[2])) { for (int d = 0; d < 3; d++) { mn[d] = 0.0; mx[d] = 0.0; } }  // empty set
   int dims[3];
   for (;;) {
     double total = 1.0;
@@ -79,10 +68,26 @@ __device__ void grid_header_body(const unsigned long long* bbox, double cell, in
   hdr->n = 0;
 }
 
+__device__ void grid_header_body(const unsigned long long* bbox, double cell, int cap_cells, GridHeader* hdr) {
+  double mn[3], mx[3];
+  for (int d = 0; d < 3; d++) { mn[d] = ord_decode(bbox[d]); mx[d] = ord_decode(bbox[3 + d]); }
+  grid_header_of(mn, mx, cell, cap_cells, hdr);
+}
+
 __global__ void grid_header_kernel(const unsigned long long* bbox, double cell, int cap_cells, GridHeader* hdr) {
   pdl_wait();
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   grid_header_body(bbox, cell, cap_cells, hdr);
+}
+
+// The axis-aligned box [lo, hi] that holds what crop_within can accept, up to the rounding of crop_within itself (a point a few ulps
+// outside may pass); false when the cropper is not bounded (no box).  The cylinder compares the absolute z.
+__device__ __forceinline__ bool crop_aabb(const CropDev& crop, double* lo, double* hi) {
+  double c[3] = {crop.cx, crop.cy, crop.cz};
+  if (crop.pose_dev) { c[0] = crop.pose_dev[3]; c[1] = crop.pose_dev[7]; c[2] = crop.pose_dev[11]; }
+  for (int d = 0; d < 3; d++) { lo[d] = c[d] - crop.rmax; hi[d] = c[d] + crop.rmax; }
+  if (crop.kind == B2S_CROP_CYLINDER) { lo[2] = crop.zmin; hi[2] = crop.zmax; }
+  return !crop.invert && (crop.kind == B2S_CROP_MAX_RADIUS || crop.kind == B2S_CROP_MINMAX_RADIUS || crop.kind == B2S_CROP_CYLINDER);
 }
 
 __device__ __forceinline__ int grid_cell_of(const GridHeader& g, double x, double y, double z) {
@@ -146,6 +151,20 @@ __global__ void __launch_bounds__(GB_THREADS) grid_scatter_kernel(const double* 
   grid_scatter_body(xyz, d_n, hdr, cell_start, rank, pts, orig);
 }
 
+// ---- map index: the grid box from the submap's box -----------------------------------------------------------------------------
+// The grid box is the submap's box (it holds every live slot) cut to the cropper's box: a superset of the patch, so only the cell
+// geometry differs from the measured box, never the indexed set (a point outside the grid box lands in a border cell, which the search
+// treats as semi-infinite).  No pass over the map: the header comes from twelve words.
+__global__ void grid_header_box_kernel(const unsigned long long* __restrict__ map_box, CropDev crop, double cell, int cap_cells, GridHeader* hdr) {
+  pdl_wait();
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  double mn[3], mx[3], lo[3], hi[3];
+  for (int d = 0; d < 3; d++) { mn[d] = ord_decode(map_box[d]); mx[d] = ord_decode(map_box[3 + d]); }
+  if (crop_aabb(crop, lo, hi))
+    for (int d = 0; d < 3; d++) { mn[d] = fmax(mn[d], lo[d]); mx[d] = fmin(mx[d], hi[d]); }   // a NaN bound keeps the map's
+  grid_header_of(mn, mx, cell, cap_cells, hdr);
+}
+
 // ---- batched build: blockIdx.y = job -------------------------------------------------------------------------------
 struct GridJob {
   const double* xyz; const int32_t* d_n;
@@ -189,6 +208,13 @@ __global__ void __launch_bounds__(GB_THREADS) gridb_scatter_kernel(const GridJob
   grid_scatter_body(j.xyz, j.d_n, j.hdr, j.starts, j.rank, j.pts, nullptr);
 }
 
+int32_t box_reset(b2s_handle* h, unsigned long long* box) {
+  launch_pdl(grid_bbox_init_kernel, 1, 32, 0, h->stream, box);
+  h->launches++;
+  B2S_CUDA(cudaGetLastError());
+  return B2S_OK;
+}
+
 CropDev make_crop(const b2s_cropper* c, const double* pose_dev) {
   CropDev d;
   memset(&d, 0, sizeof(d));
@@ -200,8 +226,13 @@ CropDev make_crop(const b2s_cropper* c, const double* pose_dev) {
   return d;
 }
 
-int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch, const int32_t* orig) {
+int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double cell, const CropDev* patch, const int32_t* orig,
+                   const unsigned long long* map_box, const CropDev* map_crop) {
   B2S_REQUIRE(cell > 0.0, B2S_E_INVALID, "grid_build: cell size must be > 0");
+  // B2S_GRID_BBOX_PASS=1: the map index measures its grid box with a pass over the map, as every other index build does (A/B switch
+  // and test reference; read once per process)
+  static const bool bbox_pass = getenv("B2S_GRID_BBOX_PASS") && atoi(getenv("B2S_GRID_BBOX_PASS")) != 0;
+  const bool from_box = map_box && map_crop && !bbox_pass;
   const size_t n_max = cloud->n_max > 0 ? cloud->n_max : 1;
   // buffers follow the ALLOCATION of the cloud, not its current size: a growing map never re-allocates its index
   // (a cudaMalloc/cudaFree pair is a device-wide synchronisation)
@@ -228,12 +259,18 @@ int32_t grid_build(b2s_handle* h, GridIndex* g, const b2s_cloud* cloud, double c
   const int32_t* d_n = cloud->dn.as<int32_t>();
   GridHeader* hdr = g->hdr.as<GridHeader>();
   ProfScope prof(h, PK_GRID);
-  launch_pdl(grid_bbox_init_kernel, 1, 32, 0, h->stream, g->bbox.as<unsigned long long>());
-  launch_pdl(grid_bbox_kernel, blocks, GB_THREADS, 0, h->stream, cloud->xyz.as<double>(), d_n, cd, use_crop, g->bbox.as<unsigned long long>());
-  launch_pdl(grid_header_kernel, 1, 32, 0, h->stream, g->bbox.as<unsigned long long>(), cell, g->cap_cells, hdr);
+  if (from_box) {
+    launch_pdl(grid_header_box_kernel, 1, 32, 0, h->stream, map_box, *map_crop, cell, g->cap_cells, hdr);
+    h->launches++;
+  } else {
+    launch_pdl(grid_bbox_init_kernel, 1, 32, 0, h->stream, g->bbox.as<unsigned long long>());
+    launch_pdl(grid_bbox_kernel, blocks, GB_THREADS, 0, h->stream, cloud->xyz.as<double>(), d_n, cd, use_crop, g->bbox.as<unsigned long long>());
+    launch_pdl(grid_header_kernel, 1, 32, 0, h->stream, g->bbox.as<unsigned long long>(), cell, g->cap_cells, hdr);
+    h->launches += 3;
+  }
   launch_pdl(grid_zero_kernel, 4 * device_sms(), 256, 0, h->stream, hdr, counts);
   launch_pdl(grid_count_kernel, blocks, GB_THREADS, 0, h->stream, cloud->xyz.as<double>(), d_n, cd, use_crop, hdr, counts, g->rank.as<int32_t>());
-  h->launches += 5;
+  h->launches += 2;
   // scan over ncell (device-known) counts; launch sized for the capacity
   B2S_TRY(scan_exclusive_i32(h, counts, starts, &hdr->ncell, (size_t)g->cap_cells, nullptr));
   launch_pdl(grid_scatter_kernel, blocks, GB_THREADS, 0, h->stream, cloud->xyz.as<double>(), d_n, hdr, starts, g->rank.as<int32_t>(),
@@ -324,8 +361,8 @@ int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* co
 // Per registration: tile_gather_kernel reads the sensor position from the device pose (or the host-given centre), takes the tiles the
 // cropper's box overlaps, grown by TILE_MARGIN tiles on every side (the box is computed in rounded arithmetic, and crop_within accepts a
 // point up to a few ulps outside it), and appends the points of those tiles that pass the unchanged crop_within, each with its map slot.
-// The NN grid is then built over exactly those points with the slot as original index: the same set, bbox, header and original indices
-// as the full path's crop inside the build, at O(points in the touched tiles) instead of O(map).  Why 2 m: a few map voxels, fine enough
+// The NN grid is then built over exactly those points with the slot as original index: the same set, header (both paths take it from
+// the submap's box and the cropper) and original indices as the full path's crop inside the build, at O(points in the touched tiles) instead of O(map).  Why 2 m: a few map voxels, fine enough
 // that the cube of tiles around a 20-30 m cropper holds little beyond the sphere's own box, coarse enough that a site-sized map's table
 // stays within the cell budget.  Launches are sized from the map's bound (grid-stride over the device count): graph-capturable.
 __global__ void tile_zero_kernel(int32_t* n) {
@@ -335,11 +372,8 @@ __global__ void tile_zero_kernel(int32_t* n) {
 
 // the tile box of the cropper: [lo, hi] per axis, clamped to the table; empty when lo > hi on an axis
 __device__ __forceinline__ void tile_box(const GridHeader& g, const CropDev& crop, int* box) {
-  double c[3] = {crop.cx, crop.cy, crop.cz};
-  if (crop.pose_dev) { c[0] = crop.pose_dev[3]; c[1] = crop.pose_dev[7]; c[2] = crop.pose_dev[11]; }
   double lo[3], hi[3];
-  for (int d = 0; d < 3; d++) { lo[d] = c[d] - crop.rmax; hi[d] = c[d] + crop.rmax; }
-  if (crop.kind == B2S_CROP_CYLINDER) { lo[2] = crop.zmin; hi[2] = crop.zmax; }   // crop_within compares the absolute z
+  crop_aabb(crop, lo, hi);   // bounded: tile_patch_usable
   for (int d = 0; d < 3; d++) {
     const double a = fmax(floor((lo[d] - g.origin[d]) * g.inv_cell) - TILE_MARGIN, 0.0);
     const double b = fmin(floor((hi[d] - g.origin[d]) * g.inv_cell) + TILE_MARGIN, (double)(g.dims[d] - 1));
@@ -414,7 +448,7 @@ int32_t tile_patch_build(b2s_handle* h, b2s_submap* sm, const CropDev& crop, dou
                sm->patch_idx.as<int32_t>(), pc->dn.as<int32_t>());
     h->launches += 2;
   }
-  return grid_build(h, g, pc, cell, nullptr, sm->patch_idx.as<int32_t>());
+  return grid_build(h, g, pc, cell, nullptr, sm->patch_idx.as<int32_t>(), sm->bbox.as<unsigned long long>(), &crop);   // the full path's header
 }
 
 }  // namespace b2s
