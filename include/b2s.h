@@ -159,10 +159,10 @@ int32_t b2s_estimate_normals(b2s_handle* h, b2s_cloud* cloud, int32_t knn, doubl
  * kernels decided.  rec_out (n x 10): the nine cumulants sum x, y, z, xx, xy, xz, yy, yz, zz and the neighbour count exactly as the
  * eigen-solver received them; NaN for a point that was not queried.  path_out (n): 1, 2 or 3 = resolved by the block gather at that
  * block radius, 4 = by the block that covers the whole search radius, 5 = by the ring walk after a block held too many candidates,
- * 6 = by the ring walk after the last block could not certify the k-th neighbour; 0 = not queried (or an A/B search variant chosen in
- * the environment).  sel_out (n x 4, nullable): the block gather's selection at the last block it tried -- candidates inside the
- * certified ball (over NS2_CAP = 256: the block went over capacity), the 32-bin d2 histogram bin of the k-th key (-1: at most k
- * candidates, no histogram), that bin's member count, and the ball's squared radius lim2 the histogram spans; NaN where not queried.
+ * 6 = by the ring walk after the last block could not certify the k-th neighbour; 0 = not queried.  sel_out (n x 4, nullable): the
+ * block gather's selection at the last block it tried -- candidates inside the certified ball (over NS2_CAP = 256: the block went over
+ * capacity), the 32-bin d2 histogram bin of the k-th key (-1: at most k candidates, no histogram), that bin's member count, and the
+ * ball's squared radius lim2 the histogram spans; NaN where not queried.
  * The kernels run in their debug instantiations (the production ones compile none of the recording).  Synchronises. */
 int32_t b2s_debug_estimate_normals(b2s_handle* h, b2s_cloud* cloud, int32_t knn, double radius, double cell_hint, const int32_t* flags_host,
                                    int32_t with_prior, double* rec_out, int32_t* path_out, double* sel_out);

@@ -22,8 +22,6 @@ __global__ void f32_to_f64_kernel(const unsigned char* __restrict__ src, size_t 
 
 __global__ void write_i32_kernel(int32_t* p, int32_t v) {
   pdl_wait(); *p = v; }
-__global__ void pad_kernel() {
-  pdl_wait();}   // B2S_PAD_LAUNCHES=n: n empty launches per scan, to measure what a launch costs the chain (tuning aid)
 
 __global__ void empty_check_kernel(const int32_t* a, const int32_t* b, uint32_t* status) {
   pdl_wait();
@@ -161,8 +159,6 @@ int32_t process_scan_impl(b2s_handle* h, const b2s_cloud* raw, b2s_cloud* merge,
   B2S_TRY(op_crop(h, merge, make_crop(&c1), match));
   launch_pdl(empty_check_kernel, 1, 1, 0, h->stream, merge->dn.as<int32_t>(), match->dn.as<int32_t>(), h->status.as<uint32_t>());
   h->launches++;
-  static const int pad = getenv("B2S_PAD_LAUNCHES") ? atoi(getenv("B2S_PAD_LAUNCHES")) : 0;
-  for (int i = 0; i < pad; i++) launch_pdl(pad_kernel, 1, 32, 0, h->stream);
   return B2S_OK;
 }
 

@@ -2,7 +2,7 @@
 // (core/src/CloudRegistration.cpp:49-56) = [O3D] EstimateNormals(KDTreeSearchParamHybrid(radius, knn)) +
 // NormalizeNormals + OrientNormalsTowardsCameraLocation(0,0,0).
 //
-// One WARP per query point, three kernels (default path):
+// One WARP per query point, three kernels:
 //   normals_select2_kernel  gathers the (2R+1)^3 block of grid cells (grid_index.cu) around the query into a per-warp shared-memory
 //                           buffer, R grown until the k-th neighbour provably lies inside the block (ball-within-bounds, like a
 //                           KD-tree), selects the k nearest by counting (32-bin histogram of d2 + exact ranking of the boundary
@@ -12,7 +12,7 @@
 //   normals_phase2_kernel   the few queries the block gather cannot certify (more than NS2_CAP candidates, or a search radius the
 //                           row table cannot cover): ring walk with a sorted k-best list, one entry per lane, shuffle insert.
 // The neighbour SET is the oracle's exactly; the cumulants are summed in butterfly order instead of ascending-distance order, which
-// moves the normal by < 1e-9.  A thread-per-query variant (normals_kernel<K>) is kept behind B2S_NORMALS_RING_LIMIT for comparison.
+// moves the normal by < 1e-9.
 #include "common.cuh"
 
 namespace b2s {
@@ -128,7 +128,7 @@ __device__ void fast_eigen3x3_dev(const double* cov, double* out) {
 }
 
 
-// Post-search part shared by all KMAX: covariance in the reference's neighbour order (ascending (d2, index)) with
+// Post-search part shared by the finish and phase-2 kernels: covariance in the reference's neighbour order (ascending (d2, index)) with
 // the reference's single-pass cumulant formula in explicitly rounded fp64, analytic eigen-solver, normalise, orient.
 // prior (optional): the query's normal before the estimation -- [O3D] EstimateNormals on a cloud that already has normals keeps
 // the prior where the solver returns a zero vector and otherwise flips the new normal when it points against the prior.  The
@@ -164,127 +164,6 @@ __device__ __forceinline__ void finish_normal(const double c_in[9], int kk, doub
     if (rn == 0.0) { nr[0] = 0; nr[1] = 0; nr[2] = 1; }
     else { nr[0] = ref[0] / rn; nr[1] = ref[1] / rn; nr[2] = ref[2] / rn; }
   } else if (dot3d(nr, ref) < 0.0) { nr[0] *= -1.0; nr[1] *= -1.0; nr[2] *= -1.0; }
-}
-
-// One THREAD per query point, queries taken in grid-slot order so that the 32 lanes of a warp sit in the same or
-// in adjacent cells and walk (nearly) the same candidate ranges: the candidate loads are warp-broadcasts out of L1.
-// The k best are a sorted list held entirely in REGISTERS (KMAX compile-time, insertion fully unrolled into
-// predicated moves; no local memory).  Exact k-NN: ring expansion stops when the k-th distance is below the distance
-// to the unvisited shell or the shell is beyond the radius; ties are broken towards the lower original index.
-// Queries that still need rings beyond `ring_limit` (sparse far-range areas, isolated points) are NOT finished here:
-// their slot is pushed to `queue` and normals_phase2_kernel finishes them with one warp each.  Without that split a
-// few threads walking hundreds of empty cells serially set the duration of the whole kernel.
-template <int KMAX, bool EXACT>
-__global__ void __launch_bounds__(NK_THREADS) normals_kernel(const GridHeader* __restrict__ hdr, const int32_t* __restrict__ cs,
-                                                             const double4* __restrict__ pts, int knn, double radius, int ring_limit,
-                                                             int32_t* __restrict__ queue, int32_t* queue_n,
-                                                             const int32_t* __restrict__ qlist, const int32_t* __restrict__ qcount,
-                                                             const double* prior_nrm, double* out_nrm) {
-  pdl_wait();
-  __shared__ GridHeader g;
-  if (threadIdx.x == 0) g = *hdr;
-  __syncthreads();
-  const int n = g.n;
-  const double r2 = radius * radius;
-  const double eps = 1e-9 * g.cell;
-  const int nx = g.dims[0], ny = g.dims[1], nz = g.dims[2];
-  const int nq = qlist ? *qcount : n;   // optional query list: only these slots get a normal (fused down-sample)
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < nq; t += gridDim.x * blockDim.x) {
-    const int s = qlist ? qlist[t] : t;
-    if (ring_limit < 0) { queue[atomicAdd(queue_n, 1)] = s; continue; }   // everything to the warp-cooperative kernel
-    const double4 qp = pts[s];
-    const double qx = qp.x, qy = qp.y, qz = qp.z;
-    const int qi = (int)__double_as_longlong(qp.w);
-    const int cx = (int)fmin(fmax(floor((qx - g.origin[0]) * g.inv_cell), 0.0), (double)(nx - 1));
-    const int cy = (int)fmin(fmax(floor((qy - g.origin[1]) * g.inv_cell), 0.0), (double)(ny - 1));
-    const int cz = (int)fmin(fmax(floor((qz - g.origin[2]) * g.inv_cell), 0.0), (double)(nz - 1));
-    double bd[KMAX];
-    int bs[KMAX];
-#pragma unroll
-    for (int j = 0; j < KMAX; j++) { bd[j] = INFINITY; bs[j] = -1; }
-    double kd = INFINITY;   // current k-th best distance (entry knn-1); +inf until k neighbours are known
-    int kslot = -1;
-    bool unresolved = false;
-    for (int R = 0;; ++R) {
-      const int z0 = max(cz - R, 0), z1 = min(cz + R, nz - 1);
-      const int y0 = max(cy - R, 0), y1 = min(cy + R, ny - 1);
-      const int x0 = max(cx - R, 0), x1 = min(cx + R, nx - 1);
-      for (int z = z0; z <= z1; ++z) {
-        const double gz = slab_gap_n(qz, g.origin[2], g.cell, z, nz, eps);
-        const double gz2 = gz * gz;
-        if (gz2 > fmin(kd, r2)) continue;
-        const bool zface = (z == cz - R) || (z == cz + R);
-        for (int y = y0; y <= y1; ++y) {
-          const double gy = slab_gap_n(qy, g.origin[1], g.cell, y, ny, eps);
-          if (gz2 + gy * gy > fmin(kd, r2)) continue;
-          const int row = (z * ny + y) * nx;
-          const bool shell = zface || y == cy - R || y == cy + R;
-          for (int part = 0; part < 2; ++part) {
-            int a, b;
-            if (shell) { if (part == 1) break; a = cs[row + x0]; b = cs[row + x1 + 1]; }
-            else if (part == 0) { if (cx - R < 0) continue; a = cs[row + cx - R]; b = cs[row + cx - R + 1]; }
-            else { if (cx + R > nx - 1) continue; a = cs[row + cx + R]; b = cs[row + cx + R + 1]; }
-            for (int j = a; j < b; ++j) {
-              const double4 p = pts[j];
-              const double d = dist2_exact(qx, qy, qz, p.x, p.y, p.z);
-              if (!(d < r2)) continue;
-              if (d > kd) continue;
-              if (d == kd) {  // exact tie with the current k-th: lower original index wins (rare path)
-                const int ik = (int)__double_as_longlong(pts[kslot].w), ic = (int)__double_as_longlong(p.w);
-                if (!(ic < ik)) continue;
-              }
-              // sorted insertion, fully unrolled (registers only).  Equal distances: order by original index.
-              const int ic = (int)__double_as_longlong(p.w);
-#pragma unroll
-              for (int t = KMAX - 1; t >= 1; --t) {
-                bool before_prev = d < bd[t - 1];
-                if (d == bd[t - 1]) before_prev = ic < (int)__double_as_longlong(pts[bs[t - 1]].w);
-                bool before_cur = d < bd[t];
-                if (d == bd[t] && bs[t] >= 0) before_cur = ic < (int)__double_as_longlong(pts[bs[t]].w);
-                if (before_prev) { bd[t] = bd[t - 1]; bs[t] = bs[t - 1]; }
-                else if (before_cur) { bd[t] = d; bs[t] = j; }
-              }
-              {
-                bool before0 = d < bd[0];
-                if (d == bd[0] && bs[0] >= 0) before0 = ic < (int)__double_as_longlong(pts[bs[0]].w);
-                if (before0) { bd[0] = d; bs[0] = j; }
-              }
-              if (EXACT) { kd = bd[KMAX - 1]; kslot = bs[KMAX - 1]; }   // knn == KMAX: static index, the list stays in registers
-              else { kd = bd[knn - 1]; kslot = bs[knn - 1]; }          // generic knn: dynamic index (list lives in local memory)
-            }
-          }
-        }
-      }
-      double bound = INFINITY;
-      if (cx - R > 0) bound = fmin(bound, qx - (g.origin[0] + (double)(cx - R) * g.cell));
-      if (cx + R < nx - 1) bound = fmin(bound, (g.origin[0] + (double)(cx + R + 1) * g.cell) - qx);
-      if (cy - R > 0) bound = fmin(bound, qy - (g.origin[1] + (double)(cy - R) * g.cell));
-      if (cy + R < ny - 1) bound = fmin(bound, (g.origin[1] + (double)(cy + R + 1) * g.cell) - qy);
-      if (cz - R > 0) bound = fmin(bound, qz - (g.origin[2] + (double)(cz - R) * g.cell));
-      if (cz + R < nz - 1) bound = fmin(bound, (g.origin[2] + (double)(cz + R + 1) * g.cell) - qz);
-      bound -= eps;
-      if (bound < 0.0) bound = 0.0;
-      if (bound == INFINITY || bound * bound > fmin(kd, r2)) break;
-      if (R >= ring_limit) { unresolved = true; break; }
-    }
-    if (unresolved) { queue[atomicAdd(queue_n, 1)] = s; continue; }
-    // cumulants over the kk <= knn neighbours in ascending (d2, index) order
-    double c[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-    int kk = 0;
-#pragma unroll
-    for (int t = 0; t < KMAX; ++t) {
-      if (t < knn && bs[t] >= 0) {
-        const double4 p = pts[bs[t]];
-        c[0] = __dadd_rn(c[0], p.x); c[1] = __dadd_rn(c[1], p.y); c[2] = __dadd_rn(c[2], p.z);
-        c[3] = __dadd_rn(c[3], __dmul_rn(p.x, p.x)); c[4] = __dadd_rn(c[4], __dmul_rn(p.x, p.y)); c[5] = __dadd_rn(c[5], __dmul_rn(p.x, p.z));
-        c[6] = __dadd_rn(c[6], __dmul_rn(p.y, p.y)); c[7] = __dadd_rn(c[7], __dmul_rn(p.y, p.z)); c[8] = __dadd_rn(c[8], __dmul_rn(p.z, p.z));
-        kk++;
-      }
-    }
-    double nr[3];
-    finish_normal(c, kk, qx, qy, qz, prior_nrm ? prior_nrm + 3 * (size_t)qi : nullptr, nr);
-    out_nrm[3 * (size_t)qi] = nr[0]; out_nrm[3 * (size_t)qi + 1] = nr[1]; out_nrm[3 * (size_t)qi + 2] = nr[2];
-  }
 }
 
 // Phase 2: one WARP per queued query, restarted from ring 0.  Per ring, each lane first resolves ONE (y, z) row --
@@ -408,177 +287,6 @@ __global__ void __launch_bounds__(NK_THREADS) normals_phase2_kernel(const GridHe
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------------
-// Fast path: one warp per query, GATHER the candidates of the 3x3x3 cell block once, SELECT the k nearest by counting,
-// reduce the covariance with warp shuffles.
-//   1. lanes 0..8 resolve the nine (y, z) rows of the block (one contiguous slot range each);
-//   2. the candidates (at most NS_CHUNKS*32) are dealt round-robin to the lanes: distance + index live in registers;
-//   3. the k-th smallest (d2, index) is found WITHOUT sorting: a 32-bin histogram over d2 (neighbours on a surface are
-//      ~uniform in d2) built with shared-memory atomics, a warp prefix sum to locate the bin that holds the k-th, and a
-//      few warp arg-min rounds inside that bin;
-//   4. every lane accumulates the cumulants of its own selected candidates, a butterfly of shuffles sums them
-//      (the covariance is therefore summed in a different order than the reference's ascending-distance order: the
-//      difference is O(1e-16) relative);
-//   5. the query is exact iff the k-th distance lies inside the scanned block (or the block already covers the radius);
-//      anything else -- sparse neighbourhoods, more than NS_CHUNKS*32 candidates -- is queued for normals_phase2_kernel.
-// A warp handles 32 consecutive queries and only then runs the eigen-solver, one query per lane.
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr int NS_CHUNKS = 8;
-
-__global__ void __launch_bounds__(NK_THREADS) normals_select_kernel(const GridHeader* __restrict__ hdr, const int32_t* __restrict__ cs,
-                                                                    const double4* __restrict__ pts, int knn, double radius,
-                                                                    const int32_t* __restrict__ qlist, const int32_t* __restrict__ qcount,
-                                                                    int32_t* __restrict__ queue, int32_t* queue_n,
-                                                                    double* __restrict__ cum) {
-  pdl_wait();
-  __shared__ GridHeader g;
-  __shared__ int s_hist[NK_THREADS / 32][32];
-  if (threadIdx.x == 0) g = *hdr;
-  __syncthreads();
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-  const int n = g.n;
-  const int nq = qlist ? *qcount : n;
-  const double r2 = radius * radius;
-  const double eps = 1e-9 * g.cell;
-  const int nx = g.dims[0], ny = g.dims[1], nz = g.dims[2];
-  const int warps_total = gridDim.x * (NK_THREADS / 32);
-  {
-    for (int tq = blockIdx.x * (NK_THREADS / 32) + wib; tq < nq; tq += warps_total) {
-      const int s = qlist ? qlist[tq] : tq;
-      const double4 qp = pts[s];
-      const double qx = qp.x, qy = qp.y, qz = qp.z;
-      const int cx = (int)fmin(fmax(floor((qx - g.origin[0]) * g.inv_cell), 0.0), (double)(nx - 1));
-      const int cy = (int)fmin(fmax(floor((qy - g.origin[1]) * g.inv_cell), 0.0), (double)(ny - 1));
-      const int cz = (int)fmin(fmax(floor((qz - g.origin[2]) * g.inv_cell), 0.0), (double)(nz - 1));
-      // 1. rows of the 3x3x3 block
-      int a = 0, cnt = 0;
-      if (lane < 9) {
-        const int y = cy - 1 + lane % 3, z = cz - 1 + lane / 3;
-        if (y >= 0 && y < ny && z >= 0 && z < nz) {
-          const int row = (z * ny + y) * nx;
-          a = cs[row + max(cx - 1, 0)];
-          cnt = cs[row + min(cx + 1, nx - 1) + 1] - a;
-        }
-      }
-      int inc = cnt;
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-      const int ntot = __shfl_sync(0xffffffffu, inc, 8);
-      const int delta_l = a - (inc - cnt);   // slot = t + delta for candidate number t of this row
-      int offs[9], delta[9];
-#pragma unroll
-      for (int r = 0; r < 9; r++) { offs[r] = __shfl_sync(0xffffffffu, inc - cnt, r); delta[r] = __shfl_sync(0xffffffffu, delta_l, r); }
-      bool fallback = ntot > NS_CHUNKS * 32;
-      if (fallback && lane == 0) atomicAdd(queue_n + 2, 1);   // debug counter: block holds too many candidates
-      // 2. candidates -> registers
-      double d[NS_CHUNKS]; int idx[NS_CHUNKS], sl[NS_CHUNKS];
-      int nvalid = 0;
-      double dmax = 0.0;
-      if (!fallback) {
-#pragma unroll
-        for (int c = 0; c < NS_CHUNKS; c++) {
-          const int t = c * 32 + lane;
-          int dl = delta[0];
-#pragma unroll
-          for (int r = 1; r < 9; r++) if (t >= offs[r]) dl = delta[r];
-          d[c] = INFINITY; idx[c] = 0x7fffffff; sl[c] = -1;
-          if (t < ntot) {
-            const int slot = t + dl;
-            const double4 p = pts[slot];
-            const double dd = dist2_exact(qx, qy, qz, p.x, p.y, p.z);
-            if (dd < r2) { d[c] = dd; idx[c] = (int)__double_as_longlong(p.w); sl[c] = slot; dmax = fmax(dmax, dd); }
-          }
-          nvalid += __popc(__ballot_sync(0xffffffffu, sl[c] >= 0));
-        }
-      }
-      // 3. threshold (td, ti): the `need`-th smallest (d2, index)
-      const int need = min(knn, nvalid);
-      double td = INFINITY; int ti = 0x7fffffff;   // nvalid <= knn: everything valid is selected
-      if (!fallback && nvalid > knn) {
-        dmax = warp_max(dmax);
-        const double scale = dmax > 0.0 ? 32.0 / dmax : 0.0;
-        s_hist[wib][lane] = 0;
-        __syncwarp();
-        int bin[NS_CHUNKS];
-#pragma unroll
-        for (int c = 0; c < NS_CHUNKS; c++) {
-          bin[c] = 32;
-          if (sl[c] >= 0) { bin[c] = min(31, (int)(d[c] * scale)); atomicAdd(&s_hist[wib][bin[c]], 1); }
-        }
-        __syncwarp();
-        int cum = s_hist[wib][lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, cum, o); if (lane >= o) cum += t; }
-        const int B = __ffs(__ballot_sync(0xffffffffu, cum >= need)) - 1;
-        const int below = B > 0 ? __shfl_sync(0xffffffffu, cum, B - 1) : 0;
-        const int m = need - below;    // how many of bin B belong to the k nearest (>= 1)
-        double ld = -1.0; int li = -1; // last extracted (d2, index), lexicographic lower bound
-        for (int round = 0; round < m; ++round) {
-          double bd = INFINITY; int bi = 0x7fffffff;
-#pragma unroll
-          for (int c = 0; c < NS_CHUNKS; c++) {
-            const bool in_bin = bin[c] == B;
-            const bool after = d[c] > ld || (d[c] == ld && idx[c] > li);
-            const bool better = d[c] < bd || (d[c] == bd && idx[c] < bi);
-            if (in_bin && after && better) { bd = d[c]; bi = idx[c]; }
-          }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
-            const double od = __shfl_xor_sync(0xffffffffu, bd, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (od < bd || (od == bd && oi < bi)) { bd = od; bi = oi; }
-          }
-          ld = bd; li = bi;
-        }
-        td = ld; ti = li;
-        // everything in a lower bin is selected, bin B up to (td, ti): express both with one lexicographic threshold
-#pragma unroll
-        for (int c = 0; c < NS_CHUNKS; c++) if (bin[c] > B) sl[c] = -1;   // beyond the k-th
-#pragma unroll
-        for (int c = 0; c < NS_CHUNKS; c++) if (bin[c] == B && (d[c] > td || (d[c] == td && idx[c] > ti))) sl[c] = -1;
-      }
-      // 5. exact?  the k-th distance must lie inside the scanned block, or the block must cover the whole radius
-      double bound = INFINITY;
-      if (cx - 1 > 0) bound = fmin(bound, qx - (g.origin[0] + (double)(cx - 1) * g.cell));
-      if (cx + 1 < nx - 1) bound = fmin(bound, (g.origin[0] + (double)(cx + 2) * g.cell) - qx);
-      if (cy - 1 > 0) bound = fmin(bound, qy - (g.origin[1] + (double)(cy - 1) * g.cell));
-      if (cy + 1 < ny - 1) bound = fmin(bound, (g.origin[1] + (double)(cy + 2) * g.cell) - qy);
-      if (cz - 1 > 0) bound = fmin(bound, qz - (g.origin[2] + (double)(cz - 1) * g.cell));
-      if (cz + 1 < nz - 1) bound = fmin(bound, (g.origin[2] + (double)(cz + 2) * g.cell) - qz);
-      if (bound != INFINITY) { bound -= eps; if (bound < 0.0) bound = 0.0; }
-      const double b2 = bound == INFINITY ? INFINITY : bound * bound;
-      const double kth = nvalid >= knn ? td : INFINITY;   // fewer than k found: only exact if the block covers the radius
-      if (!fallback && !(b2 > fmin(kth, r2))) { fallback = true; if (lane == 0) atomicAdd(queue_n + (nvalid >= knn ? 3 : 4), 1); }  // debug counters: k-th outside the block / fewer than k in the block
-      if (fallback) {
-        if (lane == 0) { queue[atomicAdd(queue_n, 1)] = s; cum[10 * (size_t)tq + 9] = -1.0; }
-        continue;
-      }
-      // 4. cumulants of the selected candidates, butterfly sum
-      double c9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-#pragma unroll
-      for (int c = 0; c < NS_CHUNKS; c++) {
-        if (sl[c] >= 0) {
-          const double4 p = pts[sl[c]];
-          c9[0] += p.x; c9[1] += p.y; c9[2] += p.z;
-          c9[3] += p.x * p.x; c9[4] += p.x * p.y; c9[5] += p.x * p.z;
-          c9[6] += p.y * p.y; c9[7] += p.y * p.z; c9[8] += p.z * p.z;
-        }
-      }
-#pragma unroll
-      for (int t = 0; t < 9; t++) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) c9[t] += __shfl_xor_sync(0xffffffffu, c9[t], o);
-      }
-      {
-        double v = (double)need;   // lane 9 writes the neighbour count, lanes 0..8 one cumulant each (all lanes hold the sums)
-#pragma unroll
-        for (int t = 0; t < 9; t++) if (lane == t) v = c9[t];
-        if (lane < 10) cum[10 * (size_t)tq + lane] = v;
-      }
-    }
-  }
-}
-
 // Butterfly sum of 9 values over the warp with the exchanges TRANSPOSED: at distance 16 the two halves of the warp split the values
 // between them (each lane keeps the half it will finish and receives the partner's copy of it), at distance 8 the quarters do, and so
 // on -- 8 + 4 + 2 + 1 + 1 = 16 exchanges instead of 9 x 5.  Every partial sum is the same pair of operands the plain xor butterfly
@@ -628,13 +336,11 @@ __device__ __forceinline__ void warp_sum9_transposed(double (&v)[9], int lane) {
   v[0] = d;
 }
 
-// Second-generation fast path: same GATHER -> SELECT-BY-COUNTING -> BUTTERFLY pipeline as normals_select_kernel, but the
-// gathered candidates go through a per-warp shared-memory buffer, which lets the block radius R grow (1, 2, 3 cells)
+// Block gather: one warp per query GATHERs the candidates of a cell block into a per-warp shared-memory buffer, SELECTs the k
+// nearest by counting and sums their cumulants with a BUTTERFLY of shuffles.  The buffer lets the block radius R grow (1, 2, 3 cells)
 // until the k-th neighbour provably lies inside the block: dense areas finish at R = 1, sparse far-range areas at
 // R = 2 or 3, and only what is still unresolved (or holds more than NS2_CAP candidates) goes to normals_phase2_kernel.
-#ifndef B2S_NS2_MINBLOCKS
-#define B2S_NS2_MINBLOCKS 8   // resident CTAs per SM the select kernel is compiled for (8 -> 64 registers; A/B knob of the build)
-#endif
+constexpr int NS2_MIN_BLOCKS = 8;   // resident CTAs per SM the select kernel is compiled for (8 -> 64 registers)
 constexpr int NS2_CAP = 256;
 constexpr int NS2_CHUNKS = NS2_CAP / 32;
 constexpr int NS2_RMAX = 3;
@@ -647,7 +353,7 @@ enum : int32_t { NPATH_FULL_BLOCK = NS2_RMAX + 1, NPATH_OVER_CAPACITY, NPATH_NOT
 // 4 doubles: candidates inside the certified ball nc, the histogram bin of the k-th key or -1 without a histogram, that bin's member count,
 // lim2).  The production instantiation (kDebug = false) compiles none of it.
 template <bool kDebug>
-__global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2_kernel(const GridHeader* __restrict__ hdr, const int32_t* __restrict__ cs,
+__global__ void __launch_bounds__(NK_THREADS, NS2_MIN_BLOCKS) normals_select2_kernel(const GridHeader* __restrict__ hdr, const int32_t* __restrict__ cs,
                                                                      const double4* __restrict__ pts, int knn, double radius,
                                                                      const int32_t* __restrict__ qlist, const int32_t* __restrict__ qcount,
                                                                      int32_t* __restrict__ queue, int32_t* queue_n,
@@ -762,10 +468,7 @@ __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2
       }
       __syncwarp();
       if (nc > NS2_CAP) {   // too dense for the buffer: general kernel
-        if (lane == 0) {
-          atomicAdd(queue_n + 2, 1);
-          if (kDebug) { dbg_path[s] = NPATH_OVER_CAPACITY; dbg_sel[4 * (size_t)s] = nc; dbg_sel[4 * (size_t)s + 1] = -1; dbg_sel[4 * (size_t)s + 2] = 0; dbg_sel[4 * (size_t)s + 3] = lim2; }
-        }
+        if (kDebug && lane == 0) { dbg_path[s] = NPATH_OVER_CAPACITY; dbg_sel[4 * (size_t)s] = nc; dbg_sel[4 * (size_t)s + 1] = -1; dbg_sel[4 * (size_t)s + 2] = 0; dbg_sel[4 * (size_t)s + 3] = lim2; }
         break;
       }
       // ---- candidates -> registers (round-robin), statistics ----
@@ -853,10 +556,7 @@ __global__ void __launch_bounds__(NK_THREADS, B2S_NS2_MINBLOCKS) normals_select2
       }
       warp_sum9_transposed(c9, lane);   // lane l now holds the warp total of cumulant l >> 1 in c9[0] (l < 18)
       resolved = true;
-      if (lane == 0) {
-        if (R > 1) atomicAdd(queue_n + 2 + min(R, 3), 1);   // statistics (B2S_DEBUG_NORMALS): resolved at R = 2 / at R >= 3
-        if (kDebug) { dbg_path[s] = R <= NS2_RMAX ? R : NPATH_FULL_BLOCK; dbg_sel[4 * (size_t)s] = nc; dbg_sel[4 * (size_t)s + 1] = dbg_bin; dbg_sel[4 * (size_t)s + 2] = dbg_nb; dbg_sel[4 * (size_t)s + 3] = lim2; }
-      }
+      if (kDebug && lane == 0) { dbg_path[s] = R <= NS2_RMAX ? R : NPATH_FULL_BLOCK; dbg_sel[4 * (size_t)s] = nc; dbg_sel[4 * (size_t)s + 1] = dbg_bin; dbg_sel[4 * (size_t)s + 2] = dbg_nb; dbg_sel[4 * (size_t)s + 3] = lim2; }
     }
     if (!resolved) {
       if (lane == 0) { queue[atomicAdd(queue_n, 1)] = s; cum[10 * (size_t)tq + 9] = -1.0; }
@@ -899,7 +599,7 @@ __global__ void __launch_bounds__(NK_THREADS) normals_finish_kernel(const GridHe
 
 
 __global__ void zero_i32_kernel(int32_t* p) {
-  pdl_wait(); for (int i = 0; i < 6; i++) p[i] = 0; }
+  pdl_wait(); p[0] = 0; p[1] = 0; }
 
 // query list = grid slots whose original point is flagged; warp-aggregated append keeps neighbouring slots together
 __global__ void __launch_bounds__(NK_THREADS) normals_qlist_kernel(const GridHeader* __restrict__ hdr, const double4* __restrict__ pts,
@@ -940,67 +640,40 @@ int32_t op_estimate_normals(b2s_handle* h, b2s_cloud* c, int knn, double radius,
   int32_t* queue = h->tmp_i32.as<int32_t>() + 16;
   int32_t* qlist = flags ? queue + n_max : nullptr;
   const int32_t* qcount = flags ? qn + 1 : nullptr;
-  // rings the thread-per-query kernel may walk before handing a query to the warp-cooperative kernel
-  // (B2S_NORMALS_RING_LIMIT: tuning knob; -1 = every query goes to the warp-cooperative kernel)
-  // default -1: on the config-2 scans the all-warp path beat the thread kernel plus warp stragglers
-  static const int ring_limit_env = getenv("B2S_NORMALS_RING_LIMIT") ? atoi(getenv("B2S_NORMALS_RING_LIMIT")) : -1;
-  const int ring_limit = ring_limit_env;
   ProfScope prof(h, PK_NORMALS);
   const GridHeader* hdr = h->grid_b.hdr.as<GridHeader>();
   const int32_t* cs = grid_starts(&h->grid_b);
   const double4* pts = h->grid_b.pts.as<double4>();
   double* out = c->nrm.as<double>();
   // The prior normals are the output array itself.  That is safe because every kernel below reads only the POSITIONS of other
-  // points, and each point's normal slot is read (its prior) and then written by exactly one thread: the finish kernel, the
-  // phase-2 kernel or the thread-per-query kernel, whichever resolves the query.  Keep it so: a kernel that read another
-  // point's normal, or two kernels writing the same slot, would see overwritten priors.
+  // points, and each point's normal slot is read (its prior) and then written by exactly one thread: the finish kernel or the
+  // phase-2 kernel, whichever resolves the query.  Keep it so: a kernel that read another point's normal, or two kernels writing
+  // the same slot, would see overwritten priors.
   const double* prior = with_prior ? out : nullptr;
   launch_pdl(zero_i32_kernel, 1, 1, 0, h->stream, qn);
   if (flags) {
     launch_pdl(normals_qlist_kernel, blocks, NK_THREADS, 0, h->stream, hdr, pts, flags, qlist, qn + 1);
     h->launches++;
   }
-  // exact instantiations for the knn values the reference's presets use (Lua default 20, C++ struct default 5,
-  // place-recognition normals 10); any other knn <= 32 takes the generic variants
-  if (ring_limit == -1) {   // default: gather + select (one warp per query), stragglers to the general warp kernel
-    // one warp per query, grid-stride (B2S_NS2_GRID: A/B knob of the grid size)
-    static const int ns2_grid_env = getenv("B2S_NS2_GRID") ? atoi(getenv("B2S_NS2_GRID")) : 0;
-    const int ns2_cap = ns2_grid_env > 0 ? ns2_grid_env : 16 * device_sms();
-    int wblocks = (int)((n_max + (NK_THREADS / 32) - 1) / (NK_THREADS / 32));
-    if (wblocks > ns2_cap) wblocks = ns2_cap;
-    if (wblocks < 1) wblocks = 1;
-    B2S_TRY(h->tmp_f64.ensure((n_max + 1) * 80, h->stream));
-    double* cum = h->tmp_f64.as<double>();
-    static const bool use_v1 = getenv("B2S_NORMALS_SELECT_V1") != nullptr;   // A/B knob: fixed 3x3x3 block, register gather
-    if (use_v1) launch_pdl(normals_select_kernel, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn, cum);
-    else if (dbg) launch_pdl(normals_select2_kernel<true>, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn,
-                             cum, dbg->path, dbg->sel);
-    else launch_pdl(normals_select2_kernel<false>, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn, cum,
-                    nullptr, nullptr);
-    if (dbg) launch_pdl(normals_finish_kernel<true>, blocks, NK_THREADS, 0, h->stream, hdr, pts, qlist, qcount, cum, prior, out, dbg->rec);
-    else launch_pdl(normals_finish_kernel<false>, blocks, NK_THREADS, 0, h->stream, hdr, pts, qlist, qcount, cum, prior, out, nullptr);
-    h->launches++;
-  } else if (knn == 20) launch_pdl(normals_kernel<20, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
-  else if (knn == 10) launch_pdl(normals_kernel<10, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
-  else if (knn == 5) launch_pdl(normals_kernel<5, true>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
-  else if (knn <= 16) launch_pdl(normals_kernel<16, false>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
-  else launch_pdl(normals_kernel<32, false>, blocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, ring_limit, queue, qn, qlist, qcount, prior, out);
-  static const bool dbg_counts = getenv("B2S_DEBUG_NORMALS") != nullptr;
-  if (dbg_counts) {   // debug aid: how many queries the fast path left to the general kernel
-    int32_t hq[6] = {0, 0, 0, 0, 0, 0};
-    GridHeader gh;
-    cudaMemcpyAsync(hq, qn, 24, cudaMemcpyDeviceToHost, h->stream);
-    cudaMemcpyAsync(&gh, hdr, sizeof(gh), cudaMemcpyDeviceToHost, h->stream);
-    cudaStreamSynchronize(h->stream);
-    fprintf(stderr, "[b2s normals] select2: over-capacity %d, resolved at R=2 %d, at R=3 %d\n", hq[2], hq[4], hq[5]);
-    fprintf(stderr, "[b2s normals] indexed %d queries %d fallback %d cell %.3f dims %dx%dx%d\n", gh.n, flags ? hq[1] : gh.n, hq[0], gh.cell,
-            gh.dims[0], gh.dims[1], gh.dims[2]);
-  }
+  // gather + select (one warp per query, grid-stride; B2S_NS2_GRID: A/B knob of the grid size), stragglers to the phase-2 kernel
+  static const int ns2_grid_env = getenv("B2S_NS2_GRID") ? atoi(getenv("B2S_NS2_GRID")) : 0;
+  const int ns2_cap = ns2_grid_env > 0 ? ns2_grid_env : 16 * device_sms();
+  int wblocks = (int)((n_max + (NK_THREADS / 32) - 1) / (NK_THREADS / 32));
+  if (wblocks > ns2_cap) wblocks = ns2_cap;
+  if (wblocks < 1) wblocks = 1;
+  B2S_TRY(h->tmp_f64.ensure((n_max + 1) * 80, h->stream));
+  double* cum = h->tmp_f64.as<double>();
+  if (dbg) launch_pdl(normals_select2_kernel<true>, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn,
+                      cum, dbg->path, dbg->sel);
+  else launch_pdl(normals_select2_kernel<false>, wblocks, NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, qlist, qcount, queue, qn, cum,
+                  nullptr, nullptr);
+  if (dbg) launch_pdl(normals_finish_kernel<true>, blocks, NK_THREADS, 0, h->stream, hdr, pts, qlist, qcount, cum, prior, out, dbg->rec);
+  else launch_pdl(normals_finish_kernel<false>, blocks, NK_THREADS, 0, h->stream, hdr, pts, qlist, qcount, cum, prior, out, nullptr);
   if (dbg) launch_pdl(normals_phase2_kernel<true>, 4 * device_sms(), NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, queue, qn, prior, out,
                       dbg->rec);
   else launch_pdl(normals_phase2_kernel<false>, 4 * device_sms(), NK_THREADS, 0, h->stream, hdr, cs, pts, knn, radius, queue, qn, prior, out,
                   nullptr);
-  h->launches += 3;
+  h->launches += 4;
   c->has_normals = true;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;

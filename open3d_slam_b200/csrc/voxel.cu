@@ -431,8 +431,7 @@ int32_t select_flags(b2s_handle* h, const b2s_cloud* in, double ratio, uint32_t 
   launch_pdl(select_keys_kernel, blocks, VX_THREADS, 0, h->stream, in->xyz.as<double>(), in->dn.as<int32_t>(), seed, keys, vals,
                                                            h->flags.as<int32_t>());
   h->launches++;
-  static const bool sort_select = getenv("B2S_SELECT_SORT") != nullptr;   // A/B knob: the full sort this replaced
-  if (!sort_select && n_max <= ((size_t)1 << 18)) {
+  if (n_max <= ((size_t)1 << 18)) {
     ProfScope prof(h, PK_SELECT);
     B2S_TRY(h->misc.ensure(256, h->stream));
     uint32_t* sel = h->misc.as<uint32_t>() + 32;   // words 0..11 of misc hold the voxel bounding box

@@ -1,10 +1,10 @@
 """Child process of tests/test_gpu_boundaries.py for the cases that depend on process-wide knobs.
 
-The library reads B2S_GRID_CAP, B2S_SORT and B2S_DEBUG_NORMALS once per process, so each setting needs a process of its own.
+The library reads B2S_GRID_CAP and B2S_SORT once per process, so each setting needs a process of its own.
 
     python tests/boundary_child.py ops OUT.npz        -- a fixed set of operations, every output written to OUT.npz
-    python tests/boundary_child.py normals-exits      -- normal estimation on clouds that reach every exit of the select kernel
-                                                         (the counters go to stderr when B2S_DEBUG_NORMALS is set)
+
+It also holds the clouds and parameters that reach every exit of the normals select kernel (imported by the tests).
 """
 import os
 import sys
@@ -49,21 +49,6 @@ def two_patches(seed=5, n=3000, offset=(2500.0, 1500.0, 400.0)):
                    np.c_[rng.uniform(-2, 2, k), np.full(k, 2.0) + 0.01 * rng.standard_normal(k), rng.uniform(0, 1.5, k)],
                    np.c_[np.full(k, -2.0) + 0.01 * rng.standard_normal(k), rng.uniform(-2, 2, k), rng.uniform(0, 1.5, k)]])
     return np.ascontiguousarray(np.vstack([a, a[::-1] + np.asarray(offset)]))
-
-
-def run_normals_exits():
-    from open3d_slam_b200 import _lib as L
-    import ctypes as C
-    p = exits_params()
-    eng = E.Engine(p)
-    s2m = E.scanToMapRegistrationFactory(eng, p)
-    s2m.processForScanMatchingAndMerging(eng.cloud(exits_scan()))
-    eng.synchronize()
-    sys.stderr.write("[boundary] two-patch cloud\n")
-    cl = eng.cloud(two_patches())
-    L.check(L.lib().b2s_estimate_normals(eng._h, cl._c, 10, C.c_double(1.0)))
-    eng.synchronize()
-    eng.close()
 
 
 def run_ops(out_path):
@@ -111,7 +96,5 @@ def run_ops(out_path):
 if __name__ == "__main__":
     if sys.argv[1] == "ops":
         run_ops(sys.argv[2])
-    elif sys.argv[1] == "normals-exits":
-        run_normals_exits()
     else:
         raise SystemExit(f"unknown mode {sys.argv[1]}")

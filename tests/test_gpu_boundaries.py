@@ -3,7 +3,7 @@
 The kernels choose their code paths from the input size, from knn and from the SM count.  Each switch is crossed here by a pair of
 inputs, one on either side, and both sides are held to the oracle with the idioms of test_gpu_parity.py (iterations and
 correspondences equal, fitness to 1e-12, T to 1e-9, keyed bit-exact voxel means).  Where the library exposes which side a run took
-(the ICP debug counters, the B2S_DEBUG_NORMALS lines), the test asserts it, so that a change of a launch constant makes these
+(the ICP debug counters, the normals debug record), the test asserts it, so that a change of a launch constant makes these
 tests fail instead of silently testing one side twice.  Run with -s to see the sides that were reached.
 
   ICP (csrc/icp.cu)        cluster size: doubles while size x threads < n (768 threads point-to-plane, 512 GICP), up to 8 or 16 CTAs
@@ -18,7 +18,6 @@ tests fail instead of silently testing one side twice.  Run with -s to see the s
 """
 import ctypes as C
 import os
-import re
 import subprocess
 import sys
 
@@ -465,31 +464,50 @@ def run_child(args, env_extra, timeout=600):
     return proc
 
 
-def test_normals_select_exits_and_coarse_grid(engine_factory):
-    """Every exit of the select kernel (R = 1, R = 2, R >= 3, more candidates than its buffer, unresolved after the last block) is
-    taken at least once -- counted by B2S_DEBUG_NORMALS in a child process -- and the same clouds match the oracle here."""
+def test_normals_select_exits_and_coarse_grid_from_the_record(engine_factory):
+    """Every exit of the select kernel -- R = 1, R = 2, R = 3 (path codes 1-3), more candidates than its buffer (5), unresolved after
+    the last block (6) -- is taken on the cloud processForScanMatchingAndMerging estimates: exits_scan cropped and voxelized, at the
+    0.4 m process-scan cell.  b2s_debug_estimate_normals records the path of every query on that cloud (held to tests/normals_checks.py)
+    and the production merge_ normals agree with its record; then the same clouds match the oracle.
+
+    The two-patch cloud's index cell must have been coarsened from radius / 4 = 0.25 m to at least 1 m.  Shown from the selection
+    record rather than the grid header, because the record is what the normals kernels saw: a query resolved at R = 1 sits in the
+    middle cell of a block three cells wide, so every bounded block face lies at most 2 cells from it and its certified ball has
+    lim2 < (2 cell)^2.  lim2 == r^2 at every such query therefore needs 2 cell > r = 1 m (or a block without a bounded face, which over
+    the kilometres-wide box needs far larger cells), and the header only ever doubles the cell, 0.25 m x 2^j, so cell >= 1 m.  With the
+    0.25 m cell, lim2 < 0.25 at R = 1."""
     sys.path.insert(0, HERE)
     try:
         import boundary_child as BC
+        from test_gpu_normals_kernels import run_and_check
     finally:
         sys.path.remove(HERE)
-    proc = run_child(["normals-exits"], {"B2S_DEBUG_NORMALS": "1"})
-    sel = [tuple(map(int, m)) for m in re.findall(r"over-capacity (\d+), resolved at R=2 (\d+), at R=3 (\d+)", proc.stderr)]
-    idx = [(int(a), int(b), int(c), float(d)) for a, b, c, d in re.findall(r"indexed (\d+) queries (\d+) fallback (\d+) cell ([0-9.]+)", proc.stderr)]
-    assert len(sel) >= 2 and len(idx) == len(sel), proc.stderr
-    over, r2, r3 = sel[0]
-    _, queries, fallback, cell = idx[0]
-    r1, unresolved = queries - r2 - r3 - fallback, fallback - over
-    print(f"select exits: R=1 {r1}, R=2 {r2}, R>=3 {r3}, over capacity {over}, unresolved {unresolved} (cell {cell})")
-    assert min(r1, r2, r3, over, unresolved) > 0, f"not every exit of the select kernel was taken:\n{proc.stderr}"
-    # the two-patch cloud: the last lines; its index cell must have been coarsened from radius / 4
-    coarse_cell = idx[-1][3]
-    print(f"two-patch cloud: cell {coarse_cell} m instead of 0.25 m")
-    assert coarse_cell >= 4 * 0.25, proc.stderr
+    p = BC.exits_params()
+    es = engine_factory(p)
+    raw = BC.exits_scan()
+    ps = E.scanToMapRegistrationFactory(es, p).processForScanMatchingAndMerging(es.cloud(raw))
+    gx, gn = ps.merge_.download()
+    # the voxel cloud the estimation ran on, in the device's order: the map builder's cropper (sensor frame), then the voxel down-sample
+    cropped = E.crop(es, es.cloud(raw), p.mapBuilder.cropper.to_c(center=(0.0, 0.0, 0.0)))
+    t0, _ = E.voxelize(es, cropped, p.scanProcessing.voxelSize).download()
+    knn, radius, cell = p.icp.knn, p.icp.maxDistanceKnn, 4 * p.scanProcessing.voxelSize
+    _, path, dbg = run_and_check(es, f"exits_scan process-scan cell {cell:g}", t0, knn, radius, cell_hint=cell, full=True)[:3]
+    counts = np.bincount(path, minlength=7)
+    print(f"select exits: R=1 {counts[1]}, R=2 {counts[2]}, R=3 {counts[3]}, full-radius block {counts[4]}, over capacity {counts[5]}, "
+          f"unresolved {counts[6]}")
+    assert all(counts[c] > 0 for c in (1, 2, 3, 5, 6)), f"not every exit of the select kernel was taken: {counts.tolist()}"
+    idx = NC.rows_in(gx, t0)
+    worst = NC.assert_normals_close(gn, dbg[idx], t0, knn, radius, queries=idx)
+    print(f"processForScanMatchingAndMerging merge_ vs the debug entry: worst {worst:.3g} of the gap-aware bound ({len(idx)} of {len(t0)})")
+
+    eng = engine_factory(params())
+    _, path, _, sel = run_and_check(eng, "two_patches", BC.two_patches(), 10, 1.0, full=True)
+    r1 = path == 1
+    print(f"two-patch cloud: {r1.sum()} queries resolved at R = 1, lim2 {np.unique(sel[r1, 3])}")
+    assert r1.any() and (sel[r1, 3] == 1.0).all(), "the two-patch index cell was not coarsened to at least 4 x radius / 4"
 
     _process_scan_matches(engine_factory, BC.exits_scan(), BC.exits_params())
 
-    eng = engine_factory(params())
     xyz = BC.two_patches()
     cl = eng.cloud(xyz)
     L.check(L.lib().b2s_estimate_normals(eng._h, cl._c, 10, C.c_double(1.0)))
