@@ -366,6 +366,78 @@ int32_t b2s_debug_nn_index(b2s_handle* h, double origin_cell[4], int32_t dims_n[
  * its grid box with a pass over the map instead (read once per process). */
 int32_t b2s_debug_submap_bbox(b2s_handle* h, const b2s_submap* sm, double box[6]);
 
+/* ---- global localisation in a prior map: no initial pose needed (DESIGN.md row M3) --------------------------------------------------
+ * The reference takes the first pose in a prior map from an operator (SlamMapInitializer's interactive marker or /initialpose,
+ * ros/open3d_slam_ros/src/SlamMapInitializer.cpp) or from the fixed MapInitializingParameters::initialPose_.  This call finds it: an
+ * exhaustive search over (x, y, yaw[, z]) scored with the measure the reference uses to accept a revisit (the share of scan points in an
+ * occupied voxel, SubmapCollection::isSwitchingSubmapsConsistant), then the best distinct hypotheses refined by the scan-to-map ICP.
+ * It reads the submap and changes nothing (map, pose slot, counters, the mapper's last processed scan).  Applying the pose is the caller's
+ * job: b2s_submap_set_initial_transform (and b2s_odometry_set_initial_transform), as SlamWrapper::setInitialTransform does.
+ *   1. query: crop(raw, scan-matcher cropper at identity) -- the crop S1 applies to match_ -- then VoxelDownSample(score_voxel) exactly as
+ *      b2s_voxel_down_sample.  Empty -> B2S_E_EMPTY.
+ *   2. hypotheses: n_x = floor((x_max - x_min) / step) + 1, n_y likewise; h = ((iz n_yaw + j) n_y + iy) n_x + ix;
+ *      t = (x_min + ix step, y_min + iy step, z0 + iz z_step) (each one rounded multiply then one rounded add, no contraction);
+ *      R_j = Rz(yaw0 + j yaw_step) Ry(pitch) Rx(roll), built on the host with the C library's cos / sin as (Rz Ry) Rx, every entry a sum
+ *      of three products left to right.  A box with x_min > x_max (the default) is the xy extent of the submap's live points.
+ *   3. score: hits(h) = number of query points q with p = (R_j q) + t in an occupied voxel, R_j q summed left to right per row;
+ *      key floor(p * (1 / score_voxel)) per axis, a voxel is occupied when it holds a live map slot (tombstones skipped), a key with
+ *      |k| >= 2^20 - 1 on an axis is a miss.  Integers: the device and the oracle agree exactly.
+ *   4. candidates: the hypotheses ordered by (hits descending, h ascending); over the first M = 64 n_candidates of them, greedy
+ *      suppression in that order: a hypothesis survives when every kept one differs from it by sqrt((dx^2 + dy^2) + dz^2) > nms_distance
+ *      in translation or |remainder(yaw_a - yaw_b, 2 pi)| > nms_yaw in yaw; stop at n_candidates (fewer may survive).
+ *   5. refinement: per candidate, exactly the result of b2s_register_to_submap(match_, sm, T_c, T_c) with match_ = S1's match_ of the raw
+ *      scan (the handle's estimator and ICP parameters), 16 per batched ICP launch.  Equal to that call up to the last bits of the
+ *      ICP's fp64 sums, which are not reproducible from launch to launch (two b2s_register_to_submap calls differ there too).  A candidate whose map patch is empty (where
+ *      b2s_register_to_submap reports B2S_E_EMPTY) gets fitness 0, rmse 0, T = T_c, no correspondences.
+ *   6. decision: the winner is the candidate with the highest ICP fitness (ties -> lower rank); found = fitness >= min_refinement_fitness.
+ *      runner_up_fitness: the best fitness among candidates whose refined pose lies beyond nms_distance (translation, as in 4) or nms_yaw
+ *      (yaw = atan2(R10, R00), wrapped as in 4) of the winner's; -1 when there is none.  A runner-up close to the winner's fitness marks
+ *      an ambiguous site.
+ *   7. errors: empty map or query -> B2S_E_EMPTY; non-positive or non-finite step / score_voxel, n_yaw, n_z or n_candidates < 1,
+ *      n_candidates > 256, a non-finite box bound or parameter, y_min > y_max with an explicit box, more than 2^31 - 1 hypotheses ->
+ *      B2S_E_INVALID; the occupancy grid or the score array (4 bytes per hypothesis) over 2^30 bytes -> B2S_E_CAPACITY; the estimator's
+ *      normals rules as b2s_register_to_submap.
+ * Synchronises three times: query size, candidates, result. */
+typedef struct b2s_global_localization_params {
+  double x_min, x_max, y_min, y_max;   /* translation box [m]; x_min > x_max (default): the xy extent of the submap's live points */
+  double step;                         /* translation step, 0.25 m */
+  double z0, z_step;                   /* z levels z0 + iz z_step, iz < n_z: 0, 0.25 m */
+  int32_t n_z;                         /* 1 */
+  int32_t n_yaw;                       /* 144 */
+  double yaw0, yaw_step;               /* -pi, 2 pi / 144 */
+  double roll, pitch;                  /* fixed attitude (an IMU gives it), 0 */
+  double score_voxel;                  /* voxel of the query and of the occupancy, 1.0 m */
+  int32_t n_candidates;                /* 16, at most 256 */
+  int32_t reserved_;
+  double nms_distance, nms_yaw;        /* 1.0 m, 10 degrees (in radians) */
+} b2s_global_localization_params;
+void b2s_default_global_localization_params(b2s_global_localization_params* p);
+typedef struct b2s_global_localization_candidate {
+  double T_hypothesis[16];             /* [R_j | t] of the hypothesis (row-major) */
+  int32_t hypothesis;                  /* h */
+  int32_t hits;
+  b2s_result icp;                      /* its refinement */
+} b2s_global_localization_candidate;
+typedef struct b2s_global_localization_result {
+  double T[16];                        /* the winner's refined map_to_sensor */
+  double fitness, inlier_rmse;
+  double runner_up_fitness;            /* -1: no candidate beyond the suppression distances of the winner */
+  int64_t n_hypotheses;
+  int32_t found;
+  int32_t winner_rank;                 /* -1: no candidate */
+  int32_t n_query;
+  int32_t n_candidates;
+} b2s_global_localization_result;
+/* candidates_or_null receives the first min(n_candidates, capacity) candidates in rank order */
+int32_t b2s_submap_global_localization(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* raw_scan, const b2s_global_localization_params* p,
+                                       double min_refinement_fitness, b2s_global_localization_candidate* candidates_or_null, int32_t capacity,
+                                       b2s_global_localization_result* out);
+/* Debug aid: steps 1-3 on their own, the hits of every hypothesis (hits_out[h], capacity >= the hypothesis count) and, optionally, the
+ * query cloud (3 x f64 per point).  The counts are written before the capacity checks. */
+int32_t b2s_debug_global_localization_scores(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* raw_scan, const b2s_global_localization_params* p,
+                                             int32_t* hits_out, size_t capacity, size_t* n_hypotheses, double* query_out_or_null,
+                                             size_t query_capacity, size_t* n_query);
+
 /* ---- device-resident LidarOdometry (src/Odometry.cpp:19-110) and the combined per-scan step of SlamWrapper: odometry, then
  *      Mapper::addRangeMeasurement with the prediction read from the odometry's TransformInterpolationBuffer on the device.
  *      Every decision (initialise / ok / failed, the buffer, the prediction, the mapper gates) is taken on the device.

@@ -144,6 +144,23 @@ class MapperCounters(C.Structure):
                                          "dense_carve_runs", "carved_voxels_total")]
 
 
+class GlobalLocalizationParams(C.Structure):
+    _fields_ = [("x_min", C.c_double), ("x_max", C.c_double), ("y_min", C.c_double), ("y_max", C.c_double), ("step", C.c_double),
+                ("z0", C.c_double), ("z_step", C.c_double), ("n_z", C.c_int32), ("n_yaw", C.c_int32), ("yaw0", C.c_double),
+                ("yaw_step", C.c_double), ("roll", C.c_double), ("pitch", C.c_double), ("score_voxel", C.c_double),
+                ("n_candidates", C.c_int32), ("reserved_", C.c_int32), ("nms_distance", C.c_double), ("nms_yaw", C.c_double)]
+
+
+class GlobalLocalizationCandidate(C.Structure):
+    _fields_ = [("T_hypothesis", C.c_double * 16), ("hypothesis", C.c_int32), ("hits", C.c_int32), ("icp", Result)]
+
+
+class GlobalLocalizationResult(C.Structure):
+    _fields_ = [("T", C.c_double * 16), ("fitness", C.c_double), ("inlier_rmse", C.c_double), ("runner_up_fitness", C.c_double),
+                ("n_hypotheses", C.c_int64), ("found", C.c_int32), ("winner_rank", C.c_int32), ("n_query", C.c_int32),
+                ("n_candidates", C.c_int32)]
+
+
 # every symbol include/b2s.h declares (checked by tests/test_abi.py without needing a GPU)
 SYMBOLS = [
     "b2s_default_config", "b2s_create", "b2s_destroy", "b2s_set_config", "b2s_synchronize", "b2s_last_error", "b2s_version",
@@ -173,6 +190,7 @@ SYMBOLS = [
     "b2s_submap_set_initial_map", "b2s_submap_set_initial_transform", "b2s_submap_set_merge_scans", "b2s_debug_nn_index",
     "b2s_assemble_map", "b2s_assemble_colored_map", "b2s_debug_pose_graph_solve", "b2s_debug_pose_graph_linearize",
     "b2s_debug_estimate_normals", "b2s_debug_submap_bbox",
+    "b2s_default_global_localization_params", "b2s_submap_global_localization", "b2s_debug_global_localization_scores",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 ASSEMBLY_MAX_SUBMAPS = 65535             # B2S_ASSEMBLY_MAX_SUBMAPS
@@ -223,6 +241,7 @@ def lib():
         L.b2s_default_odometry_constraint_params.restype = None
         L.b2s_default_loop_closure_refinement_params.restype = None
         L.b2s_default_global_optimization_params.restype = None
+        L.b2s_default_global_localization_params.restype = None
         _lib = L
     return _lib
 

@@ -12,6 +12,7 @@ bench.py read like tests of the reference interface.  All arithmetic happens in 
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -997,6 +998,12 @@ class Submap:
         """Mapper::setMapToRangeSensorInitial (src/Mapper.cpp:87-91) on the device pose slot: the next step keeps T (see b2s.h)"""
         L.check(L.lib().b2s_submap_set_initial_transform(self.eng._h, self._s, _pd(_mat(T))))
 
+    def globalLocalization(self, rawCloud: "Cloud", params: "GlobalLocalizationParameters | None" = None,
+                           minRefinementFitness: float = 0.0) -> "GlobalLocalizationResult":
+        """b2s_submap_global_localization (include/b2s.h): the map_to_sensor of rawCloud in this submap's map without an initial pose.
+        Reads the submap and changes nothing; apply the pose with setInitialTransform."""
+        return globalLocalization(self.eng, self, rawCloud, params, minRefinementFitness)
+
     def setMergeScans(self, on: bool) -> None:
         """isMergeScansIntoMap_ for the device chain on this submap: off = pure localisation (src/Mapper.cpp:163-167)"""
         L.check(L.lib().b2s_submap_set_merge_scans(self.eng._h, self._s, C.c_int32(1 if on else 0)))
@@ -1566,3 +1573,86 @@ class Mapper:
         L.check(L.lib().b2s_slam_step_host_async(self.eng._h, self.submap._s, odometry._o, C.c_void_p(xyz_f32_ptr), C.c_size_t(n), C.c_size_t(stride),
                                                  C.c_int64(int(t)), C.c_double(self.params_.minRefinementFitness),
                                                  C.c_int32(int(self.params_.isIgnoreMinRefinementFitness)), C.c_void_p(out_pinned_ptr)))
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# global localisation in a prior map (b2s_submap_global_localization, DESIGN.md row M3)
+# --------------------------------------------------------------------------------------------------------------------
+@dataclass
+class GlobalLocalizationParameters:
+    """b2s_global_localization_params.  A box with xMin > xMax (the default) is the xy extent of the map's live points."""
+    xMin: float = 1.0
+    xMax: float = -1.0
+    yMin: float = 1.0
+    yMax: float = -1.0
+    step: float = 0.25
+    z0: float = 0.0
+    zStep: float = 0.25
+    nZ: int = 1
+    nYaw: int = 144
+    yaw0: float = -math.pi
+    yawStep: float = 2.0 * math.pi / 144.0
+    roll: float = 0.0
+    pitch: float = 0.0
+    scoreVoxel: float = 1.0
+    nCandidates: int = 16
+    nmsDistance: float = 1.0
+    nmsYaw: float = math.radians(10.0)
+
+    def to_c(self) -> L.GlobalLocalizationParams:
+        return L.GlobalLocalizationParams(self.xMin, self.xMax, self.yMin, self.yMax, self.step, self.z0, self.zStep, int(self.nZ), int(self.nYaw),
+                                          self.yaw0, self.yawStep, self.roll, self.pitch, self.scoreVoxel, int(self.nCandidates), 0,
+                                          self.nmsDistance, self.nmsYaw)
+
+
+@dataclass
+class GlobalLocalizationCandidate:
+    T_hypothesis: np.ndarray
+    hypothesis: int
+    hits: int
+    icp: RegistrationResult
+
+
+@dataclass
+class GlobalLocalizationResult:
+    found: bool
+    T: np.ndarray
+    fitness: float
+    inlier_rmse: float
+    runner_up_fitness: float     # -1: no candidate beyond the suppression distances of the winner
+    winner_rank: int             # -1: no candidate
+    n_hypotheses: int
+    n_query: int
+    candidates: list             # GlobalLocalizationCandidate in rank order
+
+
+def globalLocalization(eng: Engine, submap: "Submap", rawCloud: "Cloud", params: GlobalLocalizationParameters | None = None,
+                       minRefinementFitness: float = 0.0) -> GlobalLocalizationResult:
+    """Localise rawCloud (sensor frame) in submap's map with no initial pose (b2s_submap_global_localization)."""
+    p = (params or GlobalLocalizationParameters()).to_c()
+    cap = max(int(p.n_candidates), 1)
+    cands = (L.GlobalLocalizationCandidate * cap)()
+    out = L.GlobalLocalizationResult()
+    L.check(L.lib().b2s_submap_global_localization(eng._h, submap._s, rawCloud._c, C.byref(p), C.c_double(float(minRefinementFitness)), cands,
+                                                   C.c_int32(cap), C.byref(out)))
+    cl = [GlobalLocalizationCandidate(np.array(c.T_hypothesis, dtype=np.float64).reshape(4, 4), int(c.hypothesis), int(c.hits), _res(c.icp))
+          for c in cands[:out.n_candidates]]
+    return GlobalLocalizationResult(bool(out.found), np.array(out.T, dtype=np.float64).reshape(4, 4), float(out.fitness), float(out.inlier_rmse),
+                                    float(out.runner_up_fitness), int(out.winner_rank), int(out.n_hypotheses), int(out.n_query), cl)
+
+
+def debugGlobalLocalizationScores(eng: Engine, submap: "Submap", rawCloud: "Cloud", params: GlobalLocalizationParameters | None = None):
+    """b2s_debug_global_localization_scores: (hits per hypothesis, query cloud)"""
+    p = (params or GlobalLocalizationParameters()).to_c()
+    nh, nq = C.c_size_t(0), C.c_size_t(0)
+    one = np.zeros(1, dtype=np.int32)
+    rc = L.lib().b2s_debug_global_localization_scores(eng._h, submap._s, rawCloud._c, C.byref(p), one.ctypes.data_as(C.c_void_p), C.c_size_t(0),
+                                                      C.byref(nh), None, C.c_size_t(0), C.byref(nq))
+    if rc != L.E_CAPACITY or nh.value == 0:
+        L.check(rc)
+    hits = np.zeros(nh.value, dtype=np.int32)
+    q = np.zeros((nq.value, 3), dtype=np.float64)
+    L.check(L.lib().b2s_debug_global_localization_scores(eng._h, submap._s, rawCloud._c, C.byref(p), hits.ctypes.data_as(C.c_void_p),
+                                                         C.c_size_t(hits.size), C.byref(nh), q.ctypes.data_as(C.c_void_p), C.c_size_t(len(q)),
+                                                         C.byref(nq)))
+    return hits, q

@@ -399,6 +399,19 @@ class SegmentMapper:
         self.isNewInitialValueSet = True
         self.backend.set_initial_transform(self.submaps.getActiveSubmap().handle, self.mapToRangeSensor)
 
+    def globalLocalization(self, rawScanF32: np.ndarray, params=None):
+        """Localise the raw scan in the loaded prior map with no pose given (b2s_submap_global_localization, DESIGN.md row M3) -- what
+        SlamMapInitializer's marker pose does in the reference.  When the winner passes the mapper's fitness gate, setInitialTransform(T)
+        follows, so the next step keeps T (rule 3 of M2).  Logged as ("global_localization", k, found, T, fitness, runner_up) in
+        submaps.events, k = the index of the next scan.  Returns the backend's GlobalLocalizationResult."""
+        if not self.submaps.submaps:
+            raise RuntimeError("globalLocalization: no map loaded (call setInitialMap first)")
+        r = self.backend.global_localization(self.submaps.getActiveSubmap().handle, rawScanF32, params)
+        self.submaps.events.append(("global_localization", self._k, r.found, r.T.copy(), r.fitness, r.runner_up_fitness))
+        if r.found:
+            self.setInitialTransform(r.T)
+        return r
+
     def addRangeMeasurement(self, rawScanF32: np.ndarray, odometryMotion: np.ndarray):
         sc = self.submaps
         k = self._k
@@ -932,6 +945,15 @@ class DeviceBackend:
         self._odo_initial = np.array(T, dtype=np.float64)
         if self._odo is not None:
             self._odo.setInitialTransform(T)
+
+    def global_localization(self, sm, raw: np.ndarray, params: E.GlobalLocalizationParameters | None = None) -> E.GlobalLocalizationResult:
+        """b2s_submap_global_localization of a raw float32 scan in the submap's map, judged by the mapper's fitness gate
+        (MapperParameters::minRefinementFitness_); the submap is left as it was"""
+        raw_c = self.eng.cloud(np.ascontiguousarray(raw, dtype=np.float32))
+        try:
+            return sm.globalLocalization(raw_c, params, self.params.minRefinementFitness)
+        finally:
+            raw_c.free()
 
     def _activate(self, sm):
         self.mapper.submap = sm

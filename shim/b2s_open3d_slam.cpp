@@ -346,6 +346,15 @@ void SubmapB200::setMergeScans(bool on) {   // Mapper.cpp:163-167; off also keep
   if (rc != B2S_OK) b2sThrow(rc);
 }
 
+b2s_global_localization_result SubmapB200::globalLocalization(const PointCloud& rawScan, const b2s_global_localization_params& params,
+                                                              double minRefinementFitness) const {
+  DeviceCloud raw(h_, rawScan, false);
+  b2s_global_localization_result r;
+  const int32_t rc = b2s_submap_global_localization(h_, sm_, raw.c, &params, minRefinementFitness, nullptr, 0, &r);
+  if (rc != B2S_OK) b2sThrow(rc);
+  return r;
+}
+
 void SubmapB200::computeFeatures(const PlaceRecognitionParameters& p) {
   int32_t rc = B2S_OK;
   if (!sparse_ && (rc = b2s_cloud_create(h_, &sparse_)) != B2S_OK) b2sThrow(rc);

@@ -90,6 +90,10 @@ class SubmapB200 {
   bool isEmpty() const;
   void setMapPointCloud(const PointCloud& cloud);           // initial map (SlamWrapper::setInitialMap)
   void setMergeScans(bool on);                              // isMergeScansIntoMap_ for the device chain: false = pure localisation
+  // stands in for SlamMapInitializer's marker pose: the raw scan's mapToRangeSensor in this submap's map without an initial pose
+  // (b2s_submap_global_localization); the submap is left as it was.  If result.found, pass result.T to SlamWrapper::setInitialTransform.
+  b2s_global_localization_result globalLocalization(const PointCloud& rawScan, const b2s_global_localization_params& params,
+                                                    double minRefinementFitness) const;
   void computeFeatures(const PlaceRecognitionParameters& p);
   const PointCloud& getSparseMapPointCloud() const;
   const Feature& getFeatures() const;                       // throws before the first computeFeatures, like the reference
