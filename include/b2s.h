@@ -877,6 +877,27 @@ int32_t b2s_assemble_map(b2s_handle* h, int32_t n_submaps, const b2s_submap* con
 int32_t b2s_assemble_colored_map(b2s_handle* h, int32_t n_submaps, const b2s_submap* const* submaps, double voxel_size, b2s_cloud* out,
                                  double* rgb, size_t capacity, size_t* n_out);
 
+/* ---- the dense maps exported: VoxelizedPointCloud::toPointCloud (src/Voxel.cpp:90-115) of every submap's dense map, which
+ *      SlamWrapper::saveDenseSubmaps writes one PCD per submap from (SubmapCollection::dumpToFile(dir, "denseSubmap", true),
+ *      src/SubmapCollection.cpp:269-283) and SlamWrapperRos::publishDenseMap publishes for the active submap
+ *      (ros/open3d_slam_ros/src/SlamWrapperRos.cpp:213-220).  Restated rules (DESIGN.md row A2):
+ *   - content: for submaps[0], then submaps[1], ...: every slot of its dense table whose count is > 0, in slot order, as one point
+ *     sum / count per axis -- for every submap bit-identical to the xyz of b2s_submap_dense_download.  Voxels emptied by dense carving,
+ *     b2s_dense_remove or b2s_dense_clear are skipped (toPointCloud skips numAggregatedPoints_ == 0); after b2s_submap_transform the
+ *     points are what the transformed sums give (VoxelizedPointCloud::transform, Voxel.cpp:49-64)
+ *   - no normals and no colours: `out` has no normals, like the dense download
+ *   - offsets (host, n_submaps + 1 entries, NULL: not written): offsets[k] = index of submaps[k]'s first point, offsets[n_submaps] = the
+ *     total, so one download serves one file per submap.  A submap whose dense map was never initialised contributes an empty range
+ *   - a submap may appear more than once; the submaps are only read
+ *   - n_submaps = 0 or only empty dense maps: an empty cloud, B2S_OK.  Errors as b2s_assemble_map: n_submaps < 0, a null submap, a
+ *     submap or output of another handle, a fixed-capacity staging cloud as output -> B2S_E_INVALID; more than (2^31 - 1) / 3 points in
+ *     total -> B2S_E_CAPACITY, found on the device before anything is written (`out` and `offsets` untouched); n_submaps >
+ *     B2S_ASSEMBLY_MAX_SUBMAPS -> B2S_E_UNSUPPORTED.
+ * One set of launches for every dense map; synchronises exactly once, for the total and the offsets, and returns with the points
+ * still being written on the handle's stream (a download of `out` waits for them).  The scratch is the library's own and sized by the
+ * tiles of the tables, not their slots: exporting between graph-replayed mapper steps never makes a chain re-capture. */
+int32_t b2s_assemble_dense_maps(b2s_handle* h, int32_t n_submaps, const b2s_submap* const* submaps, b2s_cloud* out, int64_t* offsets);
+
 /* ---- device-to-device hand-over of a cloud's arrays (SURVEY.md section 8e: a submap that is the registration target on
  *      several GPUs is built once by its owner and broadcast over NVLink by the host side -- torch.distributed / NCCL own
  *      the transfer, this library only copies between its cloud and the caller's device buffers on the handle's stream).

@@ -191,6 +191,7 @@ SYMBOLS = [
     "b2s_assemble_map", "b2s_assemble_colored_map", "b2s_debug_pose_graph_solve", "b2s_debug_pose_graph_linearize",
     "b2s_debug_estimate_normals", "b2s_debug_submap_bbox",
     "b2s_default_global_localization_params", "b2s_submap_global_localization", "b2s_debug_global_localization_scores",
+    "b2s_assemble_dense_maps",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 ASSEMBLY_MAX_SUBMAPS = 65535             # B2S_ASSEMBLY_MAX_SUBMAPS

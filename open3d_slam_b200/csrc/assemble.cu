@@ -1,8 +1,9 @@
-// assemble.cu -- A1: the global map assembled on the device, for saving and publishing it.
+// assemble.cu -- A1: the global map assembled on the device, for saving and publishing it; A2: every submap's dense map exported.
 //
 //   Mapper::getAssembledMapPointCloud                      core/src/Mapper.cpp:183-208 (SlamWrapper::saveMap, SlamWrapperRos::publishMaps)
 //   assembleColoredPointCloud                              ros/open3d_slam_ros/src/helpers_ros.cpp:51-70
 //   o3d_slam::voxelize -> [O3D] VoxelDownSample             core/src/helpers.cpp:107-113 (assembledMapVoxelSize_, submapVoxelSize_)
+//   VoxelizedPointCloud::toPointCloud of every submap       core/src/Voxel.cpp:90-115 (SubmapCollection::dumpToFile(.., true), publishDenseMap)
 //
 // K-assemble is one set of launches over every submap, whatever their number: a job table holds each submap's map slots, device count
 // and list position; a live flag per slot (fusion's tombstones are NaN) with blockIdx.y = job, the batched scan of the flags gives each
@@ -28,6 +29,8 @@ struct AsmJob {
   int32_t* flags; int32_t* offs;                                 // per slot: live, offset of the live point within the submap
   int32_t label;                                                 // palette entry: list position % 11
   int32_t no_normals;                                            // the map has no normals (b2s_submap::no_normals)
+  __device__ long long live() const { return offs[*d_n]; }       // the job's contribution (after the batched scan)
+  __device__ bool lacks_normals() const { return no_normals != 0; }
 };
 
 __global__ void __launch_bounds__(AS_THREADS) asm_flags_kernel(const AsmJob* __restrict__ jobs) {
@@ -40,9 +43,11 @@ __global__ void __launch_bounds__(AS_THREADS) asm_flags_kernel(const AsmJob* __r
   }
 }
 
-// one CTA: base[k] = live points of the jobs before k (int64, job order); words[0] = the assembled count (0 above AS_MAX_POINTS, which
-// is reported as ST_CAPACITY), words[1] = a job that contributes a point has no normals
-__global__ void __launch_bounds__(AS_BASE_THREADS) asm_base_kernel(const AsmJob* __restrict__ jobs, int njobs, long long* __restrict__ base,
+// one CTA: base[k] = live points of the jobs before k (int64, job order), base[njobs] = their total; words[0] = *out_n = the assembled
+// count (0 above AS_MAX_POINTS, which is reported as ST_CAPACITY), words[1] = a job that contributes a point has no normals.
+// Job: AsmJob (A1) or DenseJob (A2), read through live() and lacks_normals()
+template <typename Job>
+__global__ void __launch_bounds__(AS_BASE_THREADS) asm_base_kernel(const Job* __restrict__ jobs, int njobs, long long* __restrict__ base,
                                                                    int32_t* out_n, int32_t* words, uint32_t* status) {
   pdl_wait();
   __shared__ long long s_warp[AS_BASE_THREADS / 32];
@@ -55,8 +60,8 @@ __global__ void __launch_bounds__(AS_BASE_THREADS) asm_base_kernel(const AsmJob*
     const int k = r0 + tid;
     long long t = 0;
     if (k < njobs) {
-      t = jobs[k].offs[*jobs[k].d_n];
-      if (t > 0 && jobs[k].no_normals) mixed = 1;
+      t = jobs[k].live();
+      if (t > 0 && jobs[k].lacks_normals()) mixed = 1;
     }
     long long inc = t;
 #pragma unroll
@@ -175,7 +180,7 @@ int32_t op_assemble_map(b2s_handle* h, int n, const b2s_submap* const* submaps, 
   launch_pdl(asm_flags_kernel, dim3((unsigned)bx, (unsigned)n), AS_THREADS, 0, h->stream, dj);
   h->launches++;
   B2S_TRY(scan_exclusive_i32_batch(h, ds, n, max_n));
-  launch_pdl(asm_base_kernel, 1, AS_BASE_THREADS, 0, h->stream, dj, n, base, dst->dn.as<int32_t>(), words, h->status.as<uint32_t>());
+  launch_pdl(asm_base_kernel<AsmJob>, 1, AS_BASE_THREADS, 0, h->stream, dj, n, base, dst->dn.as<int32_t>(), words, h->status.as<uint32_t>());
   launch_pdl(asm_scatter_kernel, dim3((unsigned)bx, (unsigned)n), AS_THREADS, 0, h->stream, dj, base, words, palette, dst->xyz.as<double>(),
              colored ? nullptr : dst->nrm.as<double>(), colored && vox ? A.labels.as<int32_t>() : nullptr,
              colored && !vox ? A.rgb.as<double>() : nullptr);
@@ -221,6 +226,182 @@ int32_t op_assemble_map(b2s_handle* h, int n, const b2s_submap* const* submaps, 
     B2S_CUDA(cudaMemcpyAsync(rgb, A.rgb.p, cnt * 24, cudaMemcpyDeviceToHost, h->stream));
     B2S_CUDA(cudaStreamSynchronize(h->stream));
   }
+  return B2S_OK;
+}
+
+// ---- A2: the dense maps ---------------------------------------------------------------------------------------------------------------
+// K-dense-export is one set of launches over every listed dense table.  The tables are mostly empty (2^22 slots, at most 7/8 usable), so
+// nothing is kept per slot: a count pass writes the live slots of every 2048-slot tile (blockIdx.y = table), the batched scan turns them
+// into tile offsets, asm_base_kernel scans the per-entry totals into int64 bases and checks the capacity, and after the one
+// synchronisation (the total sizes the output) a gather recomputes each live slot's rank within its tile and writes sum / count.
+constexpr int DX_ITEMS = 8;                        // consecutive slots per thread: two int4 loads of the counts
+constexpr int DX_TILE = AS_THREADS * DX_ITEMS;     // slots per CTA
+
+struct DenseTable {                  // one listed entry that has a dense map
+  const int32_t* cnt; const double* sum;         // the table: count and 6 running sums per slot
+  int32_t* tiles; int32_t* toffs;                // per tile: live slots; their exclusive scan (toffs[ntiles] = the table's live voxels)
+  long long cap;                                 // slots
+  int32_t ntiles;                                // tiles of DX_TILE slots (the batched scan reads its length here)
+  int32_t entry;                                 // list position: where its points go
+};
+struct DenseJob {                    // one listed entry, for asm_base_kernel
+  const int32_t* total;                          // its table's toffs[ntiles], or a zero word without a dense map
+  __device__ long long live() const { return *total; }
+  __device__ bool lacks_normals() const { return true; }   // the dense export has no normals
+};
+
+// the counts of slots s0 .. s0 + DX_ITEMS - 1 (0 past the table) into c; returns how many are live (count > 0)
+__device__ __forceinline__ int dx_load(const int32_t* __restrict__ cnt, long long cap, long long s0, int32_t c[DX_ITEMS]) {
+  if (s0 + DX_ITEMS <= cap) {
+    const int4 a = *reinterpret_cast<const int4*>(cnt + s0), b = *reinterpret_cast<const int4*>(cnt + s0 + 4);
+    c[0] = a.x; c[1] = a.y; c[2] = a.z; c[3] = a.w; c[4] = b.x; c[5] = b.y; c[6] = b.z; c[7] = b.w;
+  } else {
+#pragma unroll
+    for (int k = 0; k < DX_ITEMS; k++) c[k] = s0 + k < cap ? cnt[s0 + k] : 0;
+  }
+  int live = 0;
+#pragma unroll
+  for (int k = 0; k < DX_ITEMS; k++) live += c[k] > 0;
+  return live;
+}
+
+__global__ void __launch_bounds__(AS_THREADS) dx_count_kernel(const DenseTable* __restrict__ tabs) {
+  pdl_wait();
+  const DenseTable t = tabs[blockIdx.y];
+  if ((int)blockIdx.x >= t.ntiles) return;
+  __shared__ int s_warp[AS_THREADS / 32];
+  int32_t c[DX_ITEMS];
+  const int live = warp_sum_i(dx_load(t.cnt, t.cap, (long long)blockIdx.x * DX_TILE + threadIdx.x * DX_ITEMS, c));
+  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = live;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int s = 0;
+    for (int w = 0; w < AS_THREADS / 32; w++) s += s_warp[w];
+    t.tiles[blockIdx.x] = s;
+  }
+}
+
+// Voxel.cpp:90-115 per live slot, in slot order: the same division as dense_gather_kernel (b2s_submap_dense_download)
+__global__ void __launch_bounds__(AS_THREADS) dx_gather_kernel(const DenseTable* __restrict__ tabs, const long long* __restrict__ base,
+                                                               double* __restrict__ oxyz) {
+  pdl_wait();
+  const DenseTable t = tabs[blockIdx.y];
+  if ((int)blockIdx.x >= t.ntiles) return;
+  __shared__ int s_warp[AS_THREADS / 32];
+  const long long s0 = (long long)blockIdx.x * DX_TILE + threadIdx.x * DX_ITEMS;
+  int32_t c[DX_ITEMS];
+  const int live = dx_load(t.cnt, t.cap, s0, c);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int inc = live;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += v; }
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  int woff = 0;
+  for (int w = 0; w < warp; w++) woff += s_warp[w];
+  if (live == 0) return;
+  size_t o = (size_t)(base[t.entry] + t.toffs[blockIdx.x] + woff + inc - live);
+#pragma unroll
+  for (int k = 0; k < DX_ITEMS; k++) {
+    if (c[k] <= 0) continue;
+    const double* s = t.sum + 6 * (size_t)(s0 + k);
+    const double n = (double)c[k];
+    oxyz[3 * o] = s[0] / n; oxyz[3 * o + 1] = s[1] / n; oxyz[3 * o + 2] = s[2] / n;
+    o++;
+  }
+}
+
+int32_t op_assemble_dense_maps(b2s_handle* h, int n, const b2s_submap* const* submaps, b2s_cloud* out, int64_t* offsets) {
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  int m = 0;   // entries with a dense map
+  size_t max_tiles = 1, slot_bytes = 0;
+  for (int k = 0; k < n; k++) {
+    const size_t cap = submaps[k]->dense_cap;
+    if (cap == 0) continue;
+    const size_t nt = (cap + DX_TILE - 1) / DX_TILE;
+    if (nt > max_tiles) max_tiles = nt;
+    slot_bytes += al(scan_state_bytes(nt)) + al(nt * 4) + al((nt + 2) * 4);
+    m++;
+  }
+  if (m == 0) {   // nothing to read: every range is empty
+    if (offsets) for (int k = 0; k <= n; k++) offsets[k] = 0;
+    B2S_TRY(cloud_reserve(h, out, 0, false));
+    B2S_TRY(cloud_set_count(h, out, 0));
+    out->has_normals = false;
+    return B2S_OK;
+  }
+  AssemblyScratch& A = h->assembly;
+  // tables: [DenseTable x m][ScanJob x m][DenseJob x n][zero word] staged from the host, then [base x (n + 1)][out_n, words x 2] written
+  // on the device.  The stage also receives the bases.
+  const size_t t_tab = al((size_t)m * sizeof(DenseTable)), t_scan = al((size_t)m * sizeof(ScanJob)), t_jobs = al((size_t)n * sizeof(DenseJob));
+  const size_t staged = t_tab + t_scan + t_jobs + 256, t_base = al(((size_t)n + 1) * 8);
+  B2S_TRY(A.tables.ensure(staged + t_base + 256, h->stream));
+  B2S_TRY(A.slots.ensure(slot_bytes, h->stream));
+  if (A.stage.cap < staged + t_base) B2S_TRY(A.stage.alloc(2 * (staged + t_base)));   // every earlier call synchronised after its upload
+  unsigned char* st = A.stage.as<unsigned char>();
+  unsigned char* tab = A.tables.as<unsigned char>();
+  DenseTable* ht = reinterpret_cast<DenseTable*>(st);
+  ScanJob* hs = reinterpret_cast<ScanJob*>(st + t_tab);
+  DenseJob* hj = reinterpret_cast<DenseJob*>(st + t_tab + t_scan);
+  memset(st + t_tab + t_scan + t_jobs, 0, 256);
+  const int32_t* zero = reinterpret_cast<const int32_t*>(tab + t_tab + t_scan + t_jobs);
+  unsigned char* slots = A.slots.as<unsigned char>();
+  size_t off = 0;
+  for (int k = 0, t = 0; k < n; k++) {   // tile states first: they are the region zeroed below
+    const size_t cap = submaps[k]->dense_cap;
+    if (cap == 0) continue;
+    const size_t nt = (cap + DX_TILE - 1) / DX_TILE;
+    unsigned long long* s = reinterpret_cast<unsigned long long*>(slots + off);
+    hs[t].state = s;
+    hs[t].counter = reinterpret_cast<int32_t*>(s + (scan_state_bytes(nt) - 64) / 8);
+    off += al(scan_state_bytes(nt));
+    t++;
+  }
+  const size_t state_bytes = off;
+  for (int k = 0, t = 0; k < n; k++) {
+    const b2s_submap* sm = submaps[k];
+    if (sm->dense_cap == 0) { hj[k].total = zero; continue; }
+    const size_t nt = (sm->dense_cap + DX_TILE - 1) / DX_TILE;
+    DenseTable& T = ht[t];
+    T.cnt = sm->dense_cnt.as<int32_t>(); T.sum = sm->dense_sum.as<double>();
+    T.tiles = reinterpret_cast<int32_t*>(slots + off); off += al(nt * 4);
+    T.toffs = reinterpret_cast<int32_t*>(slots + off); off += al((nt + 2) * 4);
+    T.cap = (long long)sm->dense_cap; T.ntiles = (int32_t)nt; T.entry = k;
+    hs[t].in = T.tiles; hs[t].out = T.toffs;
+    hs[t].d_n = reinterpret_cast<const int32_t*>(tab + (size_t)t * sizeof(DenseTable) + offsetof(DenseTable, ntiles));
+    hj[k].total = T.toffs + nt;
+    t++;
+  }
+  B2S_CUDA(cudaMemcpyAsync(tab, st, staged, cudaMemcpyHostToDevice, h->stream));
+  B2S_CUDA(cudaMemsetAsync(slots, 0, state_bytes, h->stream));
+  const DenseTable* dt = reinterpret_cast<const DenseTable*>(tab);
+  const ScanJob* ds = reinterpret_cast<const ScanJob*>(tab + t_tab);
+  const DenseJob* dj = reinterpret_cast<const DenseJob*>(tab + t_tab + t_scan);
+  long long* base = reinterpret_cast<long long*>(tab + staged);
+  int32_t* words = reinterpret_cast<int32_t*>(tab + staged + t_base);   // [0] the count, [1..2] asm_base_kernel's words
+
+  launch_pdl(dx_count_kernel, dim3((unsigned)max_tiles, (unsigned)m), AS_THREADS, 0, h->stream, dt);
+  h->launches++;
+  B2S_TRY(scan_exclusive_i32_batch(h, ds, m, max_tiles));
+  launch_pdl(asm_base_kernel<DenseJob>, 1, AS_BASE_THREADS, 0, h->stream, dj, n, base, words, words + 1, h->status.as<uint32_t>());
+  h->launches++;
+  B2S_CUDA(cudaGetLastError());
+
+  // the one synchronisation: the bases are the offsets, the last one the total; above AS_MAX_POINTS the status reports ST_CAPACITY
+  // and nothing has been written
+  long long* hb = reinterpret_cast<long long*>(st + staged);
+  B2S_CUDA(cudaMemcpyAsync(hb, base, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, h->stream));
+  B2S_TRY(check_status(h));
+  const size_t total = (size_t)hb[n];
+  if (offsets) for (int k = 0; k <= n; k++) offsets[k] = hb[k];
+  B2S_TRY(cloud_reserve(h, out, total, false));
+  if (total > 0) {
+    launch_pdl(dx_gather_kernel, dim3((unsigned)max_tiles, (unsigned)m), AS_THREADS, 0, h->stream, dt, base, out->xyz.as<double>());
+    h->launches++;
+  }
+  B2S_TRY(cloud_set_count(h, out, total));
+  out->has_normals = false;
+  B2S_CUDA(cudaGetLastError());
   return B2S_OK;
 }
 

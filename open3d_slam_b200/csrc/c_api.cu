@@ -1504,6 +1504,14 @@ int32_t b2s_assemble_colored_map(b2s_handle* h, int32_t n, const b2s_submap* con
   return op_assemble_map(h, n, submaps, voxel_size, out, true, rgb, capacity, n_out);
 }
 
+// VoxelizedPointCloud::toPointCloud (Voxel.cpp:90-115) of every submap's dense map: SubmapCollection::dumpToFile(dir, "denseSubmap", true)
+// (SubmapCollection.cpp:269-283) and SlamWrapperRos::publishDenseMap (SlamWrapperRos.cpp:213-220)
+int32_t b2s_assemble_dense_maps(b2s_handle* h, int32_t n, const b2s_submap* const* submaps, b2s_cloud* out, int64_t* offsets) {
+  B2S_TRY(check_assembly_args(h, n, submaps, out));
+  LOCK(h);
+  return op_assemble_dense_maps(h, n, submaps, out, offsets);
+}
+
 // debug aid for tests: the header, cell starts and original indices of the NN index the last registration built (h->grid_a).
 // dims_n = {dims[0..2], ncell, n}; cell_start (ncell + 1 entries) and orig (n entries) are skipped when null or too small.
 int32_t b2s_debug_nn_index(b2s_handle* h, double origin_cell[4], int32_t dims_n[5], int32_t* cell_start, size_t cap_cells, int32_t* orig,

@@ -238,15 +238,16 @@ struct b2s_submap {
 };
 
 namespace b2s {
-// Scratch of the operators that work on the whole map (b2s_assemble_map, assemble.cu).  Every buffer is sized to the assembled map and
+// Scratch of the operators that work on the whole map (b2s_assemble_map, b2s_assemble_dense_maps, assemble.cu).  Every buffer is sized to the assembled map and
 // grows with it, so none is tracked: no captured chain reads them, and their growth must not make the mapper chains re-capture.
 struct VoxelScratch {    // op_voxel_down_sample's own scratch instead of the handle's keys / vals / flags / offs, scan state and sort histogram
   DevBuf keys, vals, flags, offs, scan_state, sort_hist;
   VoxelScratch() { for (DevBuf* b : {&keys, &vals, &flags, &offs, &scan_state, &sort_hist}) b->tracked = false; }
 };
 struct AssemblyScratch {
-  DevBuf tables;         // AsmJob + ScanJob tables, the per-job base offsets and the palette
-  DevBuf slots;          // per map slot of every job: live flag, offset within the submap; the batched scan's tile states
+  DevBuf tables;         // AsmJob / DenseTable + ScanJob tables, the per-job base offsets and the palette
+  DevBuf slots;          // per map slot of every job: live flag, offset within the submap (A1); per dense-table tile: live voxels,
+                         // their offset within the table (A2); the batched scan's tile states
   DevBuf labels;         // int32 per assembled point: palette entry (coloured call, voxel path)
   DevBuf rgb;            // 3 x f64 per output point (coloured call)
   PinnedBuf stage;       // page-locked staging of the tables
@@ -354,7 +355,7 @@ struct b2s_handle {
   b2s::DevBuf pg_A, pg_F, pg_W, pg_vec, pg_nodes, pg_edges;
   int32_t pg_edge_cap = 0;
   b2s::GraphCache pg_graph;
-  b2s::AssemblyScratch assembly;      // b2s_assemble_map / b2s_assemble_colored_map (assemble.cu owns the layouts)
+  b2s::AssemblyScratch assembly;      // b2s_assemble_map / _colored_map / _dense_maps (assemble.cu owns the layouts)
 };
 
 // every entry point that touches a handle's stream or buffers holds its lock and works on its device
@@ -446,6 +447,9 @@ int32_t bbox_reduce(b2s_handle* h, const double* xyz, const int32_t* d_n, size_t
 // n x 3, capacity / n_out like b2s_submap_dense_download.  Validated arguments.
 int32_t op_assemble_map(b2s_handle* h, int n, const b2s_submap* const* submaps, double voxel, b2s_cloud* out, bool colored, double* rgb,
                         size_t capacity, size_t* n_out);
+// A2 (assemble.cu): VoxelizedPointCloud::toPointCloud of every listed submap's dense map, concatenated; offsets (optional, host): n + 1
+// entries.  Validated arguments.
+int32_t op_assemble_dense_maps(b2s_handle* h, int n, const b2s_submap* const* submaps, b2s_cloud* out, int64_t* offsets);
 // flags (optional, one int per point of c): only flagged points get a normal.  with_prior: c's normals on entry are the priors of
 // [O3D] EstimateNormals on a cloud that has normals (keep the prior for a zero solver result, flip against it otherwise)
 // dbg (b2s_debug_estimate_normals only; nullptr everywhere else): rec, 10 doubles per ORIGINAL point index, receives the nine cumulants

@@ -549,6 +549,17 @@ def assembleColoredPointCloud(eng: Engine, submaps, voxelSize: float = 0.0):
     return out, rgb[:m.value].copy()
 
 
+def assembleDenseMaps(eng: Engine, submaps, out: "Cloud | None" = None):
+    """VoxelizedPointCloud::toPointCloud (src/Voxel.cpp:90-115) of every Submap's dense map in list order, in one device call
+    (b2s_assemble_dense_maps; rules in include/b2s.h): (Cloud without normals, int64 offsets of n + 1 entries -- submap k's points are
+    rows offsets[k]:offsets[k + 1]).  A submap without a dense map gives an empty range."""
+    n, arr = _submap_array(submaps)
+    out = out if out is not None else Cloud(eng)
+    offsets = np.zeros(n + 1, dtype=np.int64)
+    L.check(L.lib().b2s_assemble_dense_maps(eng._h, C.c_int32(n), arr, out._c, offsets.ctypes.data_as(C.POINTER(C.c_int64))))
+    return out, offsets
+
+
 @dataclass
 class PoseGraphNode:
     """[O3D] PoseGraphNode: pose_ (4x4)"""
@@ -953,6 +964,11 @@ class Submap:
         L.check(L.lib().b2s_submap_dense_download(self.eng._h, self._s, _pd(xyz), None, keys.ctypes.data_as(C.POINTER(C.c_int32)),
                                                   C.c_size_t(capacity), C.byref(m)))
         return xyz[:m.value].copy(), keys[:m.value].copy()
+
+    def getDenseMapPointCloud(self, out: "Cloud | None" = None) -> "Cloud":
+        """getDenseMapCopy().toPointCloud() (src/Voxel.cpp:90-115) without leaving the device: the dense map's voxel means in slot
+        order, no normals (b2s_assemble_dense_maps of this submap alone)"""
+        return assembleDenseMaps(self.eng, [self], out)[0]
 
     # ---- VoxelHashMap query interface on the dense map (include/open3d_slam/VoxelHashMap.hpp:104-158), batched ----
     def denseQuery(self, points: Cloud, with_means: bool = True):

@@ -464,6 +464,19 @@ class SegmentMapper:
         """assembleColoredPointCloud (ros/open3d_slam_ros/src/helpers_ros.cpp:51-70) + voxelize(submapVoxelSize_): (cloud, rgb)"""
         return self.backend.assembled_colored_map([s.handle for s in self.submaps.submaps], voxelSize)
 
+    def getDenseSubmapPointClouds(self) -> list:
+        """SubmapCollection::dumpToFile(dir, "denseSubmap", true) (src/SubmapCollection.cpp:269-283), which SlamWrapper::saveDenseSubmaps
+        calls: getDenseMapCopy().toPointCloud() of every submap, one n x 3 array per submap in submap order (a submap without a dense
+        map gives an empty one).  Writing the files stays with the caller.  The mapper never calls it on its own."""
+        return self.backend.dense_map_clouds([s.handle for s in self.submaps.submaps])
+
+    def getActiveDenseMapPointCloud(self):
+        """The active submap's getDenseMapCopy().toPointCloud(), as SlamWrapperRos::publishDenseMap publishes it
+        (ros/open3d_slam_ros/src/SlamWrapperRos.cpp:213-220): an n x 3 array"""
+        if not self.submaps.submaps:
+            return np.zeros((0, 3))
+        return self.backend.dense_map_clouds([self.submaps.getActiveSubmap().handle])[0]
+
     def _after_step(self, k: int, res, inserted: bool, t: int | None = None):
         sc = self.submaps
         self.results.append(res)
@@ -1052,6 +1065,13 @@ class DeviceBackend:
     def assembled_colored_map(self, sms, voxelSize: float):
         """(device Cloud, host rgb) of one b2s_assemble_colored_map call"""
         return E.assembleColoredPointCloud(self.eng, sms, voxelSize)
+
+    def dense_map_clouds(self, sms) -> list:
+        """toPointCloud of every submap's dense map: one b2s_assemble_dense_maps call and one download, split by its offsets"""
+        c, offsets = E.assembleDenseMaps(self.eng, sms)
+        xyz, _ = c.download()
+        c.free()
+        return [xyz[offsets[k]:offsets[k + 1]] for k in range(len(sms))]
 
     def map_center(self, sm) -> np.ndarray:
         xyz, _ = sm.getMapPointCloud()

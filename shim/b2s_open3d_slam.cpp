@@ -588,4 +588,21 @@ PointCloud assembleColoredPointCloudB200(const std::vector<const SubmapB200*>& s
   return cloud;
 }
 
+std::vector<PointCloud> getDenseSubmapPointCloudsB200(const std::vector<const SubmapB200*>& submaps) {
+  std::vector<PointCloud> clouds(submaps.size());
+  if (submaps.empty()) return clouds;
+  b2s_handle* h = nullptr;
+  const std::vector<const b2s_submap*> sms = assemblyInputs(submaps, &h);
+  DeviceCloud out(h);
+  std::vector<int64_t> offsets(sms.size() + 1);
+  const int32_t rc = b2s_assemble_dense_maps(h, (int32_t)sms.size(), sms.data(), out.c, offsets.data());
+  if (rc != B2S_OK) b2sThrow(rc);
+  const PointCloudPtr all = out.download();
+  for (size_t k = 0; k < sms.size(); ++k)
+    clouds[k].points_.assign(all->points_.begin() + offsets[k], all->points_.begin() + offsets[k + 1]);
+  return clouds;
+}
+
+PointCloud SubmapB200::getDenseMapPointCloud() const { return std::move(getDenseSubmapPointCloudsB200({this}).front()); }
+
 }  // namespace o3d_slam

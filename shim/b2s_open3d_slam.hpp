@@ -87,6 +87,9 @@ class SubmapB200 {
   bool insertScanDenseMap(const PointCloud& rawScan, const Transform& mapToRangeSensor, bool isPerformCarving);
   void transform(const Transform& T);
   const PointCloud& getMapPointCloud() const;
+  // getDenseMapCopy().toPointCloud() (src/Voxel.cpp:90-115) as SlamWrapperRos::publishDenseMap publishes it for the active submap: the
+  // dense map's voxel means, no normals, no colours.  One b2s_assemble_dense_maps call and one download (DESIGN.md row A2).
+  PointCloud getDenseMapPointCloud() const;
   bool isEmpty() const;
   void setMapPointCloud(const PointCloud& cloud);           // initial map (SlamWrapper::setInitialMap)
   void setMergeScans(bool on);                              // isMergeScansIntoMap_ for the device chain: false = pure localisation
@@ -167,6 +170,11 @@ PointCloud getAssembledMapPointCloudB200(const std::vector<const SubmapB200*>& s
 // assembleColoredPointCloud (ros/open3d_slam_ros/src/helpers_ros.cpp:51-70) + voxelize(voxelSize) as publishMaps runs it with
 // submapVoxelSize_: points_ and colors_ (submap j in Color::getColor(j % 11 + 2)), no normals.  One b2s_assemble_colored_map call.
 PointCloud assembleColoredPointCloudB200(const std::vector<const SubmapB200*>& submaps, double voxelSize);
+// SubmapCollection::dumpToFile(dir, "denseSubmap", true) (src/SubmapCollection.cpp:269-283), which SlamWrapper::saveDenseSubmaps calls:
+// getDenseMapCopy().toPointCloud() of every submap (all on one handle), one PointCloud per submap in the order given (empty for a submap
+// whose dense map was never fed).  One b2s_assemble_dense_maps call, one download, split by its offsets; writing the PCDs stays with the
+// caller, as for saveMap.
+std::vector<PointCloud> getDenseSubmapPointCloudsB200(const std::vector<const SubmapB200*>& submaps);
 
 // OptimizationProblem::solve (src/OptimizationProblem.cpp:25-44): in place of GlobalOptimization(poseGraph_, LevenbergMarquardt, criteria,
 // option) at :40, with option from params_.globalOptimization_ and [O3D]'s default GlobalOptimizationConvergenceCriteria.  One
