@@ -99,7 +99,7 @@ void destroy_object(T* obj) {
 // device-side status word: kernels OR error bits into it, the host checks it when it synchronises
 enum : uint32_t { ST_KEY_OVERFLOW = 1u, ST_CAPACITY = 2u, ST_EMPTY = 4u, ST_HASH_FULL = 8u };
 
-struct GridHeader {      // one per nearest-neighbour grid, lives in device memory
+struct GridHeader {      // one per nearest-neighbour grid, lives in device memory; searched through the helpers after dist2_exact
   double origin[3];
   double cell, inv_cell;
   int32_t dims[3];
@@ -709,6 +709,179 @@ __device__ __forceinline__ void vec6_to_mat4_dev(const double (&x)[6], double* T
 __device__ __forceinline__ double dist2_exact(double ax, double ay, double az, double bx, double by, double bz) {
   double dx = __dsub_rn(ax, bx), dy = __dsub_rn(ay, by), dz = __dsub_rn(az, bz);
   return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
+// ---- Searches over a K-index grid (GridHeader, grid_index.cu) ----
+// Every search follows the rules of the build and of the oracle's KD-tree, so that its neighbours match the oracle's bit for bit:
+// a coordinate's cell is grid_axis_cell, a neighbour qualifies only if d2 < r2 (dist2_exact), and neighbours are ordered by
+// (d2, original index).  icp.cu keeps its own tuned scan over a register copy of the header (GridView), on the same rules.
+
+// cell of coordinate v on an axis with origin o and n cells, clamped into the grid: the build files every point with it, outside
+// points into the border cells
+__device__ __forceinline__ int grid_axis_cell(double v, double o, double inv_cell, int n) {
+  return (int)fmin(fmax(floor((v - o) * inv_cell), 0.0), (double)(n - 1));
+}
+
+// the (d2, original index) order of neighbours: equal distances go to the lower index
+__device__ __forceinline__ bool nn_key_less(double da, int ia, double db, int ib) { return da < db || (da == db && ia < ib); }
+
+// distance from q to cell i of an axis with n cells (border cells reach to infinity), less eps and at least 0
+__device__ __forceinline__ double slab_gap(double q, double o, double cell, int i, int n, double eps) {
+  double g = 0.0;
+  if (i > 0) { double lo = o + (double)i * cell; if (q < lo) g = lo - q; }
+  if (i < n - 1) { double hi = o + (double)(i + 1) * cell; if (q > hi) g = q - hi; }
+  g -= eps;  // slack: cell membership was decided with floor((p-o)*inv), which can disagree with o+i*cell by an ulp
+  return g > 0.0 ? g : 0.0;
+}
+
+// distance from q to the nearest face of the (2R+1)^3 block around cell c that has cells beyond it, less eps and at least 0: every
+// point outside the block lies further away.  INFINITY once the block covers the grid.
+__device__ __forceinline__ double ring_bound(const GridHeader& g, const double (&q)[3], const int (&c)[3], int R, double eps) {
+  double bound = INFINITY;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    if (c[a] - R > 0) bound = fmin(bound, q[a] - (g.origin[a] + (double)(c[a] - R) * g.cell));
+    if (c[a] + R < g.dims[a] - 1) bound = fmin(bound, (g.origin[a] + (double)(c[a] + R + 1) * g.cell) - q[a]);
+  }
+  if (bound == INFINITY) return bound;
+  bound -= eps;
+  return bound > 0.0 ? bound : 0.0;
+}
+
+// Exact hybrid k-NN of q -- the knn nearest with d2 < r2, in (d2, index) order -- by one warp, every lane with the same query.
+// Rings R = 0, 1, .. of cells around q's cell: per ring each lane first resolves ONE (y, z) row (the slab-gap test and the two
+// dependent cell_start loads, the latency that dominates in empty space), then the warp walks the non-empty rows together, 32
+// candidates per step.  The k best are a sorted list of ROWS * 32 entries: position p = m * 32 + lane is register row m of that
+// lane, holding d2 (ed), original index (ei) and, with kSlot, slot in pts (es; left untouched without, which keeps the registers
+// of a caller that does not need it); empty entries are (INFINITY, 0x7fffffff, -1).  A qualifying
+// candidate is inserted with one shuffle-up of every row, lane 31 of row m - 1 carried into lane 0 of row m.  The walk ends once
+// the nearest block face with cells behind it lies beyond the k-th best.  Requires 1 <= knn <= ROWS * 32.
+template <int ROWS, bool kSlot>
+__device__ __forceinline__ void grid_knn_walk(const GridHeader& g, const int32_t* __restrict__ cs, const double4* __restrict__ pts,
+                                              double qx, double qy, double qz, int knn, double r2,
+                                              double (&ed)[ROWS], int (&ei)[ROWS], int (&es)[ROWS]) {
+  const unsigned FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const double eps = 1e-9 * g.cell;
+  const int nx = g.dims[0], ny = g.dims[1], nz = g.dims[2];
+  const double q[3] = {qx, qy, qz};
+  const int c[3] = {grid_axis_cell(qx, g.origin[0], g.inv_cell, nx), grid_axis_cell(qy, g.origin[1], g.inv_cell, ny),
+                    grid_axis_cell(qz, g.origin[2], g.inv_cell, nz)};
+  const int cx = c[0], cy = c[1], cz = c[2];
+  const int km = (knn - 1) >> 5, kl = (knn - 1) & 31;   // list position of the k-th neighbour
+#pragma unroll
+  for (int m = 0; m < ROWS; ++m) { ed[m] = INFINITY; ei[m] = 0x7fffffff; if (kSlot) es[m] = -1; }
+  double kd = INFINITY; int ki = 0x7fffffff;   // current k-th best
+  for (int R = 0;; ++R) {
+    const int side = 2 * R + 1;
+    const int x0 = max(cx - R, 0), x1 = min(cx + R, nx - 1);
+    for (int t0 = 0; t0 < side * side; t0 += 32) {
+      int a0 = 0, b0 = 0, a1 = 0, b1 = 0;   // this lane's row: the whole x-run on the ring's shell, else its two end cells
+      const int t = t0 + lane;
+      if (t < side * side) {
+        const int z = cz - R + t / side, y = cy - R + t % side;
+        if (z >= 0 && z < nz && y >= 0 && y < ny) {
+          const double gz = slab_gap(qz, g.origin[2], g.cell, z, nz, eps);
+          const double gy = slab_gap(qy, g.origin[1], g.cell, y, ny, eps);
+          if (gz * gz + gy * gy <= fmin(kd, r2)) {
+            const int row = (z * ny + y) * nx;
+            if (z == cz - R || z == cz + R || y == cy - R || y == cy + R) { a0 = cs[row + x0]; b0 = cs[row + x1 + 1]; }
+            else {
+              if (cx - R >= 0) { a0 = cs[row + cx - R]; b0 = cs[row + cx - R + 1]; }
+              if (cx + R <= nx - 1) { a1 = cs[row + cx + R]; b1 = cs[row + cx + R + 1]; }
+            }
+          }
+        }
+      }
+      for (int part = 0; part < 2; ++part) {
+        unsigned rows = __ballot_sync(FULL, part == 0 ? (b0 > a0) : (b1 > a1));
+        while (rows) {
+          const int src_lane = __ffs(rows) - 1;
+          rows &= rows - 1;
+          const int a = __shfl_sync(FULL, part == 0 ? a0 : a1, src_lane);
+          const int b = __shfl_sync(FULL, part == 0 ? b0 : b1, src_lane);
+          for (int j0 = a; j0 < b; j0 += 32) {
+            const int j = j0 + lane;
+            double d = INFINITY; int idx = 0x7fffffff;
+            if (j < b) {
+              const double4 p = pts[j];
+              d = dist2_exact(qx, qy, qz, p.x, p.y, p.z);
+              idx = (int)__double_as_longlong(p.w);
+            }
+            unsigned mask = __ballot_sync(FULL, j < b && d < r2 && nn_key_less(d, idx, kd, ki));
+            while (mask) {
+              const int src = __ffs(mask) - 1;
+              mask &= mask - 1;
+              const double cd = __shfl_sync(FULL, d, src);
+              const int ci = __shfl_sync(FULL, idx, src);
+              if (!nn_key_less(cd, ci, kd, ki)) continue;   // an earlier insertion of this batch moved the k-th entry
+              double pd[ROWS], td[ROWS]; int pi[ROWS], ti[ROWS], ps[ROWS], ts[ROWS];
+#pragma unroll
+              for (int m = 0; m < ROWS; ++m) {
+                pd[m] = __shfl_up_sync(FULL, ed[m], 1); pi[m] = __shfl_up_sync(FULL, ei[m], 1);
+                td[m] = __shfl_sync(FULL, ed[m], 31); ti[m] = __shfl_sync(FULL, ei[m], 31);
+                if (kSlot) { ps[m] = __shfl_up_sync(FULL, es[m], 1); ts[m] = __shfl_sync(FULL, es[m], 31); }
+              }
+#pragma unroll
+              for (int m = 0; m < ROWS; ++m) {   // the entry one position before this lane's: lane - 1, or lane 31 of the row above
+                const bool has_prev = lane > 0 || m > 0;
+                const double prd = lane > 0 ? pd[m] : (m > 0 ? td[m > 0 ? m - 1 : 0] : -INFINITY);
+                const int pri = lane > 0 ? pi[m] : (m > 0 ? ti[m > 0 ? m - 1 : 0] : -1);
+                if (nn_key_less(cd, ci, ed[m], ei[m])) {
+                  if (has_prev && nn_key_less(cd, ci, prd, pri)) {
+                    ed[m] = prd; ei[m] = pri;
+                    if (kSlot) es[m] = lane > 0 ? ps[m] : ts[m > 0 ? m - 1 : 0];
+                  } else {
+                    ed[m] = cd; ei[m] = ci;
+                    if (kSlot) es[m] = j0 + src;
+                  }
+                }
+              }
+              double kdl = ed[0]; int kil = ei[0];
+#pragma unroll
+              for (int m = 1; m < ROWS; ++m) if (m == km) { kdl = ed[m]; kil = ei[m]; }
+              kd = __shfl_sync(FULL, kdl, kl);
+              ki = __shfl_sync(FULL, kil, kl);
+            }
+          }
+        }
+      }
+    }
+    const double bound = ring_bound(g, q, c, R, eps);
+    if (bound == INFINITY || bound * bound > fmin(kd, r2)) break;
+  }
+}
+
+// Exact 1-NN of q within r: the (d2, index)-least point with d2 < r * r, or -1.  Returns its slot in pts and its d2 in *d2.
+// It scans every cell of the box floor((q -+ r - o) * inv_cell -+ 1e-6): the build's cell rule, widened by a millionth of a cell on
+// either side.  That holds every point with d2 < r2: such a point lies within r (1 + a few ulp) of q on every axis, and the rounding
+// of its cell coordinate and of the box edge's can put it across the edge only by a few ulp of those coordinates -- far below 1e-6
+// cell while points and queries lie within ~1e8 cells of the origin.  A larger box holds the same qualifying points, so any box
+// that holds them all returns the same point.
+__device__ __forceinline__ int grid_nearest(const GridHeader& g, const int32_t* __restrict__ cs, const double4* __restrict__ pts,
+                                            double qx, double qy, double qz, double r, double* d2) {
+  const double r2 = r * r, q[3] = {qx, qy, qz};
+  int lo[3], hi[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const double top = (double)(g.dims[a] - 1);
+    lo[a] = (int)fmin(fmax(floor((q[a] - r - g.origin[a]) * g.inv_cell - 1e-6), 0.0), top);
+    hi[a] = (int)fmin(fmax(floor((q[a] + r - g.origin[a]) * g.inv_cell + 1e-6), 0.0), top);
+  }
+  double bd = INFINITY; int bi = 0x7fffffff, bslot = -1;
+  for (int z = lo[2]; z <= hi[2]; z++)
+    for (int y = lo[1]; y <= hi[1]; y++) {
+      const int row = (z * g.dims[1] + y) * g.dims[0];
+      const int e = cs[row + hi[0] + 1];
+      for (int j = cs[row + lo[0]]; j < e; j++) {
+        const double4 p = pts[j];
+        const double d = dist2_exact(qx, qy, qz, p.x, p.y, p.z);
+        const int idx = (int)__double_as_longlong(p.w);
+        if (d < r2 && nn_key_less(d, idx, bd, bi)) { bd = d; bi = idx; bslot = j; }
+      }
+    }
+  *d2 = bd;
+  return bslot;
 }
 
 // 3x3 SVD by one-sided Jacobi (Hestenes), singular values sorted descending like Eigen's JacobiSVD (the rotation that

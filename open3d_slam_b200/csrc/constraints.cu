@@ -43,35 +43,6 @@ __device__ bool wi_is_identity(const double* T) {
   return true;
 }
 
-// exact 1-NN within r: every cell that overlaps the box [q - r, q + r] (cell indices by the build's floor((v - o) * inv), which is
-// monotone, clamped like the build clamps), strict d2 < r2 with dist2_exact, equal distances to the lower original index.
-// Returns the slot in g's point array, -1 = none.
-__device__ __forceinline__ int wi_nearest(const GridHeader& g, const int32_t* __restrict__ cs, const double4* __restrict__ pts, double qx, double qy,
-                                          double qz, double rad, double r2) {
-  const double ox = g.origin[0], oy = g.origin[1], oz = g.origin[2], inv = g.inv_cell;
-  const int nx = g.dims[0], ny = g.dims[1], nz = g.dims[2];
-  const int ix0 = (int)fmin(fmax(floor((qx - rad - ox) * inv), 0.0), (double)(nx - 1));
-  const int ix1 = (int)fmin(fmax(floor((qx + rad - ox) * inv), 0.0), (double)(nx - 1));
-  const int iy0 = (int)fmin(fmax(floor((qy - rad - oy) * inv), 0.0), (double)(ny - 1));
-  const int iy1 = (int)fmin(fmax(floor((qy + rad - oy) * inv), 0.0), (double)(ny - 1));
-  const int iz0 = (int)fmin(fmax(floor((qz - rad - oz) * inv), 0.0), (double)(nz - 1));
-  const int iz1 = (int)fmin(fmax(floor((qz + rad - oz) * inv), 0.0), (double)(nz - 1));
-  double best = r2;
-  int bidx = 0x7fffffff, bslot = -1;
-  for (int z = iz0; z <= iz1; z++)
-    for (int y = iy0; y <= iy1; y++) {
-      const int row = (z * ny + y) * nx;
-      const int s = cs[row + ix0], e = cs[row + ix1 + 1];
-      for (int j = s; j < e; j++) {
-        const double4 p = pts[j];
-        const double d = dist2_exact(qx, qy, qz, p.x, p.y, p.z);
-        const int idx = (int)__double_as_longlong(p.w);
-        if (d < best || (d == best && bslot >= 0 && idx < bidx)) { best = d; bidx = idx; bslot = j; }
-      }
-    }
-  return bslot;
-}
-
 __global__ void __launch_bounds__(WI_THREADS) info_wide_kernel(const InfoPair* __restrict__ pairs, int npairs, int total_tiles, double r,
                                                                double* __restrict__ partials) {
   pdl_wait();
@@ -80,8 +51,6 @@ __global__ void __launch_bounds__(WI_THREADS) info_wide_kernel(const InfoPair* _
   __shared__ int s_apply;
   __shared__ double sred[WI_THREADS / 32][WI_MOM];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const double r2 = r * r;
-  const double rad = r * (1.0 + 1e-12) + 1e-300;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     int lo = 0, hi = npairs - 1;   // the pair whose tile range holds `tile` (tile0 ascending)
     while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (pairs[mid].tile0 <= tile) lo = mid; else hi = mid - 1; }
@@ -109,7 +78,8 @@ __global__ void __launch_bounds__(WI_THREADS) info_wide_kernel(const InfoPair* _
           px = x; py = y; pz = z;
         }
         if (!(px == px && py == py && pz == pz) || sg.n == 0) continue;
-        const int slot = wi_nearest(sg, P.cell_start, P.pts, px, py, pz, rad, r2);
+        double d2;
+        const int slot = grid_nearest(sg, P.cell_start, P.pts, px, py, pz, r, &d2);
         if (slot < 0) continue;
         const double4 q = P.pts[slot];   // the moments of the matched TARGET point (EST_INFORMATION)
         acc[0] += q.x; acc[1] += q.y; acc[2] += q.z;

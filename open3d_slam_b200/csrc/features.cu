@@ -3,8 +3,9 @@
 //
 // Three kernels over a K-index grid of the cloud (grid_index.cu):
 //   fpfh_knn_kernel   one WARP per query: the exact hybrid search (k nearest with d2 < r2, ties -> lower index, ascending
-//                     (d2, index)) as a ring walk over the grid, the k best kept as a sorted list of up to B2S_FEATURE_MAX_KNN
-//                     entries, FK_PER_LANE per lane.  Each neighbour list (index + d2) is written once and read by both passes.
+//                     (d2, index)) by the warp ring walk grid_knn_walk (common.cuh), the k best kept as a sorted list of up to
+//                     B2S_FEATURE_MAX_KNN entries, FK_PER_LANE per lane.  Each neighbour list (index + d2) is written once and
+//                     read by both passes.
 //   fpfh_spfh_kernel  one thread per point: SPFH.  The first list entry is skipped as "self" (kept literally, also when a
 //                     coincident lower-index point takes that place); bins are counted, then every bin is the count-fold sum
 //                     of hist_incr -- the reference's sequential `+= hist_incr`, whose value depends on the count only.
@@ -22,19 +23,7 @@ constexpr int FK_THREADS = 128;
 constexpr int FK_PER_LANE = B2S_FEATURE_MAX_KNN / 32;
 static_assert(B2S_FEATURE_MAX_KNN % 32 == 0, "the k-best list is FK_PER_LANE entries per lane");
 
-__device__ __forceinline__ bool fk_less(double da, int ia, double db, int ib) { return da < db || (da == db && ia < ib); }
-
-__device__ __forceinline__ double fk_slab_gap(double q, double o, double cell, int i, int n, double eps) {
-  double g = 0.0;
-  if (i > 0) { double lo = o + (double)i * cell; if (q < lo) g = lo - q; }
-  if (i < n - 1) { double hi = o + (double)(i + 1) * cell; if (q > hi) g = q - hi; }
-  g -= eps;
-  return g > 0.0 ? g : 0.0;
-}
-
-// Ring walk of normals_phase2_kernel (normals.cu) with a k-best list of up to FK_PER_LANE * 32 entries: list position
-// p = m * 32 + lane lives in register m of that lane; inserting shifts every entry behind the new one up by one position
-// (shuffle-up inside a register row, lane 31 of row m - 1 carried into lane 0 of row m).
+// one WARP per query: the ring walk grid_knn_walk (common.cuh) with FK_PER_LANE list entries per lane
 __global__ void __launch_bounds__(FK_THREADS) fpfh_knn_kernel(const GridHeader* __restrict__ hdr, const int32_t* __restrict__ cs,
                                                               const double4* __restrict__ pts, int knn, double radius,
                                                               int32_t* __restrict__ nb_idx, double* __restrict__ nb_d2,
@@ -47,100 +36,11 @@ __global__ void __launch_bounds__(FK_THREADS) fpfh_knn_kernel(const GridHeader* 
   const int lane = threadIdx.x & 31;
   const int warps_total = gridDim.x * (FK_THREADS / 32);
   const double r2 = radius * radius;
-  const double eps = 1e-9 * g.cell;
-  const int nx = g.dims[0], ny = g.dims[1], nz = g.dims[2];
-  const int km = (knn - 1) >> 5, kl = (knn - 1) & 31;   // list position of the k-th neighbour
   for (int w = blockIdx.x * (FK_THREADS / 32) + (threadIdx.x >> 5); w < g.n; w += warps_total) {
     const double4 qp = pts[w];
-    const double qx = qp.x, qy = qp.y, qz = qp.z;
     const int qi = (int)__double_as_longlong(qp.w);
-    const int cx = (int)fmin(fmax(floor((qx - g.origin[0]) * g.inv_cell), 0.0), (double)(nx - 1));
-    const int cy = (int)fmin(fmax(floor((qy - g.origin[1]) * g.inv_cell), 0.0), (double)(ny - 1));
-    const int cz = (int)fmin(fmax(floor((qz - g.origin[2]) * g.inv_cell), 0.0), (double)(nz - 1));
-    double ed[FK_PER_LANE]; int ei[FK_PER_LANE];
-#pragma unroll
-    for (int m = 0; m < FK_PER_LANE; ++m) { ed[m] = INFINITY; ei[m] = 0x7fffffff; }
-    double kd = INFINITY; int ki = 0x7fffffff;   // current k-th best
-    for (int R = 0;; ++R) {
-      const int side = 2 * R + 1;
-      const int x0 = max(cx - R, 0), x1 = min(cx + R, nx - 1);
-      for (int t0 = 0; t0 < side * side; t0 += 32) {
-        int a0 = 0, b0 = 0, a1 = 0, b1 = 0;   // this lane's (y, z) row: up to two slot ranges
-        const int t = t0 + lane;
-        if (t < side * side) {
-          const int z = cz - R + t / side, y = cy - R + t % side;
-          if (z >= 0 && z < nz && y >= 0 && y < ny) {
-            const double gz = fk_slab_gap(qz, g.origin[2], g.cell, z, nz, eps);
-            const double gy = fk_slab_gap(qy, g.origin[1], g.cell, y, ny, eps);
-            if (gz * gz + gy * gy <= fmin(kd, r2)) {
-              const int row = (z * ny + y) * nx;
-              if (z == cz - R || z == cz + R || y == cy - R || y == cy + R) { a0 = cs[row + x0]; b0 = cs[row + x1 + 1]; }
-              else {
-                if (cx - R >= 0) { a0 = cs[row + cx - R]; b0 = cs[row + cx - R + 1]; }
-                if (cx + R <= nx - 1) { a1 = cs[row + cx + R]; b1 = cs[row + cx + R + 1]; }
-              }
-            }
-          }
-        }
-        for (int part = 0; part < 2; ++part) {
-          unsigned rows = __ballot_sync(FULL, part == 0 ? (b0 > a0) : (b1 > a1));
-          while (rows) {
-            const int src_lane = __ffs(rows) - 1;
-            rows &= rows - 1;
-            const int a = __shfl_sync(FULL, part == 0 ? a0 : a1, src_lane);
-            const int b = __shfl_sync(FULL, part == 0 ? b0 : b1, src_lane);
-            for (int j0 = a; j0 < b; j0 += 32) {
-              const int j = j0 + lane;
-              double d = INFINITY; int idx = 0x7fffffff;
-              if (j < b) {
-                const double4 p = pts[j];
-                d = dist2_exact(qx, qy, qz, p.x, p.y, p.z);
-                idx = (int)__double_as_longlong(p.w);
-              }
-              unsigned mask = __ballot_sync(FULL, j < b && d < r2 && fk_less(d, idx, kd, ki));
-              while (mask) {
-                const int src = __ffs(mask) - 1;
-                mask &= mask - 1;
-                const double cd = __shfl_sync(FULL, d, src);
-                const int ci = __shfl_sync(FULL, idx, src);
-                if (!fk_less(cd, ci, kd, ki)) continue;   // an earlier insertion of this batch moved the k-th entry
-                double pd[FK_PER_LANE], td[FK_PER_LANE]; int pi[FK_PER_LANE], ti[FK_PER_LANE];
-#pragma unroll
-                for (int m = 0; m < FK_PER_LANE; ++m) {
-                  pd[m] = __shfl_up_sync(FULL, ed[m], 1); pi[m] = __shfl_up_sync(FULL, ei[m], 1);
-                  td[m] = __shfl_sync(FULL, ed[m], 31); ti[m] = __shfl_sync(FULL, ei[m], 31);
-                }
-#pragma unroll
-                for (int m = 0; m < FK_PER_LANE; ++m) {
-                  const bool has_prev = lane > 0 || m > 0;
-                  const double prd = lane > 0 ? pd[m] : (m > 0 ? td[m > 0 ? m - 1 : 0] : -INFINITY);
-                  const int pri = lane > 0 ? pi[m] : (m > 0 ? ti[m > 0 ? m - 1 : 0] : -1);
-                  if (fk_less(cd, ci, ed[m], ei[m])) {
-                    if (has_prev && fk_less(cd, ci, prd, pri)) { ed[m] = prd; ei[m] = pri; }
-                    else { ed[m] = cd; ei[m] = ci; }
-                  }
-                }
-                double kdl = ed[0]; int kil = ei[0];
-#pragma unroll
-                for (int m = 1; m < FK_PER_LANE; ++m) if (m == km) { kdl = ed[m]; kil = ei[m]; }
-                kd = __shfl_sync(FULL, kdl, kl);
-                ki = __shfl_sync(FULL, kil, kl);
-              }
-            }
-          }
-        }
-      }
-      double bound = INFINITY;
-      if (cx - R > 0) bound = fmin(bound, qx - (g.origin[0] + (double)(cx - R) * g.cell));
-      if (cx + R < nx - 1) bound = fmin(bound, (g.origin[0] + (double)(cx + R + 1) * g.cell) - qx);
-      if (cy - R > 0) bound = fmin(bound, qy - (g.origin[1] + (double)(cy - R) * g.cell));
-      if (cy + R < ny - 1) bound = fmin(bound, (g.origin[1] + (double)(cy + R + 1) * g.cell) - qy);
-      if (cz - R > 0) bound = fmin(bound, qz - (g.origin[2] + (double)(cz - R) * g.cell));
-      if (cz + R < nz - 1) bound = fmin(bound, (g.origin[2] + (double)(cz + R + 1) * g.cell) - qz);
-      bound -= eps;
-      if (bound < 0.0) bound = 0.0;
-      if (bound == INFINITY || bound * bound > fmin(kd, r2)) break;
-    }
+    double ed[FK_PER_LANE]; int ei[FK_PER_LANE], es[FK_PER_LANE];   // es: unused, the lists hold original indices
+    grid_knn_walk<FK_PER_LANE, false>(g, cs, pts, qp.x, qp.y, qp.z, knn, r2, ed, ei, es);
     int kk = 0;
 #pragma unroll
     for (int m = 0; m < FK_PER_LANE; ++m) {

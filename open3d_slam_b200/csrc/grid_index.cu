@@ -91,11 +91,8 @@ __device__ __forceinline__ bool crop_aabb(const CropDev& crop, double* lo, doubl
 }
 
 __device__ __forceinline__ int grid_cell_of(const GridHeader& g, double x, double y, double z) {
-  double fx = floor((x - g.origin[0]) * g.inv_cell), fy = floor((y - g.origin[1]) * g.inv_cell), fz = floor((z - g.origin[2]) * g.inv_cell);
-  int cx = (int)fmin(fmax(fx, 0.0), (double)(g.dims[0] - 1));
-  int cy = (int)fmin(fmax(fy, 0.0), (double)(g.dims[1] - 1));
-  int cz = (int)fmin(fmax(fz, 0.0), (double)(g.dims[2] - 1));
-  return (cz * g.dims[1] + cy) * g.dims[0] + cx;
+  return (grid_axis_cell(z, g.origin[2], g.inv_cell, g.dims[2]) * g.dims[1] + grid_axis_cell(y, g.origin[1], g.inv_cell, g.dims[1])) * g.dims[0] +
+         grid_axis_cell(x, g.origin[0], g.inv_cell, g.dims[0]);
 }
 
 __global__ void grid_zero_kernel(const GridHeader* hdr, int32_t* counts) {

@@ -98,14 +98,6 @@ struct NNState {
   int scanned;   // candidates looked at (only read by the counting instantiation, icp_kernel<3>)
 };
 
-__device__ __forceinline__ double slab_gap(double q, double o, double cell, int i, int n, double eps) {
-  double g = 0.0;
-  if (i > 0) { double lo = o + (double)i * cell; if (q < lo) g = lo - q; }
-  if (i < n - 1) { double hi = o + (double)(i + 1) * cell; if (q > hi) g = q - hi; }
-  g -= eps;  // slack: cell membership was decided with floor((p-o)*inv), which can disagree with o+i*cell by an ulp
-  return g > 0.0 ? g : 0.0;
-}
-
 __device__ __forceinline__ void nn_scan_range(const double4* __restrict__ pts, int s, int e, double qx, double qy, double qz, NNState& st) {
   st.scanned += e > s ? e - s : 0;   // statistics (dead code unless the counting instantiation reads it)
 #pragma unroll 4

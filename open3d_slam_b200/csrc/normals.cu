@@ -10,7 +10,7 @@
 //   normals_finish_kernel   one thread per query: analytic 3x3 eigen-solver ([O3D] FastEigen3x3, geometrictools
 //                           RobustEigenSymmetric3x3), normalise, orient;
 //   normals_phase2_kernel   the few queries the block gather cannot certify (more than NS2_CAP candidates, or a search radius the
-//                           row table cannot cover): ring walk with a sorted k-best list, one entry per lane, shuffle insert.
+//                           row table cannot cover): the warp ring walk grid_knn_walk (common.cuh), one list entry per lane.
 // The neighbour SET is the oracle's exactly; the cumulants are summed in butterfly order instead of ascending-distance order, which
 // moves the normal by < 1e-9.
 #include "common.cuh"
@@ -18,16 +18,6 @@
 namespace b2s {
 
 constexpr int NK_THREADS = 128;
-
-__device__ __forceinline__ bool lex_less(double da, int ia, double db, int ib) { return da < db || (da == db && ia < ib); }
-
-__device__ __forceinline__ double slab_gap_n(double q, double o, double cell, int i, int n, double eps) {
-  double g = 0.0;
-  if (i > 0) { double lo = o + (double)i * cell; if (q < lo) g = lo - q; }
-  if (i < n - 1) { double hi = o + (double)(i + 1) * cell; if (q > hi) g = q - hi; }
-  g -= eps;
-  return g > 0.0 ? g : 0.0;
-}
 
 __device__ __forceinline__ void cross3d(const double* a, const double* b, double* o) {
   o[0] = a[1] * b[2] - a[2] * b[1]; o[1] = a[2] * b[0] - a[0] * b[2]; o[2] = a[0] * b[1] - a[1] * b[0];
@@ -166,10 +156,7 @@ __device__ __forceinline__ void finish_normal(const double c_in[9], int kk, doub
   } else if (dot3d(nr, ref) < 0.0) { nr[0] *= -1.0; nr[1] *= -1.0; nr[2] *= -1.0; }
 }
 
-// Phase 2: one WARP per queued query, restarted from ring 0.  Per ring, each lane first resolves ONE (y, z) row --
-// pruning test and the two dependent cell_start loads, the latency that dominates in empty space -- then the warp
-// walks the non-empty rows together: 32 candidates per step, the k best kept as a sorted list with one entry per lane
-// (k <= 32), a qualifying candidate inserted with a single shuffle-up step.
+// Phase 2: one WARP per queued query, the ring walk of grid_knn_walk (common.cuh) with one list entry per lane (k <= 32).
 template <bool kDebug>
 __global__ void __launch_bounds__(NK_THREADS) normals_phase2_kernel(const GridHeader* __restrict__ hdr, const int32_t* __restrict__ cs,
                                                                     const double4* __restrict__ pts, int knn, double radius,
@@ -183,91 +170,17 @@ __global__ void __launch_bounds__(NK_THREADS) normals_phase2_kernel(const GridHe
   const int warps_total = gridDim.x * (NK_THREADS / 32);
   const int nq = *queue_n;
   const double r2 = radius * radius;
-  const double eps = 1e-9 * g.cell;
-  const int nx = g.dims[0], ny = g.dims[1], nz = g.dims[2];
   for (int w = blockIdx.x * (NK_THREADS / 32) + (threadIdx.x >> 5); w < nq; w += warps_total) {
     const int s = queue[w];
     const double4 qp = pts[s];
     const double qx = qp.x, qy = qp.y, qz = qp.z;
     const int qi = (int)__double_as_longlong(qp.w);
-    const int cx = (int)fmin(fmax(floor((qx - g.origin[0]) * g.inv_cell), 0.0), (double)(nx - 1));
-    const int cy = (int)fmin(fmax(floor((qy - g.origin[1]) * g.inv_cell), 0.0), (double)(ny - 1));
-    const int cz = (int)fmin(fmax(floor((qz - g.origin[2]) * g.inv_cell), 0.0), (double)(nz - 1));
-    double ed = INFINITY; int ei = 0x7fffffff; int es = -1;  // this lane's entry of the sorted k-best list
-    double kd = INFINITY; int ki = 0x7fffffff;               // current k-th best (lane knn-1)
-    for (int R = 0;; ++R) {
-      const int side = 2 * R + 1;
-      const int x0 = max(cx - R, 0), x1 = min(cx + R, nx - 1);
-      for (int t0 = 0; t0 < side * side; t0 += 32) {
-        // each lane resolves one row: up to two candidate ranges [a0,b0) and [a1,b1)
-        int a0 = 0, b0 = 0, a1 = 0, b1 = 0;
-        const int t = t0 + lane;
-        if (t < side * side) {
-          const int z = cz - R + t / side, y = cy - R + t % side;
-          if (z >= 0 && z < nz && y >= 0 && y < ny) {
-            const double gz = slab_gap_n(qz, g.origin[2], g.cell, z, nz, eps);
-            const double gy = slab_gap_n(qy, g.origin[1], g.cell, y, ny, eps);
-            if (gz * gz + gy * gy <= fmin(kd, r2)) {
-              const int row = (z * ny + y) * nx;
-              if (z == cz - R || z == cz + R || y == cy - R || y == cy + R) { a0 = cs[row + x0]; b0 = cs[row + x1 + 1]; }
-              else {
-                if (cx - R >= 0) { a0 = cs[row + cx - R]; b0 = cs[row + cx - R + 1]; }
-                if (cx + R <= nx - 1) { a1 = cs[row + cx + R]; b1 = cs[row + cx + R + 1]; }
-              }
-            }
-          }
-        }
-        for (int part = 0; part < 2; ++part) {
-          unsigned rows = __ballot_sync(0xffffffffu, part == 0 ? (b0 > a0) : (b1 > a1));
-          while (rows) {
-            const int src_lane = __ffs(rows) - 1;
-            rows &= rows - 1;
-            const int a = __shfl_sync(0xffffffffu, part == 0 ? a0 : a1, src_lane);
-            const int b = __shfl_sync(0xffffffffu, part == 0 ? b0 : b1, src_lane);
-            for (int j0 = a; j0 < b; j0 += 32) {
-              const int j = j0 + lane;
-              double d = INFINITY; int idx = 0x7fffffff;
-              if (j < b) {
-                const double4 p = pts[j];
-                d = dist2_exact(qx, qy, qz, p.x, p.y, p.z);
-                idx = (int)__double_as_longlong(p.w);
-              }
-              unsigned mask = __ballot_sync(0xffffffffu, j < b && d < r2 && lex_less(d, idx, kd, ki));
-              while (mask) {
-                const int src = __ffs(mask) - 1;
-                mask &= mask - 1;
-                const double cd = __shfl_sync(0xffffffffu, d, src);
-                const int ci = __shfl_sync(0xffffffffu, idx, src);
-                const int cslot = j0 + src;
-                const double pd = __shfl_up_sync(0xffffffffu, ed, 1);
-                const int pi = __shfl_up_sync(0xffffffffu, ei, 1);
-                const int ps = __shfl_up_sync(0xffffffffu, es, 1);
-                if (lex_less(cd, ci, ed, ei)) {
-                  if (lane > 0 && lex_less(cd, ci, pd, pi)) { ed = pd; ei = pi; es = ps; }
-                  else { ed = cd; ei = ci; es = cslot; }
-                }
-                kd = __shfl_sync(0xffffffffu, ed, knn - 1);
-                ki = __shfl_sync(0xffffffffu, ei, knn - 1);
-              }
-            }
-          }
-        }
-      }
-      double bound = INFINITY;
-      if (cx - R > 0) bound = fmin(bound, qx - (g.origin[0] + (double)(cx - R) * g.cell));
-      if (cx + R < nx - 1) bound = fmin(bound, (g.origin[0] + (double)(cx + R + 1) * g.cell) - qx);
-      if (cy - R > 0) bound = fmin(bound, qy - (g.origin[1] + (double)(cy - R) * g.cell));
-      if (cy + R < ny - 1) bound = fmin(bound, (g.origin[1] + (double)(cy + R + 1) * g.cell) - qy);
-      if (cz - R > 0) bound = fmin(bound, qz - (g.origin[2] + (double)(cz - R) * g.cell));
-      if (cz + R < nz - 1) bound = fmin(bound, (g.origin[2] + (double)(cz + R + 1) * g.cell) - qz);
-      bound -= eps;
-      if (bound < 0.0) bound = 0.0;
-      if (bound == INFINITY || bound * bound > fmin(kd, r2)) break;
-    }
+    double ed[1]; int ei[1], es[1];   // this lane's entry of the sorted k-best list
+    grid_knn_walk<1, true>(g, cs, pts, qx, qy, qz, knn, r2, ed, ei, es);
     // cumulants in ascending (d2, index) order: lane t holds the t-th neighbour, broadcast by shuffles
-    const int kk = __popc(__ballot_sync(0xffffffffu, lane < knn && es >= 0));
+    const int kk = __popc(__ballot_sync(0xffffffffu, lane < knn && es[0] >= 0));
     double4 np = make_double4(0, 0, 0, 0);
-    if (lane < kk) np = pts[es];
+    if (lane < kk) np = pts[es[0]];
     double c[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     for (int t = 0; t < kk; ++t) {
       const double x = __shfl_sync(0xffffffffu, np.x, t), y = __shfl_sync(0xffffffffu, np.y, t), z = __shfl_sync(0xffffffffu, np.z, t);
@@ -381,9 +294,10 @@ __global__ void __launch_bounds__(NK_THREADS, NS2_MIN_BLOCKS) normals_select2_ke
     const int s = qlist ? qlist[tq] : tq;
     const double4 qp = pts[s];
     const double qx = qp.x, qy = qp.y, qz = qp.z;
-    const int cx = (int)fmin(fmax(floor((qx - g.origin[0]) * g.inv_cell), 0.0), (double)(nx - 1));
-    const int cy = (int)fmin(fmax(floor((qy - g.origin[1]) * g.inv_cell), 0.0), (double)(ny - 1));
-    const int cz = (int)fmin(fmax(floor((qz - g.origin[2]) * g.inv_cell), 0.0), (double)(nz - 1));
+    const double q[3] = {qx, qy, qz};
+    const int c[3] = {grid_axis_cell(qx, g.origin[0], g.inv_cell, nx), grid_axis_cell(qy, g.origin[1], g.inv_cell, ny),
+                      grid_axis_cell(qz, g.origin[2], g.inv_cell, nz)};
+    const int cx = c[0], cy = c[1], cz = c[2];
     bool resolved = false;
     int need = 0;
     double c9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -416,14 +330,7 @@ __global__ void __launch_bounds__(NK_THREADS, NS2_MIN_BLOCKS) normals_select2_ke
       // ---- gather the (2R+1)^3 block into shared memory (valid = inside the radius), rows resolved by the lanes ----
       const int side = 2 * R + 1;
       const int x0 = max(cx - R, 0), x1 = min(cx + R, nx - 1);
-      double bound = INFINITY;   // distance from the query to the nearest face of the block that has cells beyond it
-      if (cx - R > 0) bound = fmin(bound, qx - (g.origin[0] + (double)(cx - R) * g.cell));
-      if (cx + R < nx - 1) bound = fmin(bound, (g.origin[0] + (double)(cx + R + 1) * g.cell) - qx);
-      if (cy - R > 0) bound = fmin(bound, qy - (g.origin[1] + (double)(cy - R) * g.cell));
-      if (cy + R < ny - 1) bound = fmin(bound, (g.origin[1] + (double)(cy + R + 1) * g.cell) - qy);
-      if (cz - R > 0) bound = fmin(bound, qz - (g.origin[2] + (double)(cz - R) * g.cell));
-      if (cz + R < nz - 1) bound = fmin(bound, (g.origin[2] + (double)(cz + R + 1) * g.cell) - qz);
-      if (bound != INFINITY) { bound -= eps; if (bound < 0.0) bound = 0.0; }
+      const double bound = ring_bound(g, q, c, R, eps);
       const double b2 = bound == INFINITY ? INFINITY : bound * bound;
       const double lim2 = fmin(r2, b2);   // candidates beyond the guaranteed ball cannot be certified at this R: drop them
       int nc = 0;

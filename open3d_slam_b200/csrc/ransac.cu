@@ -29,7 +29,6 @@ constexpr int FM_TILE = 64, FM_THREADS = 256, FM_DIM = B2S_FEATURE_DIM;
 constexpr int RS_THREADS = 128, RV_THREADS = 256;
 constexpr int NONE = 0x7fffffff;
 
-__device__ __forceinline__ bool lex_less(double da, int ia, double db, int ib) { return da < db || (da == db && ia < ib); }
 
 struct MatchJob {
   const double* tgt; int nt;
@@ -83,18 +82,18 @@ __global__ void __launch_bounds__(FM_THREADS) fm_tile_kernel(const double* __res
 #pragma unroll
       for (int r = 0; r < 4; ++r) {
         const int i = s0 + ty + 16 * r;
-        if (j < J.nt && lex_less(acc[r][c], j, rb[r], ri[r])) { rb[r] = acc[r][c]; ri[r] = j; }
-        if (i < ns && lex_less(acc[r][c], i, bd, bi)) { bd = acc[r][c]; bi = i; }
+        if (j < J.nt && nn_key_less(acc[r][c], j, rb[r], ri[r])) { rb[r] = acc[r][c]; ri[r] = j; }
+        if (i < ns && nn_key_less(acc[r][c], i, bd, bi)) { bd = acc[r][c]; bi = i; }
       }
       const double od = __shfl_xor_sync(FULL, bd, 16);   // the other row group (ty ^ 1) of this warp
       const int oi = __shfl_xor_sync(FULL, bi, 16);
-      if (lex_less(od, oi, bd, bi)) { bd = od; bi = oi; }
+      if (nn_key_less(od, oi, bd, bi)) { bd = od; bi = oi; }
       if ((tid & 16) == 0) { cd[warp][tx + 16 * c] = bd; ci[warp][tx + 16 * c] = bi; }
     }
     __syncthreads();
     if (tid < FM_TILE && t0 + tid < J.nt) {
       double bd = INFINITY; int bi = NONE;
-      for (int w = 0; w < FM_THREADS / 32; ++w) if (lex_less(cd[w][tid], ci[w][tid], bd, bi)) { bd = cd[w][tid]; bi = ci[w][tid]; }
+      for (int w = 0; w < FM_THREADS / 32; ++w) if (nn_key_less(cd[w][tid], ci[w][tid], bd, bi)) { bd = cd[w][tid]; bi = ci[w][tid]; }
       J.part_d[(size_t)blockIdx.x * J.nt + t0 + tid] = bd;
       J.part_i[(size_t)blockIdx.x * J.nt + t0 + tid] = bi;
     }
@@ -106,7 +105,7 @@ __global__ void __launch_bounds__(FM_THREADS) fm_tile_kernel(const double* __res
     for (int o = 1; o < 16; o <<= 1) {
       const double od = __shfl_xor_sync(FULL, bd, o);
       const int oi = __shfl_xor_sync(FULL, bi, o);
-      if (lex_less(od, oi, bd, bi)) { bd = od; bi = oi; }
+      if (nn_key_less(od, oi, bd, bi)) { bd = od; bi = oi; }
     }
     const int i = s0 + ty + 16 * r;
     if (tx == 0 && i < ns) J.s2t[i] = bi == NONE ? -1 : bi;
@@ -121,7 +120,7 @@ __global__ void fm_merge_kernel(int n_stiles, const MatchJob* __restrict__ jobs)
     for (int t = 0; t < n_stiles; ++t) {
       const double d = J.part_d[(size_t)t * J.nt + j];
       const int i = J.part_i[(size_t)t * J.nt + j];
-      if (lex_less(d, i, bd, bi)) { bd = d; bi = i; }
+      if (nn_key_less(d, i, bd, bi)) { bd = d; bi = i; }
     }
     J.t2s[j] = bi == NONE ? -1 : bi;
   }
@@ -292,12 +291,6 @@ __global__ void rs_compact_kernel(RansacConst c, long long h0, const RansacJob* 
   }
 }
 
-// grid cell of coordinate v along axis a, clamped into the grid.  The box [cell(q - r), cell(q + r)] is widened by a millionth of a
-// cell on either side against rounding; the d2 test that follows is exact.
-__device__ __forceinline__ int grid_cell(const GridHeader& g, int a, double v, double slack) {
-  return (int)fmin(fmax(floor((v - g.origin[a]) * g.inv_cell + slack), 0.0), (double)(g.dims[a] - 1));
-}
-
 // GetRegistrationResultAndCorrespondences of the source sparse cloud moved by T: 1-NN in the target grid with d2 < r2
 __global__ void __launch_bounds__(RV_THREADS, 1) rs_validate_kernel(RansacConst c, const RansacJob* __restrict__ jobs) {
   pdl_wait();
@@ -311,27 +304,13 @@ __global__ void __launch_bounds__(RV_THREADS, 1) rs_validate_kernel(RansacConst 
   if (threadIdx.x == 0) g = *J.ghdr;
   if (threadIdx.x < 16) T[threadIdx.x] = J.surv_T[(size_t)s * 16 + threadIdx.x];
   __syncthreads();
-  const double r = c.max_corr, r2 = r * r;
+  const double r = c.max_corr;
   double sum = 0.0; int inl = 0;
   for (int i = threadIdx.x; i < c.ns; i += RV_THREADS) {
     double q[3];
     xform(T, c.sxyz[3 * (size_t)i], c.sxyz[3 * (size_t)i + 1], c.sxyz[3 * (size_t)i + 2], q);
-    const int x0 = grid_cell(g, 0, q[0] - r, -1e-6), x1 = grid_cell(g, 0, q[0] + r, 1e-6);
-    const int y0 = grid_cell(g, 1, q[1] - r, -1e-6), y1 = grid_cell(g, 1, q[1] + r, 1e-6);
-    const int z0 = grid_cell(g, 2, q[2] - r, -1e-6), z1 = grid_cell(g, 2, q[2] + r, 1e-6);
-    double bd = INFINITY; int bi = NONE;
-    for (int z = z0; z <= z1; ++z)
-      for (int y = y0; y <= y1; ++y) {
-        const int row = (z * g.dims[1] + y) * g.dims[0];
-        const int e = J.gcs[row + x1 + 1];
-        for (int k = J.gcs[row + x0]; k < e; ++k) {
-          const double4 p = J.gpts[k];
-          const double d = dist2_exact(q[0], q[1], q[2], p.x, p.y, p.z);
-          const int idx = (int)__double_as_longlong(p.w);
-          if (d < r2 && lex_less(d, idx, bd, bi)) { bd = d; bi = idx; }
-        }
-      }
-    if (bi != NONE) { ++inl; sum += bd; }
+    double d2;
+    if (grid_nearest(g, J.gcs, J.gpts, q[0], q[1], q[2], r, &d2) >= 0) { ++inl; sum += d2; }
   }
   rsum[threadIdx.x] = sum; rinl[threadIdx.x] = inl;
   for (int o = RV_THREADS / 2; o > 0; o >>= 1) {   // fixed tree: a run is bit-reproducible
