@@ -898,6 +898,101 @@ int32_t b2s_assemble_colored_map(b2s_handle* h, int32_t n_submaps, const b2s_sub
  * tiles of the tables, not their slots: exporting between graph-replayed mapper steps never makes a chain re-capture. */
 int32_t b2s_assemble_dense_maps(b2s_handle* h, int32_t n_submaps, const b2s_submap* const* submaps, b2s_cloud* out, int64_t* offsets);
 
+/* ---- session state: a submap's and an odometry object's device state saved as host blobs and restored on any handle (DESIGN.md
+ *      row A3).  A1 / A2 and the downloads give outputs; these give the state, so a mission can pause and continue, move to another
+ *      handle or GPU, or map a site in two sessions.  The reference has no counterpart (it saves maps only).  Restated rules:
+ *   1. self-contained blobs: each blob imports on its own, on any handle and device.  The import creates a new object with the
+ *      exported capacities (submap: capacity, vcap, stage_cap, dense_cap -- dense_cap 0: the dense map was never fed and stays so;
+ *      odometry: capacity, buffer_size) and a fresh identity: it never replays another object's captured graph.
+ *   2. exact state: every device buffer a later call reads holds what the exported object held, over the ranges that are state --
+ *      submap: the 8 pose slots, the mapper options, the MS_* words, the box, the map slots [0, dn) (xyz and normals, tombstones
+ *      included), every fusion-table slot whose key is not EMPTY (key, chain head, stamp), the chain links, stamps and worklist flags
+ *      of [0, dn), the current halves of the duplicate list and of the worklist, every dense-table slot whose key is not EMPTY (key,
+ *      six sums, count; count-0 keys included: they decide probe runs), the dense table's fill counter, the normals / merge flags.
+ *      Not state: the ping-pong and staging clouds, the scan in flight, the static patch table, captured graphs, pinned read-backs.
+ *      odometry: parameters, de-skew parameters, the device state word block, both pose buffers, the previous cloud, the host's
+ *      step counter and last timestamp.
+ *   3. format: a 256-byte header of uint64 words (B2S_STATE_W_*: magic, B2S_STATE_VERSION, B2S_STATE_BYTE_ORDER as written by the
+ *      exporter, total bytes, the exporting handle's map_voxel_size, the section count and every section's byte length, then the
+ *      object's parameter words), then the sections in the order of B2S_SS_* / B2S_OS_*, each padded to a multiple of 8 bytes with
+ *      zeros.  The fusion hash is keyed by map_voxel_size: a submap blob is refused by a handle whose map_voxel_size differs.
+ *      Only this version and byte order are read.
+ *   4. validation: a blob is outside input.  B2S_E_INVALID for: fewer bytes than the header or than its total, a wrong magic,
+ *      version or byte order; section lengths that disagree with the parameter words; dn above the capacity, table sizes that are
+ *      not what a submap of that capacity has, counters of the MS_* words that disagree with the section lengths; a record slot at
+ *      or beyond its table's size, an EMPTY key, two records of one slot; a chain head or link outside [-1, dn), a map slot reached
+ *      by two links, a worklist entry outside [0, dn), a duplicate entry outside the table, a worklist flag other than 0 / 1;
+ *      odometry: invalid parameters, a ring position or count outside the buffer, more previous points than the capacity.  Every
+ *      check runs before a kernel uses the value as an index; a refused blob creates nothing and the handle stays usable.
+ *   5. export only reads: no captured graph is dropped and its scratch is the library's own (untracked), so exports between
+ *      graph-replayed steps never make a chain re-capture.  Two exports of an unchanged object are byte-identical, and so is the
+ *      re-export of an imported one.
+ *   6. b2s_submaps_export_state: host_or_null NULL computes the offsets only; otherwise the blobs of the same list are written when
+ *      their total fits `capacity` (else B2S_E_CAPACITY and nothing is written: a submap that grew since the size call).
+ *      offsets_out (n + 1 entries) receives the byte offsets, blob k = [offsets_out[k], offsets_out[k + 1]).  n < 0, a null entry or
+ *      another handle's submap -> B2S_E_INVALID; n > B2S_ASSEMBLY_MAX_SUBMAPS -> B2S_E_UNSUPPORTED.  One set of launches for every
+ *      listed submap; synchronises once for the sizes and once for the data.  b2s_odometry_export_state: the same with one blob
+ *      (*n_bytes receives its size). */
+#define B2S_STATE_VERSION 1
+#define B2S_STATE_BYTE_ORDER 0x0102030405060708ull
+#define B2S_STATE_MAGIC_SUBMAP 0x314d425553533242ull     /* the bytes "B2SSUBM1" */
+#define B2S_STATE_MAGIC_ODOMETRY 0x314d4f444f533242ull   /* the bytes "B2SODOM1" */
+#define B2S_STATE_HEADER_BYTES 256
+#define B2S_STATE_MSTATE_WORDS 32                        /* int32 MS_* words of a submap */
+#define B2S_STATE_POSE_SLOTS 8                           /* 4x4 f64 pose slots of a submap */
+enum {   /* header words (uint64) */
+  B2S_STATE_W_MAGIC = 0, B2S_STATE_W_VERSION = 1, B2S_STATE_W_BYTE_ORDER = 2, B2S_STATE_W_TOTAL_BYTES = 3,
+  B2S_STATE_W_MAP_VOXEL = 4,    /* map_voxel_size of the exporting handle, IEEE-754 bits */
+  B2S_STATE_W_N_SECTIONS = 5,
+  B2S_STATE_W_SECTIONS = 6,     /* words 6 .. 6 + n_sections - 1: byte length of every section, in blob order */
+  B2S_STATE_W_PARAMS = 20       /* words 20 .. 31: parameter words of the object (B2S_SP_* / B2S_OP_*); unused ones are 0 */
+};
+enum {   /* submap sections */
+  B2S_SS_POSE = 0,              /* B2S_STATE_POSE_SLOTS x 16 f64 */
+  B2S_SS_OPTIONS = 1,           /* b2s_mapper_options */
+  B2S_SS_MSTATE = 2,            /* B2S_STATE_MSTATE_WORDS int32 */
+  B2S_SS_BBOX = 3,              /* 6 x uint64, ordered-encoded min xyz / max xyz */
+  B2S_SS_MAP_XYZ = 4, B2S_SS_MAP_NORMALS = 5,   /* dn x 3 f64 each */
+  B2S_SS_VNEXT = 6, B2S_SS_PSTAMP = 7, B2S_SS_WFLAG = 8,   /* dn int32 each; empty while the fusion table does not exist (vcap 0) */
+  B2S_SS_DUPS = 9,              /* n_dups int32: the current half of the duplicate list */
+  B2S_SS_WLIST = 10,            /* n_wlist int32: the current half of the worklist */
+  B2S_SS_VOXELS = 11,           /* n_voxels b2s_state_voxel_record, slot order */
+  B2S_SS_DENSE_USED = 12,       /* int32 + 4 bytes of padding; empty without a dense map */
+  B2S_SS_DENSE = 13,            /* n_dense b2s_state_dense_record, slot order */
+  B2S_SS_COUNT = 14
+};
+enum {   /* submap parameter words */
+  B2S_SP_CAPACITY = 20, B2S_SP_VCAP = 21, B2S_SP_STAGE_CAP = 22, B2S_SP_DENSE_CAP = 23,
+  B2S_SP_DENSE_VOXEL = 24,      /* IEEE-754 bits */
+  B2S_SP_FLAGS = 25,            /* B2S_STATE_F_* */
+  B2S_SP_DN = 26, B2S_SP_N_VOXELS = 27, B2S_SP_N_DUPS = 28, B2S_SP_N_WLIST = 29, B2S_SP_N_DENSE = 30
+};
+enum { B2S_STATE_F_HAS_NORMALS = 1, B2S_STATE_F_NO_NORMALS = 2, B2S_STATE_F_MERGE_SCANS = 4, B2S_STATE_F_DENSE_HAS_NORMALS = 8 };
+enum {   /* odometry sections */
+  B2S_OS_PARAMS = 0,            /* b2s_odometry_params */
+  B2S_OS_MOTION = 1,            /* b2s_motion_compensation_params */
+  B2S_OS_STATE = 2,             /* the device state block (cumulative pose, initial transform, t_last, ring positions, ...) */
+  B2S_OS_RING_TIMES = 3, B2S_OS_RING_POSES = 4,   /* the odometry buffer: buffer_size int64, buffer_size x 16 f64 (physical order) */
+  B2S_OS_MAP_TIMES = 5, B2S_OS_MAP_POSES = 6,     /* the mapper's pose buffer, the same layout */
+  B2S_OS_PREV_XYZ = 7, B2S_OS_PREV_NORMALS = 8,   /* cloudPrev_: n_prev x 3 f64 each */
+  B2S_OS_COUNT = 9
+};
+enum { B2S_OP_CAPACITY = 20, B2S_OP_BUFFER_SIZE = 21, B2S_OP_N_PREV = 22, B2S_OP_HOST_STEP = 23, B2S_OP_HAS_T = 24, B2S_OP_LAST_T = 25 };
+typedef struct b2s_state_voxel_record {   /* one fusion-table slot */
+  uint64_t key;
+  int32_t slot, head, stamp, reserved_;
+} b2s_state_voxel_record;
+typedef struct b2s_state_dense_record {   /* one dense-table slot */
+  uint64_t key;
+  double sum[6];
+  int32_t slot, count;
+} b2s_state_dense_record;
+int32_t b2s_submaps_export_state(b2s_handle* h, int32_t n, const b2s_submap* const* submaps, void* host_or_null, size_t capacity,
+                                 size_t* offsets_out);
+int32_t b2s_submap_import_state(b2s_handle* h, const void* blob, size_t n_bytes, b2s_submap** out);
+int32_t b2s_odometry_export_state(b2s_handle* h, const b2s_odometry* od, void* host_or_null, size_t capacity, size_t* n_bytes);
+int32_t b2s_odometry_import_state(b2s_handle* h, const void* blob, size_t n_bytes, b2s_odometry** out);
+
 /* ---- device-to-device hand-over of a cloud's arrays (SURVEY.md section 8e: a submap that is the registration target on
  *      several GPUs is built once by its owner and broadcast over NVLink by the host side -- torch.distributed / NCCL own
  *      the transfer, this library only copies between its cloud and the caller's device buffers on the handle's stream).

@@ -192,9 +192,30 @@ SYMBOLS = [
     "b2s_debug_estimate_normals", "b2s_debug_submap_bbox",
     "b2s_default_global_localization_params", "b2s_submap_global_localization", "b2s_debug_global_localization_scores",
     "b2s_assemble_dense_maps",
+    "b2s_submaps_export_state", "b2s_submap_import_state", "b2s_odometry_export_state", "b2s_odometry_import_state",
 ]
 FEATURE_DIM, FEATURE_MAX_KNN = 33, 128   # B2S_FEATURE_DIM, B2S_FEATURE_MAX_KNN
 ASSEMBLY_MAX_SUBMAPS = 65535             # B2S_ASSEMBLY_MAX_SUBMAPS
+# session-state blobs (include/b2s.h "session state"): header words, section order, parameter words, records
+STATE_VERSION, STATE_BYTE_ORDER = 1, 0x0102030405060708
+STATE_MAGIC_SUBMAP, STATE_MAGIC_ODOMETRY = 0x314D425553533242, 0x314D4F444F533242   # the bytes "B2SSUBM1", "B2SODOM1"
+STATE_HEADER_BYTES, STATE_MSTATE_WORDS, STATE_POSE_SLOTS = 256, 32, 8
+STATE_W_MAGIC, STATE_W_VERSION, STATE_W_BYTE_ORDER, STATE_W_TOTAL_BYTES, STATE_W_MAP_VOXEL, STATE_W_N_SECTIONS, STATE_W_SECTIONS, STATE_W_PARAMS = \
+    0, 1, 2, 3, 4, 5, 6, 20
+STATE_SUBMAP_SECTIONS = ["pose", "options", "mstate", "bbox", "map_xyz", "map_normals", "vnext", "pstamp", "wflag", "dups", "wlist", "voxels",
+                         "dense_used", "dense"]
+STATE_SUBMAP_PARAMS = ["capacity", "vcap", "stage_cap", "dense_cap", "dense_voxel", "flags", "dn", "n_voxels", "n_dups", "n_wlist", "n_dense"]
+STATE_ODOMETRY_SECTIONS = ["params", "motion", "state", "ring_times", "ring_poses", "map_times", "map_poses", "prev_xyz", "prev_normals"]
+STATE_ODOMETRY_PARAMS = ["capacity", "buffer_size", "n_prev", "host_step", "has_t", "last_t"]
+STATE_F_HAS_NORMALS, STATE_F_NO_NORMALS, STATE_F_MERGE_SCANS, STATE_F_DENSE_HAS_NORMALS = 1, 2, 4, 8
+
+
+class StateVoxelRecord(C.Structure):
+    _fields_ = [("key", C.c_uint64), ("slot", C.c_int32), ("head", C.c_int32), ("stamp", C.c_int32), ("reserved_", C.c_int32)]
+
+
+class StateDenseRecord(C.Structure):
+    _fields_ = [("key", C.c_uint64), ("sum", C.c_double * 6), ("slot", C.c_int32), ("count", C.c_int32)]
 PROFILE_KINDS = ["icp", "normals", "radix_sort", "nn_grid_build", "voxel", "fuse", "select", "crop"]
 
 _lib = None

@@ -10,13 +10,9 @@
 // live point its offset within its submap, one CTA scans the per-submap totals into each submap's base, and a scatter writes points,
 // normals and, for the coloured map, the point's palette entry.  The voxel path is op_voxel_down_sample on the assembled cloud, with
 // the palette entries averaged beside the points.  Every buffer here is the assembly's own and untracked (AssemblyScratch).
-#include "common.cuh"
+#include "assemble.cuh"
 
 namespace b2s {
-
-constexpr int AS_THREADS = 256;
-constexpr int AS_BASE_THREADS = 1024;                  // the base scan walks the jobs 1024 at a time
-constexpr long long AS_MAX_POINTS = 0x7fffffffLL / 3;   // the kernels downstream index 3 i in int32
 
 // Color::getColor(j % 11 + 2) (ros/open3d_slam_ros/include/open3d_slam_ros/Color.hpp:22-32): Gray, Red, Green, Blue, Yellow, Orange,
 // Purple, Chartreuse, Teal, Pink, Magenta.  std_msgs/ColorRGBA holds float32: the values are the float32 ones promoted to double.
@@ -40,50 +36,6 @@ __global__ void __launch_bounds__(AS_THREADS) asm_flags_kernel(const AsmJob* __r
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const double x = j.xyz[3 * (size_t)i];
     j.flags[i] = (x == x) ? 1 : 0;
-  }
-}
-
-// one CTA: base[k] = live points of the jobs before k (int64, job order), base[njobs] = their total; words[0] = *out_n = the assembled
-// count (0 above AS_MAX_POINTS, which is reported as ST_CAPACITY), words[1] = a job that contributes a point has no normals.
-// Job: AsmJob (A1) or DenseJob (A2), read through live() and lacks_normals()
-template <typename Job>
-__global__ void __launch_bounds__(AS_BASE_THREADS) asm_base_kernel(const Job* __restrict__ jobs, int njobs, long long* __restrict__ base,
-                                                                   int32_t* out_n, int32_t* words, uint32_t* status) {
-  pdl_wait();
-  __shared__ long long s_warp[AS_BASE_THREADS / 32];
-  __shared__ long long s_carry;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) s_carry = 0;
-  int mixed = 0;
-  for (int r0 = 0; r0 < njobs; r0 += AS_BASE_THREADS) {
-    __syncthreads();
-    const int k = r0 + tid;
-    long long t = 0;
-    if (k < njobs) {
-      t = jobs[k].live();
-      if (t > 0 && jobs[k].lacks_normals()) mixed = 1;
-    }
-    long long inc = t;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const long long v = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += v; }
-    if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();
-    long long woff = 0, agg = 0;
-    for (int w = 0; w < AS_BASE_THREADS / 32; w++) { const long long v = s_warp[w]; if (w < warp) woff += v; agg += v; }
-    const long long carry = s_carry;
-    if (k < njobs) base[k] = carry + woff + inc - t;
-    __syncthreads();
-    if (tid == 0) s_carry = carry + agg;
-  }
-  mixed = __syncthreads_or(mixed);
-  if (tid == 0) {
-    const long long total = s_carry;
-    base[njobs] = total;
-    int32_t cnt = (int32_t)total;
-    if (total > AS_MAX_POINTS) { atomicOr(status, ST_CAPACITY); cnt = 0; }
-    *out_n = cnt;
-    words[0] = cnt;
-    words[1] = mixed;
   }
 }
 
@@ -234,15 +186,13 @@ int32_t op_assemble_map(b2s_handle* h, int n, const b2s_submap* const* submaps, 
 // nothing is kept per slot: a count pass writes the live slots of every 2048-slot tile (blockIdx.y = table), the batched scan turns them
 // into tile offsets, asm_base_kernel scans the per-entry totals into int64 bases and checks the capacity, and after the one
 // synchronisation (the total sizes the output) a gather recomputes each live slot's rank within its tile and writes sum / count.
-constexpr int DX_ITEMS = 8;                        // consecutive slots per thread: two int4 loads of the counts
-constexpr int DX_TILE = AS_THREADS * DX_ITEMS;     // slots per CTA
-
 struct DenseTable {                  // one listed entry that has a dense map
   const int32_t* cnt; const double* sum;         // the table: count and 6 running sums per slot
   int32_t* tiles; int32_t* toffs;                // per tile: live slots; their exclusive scan (toffs[ntiles] = the table's live voxels)
   long long cap;                                 // slots
   int32_t ntiles;                                // tiles of DX_TILE slots (the batched scan reads its length here)
   int32_t entry;                                 // list position: where its points go
+  __device__ unsigned live_mask(long long s0) const;
 };
 struct DenseJob {                    // one listed entry, for asm_base_kernel
   const int32_t* total;                          // its table's toffs[ntiles], or a zero word without a dense map
@@ -265,20 +215,13 @@ __device__ __forceinline__ int dx_load(const int32_t* __restrict__ cnt, long lon
   return live;
 }
 
-__global__ void __launch_bounds__(AS_THREADS) dx_count_kernel(const DenseTable* __restrict__ tabs) {
-  pdl_wait();
-  const DenseTable t = tabs[blockIdx.y];
-  if ((int)blockIdx.x >= t.ntiles) return;
-  __shared__ int s_warp[AS_THREADS / 32];
+__device__ unsigned DenseTable::live_mask(long long s0) const {
   int32_t c[DX_ITEMS];
-  const int live = warp_sum_i(dx_load(t.cnt, t.cap, (long long)blockIdx.x * DX_TILE + threadIdx.x * DX_ITEMS, c));
-  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = live;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int s = 0;
-    for (int w = 0; w < AS_THREADS / 32; w++) s += s_warp[w];
-    t.tiles[blockIdx.x] = s;
-  }
+  dx_load(cnt, cap, s0, c);
+  unsigned m = 0;
+#pragma unroll
+  for (int k = 0; k < DX_ITEMS; k++) m |= (c[k] > 0 ? 1u : 0u) << k;
+  return m;
 }
 
 // Voxel.cpp:90-115 per live slot, in slot order: the same division as dense_gather_kernel (b2s_submap_dense_download)
@@ -287,20 +230,12 @@ __global__ void __launch_bounds__(AS_THREADS) dx_gather_kernel(const DenseTable*
   pdl_wait();
   const DenseTable t = tabs[blockIdx.y];
   if ((int)blockIdx.x >= t.ntiles) return;
-  __shared__ int s_warp[AS_THREADS / 32];
   const long long s0 = (long long)blockIdx.x * DX_TILE + threadIdx.x * DX_ITEMS;
   int32_t c[DX_ITEMS];
   const int live = dx_load(t.cnt, t.cap, s0, c);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int inc = live;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += v; }
-  if (lane == 31) s_warp[warp] = inc;
-  __syncthreads();
-  int woff = 0;
-  for (int w = 0; w < warp; w++) woff += s_warp[w];
+  const int rank = tile_rank(live);
   if (live == 0) return;
-  size_t o = (size_t)(base[t.entry] + t.toffs[blockIdx.x] + woff + inc - live);
+  size_t o = (size_t)(base[t.entry] + t.toffs[blockIdx.x] + rank);
 #pragma unroll
   for (int k = 0; k < DX_ITEMS; k++) {
     if (c[k] <= 0) continue;
@@ -380,7 +315,7 @@ int32_t op_assemble_dense_maps(b2s_handle* h, int n, const b2s_submap* const* su
   long long* base = reinterpret_cast<long long*>(tab + staged);
   int32_t* words = reinterpret_cast<int32_t*>(tab + staged + t_base);   // [0] the count, [1..2] asm_base_kernel's words
 
-  launch_pdl(dx_count_kernel, dim3((unsigned)max_tiles, (unsigned)m), AS_THREADS, 0, h->stream, dt);
+  launch_pdl(tile_count_kernel<DenseTable>, dim3((unsigned)max_tiles, (unsigned)m), AS_THREADS, 0, h->stream, dt);
   h->launches++;
   B2S_TRY(scan_exclusive_i32_batch(h, ds, m, max_tiles));
   launch_pdl(asm_base_kernel<DenseJob>, 1, AS_BASE_THREADS, 0, h->stream, dj, n, base, words, words + 1, h->status.as<uint32_t>());

@@ -9,7 +9,6 @@ using namespace b2s;
 
 namespace b2s {
 int32_t pose_to_device(b2s_handle* h, const double* T, double* dst);
-int32_t dense_init(b2s_handle* h, b2s_submap* sm, size_t cap, double voxel);
 int32_t dense_to_cloud(b2s_handle* h, b2s_submap* sm, double* d_xyz, int32_t* d_keys, int32_t* d_out_n);
 
 __global__ void f32_to_f64_kernel(const unsigned char* __restrict__ src, size_t stride, int n, double* __restrict__ dst) {
@@ -317,6 +316,31 @@ int32_t make_cloud(b2s_handle* h, size_t capacity, bool normals, bool fixed, std
   b2s_cloud* c = nullptr;
   B2S_TRY(make_cloud(h, capacity, normals, fixed, true, &c));
   out->reset(c);
+  return B2S_OK;
+}
+
+int32_t submap_init(b2s_handle* h, b2s_submap* sm, size_t capacity_points) {
+  static unsigned long long next_uid = 0;
+  sm->h = h;
+  sm->device = h->device;
+  sm->uid = __atomic_add_fetch(&next_uid, 1ull, __ATOMIC_RELAXED);
+  submap_register(sm->uid);
+  sm->capacity = capacity_points;
+  for (std::unique_ptr<b2s_cloud>& c : sm->cloud) {
+    B2S_TRY(make_cloud(h, capacity_points, true, false, &c));
+    c->has_normals = true;
+  }
+  // pose slots: [0] mapToRangeSensor_, [1] pose of a host-driven insertion, [2] odometry motion, [3] initial guess, [4] carving pose,
+  //             [5] pose of the last insertion (= mapToRangeSensorLastScanInsertion_ = mapBuilderCropper_'s pose; Identity before the first)
+  B2S_TRY(sm->pose.ensure(B2S_STATE_POSE_SLOTS * 16 * 8, h->stream));
+  const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  B2S_TRY(pose_to_device(h, I, sm->pose.as<double>()));
+  B2S_TRY(pose_to_device(h, I, sm->pose.as<double>() + 5 * 16));
+  B2S_TRY(sm->mstate.ensure(MS_WORDS * 4, h->stream));
+  B2S_CUDA(cudaMemsetAsync(sm->mstate.p, 0, MS_WORDS * 4, h->stream));
+  B2S_TRY(sm->bbox.ensure(6 * 8, h->stream));
+  B2S_TRY(box_reset(h, sm->bbox.as<unsigned long long>()));   // the empty map
+  b2s_default_mapper_options(&sm->opts);
   return B2S_OK;
 }
 
@@ -823,30 +847,7 @@ int32_t b2s_register_host(b2s_handle* h, const double* src_xyz, size_t n_src, co
 int32_t b2s_submap_create(b2s_handle* h, size_t capacity_points, b2s_submap** out) {
   B2S_REQUIRE(h && out && capacity_points > 0, B2S_E_INVALID, "bad argument");
   LOCK(h);
-  static unsigned long long next_uid = 0;
-  return create_object(out, [&](b2s_submap* sm) -> int32_t {
-    sm->h = h;
-    sm->device = h->device;
-    sm->uid = __atomic_add_fetch(&next_uid, 1ull, __ATOMIC_RELAXED);
-    submap_register(sm->uid);
-    sm->capacity = capacity_points;
-    for (std::unique_ptr<b2s_cloud>& c : sm->cloud) {
-      B2S_TRY(make_cloud(h, capacity_points, true, false, &c));
-      c->has_normals = true;
-    }
-    // pose slots: [0] mapToRangeSensor_, [1] pose of a host-driven insertion, [2] odometry motion, [3] initial guess, [4] carving pose,
-    //             [5] pose of the last insertion (= mapToRangeSensorLastScanInsertion_ = mapBuilderCropper_'s pose; Identity before the first)
-    B2S_TRY(sm->pose.ensure(8 * 16 * 8, h->stream));
-    const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    B2S_TRY(pose_to_device(h, I, sm->pose.as<double>()));
-    B2S_TRY(pose_to_device(h, I, sm->pose.as<double>() + 5 * 16));
-    B2S_TRY(sm->mstate.ensure(MS_WORDS * 4, h->stream));
-    B2S_CUDA(cudaMemsetAsync(sm->mstate.p, 0, MS_WORDS * 4, h->stream));
-    B2S_TRY(sm->bbox.ensure(6 * 8, h->stream));
-    B2S_TRY(box_reset(h, sm->bbox.as<unsigned long long>()));   // the empty map
-    b2s_default_mapper_options(&sm->opts);
-    return B2S_OK;
-  });
+  return create_object(out, [&](b2s_submap* sm) -> int32_t { return submap_init(h, sm, capacity_points); });
 }
 
 void b2s_submap_destroy(b2s_submap* sm) { destroy_object(sm); }

@@ -253,8 +253,9 @@ struct AssemblyScratch {
   PinnedBuf stage;       // page-locked staging of the tables
   b2s_cloud cloud;       // the assembled map in front of the voxel path
   VoxelScratch vox;
+  DevBuf blob;           // A3 (state.cu): the exported blobs, laid out as on the host / the blob being imported
   AssemblyScratch() {
-    for (DevBuf* b : {&tables, &slots, &labels, &rgb, &cloud.xyz, &cloud.nrm, &cloud.dn}) b->tracked = false;
+    for (DevBuf* b : {&tables, &slots, &labels, &rgb, &cloud.xyz, &cloud.nrm, &cloud.dn, &blob}) b->tracked = false;
   }
 };
 }  // namespace b2s
@@ -501,6 +502,10 @@ constexpr int FUSE_STAGE_BASE = 1 << 30;   // chain members >= this are staged s
 constexpr int FUSE_DUP_CAP = 1 << 16;
 int32_t fuse_reserve(b2s_handle* h, b2s_submap* sm);
 int32_t fuse_rehash(b2s_handle* h, b2s_submap* sm, const int32_t* enable_dev = nullptr);
+int32_t dense_init(b2s_handle* h, b2s_submap* sm, size_t cap, double voxel);   // the dense table of cap (a power of two) empty slots
+size_t fuse_table_slots(const b2s_submap* sm);   // the fusion table's slots for the submap's capacity (fuse_reserve)
+// b2s_submap_create's set-up of a new submap (c_api.cu)
+int32_t submap_init(b2s_handle* h, b2s_submap* sm, size_t capacity);
 int32_t submap_compact_view(b2s_handle* h, b2s_submap* sm, b2s_cloud** view);   // -> sm->cloud[1] holding the live points in map order
 // F2 VoxelHashMap queries on the dense map (fuse.cu)
 int32_t op_dense_query(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* pts, int32_t* count_dev, double* mean_dev);

@@ -402,10 +402,15 @@ __global__ void __launch_bounds__(FZ_THREADS) fuse_table_dups_kernel(const unsig
   (void)vkeys;
 }
 
-int32_t fuse_reserve(b2s_handle* h, b2s_submap* sm) {
-  if (sm->vcap) return B2S_OK;
+size_t fuse_table_slots(const b2s_submap* sm) {
   size_t vcap = 4096;
   while (vcap < 2 * sm->capacity) vcap <<= 1;
+  return vcap;
+}
+
+int32_t fuse_reserve(b2s_handle* h, b2s_submap* sm) {
+  if (sm->vcap) return B2S_OK;
+  const size_t vcap = fuse_table_slots(sm);
   B2S_TRY(sm->vkeys.ensure(vcap * 8, h->stream));
   B2S_TRY(sm->vhead.ensure(vcap * 4, h->stream));
   B2S_TRY(sm->vstamp.ensure(vcap * 4, h->stream));

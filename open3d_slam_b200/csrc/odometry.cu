@@ -528,6 +528,51 @@ static int32_t buffer_lookup(b2s_handle* h, const b2s_odometry* od, bool map, lo
   return B2S_OK;
 }
 
+// b2s_odometry_create's set-up of a new object
+static int32_t odometry_init(b2s_handle* h, b2s_odometry* od, const b2s_odometry_params* p, size_t capacity_points) {
+  od->h = h;
+  od->device = h->device;
+  od->params = *p;
+  od->capacity = capacity_points;
+  B2S_TRY(make_cloud(h, capacity_points, true, true, &od->prev));
+  od->prev->has_normals = true;
+  B2S_TRY(make_cloud(h, 1, true, false, &od->pre));
+  B2S_TRY(make_cloud(h, 1, true, false, &od->scratch));
+  B2S_TRY(make_cloud(h, 1, false, false, &od->input));
+  B2S_TRY(od->state.ensure(sizeof(OdoState), h->stream));
+  B2S_CUDA(cudaMemsetAsync(od->state.p, 0, sizeof(OdoState), h->stream));
+  const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  B2S_TRY(pose_to_device(h, I, od->state.as<OdoState>()->cum));
+  B2S_TRY(od->ring_t.ensure((size_t)p->buffer_size * 8, h->stream));
+  B2S_TRY(od->ring_T.ensure((size_t)p->buffer_size * 128, h->stream));
+  B2S_TRY(od->map_t.ensure((size_t)p->buffer_size * 8, h->stream));
+  B2S_TRY(od->map_T.ensure((size_t)p->buffer_size * 128, h->stream));
+  b2s_default_motion_compensation_params(&od->mc);
+  B2S_TRY(od->res.ensure(2 * sizeof(b2s_result), h->stream));
+  B2S_CUDA(cudaMemsetAsync(od->res.p, 0, 2 * sizeof(b2s_result), h->stream));
+  B2S_TRY(od->odo_slots.ensure(256 * sizeof(b2s_odometry_result), h->stream));
+  B2S_CUDA(cudaMemsetAsync(od->odo_slots.p, 0, 256 * sizeof(b2s_odometry_result), h->stream));
+  B2S_TRY(od->slam_slots.ensure(256 * sizeof(b2s_slam_result), h->stream));
+  B2S_CUDA(cudaMemsetAsync(od->slam_slots.p, 0, 256 * sizeof(b2s_slam_result), h->stream));
+  B2S_TRY(od->lookup.ensure(17 * 8, h->stream));
+  B2S_TRY(od->inputs.alloc(ODO_RING * sizeof(OdoStepInput), cudaHostAllocMapped));
+  memset(od->inputs.p, 0, ODO_RING * sizeof(OdoStepInput));
+  return B2S_OK;
+}
+
+// the two de-skewed clouds and the velocity records, allocated when de-skew is first enabled
+static int32_t odometry_deskew_buffers(b2s_handle* h, b2s_odometry* od) {
+  if (od->odo_in) return B2S_OK;
+  std::unique_ptr<b2s_cloud> a, b;
+  B2S_TRY(make_cloud(h, od->capacity, false, false, &a));
+  B2S_TRY(make_cloud(h, od->capacity, false, false, &b));
+  B2S_TRY(od->motion.ensure(256 * sizeof(b2s_motion_compensation_result), h->stream));
+  B2S_CUDA(cudaMemsetAsync(od->motion.p, 0, 256 * sizeof(b2s_motion_compensation_result), h->stream));
+  od->odo_in = std::move(a);
+  od->map_in = std::move(b);
+  return B2S_OK;
+}
+
 }  // namespace b2s
 
 extern "C" {
@@ -550,36 +595,7 @@ int32_t b2s_odometry_create(b2s_handle* h, const b2s_odometry_params* p, size_t 
   B2S_REQUIRE(capacity_points < (size_t)0x7fffffff / 4, B2S_E_INVALID, "capacity too large");
   B2S_TRY(check_odometry_params(*p));
   LOCK(h);
-  return create_object(out, [&](b2s_odometry* od) -> int32_t {
-    od->h = h;
-    od->device = h->device;
-    od->params = *p;
-    od->capacity = capacity_points;
-    B2S_TRY(make_cloud(h, capacity_points, true, true, &od->prev));
-    od->prev->has_normals = true;
-    B2S_TRY(make_cloud(h, 1, true, false, &od->pre));
-    B2S_TRY(make_cloud(h, 1, true, false, &od->scratch));
-    B2S_TRY(make_cloud(h, 1, false, false, &od->input));
-    B2S_TRY(od->state.ensure(sizeof(OdoState), h->stream));
-    B2S_CUDA(cudaMemsetAsync(od->state.p, 0, sizeof(OdoState), h->stream));
-    const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    B2S_TRY(pose_to_device(h, I, od->state.as<OdoState>()->cum));
-    B2S_TRY(od->ring_t.ensure((size_t)p->buffer_size * 8, h->stream));
-    B2S_TRY(od->ring_T.ensure((size_t)p->buffer_size * 128, h->stream));
-    B2S_TRY(od->map_t.ensure((size_t)p->buffer_size * 8, h->stream));
-    B2S_TRY(od->map_T.ensure((size_t)p->buffer_size * 128, h->stream));
-    b2s_default_motion_compensation_params(&od->mc);
-    B2S_TRY(od->res.ensure(2 * sizeof(b2s_result), h->stream));
-    B2S_CUDA(cudaMemsetAsync(od->res.p, 0, 2 * sizeof(b2s_result), h->stream));
-    B2S_TRY(od->odo_slots.ensure(256 * sizeof(b2s_odometry_result), h->stream));
-    B2S_CUDA(cudaMemsetAsync(od->odo_slots.p, 0, 256 * sizeof(b2s_odometry_result), h->stream));
-    B2S_TRY(od->slam_slots.ensure(256 * sizeof(b2s_slam_result), h->stream));
-    B2S_CUDA(cudaMemsetAsync(od->slam_slots.p, 0, 256 * sizeof(b2s_slam_result), h->stream));
-    B2S_TRY(od->lookup.ensure(17 * 8, h->stream));
-    B2S_TRY(od->inputs.alloc(ODO_RING * sizeof(OdoStepInput), cudaHostAllocMapped));
-    memset(od->inputs.p, 0, ODO_RING * sizeof(OdoStepInput));
-    return B2S_OK;
-  });
+  return create_object(out, [&](b2s_odometry* od) -> int32_t { return odometry_init(h, od, p, capacity_points); });
 }
 
 void b2s_odometry_destroy(b2s_odometry* od) { destroy_object(od); }
@@ -721,15 +737,7 @@ int32_t b2s_odometry_set_motion_compensation(b2s_handle* h, b2s_odometry* od, co
   B2S_REQUIRE(p->scan_duration > 0.0, B2S_E_INVALID, "lidar scanDuration_: must be > 0");   // assert_gt at MotionCompensation.cpp:61
   B2S_REQUIRE(p->num_poses_velocity_estimation >= 1, B2S_E_INVALID, "num_poses_velocity_estimation must be >= 1");
   LOCK(h);
-  if (p->enabled && !od->odo_in) {
-    std::unique_ptr<b2s_cloud> a, b;
-    B2S_TRY(make_cloud(h, od->capacity, false, false, &a));
-    B2S_TRY(make_cloud(h, od->capacity, false, false, &b));
-    B2S_TRY(od->motion.ensure(256 * sizeof(b2s_motion_compensation_result), h->stream));
-    B2S_CUDA(cudaMemsetAsync(od->motion.p, 0, 256 * sizeof(b2s_motion_compensation_result), h->stream));
-    od->odo_in = std::move(a);
-    od->map_in = std::move(b);
-  }
+  if (p->enabled) B2S_TRY(odometry_deskew_buffers(h, od));
   od->mc = *p;
   od->params_gen++;   // the captured combined graphs bake the parameters in
   return B2S_OK;
@@ -777,6 +785,120 @@ int32_t b2s_slam_undistorted(b2s_handle* h, const b2s_odometry* od, b2s_cloud* o
     dst[i]->n_known = -1;   // a replayed graph updates only the device count: the host-side one may be that of the captured step
   }
   return B2S_OK;
+}
+
+}  // extern "C"
+
+// ---- A3: the odometry object's state (include/b2s.h "session state") ------------------------------------------------------------------
+namespace b2s {
+static_assert(sizeof(OdoState) % 8 == 0, "the state block is a section of whole words");
+
+// the byte length of every section of an odometry blob (B2S_OS_*); returns the blob's total
+static long long odometry_sections(long long buffer_size, long long n_prev, long long* len) {
+  len[B2S_OS_PARAMS] = (sizeof(b2s_odometry_params) + 7) & ~(size_t)7;
+  len[B2S_OS_MOTION] = (sizeof(b2s_motion_compensation_params) + 7) & ~(size_t)7;
+  len[B2S_OS_STATE] = sizeof(OdoState);
+  len[B2S_OS_RING_TIMES] = len[B2S_OS_MAP_TIMES] = 8 * buffer_size;
+  len[B2S_OS_RING_POSES] = len[B2S_OS_MAP_POSES] = 128 * buffer_size;
+  len[B2S_OS_PREV_XYZ] = len[B2S_OS_PREV_NORMALS] = 24 * n_prev;
+  long long total = B2S_STATE_HEADER_BYTES;
+  for (int k = 0; k < B2S_OS_COUNT; k++) total += len[k];
+  return total;
+}
+}  // namespace b2s
+
+extern "C" {
+
+int32_t b2s_odometry_export_state(b2s_handle* h, const b2s_odometry* od, void* host_or_null, size_t capacity, size_t* n_bytes) {
+  B2S_REQUIRE(h && od && n_bytes, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(od->h == h, B2S_E_INVALID, "the odometry belongs to another handle");
+  LOCK(h);
+  int32_t n_prev = 0;   // synchronisation 1: the size of cloudPrev_
+  B2S_TRY(read_back(h, {{&n_prev, od->prev->dn.p, 4}}));
+  long long len[B2S_OS_COUNT];
+  const long long bs = od->params.buffer_size;
+  const long long total = odometry_sections(bs, n_prev, len);
+  *n_bytes = (size_t)total;
+  if (!host_or_null) return B2S_OK;
+  B2S_REQUIRE((size_t)total <= capacity, B2S_E_CAPACITY, "the blob takes %lld bytes, the buffer holds %zu", total, capacity);
+  unsigned char* b = static_cast<unsigned char*>(host_or_null);
+  memset(b, 0, B2S_STATE_HEADER_BYTES);
+  unsigned long long w[B2S_STATE_HEADER_BYTES / 8] = {0};
+  w[B2S_STATE_W_MAGIC] = B2S_STATE_MAGIC_ODOMETRY; w[B2S_STATE_W_VERSION] = B2S_STATE_VERSION; w[B2S_STATE_W_BYTE_ORDER] = B2S_STATE_BYTE_ORDER;
+  w[B2S_STATE_W_TOTAL_BYTES] = (unsigned long long)total;
+  memcpy(&w[B2S_STATE_W_MAP_VOXEL], &h->cfg.map_voxel_size, 8);
+  w[B2S_STATE_W_N_SECTIONS] = B2S_OS_COUNT;
+  for (int k = 0; k < B2S_OS_COUNT; k++) w[B2S_STATE_W_SECTIONS + k] = (unsigned long long)len[k];
+  w[B2S_OP_CAPACITY] = od->capacity; w[B2S_OP_BUFFER_SIZE] = (unsigned long long)bs; w[B2S_OP_N_PREV] = (unsigned long long)n_prev;
+  w[B2S_OP_HOST_STEP] = (unsigned long long)od->host_step; w[B2S_OP_HAS_T] = od->has_t ? 1 : 0; w[B2S_OP_LAST_T] = (unsigned long long)od->last_t;
+  memcpy(b, w, sizeof(w));
+  long long off = B2S_STATE_HEADER_BYTES;
+  unsigned char* sec[B2S_OS_COUNT];
+  for (int k = 0; k < B2S_OS_COUNT; k++) { sec[k] = b + off; memset(sec[k], 0, (size_t)len[k]); off += len[k]; }
+  memcpy(sec[B2S_OS_PARAMS], &od->params, sizeof(b2s_odometry_params));
+  memcpy(sec[B2S_OS_MOTION], &od->mc, sizeof(b2s_motion_compensation_params));
+  const std::pair<const DevBuf*, int> dev[] = {{&od->state, B2S_OS_STATE}, {&od->ring_t, B2S_OS_RING_TIMES}, {&od->ring_T, B2S_OS_RING_POSES},
+                                               {&od->map_t, B2S_OS_MAP_TIMES}, {&od->map_T, B2S_OS_MAP_POSES}, {&od->prev->xyz, B2S_OS_PREV_XYZ},
+                                               {&od->prev->nrm, B2S_OS_PREV_NORMALS}};
+  for (const auto& d : dev)
+    if (len[d.second]) B2S_CUDA(cudaMemcpyAsync(sec[d.second], d.first->p, (size_t)len[d.second], cudaMemcpyDeviceToHost, h->stream));
+  return check_status(h);   // synchronisation 2: the data
+}
+
+int32_t b2s_odometry_import_state(b2s_handle* h, const void* blob, size_t n_bytes, b2s_odometry** out) {
+  B2S_REQUIRE(h && blob && out, B2S_E_INVALID, "null argument");
+  const unsigned char* b = static_cast<const unsigned char*>(blob);
+  unsigned long long w[B2S_STATE_HEADER_BYTES / 8];
+  B2S_REQUIRE(n_bytes >= B2S_STATE_HEADER_BYTES, B2S_E_INVALID, "state blob: %zu bytes, shorter than its header", n_bytes);
+  memcpy(w, b, sizeof(w));
+  B2S_REQUIRE(w[B2S_STATE_W_MAGIC] == B2S_STATE_MAGIC_ODOMETRY, B2S_E_INVALID, "state blob: not an odometry blob (magic)");
+  B2S_REQUIRE(w[B2S_STATE_W_VERSION] == B2S_STATE_VERSION, B2S_E_INVALID, "state blob: format version %llu, this library reads %d",
+              w[B2S_STATE_W_VERSION], B2S_STATE_VERSION);
+  B2S_REQUIRE(w[B2S_STATE_W_BYTE_ORDER] == B2S_STATE_BYTE_ORDER, B2S_E_INVALID, "state blob: foreign byte order");
+  B2S_REQUIRE(w[B2S_STATE_W_TOTAL_BYTES] == n_bytes, B2S_E_INVALID, "state blob: %zu bytes, its header says %llu", n_bytes, w[B2S_STATE_W_TOTAL_BYTES]);
+  B2S_REQUIRE(w[B2S_STATE_W_N_SECTIONS] == B2S_OS_COUNT, B2S_E_INVALID, "state blob: %llu sections, an odometry blob has %d",
+              w[B2S_STATE_W_N_SECTIONS], (int)B2S_OS_COUNT);
+  const unsigned long long cap = w[B2S_OP_CAPACITY], bs = w[B2S_OP_BUFFER_SIZE], n_prev = w[B2S_OP_N_PREV];
+  B2S_REQUIRE(cap >= 1 && cap < (unsigned long long)0x7fffffff / 4 && bs >= 1 && bs <= (1ull << 24) && n_prev <= cap, B2S_E_INVALID,
+              "state blob: capacity %llu, buffer size %llu, %llu previous points", cap, bs, n_prev);
+  long long len[B2S_OS_COUNT];
+  const long long total = odometry_sections((long long)bs, (long long)n_prev, len);
+  for (int k = 0; k < B2S_OS_COUNT; k++)
+    B2S_REQUIRE(w[B2S_STATE_W_SECTIONS + k] == (unsigned long long)len[k], B2S_E_INVALID, "state blob: section %d holds %llu bytes, its counts give %lld",
+                k, w[B2S_STATE_W_SECTIONS + k], len[k]);
+  B2S_REQUIRE((unsigned long long)total == n_bytes, B2S_E_INVALID, "state blob: sections of %lld bytes in %zu", total, n_bytes);
+  const unsigned char* sec[B2S_OS_COUNT];
+  long long off = B2S_STATE_HEADER_BYTES;
+  for (int k = 0; k < B2S_OS_COUNT; k++) { sec[k] = b + off; off += len[k]; }
+  b2s_odometry_params p;
+  b2s_motion_compensation_params mc;
+  OdoState s;
+  memcpy(&p, sec[B2S_OS_PARAMS], sizeof(p));
+  memcpy(&mc, sec[B2S_OS_MOTION], sizeof(mc));
+  memcpy(&s, sec[B2S_OS_STATE], sizeof(s));
+  B2S_TRY(check_odometry_params(p));
+  B2S_REQUIRE((unsigned long long)p.buffer_size == bs, B2S_E_INVALID, "state blob: buffer size %d, the header says %llu", (int)p.buffer_size, bs);
+  B2S_REQUIRE(mc.scan_duration > 0.0 && mc.num_poses_velocity_estimation >= 1, B2S_E_INVALID, "state blob: de-skew parameters");
+  const long long B = (long long)bs;
+  B2S_REQUIRE(s.head >= 0 && s.head < B && s.count >= 0 && s.count <= B && s.map_head >= 0 && s.map_head < B && s.map_count >= 0 &&
+                  s.map_count <= B && s.slot >= 0 && s.slot < 256, B2S_E_INVALID, "state blob: a buffer position or result slot out of range");
+  LOCK(h);
+  return create_object(out, [&](b2s_odometry* od) -> int32_t {
+    B2S_TRY(odometry_init(h, od, &p, (size_t)cap));
+    if (mc.enabled) B2S_TRY(odometry_deskew_buffers(h, od));
+    memcpy(&od->params, sec[B2S_OS_PARAMS], sizeof(b2s_odometry_params));   // byte for byte, padding included: a re-export is identical
+    memcpy(&od->mc, sec[B2S_OS_MOTION], sizeof(b2s_motion_compensation_params));
+    const std::pair<DevBuf*, int> dev[] = {{&od->state, B2S_OS_STATE}, {&od->ring_t, B2S_OS_RING_TIMES}, {&od->ring_T, B2S_OS_RING_POSES},
+                                           {&od->map_t, B2S_OS_MAP_TIMES}, {&od->map_T, B2S_OS_MAP_POSES}, {&od->prev->xyz, B2S_OS_PREV_XYZ},
+                                           {&od->prev->nrm, B2S_OS_PREV_NORMALS}};
+    for (const auto& d : dev)
+      if (len[d.second]) B2S_CUDA(cudaMemcpyAsync(d.first->p, sec[d.second], (size_t)len[d.second], cudaMemcpyHostToDevice, h->stream));
+    B2S_TRY(cloud_set_count(h, od->prev.get(), (size_t)n_prev));
+    od->host_step = (long long)w[B2S_OP_HOST_STEP];
+    od->has_t = w[B2S_OP_HAS_T] != 0;
+    od->last_t = (long long)w[B2S_OP_LAST_T];
+    return check_status(h);
+  });
 }
 
 }  // extern "C"

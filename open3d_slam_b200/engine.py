@@ -560,6 +560,84 @@ def assembleDenseMaps(eng: Engine, submaps, out: "Cloud | None" = None):
     return out, offsets
 
 
+# ---- session state: a submap's / an odometry object's device state as self-contained blobs (include/b2s.h "session state",
+#      DESIGN.md row A3).  Writing them to files is the caller's business.
+
+_VOXEL_REC = np.dtype([("key", "<u8"), ("slot", "<i4"), ("head", "<i4"), ("stamp", "<i4"), ("reserved_", "<i4")])
+_DENSE_REC = np.dtype([("key", "<u8"), ("sum", "<f8", (6,)), ("slot", "<i4"), ("count", "<i4")])
+
+
+@dataclass
+class StateHeader:
+    """The parsed header of a session-state blob: kind ("submap" / "odometry"), the words of include/b2s.h, and every section's
+    (offset, length) in bytes by name."""
+    kind: str
+    version: int
+    total_bytes: int
+    map_voxel_size: float
+    sections: dict
+    params: dict
+
+    def section(self, blob, name: str, dtype=np.uint8) -> np.ndarray:
+        """the bytes of one section, viewed as dtype (the records as structured arrays: dtype "voxels" / "dense")"""
+        dt = {"voxels": _VOXEL_REC, "dense": _DENSE_REC}.get(dtype, dtype) if isinstance(dtype, str) else dtype
+        o, n = self.sections[name]
+        return np.frombuffer(blob, dtype=np.uint8, count=n, offset=o).view(dt)
+
+
+def parseStateHeader(blob) -> StateHeader:
+    """Reads the header of a blob of exportSubmapStates / DeviceLidarOdometry.exportState (no checks beyond the magic: the import
+    validates)."""
+    w = np.frombuffer(blob, dtype="<u8", count=L.STATE_HEADER_BYTES // 8)
+    magic = int(w[L.STATE_W_MAGIC])
+    if magic == L.STATE_MAGIC_SUBMAP:
+        kind, names, pnames = "submap", L.STATE_SUBMAP_SECTIONS, L.STATE_SUBMAP_PARAMS
+    elif magic == L.STATE_MAGIC_ODOMETRY:
+        kind, names, pnames = "odometry", L.STATE_ODOMETRY_SECTIONS, L.STATE_ODOMETRY_PARAMS
+    else:
+        raise ValueError(f"not a session-state blob (magic {magic:#x})")
+    sections, off = {}, L.STATE_HEADER_BYTES
+    for k, name in enumerate(names):
+        n = int(w[L.STATE_W_SECTIONS + k])
+        sections[name] = (off, n)
+        off += n
+    params = {name: int(w[L.STATE_W_PARAMS + k]) for k, name in enumerate(pnames)}
+    if kind == "submap":
+        params["dense_voxel"] = float(w[L.STATE_W_PARAMS + 4:L.STATE_W_PARAMS + 5].view("<f8")[0])
+    return StateHeader(kind, int(w[L.STATE_W_VERSION]), int(w[L.STATE_W_TOTAL_BYTES]), float(w[L.STATE_W_MAP_VOXEL:L.STATE_W_MAP_VOXEL + 1].view("<f8")[0]),
+                       sections, params)
+
+
+def exportSubmapStates(eng: Engine, submaps) -> list:
+    """Every Submap's device state as one self-contained blob (bytes), in list order, in one batched device call
+    (b2s_submaps_export_state: one synchronisation for the sizes, one for the data).  The submaps are only read."""
+    n, arr = _submap_array(submaps)
+    offs = (C.c_size_t * (n + 1))()
+    L.check(L.lib().b2s_submaps_export_state(eng._h, C.c_int32(n), arr, None, C.c_size_t(0), offs))
+    buf = np.empty(max(int(offs[n]), 1), dtype=np.uint8)
+    L.check(L.lib().b2s_submaps_export_state(eng._h, C.c_int32(n), arr, buf.ctypes.data_as(C.c_void_p), C.c_size_t(int(offs[n])), offs))
+    return [buf[offs[k]:offs[k + 1]].tobytes() for k in range(n)]
+
+
+def importSubmapState(eng: Engine, blob: bytes) -> "Submap":
+    """A new Submap on eng holding exactly the exported state (b2s_submap_import_state); a blob the library refuses raises B2SError
+    with B2S_E_INVALID and creates nothing.  The host-side schedule counters and the map-builder cropper pose are taken from the
+    device words the blob restores (nScansInsertedMap_, nScansInsertedDenseMap_, the pose of the last insertion)."""
+    blob = bytes(blob)
+    s = C.c_void_p()
+    L.check(L.lib().b2s_submap_import_state(eng._h, blob, C.c_size_t(len(blob)), C.byref(s)))
+    hdr = parseStateHeader(blob)
+    sm = Submap.__new__(Submap)
+    sm.eng, sm._s, sm.capacity = eng, s, hdr.params["capacity"]
+    ms = hdr.section(blob, "mstate", "<i4")
+    sm.nScansInsertedMap_, sm.nScansInsertedDenseMap_ = int(ms[5]), int(ms[6])   # MS_NINS, MS_NDENSE
+    sm._cropperPose = hdr.section(blob, "pose", "<f8").reshape(L.STATE_POSE_SLOTS, 4, 4)[5].copy()
+    sm.lastCarvedCount = 0
+    sm.sparseMapCloud_ = None
+    sm.feature_ = None
+    return sm
+
+
 @dataclass
 class PoseGraphNode:
     """[O3D] PoseGraphNode: pose_ (4x4)"""
@@ -1381,6 +1459,24 @@ class DeviceLidarOdometry:
         c.eng = self.eng; c._c = st; c._borrowed = True
         self._staging = c
         return c
+
+    def exportState(self) -> bytes:
+        """The object's device state as one self-contained blob (b2s_odometry_export_state)"""
+        n = C.c_size_t()
+        L.check(L.lib().b2s_odometry_export_state(self.eng._h, self._o, None, C.c_size_t(0), C.byref(n)))
+        buf = np.empty(int(n.value), dtype=np.uint8)
+        L.check(L.lib().b2s_odometry_export_state(self.eng._h, self._o, buf.ctypes.data_as(C.c_void_p), C.c_size_t(int(n.value)), C.byref(n)))
+        return buf.tobytes()
+
+    @classmethod
+    def importState(cls, eng: Engine, blob: bytes, params: OdometryParameters | None = None) -> "DeviceLidarOdometry":
+        """A new object on eng holding exactly the exported state (b2s_odometry_import_state).  The device parameters come from the
+        blob; params (optional) is only the host-side copy setParameters would keep."""
+        blob = bytes(blob)
+        od = cls.__new__(cls)
+        od.eng, od.params_, od._o = eng, params, C.c_void_p()
+        L.check(L.lib().b2s_odometry_import_state(eng._h, blob, C.c_size_t(len(blob)), C.byref(od._o)))
+        return od
 
     def fetchSlamResult(self, slot: int = 0) -> SlamStepResult:
         r = L.SlamResult()

@@ -28,6 +28,7 @@ import collections
 import copy
 import ctypes as C
 import math
+import pickle
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -517,6 +518,98 @@ class SegmentMapper:
             sc.events.append(("loop_closure_correction", k, latest.sourceSubmapIdx, np.array(dT)))
         return len(constraints)
 
+    # -- session state: save a mapping session to one .npz file and continue it later, on another backend or GPU
+    SESSION_VERSION = 1
+
+    def saveSession(self, path: str) -> None:
+        """Writes everything the next scan depends on to path (.npz): the backend's state blobs of every submap and of the odometry
+        (DeviceBackend: the device blobs of include/b2s.h "session state"), the SubmapCollection (records, active index and merge count,
+        the overlap buffer's clouds and poses, finished and pending ids, adjacency and loop-closure marks, AdjacencyMatrix, odometry
+        constraints, the hand-over flag and the last insertion's pose and timestamp), the OptimizationProblem's constraints and counters,
+        this mapper's pose, scan count, initial-value flag and poses, and every finished submap's feature cloud and FPFH.  results and
+        events are history and are not written.  The host state is pickled: load only session files you wrote."""
+        sc, be = self.submaps, self.backend
+        arrays = {}
+
+        def put(name, obj):   # a backend's state: bytes go into the file as arrays, anything else (the oracle's copies) is pickled
+            if isinstance(obj, (bytes, bytearray)):
+                arrays[name] = np.frombuffer(bytes(obj), dtype=np.uint8)
+                return ("array", name)
+            return ("object", obj)
+
+        records = []
+        for i, (r, blob) in enumerate(zip(sc.submaps, be.export_submaps([r.handle for r in sc.submaps]))):
+            rec = dict(id=r.id, parent=r.parent, origin=r.origin, center=r.center, has_voxel_map=r.has_voxel_map, state=put(f"submap_{i}", blob),
+                       features=r.sparse is not None)
+            if r.sparse is not None:
+                arrays[f"sparse_xyz_{i}"], arrays[f"sparse_nrm_{i}"], arrays[f"feature_{i}"] = be.feature_arrays(r.sparse, r.feature)
+            records.append(rec)
+        overlap = []
+        for j, (cloud, T) in enumerate(sc.overlapScansBuffer):
+            if cloud is not None:
+                xyz, nrm = be.cloud_arrays(cloud)
+                arrays[f"overlap_xyz_{j}"] = xyz
+                if nrm is not None:
+                    arrays[f"overlap_nrm_{j}"] = nrm
+            overlap.append((cloud is not None, np.array(T)))
+        op = self.optimizationProblem
+        host = dict(
+            version=self.SESSION_VERSION, submapParams=sc.params, isAttemptLoopClosures=self.isAttemptLoopClosures, loopClosing=self.loopClosing,
+            records=records, odometry=put("odometry", be.export_odometry()),
+            activeSubmapIdx=sc.activeSubmapIdx, numScansMergedInActiveSubmap=sc.numScansMergedInActiveSubmap, overlap=overlap,
+            finishedSubmapsIdxs=list(sc.finishedSubmapsIdxs), pendingFinishedSubmapIds=list(sc.pendingFinishedSubmapIds),
+            adjacency=set(sc.adjacency), loopClosureSubmaps=set(sc.loopClosureSubmaps), adjacencyMatrix=sc.adjacencyMatrix,
+            collectionOdometryConstraints=list(sc.odometryConstraints), isForceNewSubmapCreation=sc.isForceNewSubmapCreation,
+            collectionMapToRangeSensor=np.array(sc.mapToRangeSensor_), timestamp=sc.timestamp_,
+            optimization={k: v for k, v in vars(op).items() if k not in ("backend", "lastStats")},
+            mapToRangeSensor=np.array(self.mapToRangeSensor), k=self._k, isNewInitialValueSet=self.isNewInitialValueSet,
+            poses=[np.array(T) for T in self.poses])
+        arrays["host"] = np.frombuffer(pickle.dumps(host), dtype=np.uint8)
+        with open(path, "wb") as f:
+            np.savez(f, **arrays)
+
+    @classmethod
+    def loadSession(cls, path: str, backend) -> "SegmentMapper":
+        """A SegmentMapper on backend continuing the session saveSession wrote: the next addRangeMeasurement / addRangeScan goes on
+        where the saved mapper stopped.  results and events start empty; the revisit check's voxel maps are rebuilt from the restored
+        maps (backend.build_voxel_map)."""
+        with np.load(path, allow_pickle=False) as z:
+            arrays = {k: z[k] for k in z.files}
+        host = pickle.loads(arrays["host"].tobytes())
+        if host["version"] != cls.SESSION_VERSION:
+            raise ValueError(f"session format {host['version']}, this version reads {cls.SESSION_VERSION}")
+
+        def get(ref):
+            kind, v = ref
+            return arrays[v].tobytes() if kind == "array" else v
+
+        m = cls(backend, host["submapParams"], host["isAttemptLoopClosures"], host["loopClosing"])
+        sc = m.submaps
+        for i, rec in enumerate(host["records"]):
+            r = SubmapRecord(backend.import_submap(get(rec["state"])), rec["id"], rec["parent"], np.array(rec["origin"]),
+                             None if rec["center"] is None else np.array(rec["center"]))
+            if rec["features"]:
+                r.sparse, r.feature = backend.restore_features(r.handle, arrays[f"sparse_xyz_{i}"], arrays[f"sparse_nrm_{i}"], arrays[f"feature_{i}"])
+            if rec["has_voxel_map"]:
+                backend.build_voxel_map(r.handle)
+                r.has_voxel_map = True
+            sc.submaps.append(r)
+        odo = get(host["odometry"])
+        if odo is not None:
+            backend.import_odometry(odo)
+        sc.activeSubmapIdx, sc.numScansMergedInActiveSubmap = host["activeSubmapIdx"], host["numScansMergedInActiveSubmap"]
+        for j, (has_cloud, T) in enumerate(host["overlap"]):
+            cloud = backend.make_cloud(arrays[f"overlap_xyz_{j}"], arrays.get(f"overlap_nrm_{j}")) if has_cloud else None
+            sc.overlapScansBuffer.append((cloud, T))
+        sc.finishedSubmapsIdxs, sc.pendingFinishedSubmapIds = host["finishedSubmapsIdxs"], host["pendingFinishedSubmapIds"]
+        sc.adjacency, sc.loopClosureSubmaps, sc.adjacencyMatrix = host["adjacency"], host["loopClosureSubmaps"], host["adjacencyMatrix"]
+        sc.odometryConstraints, sc.isForceNewSubmapCreation = host["collectionOdometryConstraints"], host["isForceNewSubmapCreation"]
+        sc.mapToRangeSensor_, sc.timestamp_ = host["collectionMapToRangeSensor"], host["timestamp"]
+        for k, v in host["optimization"].items():
+            setattr(m.optimizationProblem, k, v)
+        m.mapToRangeSensor, m._k, m.isNewInitialValueSet, m.poses = host["mapToRangeSensor"], host["k"], host["isNewInitialValueSet"], host["poses"]
+        return m
+
     def finishProcessing(self) -> None:
         """SlamWrapper::finishProcessing (src/SlamWrapper.cpp:126-166) once every scan has been mapped: forceNewSubmapCreation finishes
         the active submap, then, with isAttemptLoopClosures, attempts run until one builds no constraint or one correction has been
@@ -1004,17 +1097,56 @@ class DeviceBackend:
     # -- scan-to-scan odometry on the device, feeding the mapper step its prediction (SegmentMapper.addRangeScan)
     def odometry(self) -> E.DeviceLidarOdometry:
         if self._odo is None:
-            import torch
-            self._odo = E.DeviceLidarOdometry(self.eng, self.odometry_params, self.raw_capacity)
+            odo = E.DeviceLidarOdometry(self.eng, self.odometry_params, self.raw_capacity)
             if self.motion_compensation is not None:
-                self._odo.setMotionCompensation(self.motion_compensation)
+                odo.setMotionCompensation(self.motion_compensation)
             if self._odo_initial is not None:
-                self._odo.setInitialTransform(self._odo_initial)
-            if self.graph:
-                self._odo.enableGraph(self.raw_capacity)
-            self._slam_pin = torch.empty(C.sizeof(L.SlamResult), dtype=torch.uint8).pin_memory()
-            self._slam_out = L.SlamResult.from_address(self._slam_pin.data_ptr())
+                odo.setInitialTransform(self._odo_initial)
+            self._use_odometry(odo)
         return self._odo
+
+    def _use_odometry(self, odo: E.DeviceLidarOdometry) -> None:
+        import torch
+        if self.graph:
+            odo.enableGraph(self.raw_capacity)
+        self._slam_pin = torch.empty(C.sizeof(L.SlamResult), dtype=torch.uint8).pin_memory()
+        self._slam_out = L.SlamResult.from_address(self._slam_pin.data_ptr())
+        self._odo = odo
+
+    # -- session state (include/b2s.h "session state"): device blobs of the submaps and of the odometry, restored on this backend
+    def export_submaps(self, sms) -> list:
+        return E.exportSubmapStates(self.eng, sms)
+
+    def import_submap(self, blob: bytes):
+        return E.importSubmapState(self.eng, blob)
+
+    def export_odometry(self) -> bytes | None:
+        """None while SegmentMapper.addRangeScan has not created the odometry"""
+        return None if self._odo is None else self._odo.exportState()
+
+    def import_odometry(self, blob: bytes) -> None:
+        """the odometry of the next addRangeScan steps becomes the exported one (its parameters, buffers and de-skew settings)"""
+        if self._odo is not None:
+            self._odo.free()
+        self._use_odometry(E.DeviceLidarOdometry.importState(self.eng, blob, self.odometry_params))
+
+    def cloud_arrays(self, c):
+        """a cloud's points and normals (None without), exact fp64 copies"""
+        return c.download()
+
+    def make_cloud(self, xyz, nrm=None):
+        return self.eng.cloud(xyz, nrm)
+
+    def feature_arrays(self, sparse, feature):
+        """a finished submap's feature cloud (points, normals) and FPFH rows, exact fp64 copies"""
+        xyz, nrm = sparse.download()
+        return xyz, nrm, feature.data_
+
+    def restore_features(self, sm, xyz, nrm, data):
+        """the feature cloud and FPFH of compute_features, uploaded into the submap that owns them"""
+        sm.sparseMapCloud_ = self.eng.cloud(xyz, nrm)
+        sm.feature_ = E.Feature(self.eng, data)
+        return sm.getSparseMapPointCloud(), sm.getFeatures()
 
     def first_scan_with_odometry(self, sm, raw: np.ndarray, t: int):
         """Mapper.cpp:109-112 for the map, with mapToRangeSensorBuffer_.push(t, mapToRangeSensor_ = I), and LidarOdometry::addRangeScan

@@ -258,6 +258,30 @@ SubmapB200::SubmapB200(const MapperParameters& p, size_t capacityPoints)
   if (rc != B2S_OK) b2sThrow(rc);
 }
 
+SubmapB200::SubmapB200(const MapperParameters& p, b2s_handle* h, b2s_submap* sm)
+    : cfg_(b2sConfigFrom(p.scanMatcher_.icp_, &p.scanProcessing_, &p.mapBuilder_)), mapBuilder_(p.mapBuilder_), denseMapBuilder_(p.denseMapBuilder_),
+      h_(h), sm_(sm) {
+  cfg_.dense_voxel_size = p.denseMapBuilder_.mapVoxelSize_;
+}
+
+std::unique_ptr<SubmapB200> SubmapB200::importState(b2s_handle* h, const std::vector<uint8_t>& blob, const MapperParameters& p) {
+  b2s_submap* sm = nullptr;
+  int32_t rc = b2s_submap_import_state(h, blob.data(), blob.size(), &sm);
+  if (rc != B2S_OK) b2sThrow(rc);
+  std::unique_ptr<SubmapB200> out(new SubmapB200(p, h, sm));
+  b2s_mapper_counters c;
+  rc = b2s_submap_get_mapper_counters(h, sm, &c);
+  if (rc != B2S_OK) b2sThrow(rc);
+  out->nScansInsertedMap_ = (size_t)c.inserted_map;
+  out->nScansInsertedDenseMap_ = (size_t)c.inserted_dense;
+  // pose slot 5 of the pose section (the first section): the pose of the last insertion, mapBuilderCropper_'s
+  double T[16];
+  std::memcpy(T, blob.data() + B2S_STATE_HEADER_BYTES + 5 * sizeof(T), sizeof(T));
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j < 4; ++j) out->cropperPose_.matrix()(i, j) = T[4 * i + j];
+  return out;
+}
+
 SubmapB200::~SubmapB200() {
   b2s_feature_destroy(feature_);
   b2s_cloud_destroy(sparse_);
@@ -601,6 +625,21 @@ std::vector<PointCloud> getDenseSubmapPointCloudsB200(const std::vector<const Su
   for (size_t k = 0; k < sms.size(); ++k)
     clouds[k].points_.assign(all->points_.begin() + offsets[k], all->points_.begin() + offsets[k + 1]);
   return clouds;
+}
+
+std::vector<std::vector<uint8_t>> exportSubmapStatesB200(const std::vector<const SubmapB200*>& submaps) {
+  std::vector<std::vector<uint8_t>> blobs(submaps.size());
+  if (submaps.empty()) return blobs;
+  b2s_handle* h = nullptr;
+  const std::vector<const b2s_submap*> sms = assemblyInputs(submaps, &h);
+  std::vector<size_t> offsets(sms.size() + 1);
+  int32_t rc = b2s_submaps_export_state(h, (int32_t)sms.size(), sms.data(), nullptr, 0, offsets.data());
+  if (rc != B2S_OK) b2sThrow(rc);
+  std::vector<uint8_t> all(offsets.back());
+  rc = b2s_submaps_export_state(h, (int32_t)sms.size(), sms.data(), all.data(), all.size(), offsets.data());
+  if (rc != B2S_OK) b2sThrow(rc);
+  for (size_t k = 0; k < sms.size(); ++k) blobs[k].assign(all.begin() + offsets[k], all.begin() + offsets[k + 1]);
+  return blobs;
 }
 
 PointCloud SubmapB200::getDenseMapPointCloud() const { return std::move(getDenseSubmapPointCloudsB200({this}).front()); }

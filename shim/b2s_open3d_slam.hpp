@@ -100,12 +100,17 @@ class SubmapB200 {
   void computeFeatures(const PlaceRecognitionParameters& p);
   const PointCloud& getSparseMapPointCloud() const;
   const Feature& getFeatures() const;                       // throws before the first computeFeatures, like the reference
+  // a submap whose device state is a blob of exportSubmapStatesB200 (b2s_submap_import_state, DESIGN.md row A3), on h (any handle whose
+  // map voxel size is the exporter's; the blob's own capacities).  The insertion counters and the map-builder cropper's pose come from
+  // the blob; a blob the library refuses throws.
+  static std::unique_ptr<SubmapB200> importState(b2s_handle* h, const std::vector<uint8_t>& blob, const MapperParameters& p);
   b2s_submap* handle() const { return sm_; }
   b2s_handle* engine() const { return h_; }
   b2s_cloud* sparseCloud() const { return sparse_; }        // device-resident sparse cloud / feature (null before computeFeatures)
   b2s_feature* feature() const { return feature_; }
 
  private:
+  SubmapB200(const MapperParameters& p, b2s_handle* h, b2s_submap* sm);   // adopts sm (importState)
   b2s_config cfg_;
   MapBuilderParameters mapBuilder_;
   MapBuilderParameters denseMapBuilder_;
@@ -175,6 +180,10 @@ PointCloud assembleColoredPointCloudB200(const std::vector<const SubmapB200*>& s
 // whose dense map was never fed).  One b2s_assemble_dense_maps call, one download, split by its offsets; writing the PCDs stays with the
 // caller, as for saveMap.
 std::vector<PointCloud> getDenseSubmapPointCloudsB200(const std::vector<const SubmapB200*>& submaps);
+// Session state (DESIGN.md row A3): every submap's device state as one self-contained blob, in the order given (all on one handle), for
+// saving a mission next to saveMap / saveDenseSubmaps and restoring it with SubmapB200::importState.  One b2s_submaps_export_state size
+// call and one fill call; writing the files stays with the caller.
+std::vector<std::vector<uint8_t>> exportSubmapStatesB200(const std::vector<const SubmapB200*>& submaps);
 
 // OptimizationProblem::solve (src/OptimizationProblem.cpp:25-44): in place of GlobalOptimization(poseGraph_, LevenbergMarquardt, criteria,
 // option) at :40, with option from params_.globalOptimization_ and [O3D]'s default GlobalOptimizationConvergenceCriteria.  One
