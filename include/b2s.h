@@ -438,6 +438,39 @@ int32_t b2s_debug_global_localization_scores(b2s_handle* h, const b2s_submap* sm
                                              int32_t* hits_out, size_t capacity, size_t* n_hypotheses, double* query_out_or_null,
                                              size_t query_capacity, size_t* n_query);
 
+/* ---- global localisation over every submap of a session (DESIGN.md row M4) ------------------------------------------------------------
+ * The rules of b2s_submap_global_localization, restated for the set sms[0..n_submaps) -- typically every submap of a restored session, so
+ * that a robot restarted anywhere in the mapped site is found and the mapper re-entered there.  It reads the submaps and changes nothing.
+ *   1. query: unchanged (S1's scan-matcher crop at identity, then VoxelDownSample(score_voxel)).
+ *   2. hypotheses: unchanged; a box with x_min > x_max (the default) is the xy extent of the live points of the union of the submaps.
+ *   3. occupancy: a voxel is occupied when it holds a live slot (tombstones skipped) of ANY of the submaps -- the union, keyed in the map
+ *      frame, the frame every submap stores its points in.  The occupancy grid spans the union of the submaps' bounding boxes
+ *      (b2s_debug_submap_bbox); hits(h) as in rule 3 of the one-submap call.
+ *   4. candidates: unchanged.
+ *   A. assignment: candidate c is refined in submap s_c = the one SubmapCollection::findClosestSubmap picks for its hypothesis pose: the
+ *      smallest sqrt((dx^2 + dy^2) + dz^2) between t_c and centers[s] (Submap::getMapToSubmapCenter, map frame), ties -> the lower index
+ *      (std::min_element, src/SubmapCollection.cpp:147-158).
+ *   5. refinement: per candidate, exactly b2s_register_to_submap(match_, sms[s_c], T_c, T_c), under rule 5's last-bits caveat, 16 per
+ *      batched ICP launch; the candidates of one launch may read different submaps, each with its own patch and index.  An empty patch
+ *      -> fitness 0, rmse 0, T = T_c, no correspondences.
+ *   6. decision: unchanged (a candidate that fits well in another submap is a runner-up like any other).  *winner_submap = s_c of the
+ *      winner, -1 when there is no candidate; candidate_submaps_or_null receives s_c of every listed candidate.
+ *   7. errors: rule 7 of the one-submap call with "the map" read as "every submap" (all empty -> B2S_E_EMPTY; the occupancy grid of the
+ *      union over 2^30 bytes -> B2S_E_CAPACITY); n_submaps < 1, a null submap, a non-finite centre, a submap or the scan of another handle
+ *      -> B2S_E_INVALID; n_submaps > B2S_ASSEMBLY_MAX_SUBMAPS -> B2S_E_UNSUPPORTED.
+ * With n_submaps = 1 the hits, the candidates, their order and the decision are those of b2s_submap_global_localization on that submap
+ * (its occupancy grid spans the live box instead of the bbox; both hold every live slot, so they set the same bits).
+ * Synchronises three times: query size and boxes, candidates, result.  candidates_or_null / candidate_submaps_or_null receive the first
+ * min(n_candidates, capacity) entries in rank order. */
+int32_t b2s_submaps_global_localization(b2s_handle* h, const b2s_submap* const* sms, int32_t n_submaps, const double* centers,
+                                        const b2s_cloud* raw_scan, const b2s_global_localization_params* p, double min_refinement_fitness,
+                                        b2s_global_localization_candidate* candidates_or_null, int32_t capacity,
+                                        int32_t* candidate_submaps_or_null, b2s_global_localization_result* out, int32_t* winner_submap);
+/* Debug aid: rules 1-3 over the union, as b2s_debug_global_localization_scores */
+int32_t b2s_debug_submaps_global_localization_scores(b2s_handle* h, const b2s_submap* const* sms, int32_t n_submaps, const b2s_cloud* raw_scan,
+                                                     const b2s_global_localization_params* p, int32_t* hits_out, size_t capacity,
+                                                     size_t* n_hypotheses, double* query_out_or_null, size_t query_capacity, size_t* n_query);
+
 /* ---- device-resident LidarOdometry (src/Odometry.cpp:19-110) and the combined per-scan step of SlamWrapper: odometry, then
  *      Mapper::addRangeMeasurement with the prediction read from the odometry's TransformInterpolationBuffer on the device.
  *      Every decision (initialise / ok / failed, the buffer, the prediction, the mapper gates) is taken on the device.

@@ -191,6 +191,7 @@ SYMBOLS = [
     "b2s_assemble_map", "b2s_assemble_colored_map", "b2s_debug_pose_graph_solve", "b2s_debug_pose_graph_linearize",
     "b2s_debug_estimate_normals", "b2s_debug_submap_bbox",
     "b2s_default_global_localization_params", "b2s_submap_global_localization", "b2s_debug_global_localization_scores",
+    "b2s_submaps_global_localization", "b2s_debug_submaps_global_localization_scores",
     "b2s_assemble_dense_maps",
     "b2s_submaps_export_state", "b2s_submap_import_state", "b2s_odometry_export_state", "b2s_odometry_import_state",
 ]

@@ -12,6 +12,12 @@
 //                       first ones (by index) with hits == T, M entries in all, as (hits, h) sort keys
 //   gl_nms_kernel       one CTA: bitonic sort of the M keys in shared memory, greedy suppression, the candidates' poses
 // Refinement: every candidate's patch is built as b2s_register_to_submap builds it; the registrations run 16 per batched ICP launch.
+//
+// Over a set of submaps (b2s_submaps_global_localization, DESIGN.md row M4) two kernels take gl_occ_kernel's place, each over a device
+// job table of one {slot array, slot count, bbox} per submap (blockIdx.y = submap):
+//   gl_union_box_kernel  the live-point box of the union and the union of the submaps' b2s_submap::bbox, one pass
+//   gl_union_occ_kernel  gl_occ_kernel's bit for every live slot of every submap, into one grid spanning the union of the bboxes
+// The score, selection and suppression kernels are the same launches; each candidate is refined in the submap whose centre is nearest.
 #include "common.cuh"
 
 #include <math.h>
@@ -48,20 +54,57 @@ __device__ __forceinline__ bool gl_probe(const GlOcc& o, double x, double y, dou
   return (__ldg(&o.bits[bit >> 5]) >> (bit & 31)) & 1u;
 }
 
+// sets the bit of map point i (rule 3: tombstones and keys beyond the limit set nothing)
+__device__ __forceinline__ void gl_occ_set(const GlOcc& o, const double* __restrict__ xyz, int i, double inv, uint32_t* bits) {
+  const double x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
+  if (!(x == x && y == y && z == z)) return;   // tombstone
+  const double fx = floor(__dmul_rn(x, inv)), fy = floor(__dmul_rn(y, inv)), fz = floor(__dmul_rn(z, inv));
+  if (!(fabs(fx) < 1048575.0 && fabs(fy) < 1048575.0 && fabs(fz) < 1048575.0)) return;
+  const unsigned kx = (unsigned)((int)fx - o.kmin[0]), ky = (unsigned)((int)fy - o.kmin[1]), kz = (unsigned)((int)fz - o.kmin[2]);
+  if (kx >= (unsigned)o.dims[0] || ky >= (unsigned)o.dims[1] || kz >= (unsigned)o.dims[2]) return;
+  const size_t bit = ((size_t)kz * (size_t)o.dims[1] + ky) * (size_t)o.dims[0] + kx;
+  atomicOr(&bits[bit >> 5], 1u << (bit & 31));
+}
+
 __global__ void __launch_bounds__(GL_THREADS) gl_occ_kernel(const double* __restrict__ xyz, const int32_t* __restrict__ d_n, double inv,
                                                             GlOcc o, uint32_t* bits) {
   pdl_wait();
   const int n = *d_n;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) gl_occ_set(o, xyz, i, inv, bits);
+}
+
+struct GlJob {              // one submap of the union: its map slots, their device count and its b2s_submap::bbox words
+  const double* xyz;
+  const int32_t* d_n;
+  const unsigned long long* bbox;
+};
+
+// grid (blocks, n_jobs).  box[0..5]: the live points' box (ord_encode'd min xyz, max xyz), box[6..11]: the union of the bboxes; both
+// reset to the empty box by the caller
+__global__ void __launch_bounds__(GL_THREADS) gl_union_box_kernel(const GlJob* __restrict__ jobs, unsigned long long* box) {
+  pdl_wait();
+  const GlJob job = jobs[blockIdx.y];
+  const int n = *job.d_n;
+  double mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
-    if (!(x == x && y == y && z == z)) continue;   // tombstone
-    const double fx = floor(__dmul_rn(x, inv)), fy = floor(__dmul_rn(y, inv)), fz = floor(__dmul_rn(z, inv));
-    if (!(fabs(fx) < 1048575.0 && fabs(fy) < 1048575.0 && fabs(fz) < 1048575.0)) continue;
-    const unsigned kx = (unsigned)((int)fx - o.kmin[0]), ky = (unsigned)((int)fy - o.kmin[1]), kz = (unsigned)((int)fz - o.kmin[2]);
-    if (kx >= (unsigned)o.dims[0] || ky >= (unsigned)o.dims[1] || kz >= (unsigned)o.dims[2]) continue;
-    const size_t bit = ((size_t)kz * (size_t)o.dims[1] + ky) * (size_t)o.dims[0] + kx;
-    atomicOr(&bits[bit >> 5], 1u << (bit & 31));
+    const double p[3] = {job.xyz[3 * i], job.xyz[3 * i + 1], job.xyz[3 * i + 2]};
+    if (!(p[0] == p[0] && p[1] == p[1] && p[2] == p[2])) continue;   // tombstone
+#pragma unroll
+    for (int d = 0; d < 3; d++) { mn[d] = fmin(mn[d], p[d]); mx[d] = fmax(mx[d], p[d]); }
   }
+  box_fold_block<GL_THREADS>(mn, mx, box);
+  if (blockIdx.x == 0 && threadIdx.x < 6) {   // the empty bbox (+inf / -inf) leaves the union as it is
+    if (threadIdx.x < 3) atomicMin(&box[6 + threadIdx.x], job.bbox[threadIdx.x]);
+    else atomicMax(&box[6 + threadIdx.x], job.bbox[threadIdx.x]);
+  }
+}
+
+// grid (blocks, n_jobs): gl_occ_kernel over every submap of the job table into one grid
+__global__ void __launch_bounds__(GL_THREADS) gl_union_occ_kernel(const GlJob* __restrict__ jobs, double inv, GlOcc o, uint32_t* bits) {
+  pdl_wait();
+  const GlJob job = jobs[blockIdx.y];
+  const int n = *job.d_n;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) gl_occ_set(o, job.xyz, i, inv, bits);
 }
 
 // grid (ceil(nx ny / GL_THREADS), n_yaw, n_z).  rot: 9 doubles per yaw, row-major
@@ -221,11 +264,11 @@ __global__ void __launch_bounds__(GL_NMS_THREADS) gl_nms_kernel(const unsigned l
 // the call's own scratch, freed on return: the search runs once per (re)localisation, and none of it may count as a re-allocation of the
 // buffers a captured mapper chain holds
 struct GlScratch {
-  DevBuf box, rot, occ, hits, eq, rank, flag, pos, hist, keys, sel, cand_i32, cand_T, scan_state, problems, work, results, hdrs;
+  DevBuf box, jobs, rot, occ, hits, eq, rank, flag, pos, hist, keys, sel, cand_i32, cand_T, scan_state, problems, work, results, hdrs;
   b2s_cloud cropped, query, merge, match;   // merge / match: S1 of the raw scan, kept apart from the mapper's last processed scan
   GlScratch() {
-    for (DevBuf* d : {&box, &rot, &occ, &hits, &eq, &rank, &flag, &pos, &hist, &keys, &sel, &cand_i32, &cand_T, &scan_state, &problems, &work,
-                      &results, &hdrs})
+    for (DevBuf* d : {&box, &jobs, &rot, &occ, &hits, &eq, &rank, &flag, &pos, &hist, &keys, &sel, &cand_i32, &cand_T, &scan_state, &problems,
+                      &work, &results, &hdrs})
       d->tracked = false;
     for (b2s_cloud* c : {&cropped, &query, &merge, &match}) c->xyz.tracked = c->nrm.tracked = c->dn.tracked = false;
   }
@@ -284,12 +327,15 @@ struct GlSetup {
 };
 
 // S1 of the raw scan into match (when given), the query cloud, the live box of the map, the hypothesis grid and the occupancy grid.
-// Synchronises once (query size and box).
-static int32_t gl_prepare(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* raw, const b2s_global_localization_params& p, b2s_cloud* match,
-                          GlScratch& S, GlSetup& G) {
+// union_grid false (one submap, b2s_submap_global_localization): the occupancy grid spans the live box, set by gl_occ_kernel.
+// union_grid true (b2s_submaps_global_localization): it spans the union of the submaps' bboxes, set by gl_union_occ_kernel from every
+// submap.  Both set the same bits: every live slot lies inside either box.  Synchronises once (query size and boxes).
+static int32_t gl_prepare(b2s_handle* h, const b2s_submap* const* sms, int n_sm, bool union_grid, const b2s_cloud* raw,
+                          const b2s_global_localization_params& p, b2s_cloud* match, GlScratch& S, GlSetup& G) {
   B2S_TRY(gl_check_params(p));
-  const b2s_cloud* map = sm->cloud[0].get();
-  B2S_REQUIRE(map->n_max > 0, B2S_E_EMPTY, "global localisation: the map is empty");
+  size_t n_max = 0;
+  for (int s = 0; s < n_sm; s++) n_max = std::max(n_max, sms[s]->cloud[0]->n_max);
+  B2S_REQUIRE(n_max > 0, B2S_E_EMPTY, "global localisation: the map is empty");
   if (match) B2S_TRY(process_scan_impl(h, raw, &S.merge, match));
   b2s_cropper c1 = h->cfg.scan.scan_matcher_cropper;
   c1.center[0] = c1.center[1] = c1.center[2] = 0.0;   // the crop S1 applies to match_, at identity
@@ -298,13 +344,34 @@ static int32_t gl_prepare(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* 
     B2S_TRY(op_crop(h, raw, make_crop(&c1), &S.cropped));
     B2S_TRY(op_voxel_down_sample(h, &S.cropped, nullptr, p.score_voxel, &S.query));
   }
-  B2S_TRY(S.box.ensure(64, h->stream));
-  B2S_TRY(bbox_reduce(h, map->xyz.as<double>(), map->dn.as<int32_t>(), map->n_max, nullptr, S.box.as<unsigned long long>()));
-  unsigned long long box_enc[6];
+  B2S_TRY(S.box.ensure(96, h->stream));
+  unsigned long long* box = S.box.as<unsigned long long>();
+  if (union_grid) {
+    std::vector<GlJob> jobs((size_t)n_sm);
+    for (int s = 0; s < n_sm; s++) {
+      const b2s_cloud* map = sms[s]->cloud[0].get();
+      jobs[s] = GlJob{map->xyz.as<double>(), map->dn.as<int32_t>(), sms[s]->bbox.as<unsigned long long>()};
+    }
+    B2S_TRY(S.jobs.ensure(sizeof(GlJob) * jobs.size(), h->stream));
+    B2S_CUDA(cudaMemcpyAsync(S.jobs.p, jobs.data(), sizeof(GlJob) * jobs.size(), cudaMemcpyHostToDevice, h->stream));
+    B2S_TRY(box_reset(h, box));
+    B2S_TRY(box_reset(h, box + 6));
+    launch_pdl(gl_union_box_kernel, dim3((unsigned)grid_for(n_max, GL_THREADS), (unsigned)n_sm), GL_THREADS, 0, h->stream,
+               static_cast<const GlJob*>(S.jobs.as<GlJob>()), box);
+    h->launches++;
+  } else {
+    const b2s_cloud* map = sms[0]->cloud[0].get();
+    B2S_TRY(bbox_reduce(h, map->xyz.as<double>(), map->dn.as<int32_t>(), map->n_max, nullptr, box));
+  }
+  unsigned long long box_enc[12];
   int32_t nq = 0;
-  B2S_TRY(read_back(h, {{&nq, S.query.dn.p, 4}, {box_enc, S.box.p, 48}}));
-  double bmin[3], bmax[3];
-  for (int d = 0; d < 3; d++) { bmin[d] = ord_decode(box_enc[d]); bmax[d] = ord_decode(box_enc[3 + d]); }
+  B2S_TRY(read_back(h, {{&nq, S.query.dn.p, 4}, {box_enc, S.box.p, union_grid ? 96u : 48u}}));
+  if (!union_grid) memcpy(box_enc + 6, box_enc, 48);   // the occupancy grid spans the live box
+  double bmin[3], bmax[3], omin[3], omax[3];
+  for (int d = 0; d < 3; d++) {
+    bmin[d] = ord_decode(box_enc[d]); bmax[d] = ord_decode(box_enc[3 + d]);
+    omin[d] = fmin(ord_decode(box_enc[6 + d]), bmin[d]); omax[d] = fmax(ord_decode(box_enc[9 + d]), bmax[d]);
+  }
   B2S_REQUIRE(bmin[0] <= bmax[0], B2S_E_EMPTY, "global localisation: the map has no live point");
   B2S_REQUIRE(nq > 0, B2S_E_EMPTY, "global localisation: the query cloud is empty");
   G.nq = nq;
@@ -316,10 +383,10 @@ static int32_t gl_prepare(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* 
   B2S_REQUIRE(fx >= 1.0 && fy >= 1.0 && total <= 2147483647.0, B2S_E_INVALID, "global localisation: %.0f hypotheses, at most 2^31 - 1", total);
   G.box = GlBox{x_min, y_min, p.step, p.z0, p.z_step, 1.0 / p.score_voxel, (int32_t)fx, (int32_t)fy, p.n_yaw, p.n_z};
   G.n_hyp = (long long)total;
-  // the occupancy grid spans the voxel keys of the live box, cut to the key limit
+  // the occupancy grid spans the voxel keys of its box, cut to the key limit
   size_t nbits = 1;
   for (int d = 0; d < 3; d++) {
-    double k0 = floor(bmin[d] * G.box.inv), k1 = floor(bmax[d] * G.box.inv);
+    double k0 = floor(omin[d] * G.box.inv), k1 = floor(omax[d] * G.box.inv);
     k0 = fmax(k0, -1048574.0); k1 = fmin(k1, 1048574.0);
     if (k1 < k0) k1 = k0;
     G.occ.kmin[d] = (int32_t)k0;
@@ -333,8 +400,14 @@ static int32_t gl_prepare(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* 
   B2S_TRY(S.occ.ensure(occ_bytes, h->stream));
   B2S_CUDA(cudaMemsetAsync(S.occ.p, 0, occ_bytes, h->stream));
   G.occ.bits = S.occ.as<uint32_t>();
-  launch_pdl(gl_occ_kernel, grid_for(map->n_max, GL_THREADS), GL_THREADS, 0, h->stream, static_cast<const double*>(map->xyz.as<double>()),
-             static_cast<const int32_t*>(map->dn.as<int32_t>()), G.box.inv, G.occ, S.occ.as<uint32_t>());
+  if (union_grid) {
+    launch_pdl(gl_union_occ_kernel, dim3((unsigned)grid_for(n_max, GL_THREADS), (unsigned)n_sm), GL_THREADS, 0, h->stream,
+               static_cast<const GlJob*>(S.jobs.as<GlJob>()), G.box.inv, G.occ, S.occ.as<uint32_t>());
+  } else {
+    const b2s_cloud* map = sms[0]->cloud[0].get();
+    launch_pdl(gl_occ_kernel, grid_for(map->n_max, GL_THREADS), GL_THREADS, 0, h->stream, static_cast<const double*>(map->xyz.as<double>()),
+               static_cast<const int32_t*>(map->dn.as<int32_t>()), G.box.inv, G.occ, S.occ.as<uint32_t>());
+  }
   h->launches++;
   gl_rotations(p, G.rot);
   B2S_TRY(S.rot.ensure(G.rot.size() * 8, h->stream));
@@ -400,15 +473,16 @@ static int32_t gl_candidates(b2s_handle* h, const b2s_global_localization_params
   return B2S_OK;
 }
 
-// one registration per candidate, each what b2s_register_to_submap(match, sm, T_c, T_c) computes: the patch around T_c's translation built
-// by the same path into the candidate's own index, the same problem, GL_BATCH problems per ICP launch.  The ICP kernel's cluster-wide sums
-// are not reproducible to the last bit from one launch to the next (two b2s_register_to_submap calls on the same inputs differ there as
-// well), so batching costs nothing in exactness.  Synchronises once.
-static int32_t gl_refine(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* match, int n, const double* Ts, GlScratch& S, b2s_result* out) {
+// one registration per candidate, each what b2s_register_to_submap(match, sm_of[c], T_c, T_c) computes: the patch around T_c's translation
+// in the candidate's submap, built by the same path into the candidate's own index, the same problem, GL_BATCH problems per ICP launch
+// (the candidates of one launch may read different submaps).  The ICP kernel's cluster-wide sums are not reproducible to the last bit from
+// one launch to the next (two b2s_register_to_submap calls on the same inputs differ there as well), so batching costs nothing in
+// exactness.  Synchronises once.
+static int32_t gl_refine(b2s_handle* h, const b2s_submap* const* sm_of, const b2s_cloud* match, int n, const double* Ts, GlScratch& S,
+                         b2s_result* out) {
   if (n == 0) return B2S_OK;
   B2S_TRY(check_icp_params(h->cfg.icp));
   B2S_REQUIRE(match->has_normals || h->cfg.icp.reg_type != B2S_REG_GENERALIZED, B2S_E_NO_NORMALS, "GeneralizedIcp: the scan has no normals");
-  const b2s_cloud* map = sm->cloud[0].get();
   const double cell = nn_cell(h, h->cfg.icp.max_corr_dist);
   const size_t work_each = (icp_work_bytes(match->n_max) + 7) / 8;
   B2S_TRY(S.problems.ensure(sizeof(IcpProblem) * (size_t)n, h->stream));
@@ -420,6 +494,8 @@ static int32_t gl_refine(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* m
   for (int b0 = 0; b0 < n; b0 += GL_BATCH) {
     const int nb = n - b0 < GL_BATCH ? n - b0 : GL_BATCH;
     for (int i = 0; i < nb; i++) {
+      const b2s_submap* sm = sm_of[b0 + i];
+      const b2s_cloud* map = sm->cloud[0].get();
       const double* T = Ts + 16 * (size_t)(b0 + i);
       GridIndex* g = h->batch_grids[i].get();   // stream order keeps each build after the previous batch's ICP
       b2s_cropper c = h->cfg.scan.scan_matcher_cropper;   // ScanToMapRegistration.cpp:58 setPose(mapToRangeSensor)
@@ -447,6 +523,106 @@ static int32_t gl_refine(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* m
   return B2S_OK;
 }
 
+// SubmapCollection::findClosestSubmap (src/SubmapCollection.cpp:147-158) for the translation t: the first submap whose centre is
+// nearest, the distance sqrt((dx^2 + dy^2) + dz^2) as Eigen's norm() of a 3-vector sums it
+static int gl_closest(const double* t, const double* centers, int n_sm) {
+  int best = 0;
+  double best_d = 0.0;
+  for (int s = 0; s < n_sm; s++) {
+    const double dx = t[0] - centers[3 * s], dy = t[1] - centers[3 * s + 1], dz = t[2] - centers[3 * s + 2];
+    volatile double sx = dx * dx, sy = dy * dy, sz = dz * dz;
+    volatile double s2 = sx + sy;
+    const double d = sqrt(s2 + sz);
+    if (s == 0 || d < best_d) { best = s; best_d = d; }
+  }
+  return best;
+}
+
+// rules 1-6 over n_sm submaps.  centers (n_sm x 3, or nullptr: every candidate in sms[0]) assign each candidate its submap; union_grid as
+// in gl_prepare.  out is cleared first; cand_submaps / winner_submap (optional) receive the submap of each listed candidate / the winner.
+static int32_t gl_run(b2s_handle* h, const b2s_submap* const* sms, int n_sm, const double* centers, bool union_grid, const b2s_cloud* raw,
+                      const b2s_global_localization_params& p, double min_refinement_fitness, b2s_global_localization_candidate* cands,
+                      int32_t capacity, int32_t* cand_submaps, b2s_global_localization_result* out, int32_t* winner_submap) {
+  memset(out, 0, sizeof(*out));
+  out->winner_rank = -1; out->runner_up_fitness = -1.0;
+  if (winner_submap) *winner_submap = -1;
+  GlScratch S;
+  GlSetup G;
+  b2s_cloud* match = &S.match;
+  B2S_TRY(gl_prepare(h, sms, n_sm, union_grid, raw, p, match, S, G));
+  int32_t nc = 0;
+  std::vector<int32_t> hyp, hits;
+  std::vector<double> Ts;
+  B2S_TRY(gl_candidates(h, p, S, G, &nc, hyp, hits, Ts));
+  std::vector<int32_t> owner((size_t)nc, 0);
+  std::vector<const b2s_submap*> sm_of((size_t)nc);
+  for (int k = 0; k < nc; k++) {
+    const double* T = Ts.data() + 16 * (size_t)k;
+    const double t[3] = {T[3], T[7], T[11]};
+    if (centers) owner[k] = gl_closest(t, centers, n_sm);
+    sm_of[k] = sms[owner[k]];
+  }
+  std::vector<b2s_result> res((size_t)nc);
+  B2S_TRY(gl_refine(h, sm_of.data(), match, nc, Ts.data(), S, res.data()));
+  out->n_hypotheses = G.n_hyp; out->n_query = G.nq; out->n_candidates = nc;
+  int w = -1;
+  for (int k = 0; k < nc; k++) if (w < 0 || res[k].fitness > res[w].fitness) w = k;
+  if (w >= 0) {
+    memcpy(out->T, res[w].T, sizeof(out->T));
+    out->fitness = res[w].fitness; out->inlier_rmse = res[w].inlier_rmse; out->winner_rank = w;
+    out->found = res[w].fitness >= min_refinement_fitness ? 1 : 0;
+    if (winner_submap) *winner_submap = owner[w];
+    const double yw = gl_yaw_of(res[w].T);
+    for (int k = 0; k < nc; k++) {
+      const double dx = res[k].T[3] - res[w].T[3], dy = res[k].T[7] - res[w].T[7], dz = res[k].T[11] - res[w].T[11];
+      volatile double sx = dx * dx, sy = dy * dy, sz = dz * dz;
+      volatile double s2 = sx + sy;
+      const double d = sqrt(s2 + sz);
+      const double dyaw = fabs(remainder(gl_yaw_of(res[k].T) - yw, GL_TWO_PI));
+      if ((d > p.nms_distance || dyaw > p.nms_yaw) && res[k].fitness > out->runner_up_fitness) out->runner_up_fitness = res[k].fitness;
+    }
+  }
+  for (int k = 0; k < nc && k < capacity; k++) {
+    if (cands) {
+      b2s_global_localization_candidate& c = cands[k];
+      memcpy(c.T_hypothesis, Ts.data() + 16 * (size_t)k, sizeof(c.T_hypothesis));
+      c.hypothesis = hyp[k]; c.hits = hits[k]; c.icp = res[k];
+    }
+    if (cand_submaps) cand_submaps[k] = owner[k];
+  }
+  return B2S_OK;
+}
+
+// rules 1-3 only (the debug aids): the hits of every hypothesis and, optionally, the query cloud
+static int32_t gl_debug_scores(b2s_handle* h, const b2s_submap* const* sms, int n_sm, bool union_grid, const b2s_cloud* raw,
+                               const b2s_global_localization_params& p, int32_t* hits_out, size_t capacity, size_t* n_hypotheses,
+                               double* query_out_or_null, size_t query_capacity, size_t* n_query) {
+  GlScratch S;
+  GlSetup G;
+  B2S_TRY(gl_prepare(h, sms, n_sm, union_grid, raw, p, nullptr, S, G));
+  *n_hypotheses = (size_t)G.n_hyp; *n_query = (size_t)G.nq;
+  B2S_REQUIRE(capacity >= (size_t)G.n_hyp, B2S_E_CAPACITY, "hits_out holds %zu entries, %lld needed", capacity, G.n_hyp);
+  B2S_REQUIRE(!query_out_or_null || query_capacity >= (size_t)G.nq, B2S_E_CAPACITY, "query_out holds %zu points, %d needed", query_capacity, G.nq);
+  B2S_CUDA(cudaMemcpyAsync(hits_out, S.hits.p, (size_t)G.n_hyp * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (query_out_or_null) B2S_CUDA(cudaMemcpyAsync(query_out_or_null, S.query.xyz.p, (size_t)G.nq * 24, cudaMemcpyDeviceToHost, h->stream));
+  return check_status(h);
+}
+
+// the argument rules of the submap-set calls (rule 7 of M4)
+static int32_t gl_check_submaps(b2s_handle* h, const b2s_submap* const* sms, int32_t n_submaps, const double* centers) {
+  B2S_REQUIRE(n_submaps >= 1, B2S_E_INVALID, "global localisation: n_submaps must be >= 1");
+  B2S_REQUIRE(n_submaps <= B2S_ASSEMBLY_MAX_SUBMAPS, B2S_E_UNSUPPORTED, "global localisation: %d submaps, at most %d", n_submaps,
+              B2S_ASSEMBLY_MAX_SUBMAPS);
+  for (int32_t s = 0; s < n_submaps; s++) {
+    B2S_REQUIRE(sms[s], B2S_E_INVALID, "global localisation: null submap %d", s);
+    B2S_REQUIRE(sms[s]->h == h, B2S_E_INVALID, "global localisation: submap %d belongs to another handle", s);
+    if (centers)
+      B2S_REQUIRE(finite(centers[3 * s]) && finite(centers[3 * s + 1]) && finite(centers[3 * s + 2]), B2S_E_INVALID,
+                  "global localisation: the centre of submap %d is not finite", s);
+  }
+  return B2S_OK;
+}
+
 }  // namespace b2s
 
 extern "C" {
@@ -470,42 +646,22 @@ int32_t b2s_submap_global_localization(b2s_handle* h, const b2s_submap* sm, cons
   B2S_REQUIRE(sm->h == h && raw_scan->h == h, B2S_E_INVALID, "the submap or the scan belongs to another handle");
   B2S_REQUIRE(!candidates_or_null || capacity >= 0, B2S_E_INVALID, "negative capacity");
   LOCK(h);
-  memset(out, 0, sizeof(*out));
-  out->winner_rank = -1; out->runner_up_fitness = -1.0;
-  GlScratch S;
-  GlSetup G;
-  b2s_cloud* match = &S.match;
-  B2S_TRY(gl_prepare(h, sm, raw_scan, *p, match, S, G));
-  int32_t nc = 0;
-  std::vector<int32_t> hyp, hits;
-  std::vector<double> Ts;
-  B2S_TRY(gl_candidates(h, *p, S, G, &nc, hyp, hits, Ts));
-  std::vector<b2s_result> res((size_t)nc);
-  B2S_TRY(gl_refine(h, sm, match, nc, Ts.data(), S, res.data()));
-  out->n_hypotheses = G.n_hyp; out->n_query = G.nq; out->n_candidates = nc;
-  int w = -1;
-  for (int k = 0; k < nc; k++) if (w < 0 || res[k].fitness > res[w].fitness) w = k;
-  if (w >= 0) {
-    memcpy(out->T, res[w].T, sizeof(out->T));
-    out->fitness = res[w].fitness; out->inlier_rmse = res[w].inlier_rmse; out->winner_rank = w;
-    out->found = res[w].fitness >= min_refinement_fitness ? 1 : 0;
-    const double yw = gl_yaw_of(res[w].T);
-    for (int k = 0; k < nc; k++) {
-      const double dx = res[k].T[3] - res[w].T[3], dy = res[k].T[7] - res[w].T[7], dz = res[k].T[11] - res[w].T[11];
-      volatile double sx = dx * dx, sy = dy * dy, sz = dz * dz;
-      volatile double s2 = sx + sy;
-      const double d = sqrt(s2 + sz);
-      const double dyaw = fabs(remainder(gl_yaw_of(res[k].T) - yw, GL_TWO_PI));
-      if ((d > p->nms_distance || dyaw > p->nms_yaw) && res[k].fitness > out->runner_up_fitness) out->runner_up_fitness = res[k].fitness;
-    }
-  }
-  if (candidates_or_null)
-    for (int k = 0; k < nc && k < capacity; k++) {
-      b2s_global_localization_candidate& c = candidates_or_null[k];
-      memcpy(c.T_hypothesis, Ts.data() + 16 * (size_t)k, sizeof(c.T_hypothesis));
-      c.hypothesis = hyp[k]; c.hits = hits[k]; c.icp = res[k];
-    }
-  return B2S_OK;
+  return gl_run(h, &sm, 1, nullptr, false, raw_scan, *p, min_refinement_fitness, candidates_or_null, candidates_or_null ? capacity : 0, nullptr,
+                out, nullptr);
+}
+
+int32_t b2s_submaps_global_localization(b2s_handle* h, const b2s_submap* const* sms, int32_t n_submaps, const double* centers,
+                                        const b2s_cloud* raw_scan, const b2s_global_localization_params* p, double min_refinement_fitness,
+                                        b2s_global_localization_candidate* candidates_or_null, int32_t capacity,
+                                        int32_t* candidate_submaps_or_null, b2s_global_localization_result* out, int32_t* winner_submap) {
+  B2S_REQUIRE(h && sms && centers && raw_scan && p && out && winner_submap, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(raw_scan->h == h, B2S_E_INVALID, "the scan belongs to another handle");
+  B2S_REQUIRE((!candidates_or_null && !candidate_submaps_or_null) || capacity >= 0, B2S_E_INVALID, "negative capacity");
+  B2S_TRY(gl_check_submaps(h, sms, n_submaps, centers));
+  LOCK(h);
+  const bool listed = candidates_or_null || candidate_submaps_or_null;
+  return gl_run(h, sms, n_submaps, centers, true, raw_scan, *p, min_refinement_fitness, candidates_or_null, listed ? capacity : 0,
+                candidate_submaps_or_null, out, winner_submap);
 }
 
 int32_t b2s_debug_global_localization_scores(b2s_handle* h, const b2s_submap* sm, const b2s_cloud* raw_scan, const b2s_global_localization_params* p,
@@ -514,15 +670,17 @@ int32_t b2s_debug_global_localization_scores(b2s_handle* h, const b2s_submap* sm
   B2S_REQUIRE(h && sm && raw_scan && p && hits_out && n_hypotheses && n_query, B2S_E_INVALID, "null argument");
   B2S_REQUIRE(sm->h == h && raw_scan->h == h, B2S_E_INVALID, "the submap or the scan belongs to another handle");
   LOCK(h);
-  GlScratch S;
-  GlSetup G;
-  B2S_TRY(gl_prepare(h, sm, raw_scan, *p, nullptr, S, G));
-  *n_hypotheses = (size_t)G.n_hyp; *n_query = (size_t)G.nq;
-  B2S_REQUIRE(capacity >= (size_t)G.n_hyp, B2S_E_CAPACITY, "hits_out holds %zu entries, %lld needed", capacity, G.n_hyp);
-  B2S_REQUIRE(!query_out_or_null || query_capacity >= (size_t)G.nq, B2S_E_CAPACITY, "query_out holds %zu points, %d needed", query_capacity, G.nq);
-  B2S_CUDA(cudaMemcpyAsync(hits_out, S.hits.p, (size_t)G.n_hyp * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (query_out_or_null) B2S_CUDA(cudaMemcpyAsync(query_out_or_null, S.query.xyz.p, (size_t)G.nq * 24, cudaMemcpyDeviceToHost, h->stream));
-  return check_status(h);
+  return gl_debug_scores(h, &sm, 1, false, raw_scan, *p, hits_out, capacity, n_hypotheses, query_out_or_null, query_capacity, n_query);
+}
+
+int32_t b2s_debug_submaps_global_localization_scores(b2s_handle* h, const b2s_submap* const* sms, int32_t n_submaps, const b2s_cloud* raw_scan,
+                                                     const b2s_global_localization_params* p, int32_t* hits_out, size_t capacity,
+                                                     size_t* n_hypotheses, double* query_out_or_null, size_t query_capacity, size_t* n_query) {
+  B2S_REQUIRE(h && sms && raw_scan && p && hits_out && n_hypotheses && n_query, B2S_E_INVALID, "null argument");
+  B2S_REQUIRE(raw_scan->h == h, B2S_E_INVALID, "the scan belongs to another handle");
+  B2S_TRY(gl_check_submaps(h, sms, n_submaps, nullptr));
+  LOCK(h);
+  return gl_debug_scores(h, sms, n_submaps, true, raw_scan, *p, hits_out, capacity, n_hypotheses, query_out_or_null, query_capacity, n_query);
 }
 
 }  // extern "C"

@@ -1768,3 +1768,59 @@ def debugGlobalLocalizationScores(eng: Engine, submap: "Submap", rawCloud: "Clou
                                                          C.c_size_t(hits.size), C.byref(nh), q.ctypes.data_as(C.c_void_p), C.c_size_t(len(q)),
                                                          C.byref(nq)))
     return hits, q
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# global localisation over every submap of a session (b2s_submaps_global_localization, DESIGN.md row M4)
+# --------------------------------------------------------------------------------------------------------------------
+@dataclass
+class SubmapsGlobalLocalizationResult(GlobalLocalizationResult):
+    """GlobalLocalizationResult over a list of submaps: the submap (list index) each candidate was refined in, and the winner's"""
+    candidate_submaps: list = None   # int per entry of candidates
+    winner_submap: int = -1          # -1: no candidate
+
+
+def _centers(submaps, centers) -> np.ndarray:
+    c = np.ascontiguousarray(np.asarray(centers, dtype=np.float64).reshape(-1, 3))
+    if len(c) != len(submaps):
+        raise ValueError(f"{len(c)} centres for {len(submaps)} submaps")
+    return c
+
+
+def globalLocalizationInSubmaps(eng: Engine, submaps, centers, rawCloud: "Cloud", params: GlobalLocalizationParameters | None = None,
+                                minRefinementFitness: float = 0.0) -> SubmapsGlobalLocalizationResult:
+    """Localise rawCloud (sensor frame) in the union of the Submaps' maps with no initial pose (b2s_submaps_global_localization, one
+    device call).  centers (n x 3, map frame): Submap::getMapToSubmapCenter of each, which picks the submap a candidate is refined in."""
+    n, arr = _submap_array(submaps)
+    c = _centers(submaps, centers)
+    p = (params or GlobalLocalizationParameters()).to_c()
+    cap = max(int(p.n_candidates), 1)
+    cands = (L.GlobalLocalizationCandidate * cap)()
+    owners = (C.c_int32 * cap)()
+    out = L.GlobalLocalizationResult()
+    win = C.c_int32(-1)
+    L.check(L.lib().b2s_submaps_global_localization(eng._h, arr, C.c_int32(n), _pd(c), rawCloud._c, C.byref(p), C.c_double(float(minRefinementFitness)),
+                                                    cands, C.c_int32(cap), owners, C.byref(out), C.byref(win)))
+    cl = [GlobalLocalizationCandidate(np.array(k.T_hypothesis, dtype=np.float64).reshape(4, 4), int(k.hypothesis), int(k.hits), _res(k.icp))
+          for k in cands[:out.n_candidates]]
+    return SubmapsGlobalLocalizationResult(bool(out.found), np.array(out.T, dtype=np.float64).reshape(4, 4), float(out.fitness),
+                                           float(out.inlier_rmse), float(out.runner_up_fitness), int(out.winner_rank), int(out.n_hypotheses),
+                                           int(out.n_query), cl, [int(owners[k]) for k in range(out.n_candidates)], int(win.value))
+
+
+def debugGlobalLocalizationScoresInSubmaps(eng: Engine, submaps, rawCloud: "Cloud", params: GlobalLocalizationParameters | None = None):
+    """b2s_debug_submaps_global_localization_scores: (hits per hypothesis over the union of the submaps, query cloud)"""
+    n, arr = _submap_array(submaps)
+    p = (params or GlobalLocalizationParameters()).to_c()
+    nh, nq = C.c_size_t(0), C.c_size_t(0)
+    one = np.zeros(1, dtype=np.int32)
+    rc = L.lib().b2s_debug_submaps_global_localization_scores(eng._h, arr, C.c_int32(n), rawCloud._c, C.byref(p), one.ctypes.data_as(C.c_void_p),
+                                                              C.c_size_t(0), C.byref(nh), None, C.c_size_t(0), C.byref(nq))
+    if rc != L.E_CAPACITY or nh.value == 0:
+        L.check(rc)
+    hits = np.zeros(nh.value, dtype=np.int32)
+    q = np.zeros((nq.value, 3), dtype=np.float64)
+    L.check(L.lib().b2s_debug_submaps_global_localization_scores(eng._h, arr, C.c_int32(n), rawCloud._c, C.byref(p),
+                                                                 hits.ctypes.data_as(C.c_void_p), C.c_size_t(hits.size), C.byref(nh),
+                                                                 q.ctypes.data_as(C.c_void_p), C.c_size_t(len(q)), C.byref(nq)))
+    return hits, q

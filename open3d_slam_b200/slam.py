@@ -373,6 +373,7 @@ class SegmentMapper:
         self.isMergeScansIntoMap = bool(mp is not None and mp.isMergeScansIntoMap)
         self.submaps.isUseInitialMap = self.isUseInitialMap
         self.isNewInitialValueSet = False   # Mapper::isNewInitialValueSet_ (the backend keeps the device's copy)
+        self.isRelocalized = False          # relocalize has re-entered the map (finishing order no longer follows submap order)
         self.isAttemptLoopClosures = isAttemptLoopClosures
         self.loopClosing = loopClosing or (LoopClosingParameters.fromMapperParameters(mp) if mp is not None else LoopClosingParameters())
         self.optimizationProblem = OptimizationProblem(backend, self.loopClosing.globalOptimization)
@@ -411,6 +412,53 @@ class SegmentMapper:
         self.submaps.events.append(("global_localization", self._k, r.found, r.T.copy(), r.fitness, r.runner_up_fitness))
         if r.found:
             self.setInitialTransform(r.T)
+        return r
+
+    def relocalize(self, rawScanF32: np.ndarray, t: int | None = None, params=None):
+        """Find the raw scan in the union of every submap with no pose given and re-enter the mapper there (one
+        b2s_submaps_global_localization call, DESIGN.md row M4): after loadSession, after losing track, or on an initial-map mapper.
+        Each candidate is refined in the submap findClosestSubmap picks for it.  When the winner passes the fitness gate
+        (minRefinementFitness):
+          1. the active submap becomes the winner's submap when the found pose T lies within SubmapParameters.radius of its centre;
+             otherwise a new submap is created at T with the winner's submap as its parent (and adjacent to it), and the scan is
+             inserted into it at T as its first scan (Mapper.cpp:105-114 at T).  A submap left behind is finished as at a hand-over,
+             stamped with t (the next scan index when None).  Localisation mode (isUseInitialMap) never creates or finishes submaps:
+             the winner's submap becomes active wherever T lies;
+          2. the overlap buffer is cleared: its scans were taken at the old pose;
+          3. setInitialTransform(T) on the active submap: the next step keeps T and inserts nothing (rule 3 of M2);
+          4. the odometry starts over: the next addRangeScan is its first scan, at T, with empty pose buffers;
+          5. from then on a finished submap's loop-closure candidates are the older submaps only: a re-entered submap can finish
+             after newer ones, and the pose graph takes loop-closure edges only from a newer submap to an older one.
+        A winner that fails the gate changes nothing.  Logged as ("relocalization", k, found, T, fitness, runner_up, submap) in
+        submaps.events, k = the index of the next scan.  Returns the backend's result (with winner_submap)."""
+        sc = self.submaps
+        if not sc.submaps:
+            raise RuntimeError("relocalize: the mapper holds no submap")
+        centers = np.array([s.mapToSubmapCenter() for s in sc.submaps], dtype=np.float64)
+        r = self.backend.global_localization_submaps([s.handle for s in sc.submaps], centers, rawScanF32, params)
+        sc.events.append(("relocalization", self._k, r.found, r.T.copy(), r.fitness, r.runner_up_fitness, r.winner_submap))
+        if not r.found:
+            return r
+        T = np.array(r.T, dtype=np.float64)
+        w, prev = r.winner_submap, sc.activeSubmapIdx
+        inside = np.linalg.norm(T[:3, 3] - sc.submaps[w].mapToSubmapCenter()) < sc.params.radius
+        sc.overlapScansBuffer.clear()
+        sc.activeSubmapIdx = w
+        sc.numScansMergedInActiveSubmap = 0
+        if not inside and not self.isUseInitialMap:
+            sc.createNewSubmap(T)   # parent: the winner's submap
+            a, b = sc.submaps[w].id, sc.getActiveSubmap().id
+            sc.adjacency.add((min(a, b), max(a, b)))
+            sc.adjacencyMatrix.addEdge(a, b)
+            self.backend.first_scan_at(sc.getActiveSubmap().handle, rawScanF32, T)
+            sc.numScansMergedInActiveSubmap = 1
+        if sc.activeSubmapIdx != prev and not self.isUseInitialMap:   # the hand-over of afterInsertion, without the buffered scans
+            sc.finishSubmap(prev)
+            sc.finishedSubmapsIdxs.append(prev)
+            sc.pendingFinishedSubmapIds.append((prev, self._k if t is None else t))
+        self.backend.restart_odometry(T)
+        self.setInitialTransform(T)
+        self.isRelocalized = True
         return r
 
     def addRangeMeasurement(self, rawScanF32: np.ndarray, odometryMotion: np.ndarray):
@@ -505,6 +553,10 @@ class SegmentMapper:
         constraints = []
         for idx, t in finished:   # SubmapCollection::buildLoopClosureConstraints (src/SubmapCollection.cpp:253-267)
             cands = getLoopClosureCandidatesIdxs(sc, sc.adjacencyMatrix, idx, sc.activeSubmapIdx, lp.candidates)
+            if self.isRelocalized:
+                # an older submap re-entered by relocalize can finish after newer ones, but the pose graph takes loop-closure edges only
+                # from a newer submap to an older one (setupLoopClosureEdges)
+                cands = [i for i in cands if i < idx]
             sc.events.append(("loop_closure_candidates", k, idx, cands))
             cs, log = buildLoopClosureConstraints(self.backend, sc, idx, cands, lp.placeRecognition, lp.mapVoxelSize, lp.refinement,
                                                   lp.consistency, timestamp=t)
@@ -563,6 +615,7 @@ class SegmentMapper:
             collectionMapToRangeSensor=np.array(sc.mapToRangeSensor_), timestamp=sc.timestamp_,
             optimization={k: v for k, v in vars(op).items() if k not in ("backend", "lastStats")},
             mapToRangeSensor=np.array(self.mapToRangeSensor), k=self._k, isNewInitialValueSet=self.isNewInitialValueSet,
+            isRelocalized=self.isRelocalized,
             poses=[np.array(T) for T in self.poses])
         arrays["host"] = np.frombuffer(pickle.dumps(host), dtype=np.uint8)
         with open(path, "wb") as f:
@@ -608,6 +661,7 @@ class SegmentMapper:
         for k, v in host["optimization"].items():
             setattr(m.optimizationProblem, k, v)
         m.mapToRangeSensor, m._k, m.isNewInitialValueSet, m.poses = host["mapToRangeSensor"], host["k"], host["isNewInitialValueSet"], host["poses"]
+        m.isRelocalized = host.get("isRelocalized", False)
         return m
 
     def finishProcessing(self) -> None:
@@ -1061,6 +1115,25 @@ class DeviceBackend:
         finally:
             raw_c.free()
 
+    def global_localization_submaps(self, sms, centers, raw: np.ndarray,
+                                    params: E.GlobalLocalizationParameters | None = None) -> E.SubmapsGlobalLocalizationResult:
+        """b2s_submaps_global_localization of a raw float32 scan in the union of the submaps (centers: getMapToSubmapCenter of each),
+        judged by the mapper's fitness gate; the submaps are left as they were"""
+        raw_c = self.eng.cloud(np.ascontiguousarray(raw, dtype=np.float32))
+        try:
+            return E.globalLocalizationInSubmaps(self.eng, sms, centers, raw_c, params, self.params.minRefinementFitness)
+        finally:
+            raw_c.free()
+
+    def restart_odometry(self, T) -> None:
+        """LidarOdometry starts over at T: the odometry object is dropped, so the next step_with_odometry creates a new one (this
+        backend's odometry and de-skew parameters, initial transform T) whose first scan is an initialisation, with no previous cloud
+        and both pose buffers (odometry and map poses) empty"""
+        if self._odo is not None:
+            self._odo.free()
+            self._odo = None
+        self._odo_initial = np.array(T, dtype=np.float64)
+
     def _activate(self, sm):
         self.mapper.submap = sm
         if self.graph:
@@ -1078,11 +1151,15 @@ class DeviceBackend:
 
     def first_scan(self, sm, raw: np.ndarray):
         """Mapper.cpp:109-112: pre-process and insert at Identity (carving is a no-op on the empty map)."""
+        return self.first_scan_at(sm, raw, np.eye(4))
+
+    def first_scan_at(self, sm, raw: np.ndarray, T):
+        """the first scan of an empty submap, pre-processed and inserted at T, which becomes the submap's pose"""
         icp = self.mapper.scan2MapReg_
         raw_c = self.eng.cloud(np.ascontiguousarray(raw, dtype=np.float32))
         ps = icp.processForScanMatchingAndMerging(raw_c)
-        sm.insertScan(raw_c, ps.merge_, np.eye(4))
-        sm.setPose(np.eye(4))
+        sm.insertScan(raw_c, ps.merge_, T)
+        sm.setPose(T)
         raw_c.free()
         return ps.merge_
 

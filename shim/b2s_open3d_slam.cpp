@@ -642,6 +642,22 @@ std::vector<std::vector<uint8_t>> exportSubmapStatesB200(const std::vector<const
   return blobs;
 }
 
+GlobalLocalizationB200 globalLocalizationB200(b2s_handle* h, const std::vector<const SubmapB200*>& submaps,
+                                              const std::vector<Eigen::Vector3d>& centers, const PointCloud& rawScan,
+                                              const b2s_global_localization_params& params, double minRefinementFitness) {
+  if (centers.size() != submaps.size()) throw std::invalid_argument("globalLocalizationB200: one centre per submap");
+  b2s_handle* owner = h;
+  const std::vector<const b2s_submap*> sms = assemblyInputs(submaps, &owner);
+  std::vector<double> c;
+  for (const Eigen::Vector3d& v : centers) c.insert(c.end(), {v(0), v(1), v(2)});
+  DeviceCloud raw(h, rawScan, false);
+  GlobalLocalizationB200 out;
+  const int32_t rc = b2s_submaps_global_localization(h, sms.data(), (int32_t)sms.size(), c.data(), raw.c, &params, minRefinementFitness, nullptr,
+                                                     0, nullptr, &out.result, &out.submap);
+  if (rc != B2S_OK) b2sThrow(rc);
+  return out;
+}
+
 PointCloud SubmapB200::getDenseMapPointCloud() const { return std::move(getDenseSubmapPointCloudsB200({this}).front()); }
 
 }  // namespace o3d_slam

@@ -184,6 +184,17 @@ std::vector<PointCloud> getDenseSubmapPointCloudsB200(const std::vector<const Su
 // saving a mission next to saveMap / saveDenseSubmaps and restoring it with SubmapB200::importState.  One b2s_submaps_export_state size
 // call and one fill call; writing the files stays with the caller.
 std::vector<std::vector<uint8_t>> exportSubmapStatesB200(const std::vector<const SubmapB200*>& submaps);
+// Relocalisation in a restored session (DESIGN.md row M4), in place of SlamMapInitializer's marker pose: the raw scan's mapToRangeSensor
+// in the union of every submap (all on h) without an initial pose, each candidate refined in the submap findClosestSubmap picks for it
+// from centers (Submap::getMapToSubmapCenter of each, in the same order).  One b2s_submaps_global_localization call; the submaps are
+// left as they were.  If result.found, make `submap` the active one (or open a new submap there), then SlamWrapper::setInitialTransform.
+struct GlobalLocalizationB200 {
+  b2s_global_localization_result result;
+  int submap;                                               // the winner's submap (index into the list), -1 without a candidate
+};
+GlobalLocalizationB200 globalLocalizationB200(b2s_handle* h, const std::vector<const SubmapB200*>& submaps,
+                                              const std::vector<Eigen::Vector3d>& centers, const PointCloud& rawScan,
+                                              const b2s_global_localization_params& params, double minRefinementFitness);
 
 // OptimizationProblem::solve (src/OptimizationProblem.cpp:25-44): in place of GlobalOptimization(poseGraph_, LevenbergMarquardt, criteria,
 // option) at :40, with option from params_.globalOptimization_ and [O3D]'s default GlobalOptimizationConvergenceCriteria.  One
