@@ -71,13 +71,10 @@ int32_t op_assemble_map(b2s_handle* h, int n, const b2s_submap* const* submaps, 
   AssemblyScratch& A = h->assembly;
   A.cloud.h = h; A.cloud.device = h->device;
   const bool vox = voxel > 0.0;   // helpers.cpp:108-110: voxelize() is a no-op for voxelSize <= 0
-  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-  size_t bound = 0, max_n = 1, slot_bytes = 0;
+  size_t bound = 0, max_n = 1;
   for (int k = 0; k < n; k++) {
-    const size_t m = submaps[k]->cloud[0]->n_max > 0 ? submaps[k]->cloud[0]->n_max : 1;
     bound += submaps[k]->cloud[0]->n_max;
-    if (m > max_n) max_n = m;
-    slot_bytes += al(scan_state_bytes(m)) + 2 * al((m + 2) * 4);
+    if (submaps[k]->cloud[0]->n_max > max_n) max_n = submaps[k]->cloud[0]->n_max;
   }
   // a larger live total is refused on the device before anything is written, so the assembled cloud never needs more
   if (bound > (size_t)AS_MAX_POINTS) bound = (size_t)AS_MAX_POINTS;
@@ -88,45 +85,40 @@ int32_t op_assemble_map(b2s_handle* h, int n, const b2s_submap* const* submaps, 
   if (colored) B2S_TRY(A.rgb.ensure((bound > 0 ? bound : 1) * 24, h->stream));
 
   // tables: [AsmJob x n][ScanJob x n][palette] staged from the host, then [base x (n + 1)][words] written on the device
-  const size_t t_jobs = al((size_t)n * sizeof(AsmJob)), t_scan = al((size_t)n * sizeof(ScanJob)), t_pal = al(sizeof(kPalette));
-  const size_t staged = t_jobs + t_scan + t_pal, t_base = al(((size_t)n + 1) * 8);
-  B2S_TRY(A.tables.ensure(staged + t_base + 256, h->stream));
-  B2S_TRY(A.slots.ensure(slot_bytes, h->stream));
+  Layout T;
+  const size_t t_jobs = T.off((size_t)n * sizeof(AsmJob)), t_scan = T.off((size_t)n * sizeof(ScanJob)), t_pal = T.off(sizeof(kPalette));
+  const size_t staged = T.size, t_base = T.off(((size_t)n + 1) * 8), t_words = T.off(8);
+  B2S_TRY(A.tables.ensure(T.size, h->stream));
   if (A.stage.cap < staged) B2S_TRY(A.stage.alloc(2 * staged));   // every call ends with a synchronisation: the stage is free
   unsigned char* st = A.stage.as<unsigned char>();
   unsigned char* tab = A.tables.as<unsigned char>();
-  AsmJob* hj = reinterpret_cast<AsmJob*>(st);
-  ScanJob* hs = reinterpret_cast<ScanJob*>(st + t_jobs);
-  memcpy(st + t_jobs + t_scan, kPalette, sizeof(kPalette));
-  unsigned char* slots = A.slots.as<unsigned char>();
-  size_t off = 0;
-  for (int k = 0; k < n; k++) {   // tile states first: they are the region zeroed below
-    const size_t m = submaps[k]->cloud[0]->n_max > 0 ? submaps[k]->cloud[0]->n_max : 1;
-    unsigned long long* s = reinterpret_cast<unsigned long long*>(slots + off);
-    hs[k].state = s;
-    hs[k].counter = reinterpret_cast<int32_t*>(s + (scan_state_bytes(m) - 64) / 8);
-    off += al(scan_state_bytes(m));
-  }
-  const size_t state_bytes = off;
+  AsmJob* hj = reinterpret_cast<AsmJob*>(st + t_jobs);
+  ScanJob* hs = reinterpret_cast<ScanJob*>(st + t_scan);
+  memcpy(st + t_pal, kPalette, sizeof(kPalette));
+  // slots: every submap's tile state (the region zeroed below), then its flags and offsets
+  auto slots_of = [&](int k) { const size_t m = submaps[k]->cloud[0]->n_max; return m > 0 ? m : 1; };
+  size_t state_bytes = 0;
+  B2S_TRY(carve(A.slots, h->stream, [&](Layout& L) {
+    for (int k = 0; k < n; k++) scan_bind_state(L, hs[k], slots_of(k));
+    state_bytes = L.size;
+    for (int k = 0; k < n; k++) { hj[k].flags = L.take<int32_t>(slots_of(k) + 2); hj[k].offs = L.take<int32_t>(slots_of(k) + 2); }
+  }));
   for (int k = 0; k < n; k++) {
     const b2s_submap* sm = submaps[k];
     const b2s_cloud* map = sm->cloud[0].get();
-    const size_t m = map->n_max > 0 ? map->n_max : 1;
     AsmJob& J = hj[k];
     J.xyz = map->xyz.as<double>(); J.nrm = map->nrm.as<double>(); J.d_n = map->dn.as<int32_t>();
-    J.flags = reinterpret_cast<int32_t*>(slots + off); off += al((m + 2) * 4);
-    J.offs = reinterpret_cast<int32_t*>(slots + off); off += al((m + 2) * 4);
     J.label = k % 11;
     J.no_normals = sm->no_normals ? 1 : 0;
     hs[k].in = J.flags; hs[k].out = J.offs; hs[k].d_n = J.d_n;
   }
   B2S_CUDA(cudaMemcpyAsync(tab, st, staged, cudaMemcpyHostToDevice, h->stream));
-  B2S_CUDA(cudaMemsetAsync(slots, 0, state_bytes, h->stream));
-  const AsmJob* dj = reinterpret_cast<const AsmJob*>(tab);
-  const ScanJob* ds = reinterpret_cast<const ScanJob*>(tab + t_jobs);
-  const double* palette = reinterpret_cast<const double*>(tab + t_jobs + t_scan);
-  long long* base = reinterpret_cast<long long*>(tab + staged);
-  int32_t* words = reinterpret_cast<int32_t*>(tab + staged + t_base);
+  B2S_CUDA(cudaMemsetAsync(A.slots.p, 0, state_bytes, h->stream));
+  const AsmJob* dj = reinterpret_cast<const AsmJob*>(tab + t_jobs);
+  const ScanJob* ds = reinterpret_cast<const ScanJob*>(tab + t_scan);
+  const double* palette = reinterpret_cast<const double*>(tab + t_pal);
+  long long* base = reinterpret_cast<long long*>(tab + t_base);
+  int32_t* words = reinterpret_cast<int32_t*>(tab + t_words);
 
   const int bx = grid_for(max_n, AS_THREADS, 2 * device_sms());   // x blocks per job (grid-stride); y = job
   launch_pdl(asm_flags_kernel, dim3((unsigned)bx, (unsigned)n), AS_THREADS, 0, h->stream, dj);
@@ -247,15 +239,12 @@ __global__ void __launch_bounds__(AS_THREADS) dx_gather_kernel(const DenseTable*
 }
 
 int32_t op_assemble_dense_maps(b2s_handle* h, int n, const b2s_submap* const* submaps, b2s_cloud* out, int64_t* offsets) {
-  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  auto tiles_of = [&](int k) { return (submaps[k]->dense_cap + DX_TILE - 1) / DX_TILE; };
   int m = 0;   // entries with a dense map
-  size_t max_tiles = 1, slot_bytes = 0;
+  size_t max_tiles = 1;
   for (int k = 0; k < n; k++) {
-    const size_t cap = submaps[k]->dense_cap;
-    if (cap == 0) continue;
-    const size_t nt = (cap + DX_TILE - 1) / DX_TILE;
-    if (nt > max_tiles) max_tiles = nt;
-    slot_bytes += al(scan_state_bytes(nt)) + al(nt * 4) + al((nt + 2) * 4);
+    if (submaps[k]->dense_cap == 0) continue;
+    if (tiles_of(k) > max_tiles) max_tiles = tiles_of(k);
     m++;
   }
   if (m == 0) {   // nothing to read: every range is empty
@@ -268,52 +257,46 @@ int32_t op_assemble_dense_maps(b2s_handle* h, int n, const b2s_submap* const* su
   AssemblyScratch& A = h->assembly;
   // tables: [DenseTable x m][ScanJob x m][DenseJob x n][zero word] staged from the host, then [base x (n + 1)][out_n, words x 2] written
   // on the device.  The stage also receives the bases.
-  const size_t t_tab = al((size_t)m * sizeof(DenseTable)), t_scan = al((size_t)m * sizeof(ScanJob)), t_jobs = al((size_t)n * sizeof(DenseJob));
-  const size_t staged = t_tab + t_scan + t_jobs + 256, t_base = al(((size_t)n + 1) * 8);
-  B2S_TRY(A.tables.ensure(staged + t_base + 256, h->stream));
-  B2S_TRY(A.slots.ensure(slot_bytes, h->stream));
-  if (A.stage.cap < staged + t_base) B2S_TRY(A.stage.alloc(2 * (staged + t_base)));   // every earlier call synchronised after its upload
+  Layout L;
+  const size_t t_tab = L.off((size_t)m * sizeof(DenseTable)), t_scan = L.off((size_t)m * sizeof(ScanJob));
+  const size_t t_jobs = L.off((size_t)n * sizeof(DenseJob)), t_zero = L.off(4), staged = L.size;
+  const size_t t_base = L.off(((size_t)n + 1) * 8), t_words = L.off(12);   // words: [0] the count, [1..2] asm_base_kernel's words
+  B2S_TRY(A.tables.ensure(L.size, h->stream));
+  if (A.stage.cap < t_words) B2S_TRY(A.stage.alloc(2 * t_words));   // with the bases; every earlier call synchronised after its upload
   unsigned char* st = A.stage.as<unsigned char>();
   unsigned char* tab = A.tables.as<unsigned char>();
-  DenseTable* ht = reinterpret_cast<DenseTable*>(st);
-  ScanJob* hs = reinterpret_cast<ScanJob*>(st + t_tab);
-  DenseJob* hj = reinterpret_cast<DenseJob*>(st + t_tab + t_scan);
-  memset(st + t_tab + t_scan + t_jobs, 0, 256);
-  const int32_t* zero = reinterpret_cast<const int32_t*>(tab + t_tab + t_scan + t_jobs);
-  unsigned char* slots = A.slots.as<unsigned char>();
-  size_t off = 0;
-  for (int k = 0, t = 0; k < n; k++) {   // tile states first: they are the region zeroed below
-    const size_t cap = submaps[k]->dense_cap;
-    if (cap == 0) continue;
-    const size_t nt = (cap + DX_TILE - 1) / DX_TILE;
-    unsigned long long* s = reinterpret_cast<unsigned long long*>(slots + off);
-    hs[t].state = s;
-    hs[t].counter = reinterpret_cast<int32_t*>(s + (scan_state_bytes(nt) - 64) / 8);
-    off += al(scan_state_bytes(nt));
-    t++;
-  }
-  const size_t state_bytes = off;
+  DenseTable* ht = reinterpret_cast<DenseTable*>(st + t_tab);
+  ScanJob* hs = reinterpret_cast<ScanJob*>(st + t_scan);
+  DenseJob* hj = reinterpret_cast<DenseJob*>(st + t_jobs);
+  memset(st + t_zero, 0, 4);
+  const int32_t* zero = reinterpret_cast<const int32_t*>(tab + t_zero);
+  // slots: every table's tile state (the region zeroed below), then its tile counts and offsets
+  size_t state_bytes = 0;
+  B2S_TRY(carve(A.slots, h->stream, [&](Layout& S) {
+    for (int k = 0, t = 0; k < n; k++) if (submaps[k]->dense_cap) scan_bind_state(S, hs[t++], tiles_of(k));
+    state_bytes = S.size;
+    for (int k = 0, t = 0; k < n; k++)
+      if (submaps[k]->dense_cap) { ht[t].tiles = S.take<int32_t>(tiles_of(k)); ht[t].toffs = S.take<int32_t>(tiles_of(k) + 2); t++; }
+  }));
   for (int k = 0, t = 0; k < n; k++) {
     const b2s_submap* sm = submaps[k];
     if (sm->dense_cap == 0) { hj[k].total = zero; continue; }
-    const size_t nt = (sm->dense_cap + DX_TILE - 1) / DX_TILE;
+    const size_t nt = tiles_of(k);
     DenseTable& T = ht[t];
     T.cnt = sm->dense_cnt.as<int32_t>(); T.sum = sm->dense_sum.as<double>();
-    T.tiles = reinterpret_cast<int32_t*>(slots + off); off += al(nt * 4);
-    T.toffs = reinterpret_cast<int32_t*>(slots + off); off += al((nt + 2) * 4);
     T.cap = (long long)sm->dense_cap; T.ntiles = (int32_t)nt; T.entry = k;
     hs[t].in = T.tiles; hs[t].out = T.toffs;
-    hs[t].d_n = reinterpret_cast<const int32_t*>(tab + (size_t)t * sizeof(DenseTable) + offsetof(DenseTable, ntiles));
+    hs[t].d_n = reinterpret_cast<const int32_t*>(tab + t_tab + (size_t)t * sizeof(DenseTable) + offsetof(DenseTable, ntiles));
     hj[k].total = T.toffs + nt;
     t++;
   }
   B2S_CUDA(cudaMemcpyAsync(tab, st, staged, cudaMemcpyHostToDevice, h->stream));
-  B2S_CUDA(cudaMemsetAsync(slots, 0, state_bytes, h->stream));
-  const DenseTable* dt = reinterpret_cast<const DenseTable*>(tab);
-  const ScanJob* ds = reinterpret_cast<const ScanJob*>(tab + t_tab);
-  const DenseJob* dj = reinterpret_cast<const DenseJob*>(tab + t_tab + t_scan);
-  long long* base = reinterpret_cast<long long*>(tab + staged);
-  int32_t* words = reinterpret_cast<int32_t*>(tab + staged + t_base);   // [0] the count, [1..2] asm_base_kernel's words
+  B2S_CUDA(cudaMemsetAsync(A.slots.p, 0, state_bytes, h->stream));
+  const DenseTable* dt = reinterpret_cast<const DenseTable*>(tab + t_tab);
+  const ScanJob* ds = reinterpret_cast<const ScanJob*>(tab + t_scan);
+  const DenseJob* dj = reinterpret_cast<const DenseJob*>(tab + t_jobs);
+  long long* base = reinterpret_cast<long long*>(tab + t_base);
+  int32_t* words = reinterpret_cast<int32_t*>(tab + t_words);
 
   launch_pdl(tile_count_kernel<DenseTable>, dim3((unsigned)max_tiles, (unsigned)m), AS_THREADS, 0, h->stream, dt);
   h->launches++;
@@ -324,7 +307,7 @@ int32_t op_assemble_dense_maps(b2s_handle* h, int n, const b2s_submap* const* su
 
   // the one synchronisation: the bases are the offsets, the last one the total; above AS_MAX_POINTS the status reports ST_CAPACITY
   // and nothing has been written
-  long long* hb = reinterpret_cast<long long*>(st + staged);
+  long long* hb = reinterpret_cast<long long*>(st + t_base);
   B2S_CUDA(cudaMemcpyAsync(hb, base, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, h->stream));
   B2S_TRY(check_status(h));
   const size_t total = (size_t)hb[n];

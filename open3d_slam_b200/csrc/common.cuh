@@ -382,13 +382,37 @@ struct ReadBack { void* dst; const void* src; size_t bytes; };   // host destina
 // reports an error, and check_status's code is returned
 int32_t read_back(b2s_handle* h, std::initializer_list<ReadBack> copies);
 
+// The scratch layout of a batched call: regions in the order they are taken, each rounded up to 256 bytes.  The same layout code runs
+// twice, first on a Layout without a base, which only adds up `size`, then on one with the buffer's base, which places every region where
+// the first pass counted it, so the two cannot disagree.  off() hands out a region's offset, so that a table can be written at that offset
+// in a host stage and read at it in the device buffer; take() hands out base + offset (nullptr while measuring).
+struct Layout {
+  unsigned char* base = nullptr;
+  size_t size = 0;
+  size_t off(size_t bytes) { const size_t o = size; size += (bytes + 255) & ~(size_t)255; return o; }
+  template <typename T>
+  T* take(size_t count) { const size_t o = off(count * sizeof(T)); return base ? reinterpret_cast<T*>(base + o) : nullptr; }
+};
+// runs place(L) on a measuring Layout, ensures buf to the size it counted, then runs place(L) again on buf's base
+template <typename F>
+int32_t carve(DevBuf& buf, cudaStream_t s, F&& place) {
+  Layout L;
+  place(L);
+  B2S_TRY(buf.ensure(L.size, s));
+  L = Layout{buf.as<unsigned char>()};
+  place(L);
+  return B2S_OK;
+}
+
 // ---- primitives (scan.cu / radix_sort.cu / grid_index.cu / ...) : all asynchronous on h->stream ----
 // exclusive scan of in[0..*d_n) into out[0..*d_n]; out[*d_n] and *d_total (optional) receive the total.  state (optional): the tile
 // state buffer to use instead of the handle's
 int32_t scan_exclusive_i32(b2s_handle* h, const int32_t* in, int32_t* out, const int32_t* d_n, size_t n_max, int32_t* d_total,
                            DevBuf* state = nullptr);
-// njobs independent scans in one launch; every job's tile state (scan_state_bytes(n_max), zeroed) is supplied by the caller
-size_t scan_state_bytes(size_t n_max);
+// njobs independent scans in one launch.  Every job's tile state comes from scan_bind_state with the same n_max and is zeroed before
+// the scan: it takes the state from L and points j.state / j.counter into it (the measuring pass only counts).  A caller binds every
+// job's state before its other regions, so that the states are one range that one memset clears.
+void scan_bind_state(Layout& L, ScanJob& j, size_t n_max);
 int32_t scan_exclusive_i32_batch(b2s_handle* h, const ScanJob* jobs_dev, int njobs, size_t n_max);
 // stable LSD radix sort of (key, value) pairs, key_bits low bits significant; result ends in keys/vals
 // (pointers are swapped so that keys/vals designate the sorted arrays on return, *_alt the scratch).  own (optional): the histogram and
@@ -523,6 +547,12 @@ int32_t op_undistort(b2s_handle* h, const b2s_cloud* in, const double* lin_vel, 
 // L1 overlap selection in front of the loop-closure ICP (overlap.cu); T_dev = sourceToTarget (device, row-major)
 int32_t op_overlap(b2s_handle* h, const b2s_cloud* source, const b2s_cloud* target, const double* T_dev, double voxel, int min_pts,
                    b2s_cloud* source_overlap, b2s_cloud* target_overlap);
+// the same for n pairs in one set of launches (overlap.cu).  Its tables are staged in the caller's page-locked stage at the offsets
+// overlap_tables carved from the caller's stage layout, and uploaded to the same offsets of h->odo.
+struct OverlapTables { size_t jobs, scan, T, end; };
+OverlapTables overlap_tables(Layout& stage, int n);
+int32_t op_overlap_batch(b2s_handle* h, int n, const b2s_submap* const* maps, const double* inits, double voxel, int min_pts,
+                         b2s_cloud* const* outs, unsigned char* stage, const OverlapTables& tb);
 // L2 odometry constraints of n (parent, child) submap pairs (constraints.cu); voxel = the map voxel after getMapVoxelSize; so_out /
 // to_out: the caller's overlap clouds or nullptr; out: host records.  Synchronises once.
 int32_t op_odometry_constraints(b2s_handle* h, int n, const b2s_submap* const* sources, const b2s_submap* const* targets,

@@ -146,10 +146,6 @@ __global__ void info_finish_kernel(const InfoPair* __restrict__ pairs, const dou
   finish_record(out[blockIdx.x], P, M, min_fitness);
 }
 
-size_t op_overlap_batch_stage_bytes(int n);
-int32_t op_overlap_batch(b2s_handle* h, int n, const b2s_submap* const* maps, const double* inits, double voxel, int min_pts,
-                         b2s_cloud* const* outs, unsigned char* host_stage);
-
 namespace {
 // what one batch of pair constraints runs; the two kinds differ only here
 struct PairJob {
@@ -170,7 +166,6 @@ struct PairJob {
 template <class Rec>
 int32_t op_submap_constraints(b2s_handle* h, int n, const b2s_submap* const* sources, const b2s_submap* const* targets, const PairJob& J,
                               b2s_cloud* const* so_out, b2s_cloud* const* to_out, Rec* out) {
-  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
   // the overlap clouds: the caller's, or the handle's own
   while (h->odo_clouds.size() < (size_t)(2 * n)) {
     std::unique_ptr<b2s_cloud> c;
@@ -185,10 +180,12 @@ int32_t op_submap_constraints(b2s_handle* h, int n, const b2s_submap* const* sou
     outs[2 * k + 1] = to_out ? to_out[k] : h->odo_clouds[2 * k + 1].get();
   }
   // page-locked staging of every table this call uploads (nothing waits for the device before the final read-back)
-  const size_t st_ov = al(op_overlap_batch_stage_bytes(n)), st_icp = al((size_t)n * sizeof(IcpProblem)), st_info = (size_t)n * sizeof(InfoPair);
-  if (h->odo_stage.cap < st_ov + st_icp + st_info) B2S_TRY(h->odo_stage.alloc(2 * (st_ov + st_icp + st_info)));   // the last call synchronised
+  Layout S;
+  const OverlapTables ov = overlap_tables(S, n);
+  const size_t st_icp = S.off((size_t)n * sizeof(IcpProblem)), st_info = S.off((size_t)n * sizeof(InfoPair));
+  if (h->odo_stage.cap < S.size) B2S_TRY(h->odo_stage.alloc(2 * S.size));   // the last call synchronised
   unsigned char* stage = h->odo_stage.as<unsigned char>();
-  B2S_TRY(op_overlap_batch(h, n, maps.data(), J.inits, J.overlap_voxel, J.min_pts, outs.data(), stage));
+  B2S_TRY(op_overlap_batch(h, n, maps.data(), J.inits, J.overlap_voxel, J.min_pts, outs.data(), stage, ov));
 
   // the index of every target overlap, one batched build
   std::vector<GridIndex*> grids((size_t)n);
@@ -211,7 +208,7 @@ int32_t op_submap_constraints(b2s_handle* h, int n, const b2s_submap* const* sou
     B2S_TRY(h->work_xyz.ensure(work_total * 8, h->stream));
     B2S_TRY(h->problems.ensure(sizeof(IcpProblem) * (size_t)n, h->stream));
     B2S_TRY(h->results.ensure(sizeof(b2s_result) * (size_t)n, h->stream));
-    IcpProblem* probs = reinterpret_cast<IcpProblem*>(stage + st_ov);
+    IcpProblem* probs = reinterpret_cast<IcpProblem*>(stage + st_icp);
     const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
     size_t woff = 0;
     for (int k = 0; k < n; k++) {
@@ -224,7 +221,7 @@ int32_t op_submap_constraints(b2s_handle* h, int n, const b2s_submap* const* sou
   }
 
   // the information matrices: K-info-wide over the tiles of every pair, then one CTA per pair
-  InfoPair* ip = reinterpret_cast<InfoPair*>(stage + st_ov + st_icp);
+  InfoPair* ip = reinterpret_cast<InfoPair*>(stage + st_info);
   int tiles = 0;
   for (int k = 0; k < n; k++) {
     const b2s_cloud* s = outs[2 * k];
@@ -236,13 +233,13 @@ int32_t op_submap_constraints(b2s_handle* h, int n, const b2s_submap* const* sou
     P.tile0 = tiles; P.ntiles = (int32_t)(nt > 0 ? nt : 1);
     tiles += P.ntiles;
   }
-  const size_t b_pairs = al((size_t)n * sizeof(InfoPair)), b_part = al((size_t)tiles * WI_MOM * 8);
-  B2S_TRY(h->odo_info.ensure(b_pairs + b_part + (size_t)n * sizeof(Rec), h->stream));
-  unsigned char* dev = h->odo_info.as<unsigned char>();
-  const InfoPair* dpairs = reinterpret_cast<const InfoPair*>(dev);
-  double* partials = reinterpret_cast<double*>(dev + b_pairs);
-  Rec* dout = reinterpret_cast<Rec*>(dev + b_pairs + b_part);
-  B2S_CUDA(cudaMemcpyAsync(dev, ip, (size_t)n * sizeof(InfoPair), cudaMemcpyHostToDevice, h->stream));
+  InfoPair* dpairs = nullptr;
+  double* partials = nullptr;
+  Rec* dout = nullptr;
+  B2S_TRY(carve(h->odo_info, h->stream, [&](Layout& D) {
+    dpairs = D.take<InfoPair>(n); partials = D.take<double>((size_t)tiles * WI_MOM); dout = D.take<Rec>(n);
+  }));
+  B2S_CUDA(cudaMemcpyAsync(dpairs, ip, (size_t)n * sizeof(InfoPair), cudaMemcpyHostToDevice, h->stream));
   {
     ProfScope prof(h, PK_ICP);
     launch_pdl(info_wide_kernel, grid_for((size_t)tiles, 1, 4 * device_sms()), WI_THREADS, 0, h->stream, dpairs, n, tiles, J.radius, partials);

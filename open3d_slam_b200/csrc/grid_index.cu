@@ -307,17 +307,19 @@ int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* co
     if (clouds[i]->n_max > max_pts) max_pts = clouds[i]->n_max;
     if ((size_t)g[i]->cap_cells > max_cells) max_cells = (size_t)g[i]->cap_cells;
   }
-  // device tables: GridJob[n] | ScanJob[n] | scan tile states (zeroed)
-  const size_t st_bytes = (scan_state_bytes(max_cells) + 15) & ~(size_t)15;
-  const size_t off_scan = ((size_t)n * sizeof(GridJob) + 15) & ~(size_t)15;
-  const size_t off_state = (off_scan + (size_t)n * sizeof(ScanJob) + 15) & ~(size_t)15;
-  const size_t total = off_state + st_bytes * (size_t)n;
-  B2S_TRY(h->batch_jobs.ensure(total, h->stream));
-  h->batch_jobs_host.assign(off_state, 0);
-  GridJob* gj = reinterpret_cast<GridJob*>(h->batch_jobs_host.data());
-  ScanJob* sj = reinterpret_cast<ScanJob*>(h->batch_jobs_host.data() + off_scan);
+  // device tables: GridJob[n] | ScanJob[n], uploaded from batch_jobs_host at the same offsets, then the scan tile states (zeroed)
+  Layout T;
+  const size_t o_jobs = T.off((size_t)n * sizeof(GridJob)), o_scan = T.off((size_t)n * sizeof(ScanJob)), staged = T.size;
+  h->batch_jobs_host.assign(staged, 0);
+  GridJob* gj = reinterpret_cast<GridJob*>(h->batch_jobs_host.data() + o_jobs);
+  ScanJob* sj = reinterpret_cast<ScanJob*>(h->batch_jobs_host.data() + o_scan);
+  size_t state_end = 0;
+  B2S_TRY(carve(h->batch_jobs, h->stream, [&](Layout& D) {
+    D.off(staged);
+    for (int i = 0; i < n; i++) scan_bind_state(D, sj[i], max_cells);
+    state_end = D.size;
+  }));
   unsigned char* dev = h->batch_jobs.as<unsigned char>();
-  const size_t ntiles = (scan_state_bytes(max_cells) - 64) / 8;
   for (int i = 0; i < n; i++) {
     int32_t* counts = g[i]->cell_start.as<int32_t>();
     int32_t* starts = counts + g[i]->cap_cells + 4;
@@ -328,13 +330,12 @@ int32_t grid_build_batch(b2s_handle* h, GridIndex* const* g, const b2s_cloud* co
     gj[i].hdr = hdr; gj[i].counts = counts; gj[i].starts = starts; gj[i].rank = g[i]->rank.as<int32_t>();
     gj[i].pts = g[i]->pts.as<double4>();
     gj[i].cap_cells = g[i]->cap_cells;
-    unsigned long long* st = reinterpret_cast<unsigned long long*>(dev + off_state + st_bytes * (size_t)i);
-    sj[i].in = counts; sj[i].out = starts; sj[i].d_n = &hdr->ncell; sj[i].state = st; sj[i].counter = reinterpret_cast<int32_t*>(st + ntiles);
+    sj[i].in = counts; sj[i].out = starts; sj[i].d_n = &hdr->ncell;
   }
-  B2S_CUDA(cudaMemcpyAsync(dev, h->batch_jobs_host.data(), off_state, cudaMemcpyHostToDevice, h->stream));
-  B2S_CUDA(cudaMemsetAsync(dev + off_state, 0, st_bytes * (size_t)n, h->stream));
-  const GridJob* dj = reinterpret_cast<const GridJob*>(dev);
-  const ScanJob* ds = reinterpret_cast<const ScanJob*>(dev + off_scan);
+  B2S_CUDA(cudaMemcpyAsync(dev, h->batch_jobs_host.data(), staged, cudaMemcpyHostToDevice, h->stream));
+  B2S_CUDA(cudaMemsetAsync(dev + staged, 0, state_end - staged, h->stream));
+  const GridJob* dj = reinterpret_cast<const GridJob*>(dev + o_jobs);
+  const ScanJob* ds = reinterpret_cast<const ScanJob*>(dev + o_scan);
   int bx = grid_for(max_pts, GB_THREADS, 2 * device_sms());   // x blocks per job; y = job
   const dim3 gpts((unsigned)bx, (unsigned)n);
   ProfScope prof(h, PK_GRID);

@@ -150,31 +150,31 @@ __global__ void __launch_bounds__(OV_THREADS) ovb_compact_kernel(const OvJob* __
   }
 }
 
+OverlapTables overlap_tables(Layout& stage, int n) {
+  OverlapTables t;
+  t.jobs = stage.off((size_t)2 * n * sizeof(OvJob));
+  t.scan = stage.off((size_t)2 * n * sizeof(ScanJob));
+  t.T = stage.off((size_t)n * 16 * sizeof(double));
+  t.end = stage.size;
+  return t;
+}
+
 // maps[2k], maps[2k + 1]: pair k's source and target; outs[2k], outs[2k + 1]: their overlap clouds (reserved here).  inits: n row-major
 // 4x4 sourceToTarget (host), or nullptr for the identity.  The job tables, the transforms and the per-slot arrays live in h->odo; the
-// tables and transforms are staged through host_stage (page-locked, op_overlap_batch_stage_bytes(n)) so that nothing here waits for
-// the device.
-size_t op_overlap_batch_stage_bytes(int n) {
-  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-  return al((size_t)2 * n * sizeof(OvJob)) + al((size_t)2 * n * sizeof(ScanJob)) + (size_t)n * 16 * sizeof(double);
-}
+// tables and transforms are staged through stage (page-locked, at the offsets tb) so that nothing here waits for the device.
 int32_t op_overlap_batch(b2s_handle* h, int n, const b2s_submap* const* maps, const double* inits, double voxel, int min_pts,
-                         b2s_cloud* const* outs, unsigned char* host_stage) {
+                         b2s_cloud* const* outs, unsigned char* stage, const OverlapTables& tb) {
   const int nj = 2 * n;
-  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-  const size_t tables = al((size_t)nj * sizeof(OvJob)) + al((size_t)nj * sizeof(ScanJob));
-  size_t max_n = 1, bytes = al(op_overlap_batch_stage_bytes(n));
+  auto slots_of = [&](int j) { const size_t m = maps[j]->cloud[0]->n_max; return m > 0 ? m : 1; };
+  size_t max_n = 1;
   std::vector<size_t> caps((size_t)n);
   for (int k = 0; k < n; k++) {
-    const size_t ns = maps[2 * k]->cloud[0]->n_max > 0 ? maps[2 * k]->cloud[0]->n_max : 1;
-    const size_t nt = maps[2 * k + 1]->cloud[0]->n_max > 0 ? maps[2 * k + 1]->cloud[0]->n_max : 1;
+    const size_t ns = slots_of(2 * k), nt = slots_of(2 * k + 1);
     size_t cap = 1024;
     while (cap < 2 * (ns + nt)) cap <<= 1;
     caps[(size_t)k] = cap;
-    bytes += al(cap * 8) + al(cap * 8);
-    for (size_t m : {ns, nt}) { bytes += 3 * al((m + 2) * 4) + al(scan_state_bytes(m)); if (m > max_n) max_n = m; }
+    for (size_t m : {ns, nt}) if (m > max_n) max_n = m;
   }
-  B2S_TRY(h->odo.ensure(bytes, h->stream));
   for (int j = 0; j < nj; j++) {
     const b2s_cloud* map = maps[j]->cloud[0].get();
     B2S_TRY(cloud_reserve(h, outs[j], map->n_max, true));
@@ -182,44 +182,44 @@ int32_t op_overlap_batch(b2s_handle* h, int n, const b2s_submap* const* maps, co
     outs[j]->n_max = map->n_max;
     outs[j]->n_known = -1;
   }
-  unsigned char* dev = h->odo.as<unsigned char>();
-  OvJob* oj = reinterpret_cast<OvJob*>(host_stage);
-  ScanJob* sj = reinterpret_cast<ScanJob*>(host_stage + al((size_t)nj * sizeof(OvJob)));
-  if (inits) memcpy(host_stage + tables, inits, (size_t)n * 16 * sizeof(double));
-  const double* dT = reinterpret_cast<const double*>(dev + tables);
-  size_t off = al(op_overlap_batch_stage_bytes(n));
-  const size_t state_begin = off;
-  for (int j = 0; j < nj; j++) {   // tile states first: they are the region zeroed below
-    const size_t m = maps[j]->cloud[0]->n_max > 0 ? maps[j]->cloud[0]->n_max : 1;
-    unsigned long long* st = reinterpret_cast<unsigned long long*>(dev + off);
-    sj[j].state = st;
-    sj[j].counter = reinterpret_cast<int32_t*>(st + (scan_state_bytes(m) - 64) / 8);
-    off += al(scan_state_bytes(m));
-  }
-  const size_t state_end = off;
-  for (int k = 0; k < n; k++) {
-    unsigned long long* keys = reinterpret_cast<unsigned long long*>(dev + off); off += al(caps[(size_t)k] * 8);
-    int32_t* cnt = reinterpret_cast<int32_t*>(dev + off); off += al(caps[(size_t)k] * 8);
-    for (int w = 0; w < 2; w++) {
-      const int j = 2 * k + w;
-      const b2s_cloud* map = maps[j]->cloud[0].get();
-      const size_t m = map->n_max > 0 ? map->n_max : 1;
-      OvJob& J = oj[j];
-      J.xyz = map->xyz.as<double>(); J.nrm = map->nrm.as<double>(); J.d_n = map->dn.as<int32_t>();
-      J.keys = keys; J.cnt = cnt; J.mask = caps[(size_t)k] - 1;
-      J.slot_of = reinterpret_cast<int32_t*>(dev + off); off += al((m + 2) * 4);
-      J.keep = reinterpret_cast<int32_t*>(dev + off); off += al((m + 2) * 4);
-      J.offs = reinterpret_cast<int32_t*>(dev + off); off += al((m + 2) * 4);
-      J.oxyz = outs[j]->xyz.as<double>(); J.onrm = outs[j]->nrm.as<double>(); J.out_n = outs[j]->dn.as<int32_t>();
-      J.T = (inits && w == 0) ? dT + 16 * (size_t)k : nullptr;
-      J.which = w; J.pad = 0;
-      sj[j].in = J.keep; sj[j].out = J.offs; sj[j].d_n = J.d_n;
+  OvJob* oj = reinterpret_cast<OvJob*>(stage + tb.jobs);
+  ScanJob* sj = reinterpret_cast<ScanJob*>(stage + tb.scan);
+  if (inits) memcpy(stage + tb.T, inits, (size_t)n * 16 * sizeof(double));
+  // h->odo: the tables at their stage offsets, then every job's tile state (the region zeroed below), then per pair its hash segment
+  // and per job its slot, flag and offset arrays
+  size_t state_begin = 0, state_end = 0;
+  B2S_TRY(carve(h->odo, h->stream, [&](Layout& D) {
+    D.off(tb.end);
+    state_begin = D.size;
+    for (int j = 0; j < nj; j++) scan_bind_state(D, sj[j], slots_of(j));
+    state_end = D.size;
+    for (int k = 0; k < n; k++) {
+      unsigned long long* keys = D.take<unsigned long long>(caps[(size_t)k]);
+      int32_t* cnt = D.take<int32_t>(2 * caps[(size_t)k]);
+      for (int j = 2 * k; j < 2 * k + 2; j++) {
+        oj[j].keys = keys; oj[j].cnt = cnt;
+        oj[j].slot_of = D.take<int32_t>(slots_of(j) + 2);
+        oj[j].keep = D.take<int32_t>(slots_of(j) + 2);
+        oj[j].offs = D.take<int32_t>(slots_of(j) + 2);
+      }
     }
+  }));
+  unsigned char* dev = h->odo.as<unsigned char>();
+  for (int j = 0; j < nj; j++) {
+    const b2s_cloud* map = maps[j]->cloud[0].get();
+    const int k = j / 2, w = j % 2;
+    OvJob& J = oj[j];
+    J.xyz = map->xyz.as<double>(); J.nrm = map->nrm.as<double>(); J.d_n = map->dn.as<int32_t>();
+    J.mask = caps[(size_t)k] - 1;
+    J.oxyz = outs[j]->xyz.as<double>(); J.onrm = outs[j]->nrm.as<double>(); J.out_n = outs[j]->dn.as<int32_t>();
+    J.T = (inits && w == 0) ? reinterpret_cast<const double*>(dev + tb.T) + 16 * (size_t)k : nullptr;
+    J.which = w; J.pad = 0;
+    sj[j].in = J.keep; sj[j].out = J.offs; sj[j].d_n = J.d_n;
   }
-  B2S_CUDA(cudaMemcpyAsync(dev, host_stage, inits ? op_overlap_batch_stage_bytes(n) : tables, cudaMemcpyHostToDevice, h->stream));
+  B2S_CUDA(cudaMemcpyAsync(dev + tb.jobs, stage + tb.jobs, (inits ? tb.end : tb.T) - tb.jobs, cudaMemcpyHostToDevice, h->stream));
   B2S_CUDA(cudaMemsetAsync(dev + state_begin, 0, state_end - state_begin, h->stream));
-  const OvJob* dj = reinterpret_cast<const OvJob*>(dev);
-  const ScanJob* ds = reinterpret_cast<const ScanJob*>(dev + al((size_t)nj * sizeof(OvJob)));
+  const OvJob* dj = reinterpret_cast<const OvJob*>(dev + tb.jobs);
+  const ScanJob* ds = reinterpret_cast<const ScanJob*>(dev + tb.scan);
   size_t max_cap = 1;
   for (size_t c : caps) if (c > max_cap) max_cap = c;
   const int bx = grid_for(max_n, OV_THREADS, 2 * device_sms());   // x blocks per job (grid-stride); y = job

@@ -460,8 +460,6 @@ struct PgLayout {   // pointers into the handle's pose-graph buffers
   int32_t* contrib;
 };
 
-size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 // BFS from node 0 (ValidatePoseGraphConnectivity); certain_only: uncertain edges are ignored
 bool pg_connected(int N, const std::vector<b2s_pose_graph_edge>& E, bool certain_only) {
   std::vector<std::vector<int>> adj((size_t)N);
@@ -490,10 +488,11 @@ int32_t pg_prepare(b2s_handle* h, int N, int ne, int ntasks, int ncontrib, PgLay
   B2S_TRY(h->pg_vec.ensure((5 * (size_t)L->M + PG_R_WORDS + 8) * 8, h->stream));
   B2S_TRY(h->pg_nodes.ensure(2 * 16 * 8 * (size_t)N, h->stream));
   const size_t ec = (size_t)L->ecap;
-  const size_t o_conf = al256(ec * sizeof(b2s_pose_graph_edge)), o_hss = o_conf + al256(ec * 8), o_gv = o_hss + al256(ec * 36 * 8),
-               o_term = o_gv + al256(ec * 6 * 8), o_ne = o_term + al256(ec * 8), o_tasks = o_ne + 256,
-               o_contrib = o_tasks + al256((size_t)ntasks * sizeof(PgTask)), total = o_contrib + al256((size_t)ncontrib * 4 + 4);
-  B2S_TRY(h->pg_edges.ensure(total, h->stream));
+  B2S_TRY(carve(h->pg_edges, h->stream, [&](Layout& E) {
+    L->E = E.take<b2s_pose_graph_edge>(ec);
+    L->conf = E.take<double>(ec); L->hss = E.take<double>(ec * 36); L->gv = E.take<double>(ec * 6); L->term = E.take<double>(ec);
+    L->ne = E.take<int32_t>(1); L->tasks = E.take<PgTask>(ntasks); L->contrib = E.take<int32_t>((size_t)ncontrib + 1);
+  }));
   // K-pg-panel holds two 64 x 65 tiles, above the default 48 KB of shared memory; the attribute is per device, set on every pass
   // (a host call, cheap next to a pass) rather than cached behind an unsynchronised flag
   B2S_CUDA(cudaFuncSetAttribute(pg_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PG_PANEL_SMEM));
@@ -502,11 +501,6 @@ int32_t pg_prepare(b2s_handle* h, int N, int ne, int ntasks, int ncontrib, PgLay
   L->b = v; L->rhs = v + L->M; L->z = v + 2 * L->M; L->delta = v + 3 * L->M; L->D = v + 4 * L->M; L->rec = v + 5 * L->M;
   L->scal = L->rec + PG_R_WORDS;
   L->P = h->pg_nodes.as<double>(); L->Pt = L->P + 16 * (size_t)N;
-  unsigned char* eb = h->pg_edges.as<unsigned char>();
-  L->E = reinterpret_cast<b2s_pose_graph_edge*>(eb);
-  L->conf = reinterpret_cast<double*>(eb + o_conf); L->hss = reinterpret_cast<double*>(eb + o_hss); L->gv = reinterpret_cast<double*>(eb + o_gv);
-  L->term = reinterpret_cast<double*>(eb + o_term); L->ne = reinterpret_cast<int32_t*>(eb + o_ne);
-  L->tasks = reinterpret_cast<PgTask*>(eb + o_tasks); L->contrib = reinterpret_cast<int32_t*>(eb + o_contrib);
   return B2S_OK;
 }
 

@@ -353,13 +353,18 @@ static int ransac_batch() {   // B2S_RANSAC_BATCH: hypotheses per batch (tuning 
   return v > 0 ? v : 1024;
 }
 
-static inline size_t al(size_t b) { return (b + 255) & ~(size_t)255; }
+// Carves the per-pair partial arrays of the feature matching from L into jobs
+static void fm_carve(Layout& L, const b2s_feature* src, int n, const b2s_feature* const* tgts, MatchJob* jobs) {
+  const size_t n_stiles = (src->n + FM_TILE - 1) / FM_TILE;
+  for (int k = 0; k < n; ++k) {
+    jobs[k].part_d = L.take<double>(n_stiles * tgts[k]->n);
+    jobs[k].part_i = L.take<int32_t>(n_stiles * tgts[k]->n);
+  }
+}
 
-// Carves the per-pair device arrays of the feature matching out of h->lc and launches it; `layout` receives the offsets
-struct FmLayout { size_t part, s2t, t2s, per_pair; };
-
+// Uploads the feature matching's jobs (their partial arrays carved by fm_carve) to jobs_dev and launches it
 static int32_t feature_match(b2s_handle* h, const b2s_feature* src, int n, const b2s_feature* const* tgts, int32_t* const* s2t, int32_t* const* t2s,
-                             unsigned char* base, MatchJob* jobs_dev, std::vector<MatchJob>& jobs) {
+                             MatchJob* jobs_dev, std::vector<MatchJob>& jobs) {
   const int ns = (int)src->n;
   const int n_stiles = (ns + FM_TILE - 1) / FM_TILE;
   int max_nt = 1;
@@ -368,10 +373,6 @@ static int32_t feature_match(b2s_handle* h, const b2s_feature* src, int n, const
     max_nt = std::max(max_nt, nt);
     jobs[k].tgt = tgts[k]->data.as<double>(); jobs[k].nt = nt;
     jobs[k].s2t = s2t[k]; jobs[k].t2s = t2s[k];
-    jobs[k].part_d = reinterpret_cast<double*>(base);
-    base += al((size_t)n_stiles * nt * 8);
-    jobs[k].part_i = reinterpret_cast<int32_t*>(base);
-    base += al((size_t)n_stiles * nt * 4);
   }
   B2S_CUDA(cudaMemcpyAsync(jobs_dev, jobs.data(), sizeof(MatchJob) * n, cudaMemcpyHostToDevice, h->stream));
   if (ns > 0) launch_pdl(fm_tile_kernel, dim3(n_stiles, n), FM_THREADS, 0, h->stream, src->data.as<double>(), ns, (const MatchJob*)jobs_dev);
@@ -382,17 +383,16 @@ static int32_t feature_match(b2s_handle* h, const b2s_feature* src, int n, const
   return B2S_OK;
 }
 
-static size_t fm_bytes(size_t ns, size_t nt) { const size_t st = (ns + FM_TILE - 1) / FM_TILE; return al(st * nt * 8) + al(st * nt * 4); }
-
 int32_t op_feature_correspondences(b2s_handle* h, const b2s_feature* src, int n, const b2s_feature* const* tgts, int32_t* const* s2t,
                                    int32_t* const* t2s) {
   if (n <= 0) return B2S_OK;
-  size_t bytes = al(sizeof(MatchJob) * n);
-  for (int k = 0; k < n; ++k) bytes += fm_bytes(src->n, tgts[k]->n);
-  B2S_TRY(h->lc.ensure(bytes, h->stream));
   std::vector<MatchJob> jobs(n);
-  unsigned char* base = h->lc.as<unsigned char>();
-  return feature_match(h, src, n, tgts, s2t, t2s, base + al(sizeof(MatchJob) * n), reinterpret_cast<MatchJob*>(base), jobs);
+  MatchJob* jobs_dev = nullptr;
+  B2S_TRY(carve(h->lc, h->stream, [&](Layout& L) {
+    jobs_dev = L.take<MatchJob>(n);
+    fm_carve(L, src, n, tgts, jobs.data());
+  }));
+  return feature_match(h, src, n, tgts, s2t, t2s, jobs_dev, jobs);
 }
 
 int32_t op_ransac(b2s_handle* h, const b2s_cloud* src, size_t ns_, const b2s_feature* src_f, int n, const b2s_cloud* const* tgts, const size_t* nts,
@@ -412,46 +412,42 @@ int32_t op_ransac(b2s_handle* h, const b2s_cloud* src, size_t ns_, const b2s_fea
   std::vector<const b2s_feature*> lf(m);
   std::vector<const b2s_cloud*> lc(m);
   for (int q = 0; q < m; ++q) { lf[q] = tgt_fs[live[q]]; lc[q] = tgts[live[q]]; }
-  // scratch, carved twice (first to size it): MatchJob[m] | RansacJob[m] | ScanJob[2m] | RansacPair[m] | {ns, B} | scan states (mutual
-  // scan, survivor scan) | per pair: s2t, t2s, mutual flags / offsets, the set, survivor flags / offsets, survivors, hypothesis T
-  const size_t tb_ns = (scan_state_bytes((size_t)ns) - 64) / 8, tb_b = (scan_state_bytes((size_t)B) - 64) / 8;
-  const size_t st_ns = al(scan_state_bytes((size_t)ns)), st_b = al(scan_state_bytes((size_t)B));
+  // scratch: MatchJob[m] | RansacJob[m] | ScanJob[2m] | RansacPair[m] | {ns, B} | scan states (every mutual scan's, then every survivor
+  // scan's) | per pair: s2t, t2s, mutual flags / offsets, the set, survivor flags / offsets, survivors, hypothesis T | feature matching
   std::vector<RansacJob> rj(m);
+  std::vector<ScanJob> sj(2 * m);
+  std::vector<MatchJob> mj(m);
   std::vector<int32_t*> s2t(m), t2s(m);
   MatchJob* mj_dev = nullptr; RansacJob* rj_dev = nullptr; ScanJob* sj_dev = nullptr; RansacPair* st_dev = nullptr;
-  int32_t* d_consts = nullptr; unsigned char* states = nullptr; unsigned char* fm_base = nullptr;
-  unsigned char* base = nullptr;
-  size_t off = 0;
-  auto take = [&](size_t b) { unsigned char* r = base + off; off += al(b); return r; };
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass == 1) {
-      size_t bytes = off;
-      for (int q = 0; q < m; ++q) bytes += fm_bytes((size_t)ns, nts[live[q]]);
-      B2S_TRY(h->lc.ensure(bytes, h->stream));
-      base = h->lc.as<unsigned char>();
-      off = 0;
-    }
-    mj_dev = reinterpret_cast<MatchJob*>(take(sizeof(MatchJob) * m));
-    rj_dev = reinterpret_cast<RansacJob*>(take(sizeof(RansacJob) * m));
-    sj_dev = reinterpret_cast<ScanJob*>(take(sizeof(ScanJob) * 2 * m));
-    st_dev = reinterpret_cast<RansacPair*>(take(sizeof(RansacPair) * m));
-    d_consts = reinterpret_cast<int32_t*>(take(8));
-    states = take((st_ns + st_b) * m);
+  int32_t* d_consts = nullptr;
+  size_t states = 0, surv_states = 0, states_end = 0;
+  B2S_TRY(carve(h->lc, h->stream, [&](Layout& L) {
+    mj_dev = L.take<MatchJob>(m);
+    rj_dev = L.take<RansacJob>(m);
+    sj_dev = L.take<ScanJob>(2 * m);
+    st_dev = L.take<RansacPair>(m);
+    d_consts = L.take<int32_t>(2);
+    states = L.size;
+    for (int q = 0; q < m; ++q) scan_bind_state(L, sj[q], (size_t)ns);
+    surv_states = L.size;
+    for (int q = 0; q < m; ++q) scan_bind_state(L, sj[m + q], (size_t)B);
+    states_end = L.size;
     for (int q = 0; q < m; ++q) {
       RansacJob& J = rj[q];
       J.txyz = lc[q]->xyz.as<double>(); J.nt = (int)nts[live[q]];
-      s2t[q] = reinterpret_cast<int32_t*>(take((size_t)ns * 4)); J.s2t = s2t[q];
-      t2s[q] = reinterpret_cast<int32_t*>(take((size_t)J.nt * 4)); J.t2s = t2s[q];
-      J.mflag = reinterpret_cast<int32_t*>(take((size_t)ns * 4)); J.moff = reinterpret_cast<int32_t*>(take((size_t)(ns + 1) * 4));
-      J.set_s = reinterpret_cast<int32_t*>(take((size_t)ns * 4)); J.set_t = reinterpret_cast<int32_t*>(take((size_t)ns * 4));
-      J.hflag = reinterpret_cast<int32_t*>(take((size_t)B * 4)); J.hoff = reinterpret_cast<int32_t*>(take((size_t)(B + 1) * 4));
-      J.surv_h = reinterpret_cast<long long*>(take((size_t)B * 8));
-      J.hyp_T = reinterpret_cast<double*>(take((size_t)B * 128)); J.surv_T = reinterpret_cast<double*>(take((size_t)B * 128));
-      J.surv_inl = reinterpret_cast<int32_t*>(take((size_t)B * 4)); J.surv_sum = reinterpret_cast<double*>(take((size_t)B * 8));
+      s2t[q] = L.take<int32_t>(ns); J.s2t = s2t[q];
+      t2s[q] = L.take<int32_t>(J.nt); J.t2s = t2s[q];
+      J.mflag = L.take<int32_t>(ns); J.moff = L.take<int32_t>(ns + 1);
+      J.set_s = L.take<int32_t>(ns); J.set_t = L.take<int32_t>(ns);
+      J.hflag = L.take<int32_t>(B); J.hoff = L.take<int32_t>(B + 1);
+      J.surv_h = L.take<long long>(B);
+      J.hyp_T = L.take<double>((size_t)B * 16); J.surv_T = L.take<double>((size_t)B * 16);
+      J.surv_inl = L.take<int32_t>(B); J.surv_sum = L.take<double>(B);
       J.st = st_dev + q;
     }
-    fm_base = base + off;
-  }
+    fm_carve(L, src_f, m, lf.data(), mj.data());
+  }));
+  unsigned char* base = h->lc.as<unsigned char>();
   // target grids, built once per call (cell = the validation radius: a 3 x 3 x 3 box of cells holds every candidate)
   while (h->batch_grids.size() < (size_t)m) h->batch_grids.emplace_back(new GridIndex());
   std::vector<GridIndex*> grids(m);
@@ -460,22 +456,18 @@ int32_t op_ransac(b2s_handle* h, const b2s_cloud* src, size_t ns_, const b2s_fea
   for (int q = 0; q < m; ++q) {
     rj[q].ghdr = grids[q]->hdr.as<GridHeader>(); rj[q].gcs = grid_starts(grids[q]); rj[q].gpts = grids[q]->pts.as<double4>();
   }
-  std::vector<MatchJob> mj(m);
-  B2S_TRY(feature_match(h, src_f, m, lf.data(), s2t.data(), t2s.data(), fm_base, mj_dev, mj));
+  B2S_TRY(feature_match(h, src_f, m, lf.data(), s2t.data(), t2s.data(), mj_dev, mj));
   // device tables and the initial state
-  std::vector<ScanJob> sj(2 * m);
   std::vector<RansacPair> st(m);
   for (int q = 0; q < m; ++q) {
-    unsigned long long* a = reinterpret_cast<unsigned long long*>(states + (st_ns + st_b) * q);
-    unsigned long long* b = reinterpret_cast<unsigned long long*>(states + (st_ns + st_b) * q + st_ns);
-    sj[q] = {rj[q].mflag, rj[q].moff, d_consts, a, reinterpret_cast<int32_t*>(a + tb_ns)};
-    sj[m + q] = {rj[q].hflag, rj[q].hoff, d_consts + 1, b, reinterpret_cast<int32_t*>(b + tb_b)};
+    sj[q].in = rj[q].mflag; sj[q].out = rj[q].moff; sj[q].d_n = d_consts;
+    sj[m + q].in = rj[q].hflag; sj[m + q].out = rj[q].hoff; sj[m + q].d_n = d_consts + 1;
     memset(&st[q], 0, sizeof(st[q]));
     memcpy(st[q].best_T, I, sizeof(I));
     st[q].est_k = p.max_iteration; st[q].best_h = -1; st[q].last_update = -1;
     st[q].done = p.max_iteration == 0;
   }
-  B2S_CUDA(cudaMemsetAsync(states, 0, (st_ns + st_b) * m, h->stream));
+  B2S_CUDA(cudaMemsetAsync(base + states, 0, states_end - states, h->stream));
   const int32_t consts[2] = {ns, B};
   B2S_CUDA(cudaMemcpyAsync(d_consts, consts, 8, cudaMemcpyHostToDevice, h->stream));
   B2S_CUDA(cudaMemcpyAsync(rj_dev, rj.data(), sizeof(RansacJob) * m, cudaMemcpyHostToDevice, h->stream));
@@ -496,7 +488,7 @@ int32_t op_ransac(b2s_handle* h, const b2s_cloud* src, size_t ns_, const b2s_fea
     for (int q = 0; q < m; ++q) all_done = all_done && st[q].done;
     if (all_done) break;
     // the scan states of the survivor scan are single-use: zero them for this batch
-    for (int q = 0; q < m; ++q) B2S_CUDA(cudaMemsetAsync(states + (st_ns + st_b) * q + st_ns, 0, st_b, h->stream));
+    B2S_CUDA(cudaMemsetAsync(base + surv_states, 0, states_end - surv_states, h->stream));
     launch_pdl(rs_hyp_kernel, dim3((B + RS_THREADS - 1) / RS_THREADS, m), RS_THREADS, 0, h->stream, c, h0, (const RansacJob*)rj_dev);
     h->launches++;
     B2S_TRY(scan_exclusive_i32_batch(h, sj_dev + m, m, (size_t)B));

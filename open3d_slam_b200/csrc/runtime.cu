@@ -256,17 +256,23 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_lookback_batch_kernel(const
   scan_lookback_body(j.in, j.out, j.d_n, 0, j.state, j.counter, nullptr);
 }
 
-size_t scan_state_bytes(size_t n_max) {
-  size_t ntiles = (n_max + SCAN_TILE - 1) / SCAN_TILE;
-  if (ntiles < 1) ntiles = 1;
-  return ntiles * 8 + 64;
+// A scan's tile state: one uint64 per tile, then the tile counter in the 64 bytes after them.
+static int scan_tiles(size_t n_max) {
+  const size_t ntiles = (n_max + SCAN_TILE - 1) / SCAN_TILE;
+  return ntiles < 1 ? 1 : (int)ntiles;
+}
+static size_t scan_state_bytes(size_t n_max) { return (size_t)scan_tiles(n_max) * 8 + 64; }
+static int32_t* scan_counter(unsigned long long* state, size_t n_max) { return reinterpret_cast<int32_t*>(state + scan_tiles(n_max)); }
+
+void scan_bind_state(Layout& L, ScanJob& j, size_t n_max) {
+  unsigned char* s = L.take<unsigned char>(scan_state_bytes(n_max));
+  if (!s) return;
+  j.state = reinterpret_cast<unsigned long long*>(s);
+  j.counter = scan_counter(j.state, n_max);
 }
 
-// jobs_dev[k].state / .counter must point into zeroed memory of scan_state_bytes(n_max) each (counter = state + ntiles)
 int32_t scan_exclusive_i32_batch(b2s_handle* h, const ScanJob* jobs_dev, int njobs, size_t n_max) {
-  int ntiles = (int)((n_max + SCAN_TILE - 1) / SCAN_TILE);
-  if (ntiles < 1) ntiles = 1;
-  launch_pdl(scan_lookback_batch_kernel, dim3(ntiles, njobs), SCAN_THREADS, 0, h->stream, jobs_dev);
+  launch_pdl(scan_lookback_batch_kernel, dim3(scan_tiles(n_max), njobs), SCAN_THREADS, 0, h->stream, jobs_dev);
   h->launches++;
   B2S_CUDA(cudaGetLastError());
   return B2S_OK;
@@ -274,13 +280,12 @@ int32_t scan_exclusive_i32_batch(b2s_handle* h, const ScanJob* jobs_dev, int njo
 
 static int32_t scan_impl(b2s_handle* h, const int32_t* in, int32_t* out, const int32_t* d_n, int32_t n_host, size_t n_max,
                          int32_t* d_total, DevBuf* state) {
-  int ntiles = (int)((n_max + SCAN_TILE - 1) / SCAN_TILE);
-  if (ntiles < 1) ntiles = 1;
+  const int ntiles = scan_tiles(n_max);
   DevBuf& sb = state ? *state : h->scan.state;
-  B2S_TRY(sb.ensure((size_t)ntiles * 8 + 64, h->stream));
-  B2S_CUDA(cudaMemsetAsync(sb.p, 0, (size_t)ntiles * 8 + 64, h->stream));
+  B2S_TRY(sb.ensure(scan_state_bytes(n_max), h->stream));
+  B2S_CUDA(cudaMemsetAsync(sb.p, 0, scan_state_bytes(n_max), h->stream));
   unsigned long long* st = sb.as<unsigned long long>();
-  int32_t* counter = reinterpret_cast<int32_t*>(st + ntiles);
+  int32_t* counter = scan_counter(st, n_max);
   launch_pdl(scan_lookback_kernel, ntiles, SCAN_THREADS, 0, h->stream, in, out, d_n, n_host, st, counter, d_total);
   h->launches++;
   B2S_CUDA(cudaGetLastError());

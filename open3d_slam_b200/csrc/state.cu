@@ -192,55 +192,51 @@ static unsigned long long dbits(double v) { unsigned long long u; memcpy(&u, &v,
 
 int32_t op_export_submap_states(b2s_handle* h, int n, const b2s_submap* const* submaps, void* host, size_t capacity, size_t* offsets) {
   if (n == 0) { if (offsets) offsets[0] = 0; return B2S_OK; }
-  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
   AssemblyScratch& A = h->assembly;
+  auto tiles_of = [](size_t cap) { return (cap + DX_TILE - 1) / DX_TILE; };
   int m = 0;   // tables
-  size_t max_tiles = 1, slot_bytes = 0, max_words = 1;
+  size_t max_tiles = 1, max_words = 1;
   for (int k = 0; k < n; k++) {
     const b2s_submap* sm = submaps[k];
     for (const size_t cap : {sm->vcap, sm->dense_cap}) {
       if (cap == 0) continue;
-      const size_t nt = (cap + DX_TILE - 1) / DX_TILE;
-      if (nt > max_tiles) max_tiles = nt;
-      slot_bytes += al(scan_state_bytes(nt)) + al(nt * 4) + al((nt + 2) * 4);
+      if (tiles_of(cap) > max_tiles) max_tiles = tiles_of(cap);
       m++;
     }
     const size_t w = 3 * (sm->cloud[0]->n_max > sm->capacity ? sm->capacity : sm->cloud[0]->n_max);
     if (w > max_words) max_words = w;
   }
   // tables: [StateJob x n][KeyTable x m][ScanJob x m][zero word] staged from the host; then [base x (n + 1)][c x 6n][words] on the device
-  const size_t t_jobs = al((size_t)n * sizeof(StateJob)), t_tabs = al((size_t)m * sizeof(KeyTable)), t_scan = al((size_t)m * sizeof(ScanJob));
-  const size_t staged = t_jobs + t_tabs + t_scan + 256, t_base = al(((size_t)n + 1) * 8), t_c = al((size_t)n * 48);
-  B2S_TRY(A.tables.ensure(staged + t_base + t_c + 256, h->stream));
-  B2S_TRY(A.slots.ensure(slot_bytes > 0 ? slot_bytes : 256, h->stream));
-  if (A.stage.cap < staged + t_base) B2S_TRY(A.stage.alloc(2 * (staged + t_base)));   // every earlier call synchronised after its upload
+  Layout L;
+  const size_t t_jobs = L.off((size_t)n * sizeof(StateJob)), t_tabs = L.off((size_t)m * sizeof(KeyTable));
+  const size_t t_scan = L.off((size_t)m * sizeof(ScanJob)), t_zero = L.off(4), staged = L.size;
+  const size_t t_base = L.off(((size_t)n + 1) * 8), t_c = L.off((size_t)n * 48), t_words = L.off(8);
+  B2S_TRY(A.tables.ensure(L.size, h->stream));
+  if (A.stage.cap < t_c) B2S_TRY(A.stage.alloc(2 * t_c));   // it also receives the bases; every earlier call synchronised after its upload
   unsigned char* st = A.stage.as<unsigned char>();
   unsigned char* tab = A.tables.as<unsigned char>();
-  StateJob* hj = reinterpret_cast<StateJob*>(st);
-  KeyTable* ht = reinterpret_cast<KeyTable*>(st + t_jobs);
-  ScanJob* hs = reinterpret_cast<ScanJob*>(st + t_jobs + t_tabs);
-  memset(st + t_jobs + t_tabs + t_scan, 0, 256);
-  const int32_t* zero = reinterpret_cast<const int32_t*>(tab + t_jobs + t_tabs + t_scan);
-  long long* base = reinterpret_cast<long long*>(tab + staged);
-  long long* cdev = reinterpret_cast<long long*>(tab + staged + t_base);
-  int32_t* words = reinterpret_cast<int32_t*>(tab + staged + t_base + t_c);
-  unsigned char* slots = A.slots.as<unsigned char>();
-  size_t off = 0;
-  // tile states of every table first (the region zeroed below), then the tables' tile counts and offsets
-  {
+  StateJob* hj = reinterpret_cast<StateJob*>(st + t_jobs);
+  KeyTable* ht = reinterpret_cast<KeyTable*>(st + t_tabs);
+  ScanJob* hs = reinterpret_cast<ScanJob*>(st + t_scan);
+  memset(st + t_zero, 0, 4);
+  const int32_t* zero = reinterpret_cast<const int32_t*>(tab + t_zero);
+  long long* base = reinterpret_cast<long long*>(tab + t_base);
+  long long* cdev = reinterpret_cast<long long*>(tab + t_c);
+  int32_t* words = reinterpret_cast<int32_t*>(tab + t_words);
+  // slots: the tile states of every table (the region zeroed below), then the tables' tile counts and offsets
+  memset(ht, 0, (size_t)m * sizeof(KeyTable));
+  size_t state_bytes = 0;
+  B2S_TRY(carve(A.slots, h->stream, [&](Layout& S) {
     int t = 0;
     for (int k = 0; k < n; k++)
-      for (const size_t cap : {submaps[k]->vcap, submaps[k]->dense_cap}) {
-        if (cap == 0) continue;
-        const size_t nt = (cap + DX_TILE - 1) / DX_TILE;
-        unsigned long long* s = reinterpret_cast<unsigned long long*>(slots + off);
-        hs[t].state = s;
-        hs[t].counter = reinterpret_cast<int32_t*>(s + (scan_state_bytes(nt) - 64) / 8);
-        off += al(scan_state_bytes(nt));
-        t++;
-      }
-  }
-  const size_t state_bytes = off;
+      for (const size_t cap : {submaps[k]->vcap, submaps[k]->dense_cap})
+        if (cap) scan_bind_state(S, hs[t++], tiles_of(cap));
+    state_bytes = S.size;
+    t = 0;
+    for (int k = 0; k < n; k++)
+      for (const size_t cap : {submaps[k]->vcap, submaps[k]->dense_cap})
+        if (cap) { ht[t].tiles = S.take<int32_t>(tiles_of(cap)); ht[t].toffs = S.take<int32_t>(tiles_of(cap) + 2); t++; }
+  }));
   const double mv = h->cfg.map_voxel_size;
   for (int k = 0, t = 0; k < n; k++) {
     const b2s_submap* sm = submaps[k];
@@ -266,26 +262,23 @@ int32_t op_export_submap_states(b2s_handle* h, int n, const b2s_submap* const* s
     for (int d = 0; d < 2; d++) {
       const size_t cap = d ? sm->dense_cap : sm->vcap;
       if (cap == 0) continue;
-      const size_t nt = (cap + DX_TILE - 1) / DX_TILE;
+      const size_t nt = tiles_of(cap);
       KeyTable& T = ht[t];
-      memset(&T, 0, sizeof(T));
       T.keys = (d ? sm->dense_keys : sm->vkeys).as<unsigned long long>();
       T.head = sm->vhead.as<int32_t>(); T.stamp = sm->vstamp.as<int32_t>();
       T.sum = sm->dense_sum.as<double>(); T.cnt = sm->dense_cnt.as<int32_t>();
-      T.tiles = reinterpret_cast<int32_t*>(slots + off); off += al(nt * 4);
-      T.toffs = reinterpret_cast<int32_t*>(slots + off); off += al((nt + 2) * 4);
       T.cap = (long long)cap; T.ntiles = (int32_t)nt; T.job = k; T.dense = d;
       hs[t].in = T.tiles; hs[t].out = T.toffs;
-      hs[t].d_n = reinterpret_cast<const int32_t*>(tab + t_jobs + (size_t)t * sizeof(KeyTable) + offsetof(KeyTable, ntiles));
+      hs[t].d_n = reinterpret_cast<const int32_t*>(tab + t_tabs + (size_t)t * sizeof(KeyTable) + offsetof(KeyTable, ntiles));
       (d ? J.dlive : J.vlive) = T.toffs + nt;
       t++;
     }
   }
   B2S_CUDA(cudaMemcpyAsync(tab, st, staged, cudaMemcpyHostToDevice, h->stream));
-  if (state_bytes) B2S_CUDA(cudaMemsetAsync(slots, 0, state_bytes, h->stream));
-  const StateJob* dj = reinterpret_cast<const StateJob*>(tab);
-  const KeyTable* dt = reinterpret_cast<const KeyTable*>(tab + t_jobs);
-  const ScanJob* ds = reinterpret_cast<const ScanJob*>(tab + t_jobs + t_tabs);
+  if (state_bytes) B2S_CUDA(cudaMemsetAsync(A.slots.p, 0, state_bytes, h->stream));
+  const StateJob* dj = reinterpret_cast<const StateJob*>(tab + t_jobs);
+  const KeyTable* dt = reinterpret_cast<const KeyTable*>(tab + t_tabs);
+  const ScanJob* ds = reinterpret_cast<const ScanJob*>(tab + t_scan);
   if (m > 0) {
     launch_pdl(tile_count_kernel<KeyTable>, dim3((unsigned)max_tiles, (unsigned)m), AS_THREADS, 0, h->stream, dt);
     h->launches++;
@@ -297,7 +290,7 @@ int32_t op_export_submap_states(b2s_handle* h, int n, const b2s_submap* const* s
   B2S_CUDA(cudaGetLastError());
 
   // synchronisation 1: the byte offsets
-  long long* hb = reinterpret_cast<long long*>(st + staged);
+  long long* hb = reinterpret_cast<long long*>(st + t_base);
   B2S_CUDA(cudaMemcpyAsync(hb, base, ((size_t)n + 1) * 8, cudaMemcpyDeviceToHost, h->stream));
   B2S_TRY(check_status(h));
   const size_t total = (size_t)hb[n];
